@@ -8,6 +8,9 @@ Names and argument meaning follow the reference (rrwick/Autocycler v0.6.1):
     unitig_graph.save_gfa(path, seqs)                          unitig_graph.rs:317-331
     load_sequences(assemblies_dir, k_size, max_contigs)        compress.rs:98-133
     compress(assemblies_dir, autocycler_dir, k_size, ...)      compress.rs:32-50
+    trim_path_start_end / _hairpin_start / _hairpin_end         trim.rs:288-326 (batch forms over lists of paths)
+    unitig_graph.trim(min_identity, max_unitigs, mad)          trim.rs:43-51 (trim minus the file I/O)
+    trim(cluster_dir, min_identity, max_unitigs, mad, ...)     trim.rs:36-53
 
 There is no CPU path here: if the CUDA library is missing, or no device is present, every entry
 point raises.
@@ -48,7 +51,7 @@ class AcUnitigs(C.Structure):
 
 class AcTimings(C.Structure):
     _fields_ = [(n, C.c_float) for n in ("h2d", "pack", "insert", "adjacency", "boundaries", "runs", "unitigs", "links", "seed_sort", "emit", "d2h",
-                                        "device_total", "host_graph", "host_simplify", "host_gfa", "sample", "device_simplify", "device_gfa", "insert_kernel", "reserved0")] + \
+                                        "device_total", "host_graph", "host_simplify", "host_gfa", "sample", "device_simplify", "device_gfa", "insert_kernel", "trim_kernel")] + \
                [(n, C.c_uint64) for n in ("insert_occurrences", "table_capacity", "table_used", "kernel_launches", "h2d_bytes", "d2h_bytes")]
 
     def as_dict(self):
@@ -60,7 +63,8 @@ EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_seq
            "ac_timings_get", "ac_compress_dir", "ac_compress_dir_devices", "ac_load_sequences", "ac_sequence_get",
            "ac_build_local", "ac_entries_count", "ac_entries_export", "ac_entries_merge", "ac_runs_local", "ac_runs_export",
            "ac_runs_import", "ac_runs_import_padded", "ac_build_finish", "ac_compress_finish", "ac_gfa_data",
-           "ac_compress_finish_split", "ac_path_tokens_export", "ac_path_lines_render", "ac_path_lines_data", "ac_upload_shard", "ac_strand_block"]
+           "ac_compress_finish_split", "ac_path_tokens_export", "ac_path_lines_render", "ac_path_lines_data", "ac_upload_shard", "ac_strand_block",
+           "ac_trim_paths", "ac_trim", "ac_trim_yaml", "ac_trim_stats", "ac_trim_dir"]
 
 _libs = {}
 
@@ -119,6 +123,12 @@ def load_library(path=None):
     lib.ac_path_lines_render.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
     lib.ac_path_lines_data.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
     lib.ac_gfa_data.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
+    lib.ac_trim_paths.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_uint64), C.c_uint64, C.POINTER(C.c_uint32),
+                                  C.c_uint64, C.c_double, C.c_uint32, C.POINTER(C.c_int32), C.POINTER(C.c_uint64), C.POINTER(C.c_uint8)]
+    lib.ac_trim.argtypes = [C.c_void_p, C.c_double, C.c_uint32, C.c_double]
+    lib.ac_trim_yaml.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
+    lib.ac_trim_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]
+    lib.ac_trim_dir.argtypes = [C.c_char_p, C.c_double, C.c_uint32, C.c_double, C.c_uint32, C.c_int32, C.c_int32]
     _libs[path] = lib
     return lib
 
@@ -336,6 +346,23 @@ class UnitigGraph:
         self._h.check(self._h.lib.ac_sequence_reconstruct(self._h.ptr, index, buf, n.value, C.byref(n)))
         return buf.raw[:n.value].decode()
 
+    def trim(self, min_identity=0.75, max_unitigs=5000, mad=5.0):   # trim.rs:43-51 on this (loaded) graph
+        """Start-end and hairpin trimming (alignments on the GPU), length outliers, clean-up: afterwards the graph and its sequences are
+        2_trimmed.gfa's; trimmed_yaml() is 2_trimmed.yaml and timings().trim_kernel the alignment kernels' time."""
+        self._h.check(self._h.lib.ac_trim(self._h.ptr, min_identity, max_unitigs, mad))
+
+    def trimmed_yaml(self):   # TrimmedClusterMetrics (metrics.rs:209-225) after trim()
+        n = C.c_uint64()
+        self._h.check(self._h.lib.ac_trim_yaml(self._h.ptr, None, 0, C.byref(n)))
+        buf = C.create_string_buffer(max(1, n.value))
+        self._h.check(self._h.lib.ac_trim_yaml(self._h.ptr, buf, n.value, C.byref(n)))
+        return buf.raw[:n.value].decode()
+
+    def trim_stats(self):   # what the last trim aligned
+        jobs, cells, path = C.c_uint64(), C.c_uint64(), C.c_uint64(); window = C.c_uint32()
+        self._h.check(self._h.lib.ac_trim_stats(self._h.ptr, C.byref(jobs), C.byref(cells), C.byref(window), C.byref(path)))
+        return {"alignments": jobs.value, "dp_cells": cells.value, "max_window": window.value, "max_path": path.value}
+
     def save_gfa(self, gfa_filename, sequences=None, use_other_colour=False):   # unitig_graph.rs:317-331
         with open(gfa_filename, "wb") as f:
             f.write(self.gfa_bytes())
@@ -383,5 +410,53 @@ def compress(assemblies_dir, autocycler_dir, k_size=51, max_contigs=25, threads=
     devs = list(devices) if devices else [device]
     rc = lib.ac_compress_dir_devices(os.fsencode(assemblies_dir), os.fsencode(autocycler_dir), k_size, max_contigs, threads,
                                      (C.c_int32 * len(devs))(*devs), len(devs), 1 if verbose else 0)
+    if rc != AC_OK:
+        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+
+
+TRIM_START_END, TRIM_HAIRPIN_START, TRIM_HAIRPIN_END = 0, 1, 2
+
+
+def _trim_paths(mode, paths, weights, min_identity, max_unitigs, lib=None, device=0, handle=None):
+    """One trim.rs:288-326 trim of every path in `paths` (lists of signed unitig numbers); weights: {unitig: length} or a list indexed
+    by unitig number.  -> [trimmed path or None]"""
+    lib = lib or load_library()
+    h = handle or _Handle(lib, 51, device)
+    if isinstance(weights, dict):
+        w = [0] * (max(weights) + 1 if weights else 1)
+        for u, ln in weights.items():
+            w[u] = ln
+    else:
+        w = list(weights)
+    flat = [u for p in paths for u in p]
+    off = [0]
+    for p in paths:
+        off.append(off[-1] + len(p))
+    n = len(paths)
+    vals = (C.c_int32 * max(1, len(flat)))(*flat)
+    out = (C.c_int32 * max(1, len(flat)))()
+    out_off = (C.c_uint64 * (n + 1))()
+    trimmed = (C.c_uint8 * max(1, n))()
+    h.check(lib.ac_trim_paths(h.ptr, mode, vals, (C.c_uint64 * (n + 1))(*off), n, (C.c_uint32 * max(1, len(w)))(*w), len(w),
+                              float(min_identity), max_unitigs, out, out_off, trimmed))
+    return [list(out[out_off[x]:out_off[x + 1]]) if trimmed[x] else None for x in range(n)]
+
+
+def trim_path_start_end(paths, weights, min_identity, max_unitigs, **kw):      # trim.rs:288-296
+    return _trim_paths(TRIM_START_END, paths, weights, min_identity, max_unitigs, **kw)
+
+
+def trim_path_hairpin_start(paths, weights, min_identity, max_unitigs, **kw):  # trim.rs:320-326
+    return _trim_paths(TRIM_HAIRPIN_START, paths, weights, min_identity, max_unitigs, **kw)
+
+
+def trim_path_hairpin_end(paths, weights, min_identity, max_unitigs, **kw):    # trim.rs:299-317
+    return _trim_paths(TRIM_HAIRPIN_END, paths, weights, min_identity, max_unitigs, **kw)
+
+
+def trim(cluster_dir, min_identity=0.75, max_unitigs=5000, mad=5.0, threads=8, device=0, verbose=False, lib=None):
+    """trim.rs:36-53: reads <cluster_dir>/1_untrimmed.gfa, writes 2_trimmed.gfa and 2_trimmed.yaml."""
+    lib = lib or load_library()
+    rc = lib.ac_trim_dir(os.fsencode(cluster_dir), float(min_identity), max_unitigs, float(mad), threads, device, 1 if verbose else 0)
     if rc != AC_OK:
         raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())

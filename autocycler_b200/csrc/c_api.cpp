@@ -16,6 +16,7 @@
 #include "backend.h"
 #include "host_graph.h"
 #include "host_io.h"
+#include "host_trim.h"
 #include <immintrin.h>
 #include <functional>
 #include <thread>
@@ -65,6 +66,8 @@ struct ac_handle {
     bool graph_ready = false;                                // h->graph describes the current graph
     ac_timings t{};
     uint64_t links_now = 0;
+    std::string trim_yaml; bool trimmed = false;           // ac_trim: 2_trimmed.yaml
+    TrimStats trim_stats;
 };
 
 static int set_error(const ac_handle* h, int code, const std::string& msg) {
@@ -281,7 +284,7 @@ static void record_timings(ac_handle* h) {
     t.h2d = pt.h2d; t.pack = pt.pack; t.insert = pt.insert; t.adjacency = pt.adjacency; t.boundaries = pt.boundaries; t.runs = pt.runs;
     t.unitigs = pt.unitigs; t.links = pt.links; t.seed_sort = pt.seed_sort; t.emit = pt.emit; t.d2h = pt.d2h; t.device_total = pt.total;
     t.sample = pt.sample; t.device_simplify = pt.simplify; t.device_gfa = pt.gfa;
-    t.insert_kernel = pt.insert_kernel; t.reserved0 = 0;
+    t.insert_kernel = pt.insert_kernel; t.trim_kernel = 0;
     uint64_t windows = 0; for (auto& s : h->seqs) windows += s.length;
     t.insert_occurrences = windows; t.table_capacity = h->res.capacity; t.table_used = h->res.n_slots_used;
     t.kernel_launches = h->pipe->kernel_launches();
@@ -553,6 +556,7 @@ int ac_load_gfa(ac_handle* h, const char* gfa_text, uint64_t length) {
     h->built = false; h->gfa_ready = false; h->uploaded = false; h->device_text_ok = false; h->fused = false; h->graph_ready = false;
     h->seqs.clear(); h->infos.clear(); h->ascii.clear(); h->loaded = LoadedInput(); h->res = PipelineResult(); h->t = ac_timings{};   // a loaded graph has no sequence bytes: ac_upload / ac_build need ac_add_sequence again
     h->graph.device_sort = nullptr;
+    h->trimmed = false; h->trim_yaml.clear();
     h->graph.load_gfa(gfa_text, (size_t)length, h->seqs);
     h->cfg.k = h->graph.k;
     h->built = true; h->graph_ready = true;
@@ -981,6 +985,117 @@ int ac_decompress_gfa(const char* in_gfa, const char* out_dir, const char* out_f
         fclose(f);
         if (verbose) fprintf(stderr, "\n");
     }
+    return ok(h);
+    AC_GUARD_END(nullptr)
+}
+
+// trim.rs:288-326 for a batch of caller paths, one device round of overlap alignments
+int ac_trim_paths(ac_handle* h, int32_t mode, const int32_t* paths, const uint64_t* path_off, uint64_t n_paths,
+                  const uint32_t* weights, uint64_t n_weights, double min_identity, uint32_t max_unitigs,
+                  int32_t* out, uint64_t* out_off, uint8_t* trimmed) {
+    if (!h || !path_off || !weights || !out_off || !trimmed || (n_paths && path_off[n_paths] && (!paths || !out))) return set_error(h, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    if (mode != AC_TRIM_START_END && mode != AC_TRIM_HAIRPIN_START && mode != AC_TRIM_HAIRPIN_END) return set_error(h, AC_EINVAL, "unknown trim mode");
+    std::vector<std::vector<int32_t>> in(n_paths), res;
+    for (uint64_t x = 0; x < n_paths; ++x) {
+        if (path_off[x + 1] < path_off[x]) return set_error(h, AC_EINVAL, "path offsets must not decrease");
+        in[x].assign(paths + path_off[x], paths + path_off[x + 1]);
+        for (int32_t u : in[x]) {
+            const int64_t a = u < 0 ? -(int64_t)u : u;
+            if (u == 0 || (uint64_t)a >= n_weights) return set_error(h, AC_EINVAL, "path entry " + std::to_string(u) + " has no weight");
+        }
+    }
+    std::vector<uint32_t> w(weights, weights + n_weights);
+    std::vector<uint8_t> ok_flags;
+    TrimStats st;
+    trim_paths(*h->pipe, (TrimMode)mode, in, w, min_identity, max_unitigs, ok_flags, res, st);
+    uint64_t at = 0;
+    out_off[0] = 0;
+    for (uint64_t x = 0; x < n_paths; ++x) {
+        trimmed[x] = ok_flags[x];
+        if (ok_flags[x]) { std::copy(res[x].begin(), res[x].end(), out + at); at += res[x].size(); }
+        out_off[x + 1] = at;
+    }
+    h->t.trim_kernel = st.kernel_ms; h->trim_stats = st;
+    return ok(h);
+    AC_GUARD_END(h)
+}
+
+int ac_trim(ac_handle* h, double min_identity, uint32_t max_unitigs, double mad) {
+    if (!h) return set_error(nullptr, AC_EINVAL, "null handle");
+    AC_GUARD_BEGIN
+    if (!h->built) return set_error(h, AC_EINVAL, "a graph must be built or loaded before ac_trim");
+    ensure_graph(h);
+    TrimStats st;
+    trim_graph(h->graph, h->seqs, *h->pipe, min_identity, max_unitigs, mad, false, st);
+    h->infos.clear(); h->ascii.clear();      // the sequences are trimmed paths now: no bytes
+    h->trim_yaml = trimmed_metrics_yaml(h->seqs); h->trimmed = true;
+    h->t.trim_kernel = st.kernel_ms; h->trim_stats = st;
+    h->gfa_ready = false; h->device_text_ok = false;
+    return ok(h);
+    AC_GUARD_END(h)
+}
+
+int ac_trim_yaml(ac_handle* h, char* out, uint64_t cap, uint64_t* length) {
+    if (!h || !length) return set_error(h, AC_EINVAL, "null argument");
+    if (!h->trimmed) return set_error(h, AC_EINVAL, "ac_trim must precede ac_trim_yaml");
+    *length = h->trim_yaml.size();
+    if (!out) return ok(h);
+    if (cap < h->trim_yaml.size()) return set_error(h, AC_ERANGE, "buffer too small");
+    memcpy(out, h->trim_yaml.data(), h->trim_yaml.size());
+    return ok(h);
+}
+
+int ac_trim_stats(const ac_handle* h, uint64_t* jobs, uint64_t* cells, uint32_t* max_window, uint64_t* max_path) {
+    if (!h) return set_error(nullptr, AC_EINVAL, "null handle");
+    if (jobs) *jobs = h->trim_stats.jobs;
+    if (cells) *cells = h->trim_stats.cells;
+    if (max_window) *max_window = h->trim_stats.max_window;
+    if (max_path) *max_path = h->trim_stats.max_path;
+    return ok(h);
+}
+
+int ac_trim_dir(const char* cluster_dir, double min_identity, uint32_t max_unitigs, double mad, uint32_t threads, int32_t device, int32_t verbose) {
+    if (!cluster_dir) return set_error(nullptr, AC_EINVAL, "null argument");
+    ac_handle* h = nullptr;
+    AC_GUARD_BEGIN
+    // check_settings, trim.rs:56-67 (misc.rs:98-119)
+    const std::string dir = cluster_dir, in_gfa = dir + "/1_untrimmed.gfa", out_gfa = dir + "/2_trimmed.gfa", out_yaml = dir + "/2_trimmed.yaml";
+    struct stat st;
+    if (stat(cluster_dir, &st) != 0) return set_error(nullptr, AC_EINPUT, "directory does not exist: " + dir);
+    if (!S_ISDIR(st.st_mode)) return set_error(nullptr, AC_EINPUT, dir + " is not a directory");
+    if (stat(in_gfa.c_str(), &st) != 0) return set_error(nullptr, AC_EINPUT, "file does not exist: " + in_gfa);
+    if (!S_ISREG(st.st_mode)) return set_error(nullptr, AC_EINPUT, in_gfa + " is not a file");
+    if (!(min_identity >= 0.0 && min_identity <= 1.0)) return set_error(nullptr, AC_EINPUT, "--min_identity must be between 0.0 and 1 (inclusive)");
+    if (threads < 1) return set_error(nullptr, AC_EINPUT, "--threads cannot be less than 1");
+    if (threads > 100) return set_error(nullptr, AC_EINPUT, "--threads cannot be greater than 100");
+    if (mad < 0.0) return set_error(nullptr, AC_EINPUT, "--mad cannot be less than 0");
+    std::string text;
+    {
+        FILE* f = fopen(in_gfa.c_str(), "rb");
+        if (!f) return set_error(nullptr, AC_EIO, "cannot read " + in_gfa);
+        char buf[1 << 16]; size_t n;
+        while ((n = fread(buf, 1, sizeof buf, f)) > 0) text.append(buf, n);
+        fclose(f);
+    }
+    ac_config cfg{}; cfg.k = 51; cfg.device = device; cfg.stream = nullptr; cfg.keep_positions = 0; cfg.n_devices = 1; cfg.devices = nullptr;
+    int rc = ac_create(&h, &cfg);
+    if (rc != AC_OK) return rc;
+    std::unique_ptr<ac_handle, void (*)(ac_handle*)> guard(h, ac_destroy);
+    if ((rc = ac_load_gfa(h, text.data(), text.size())) != AC_OK) { g_error = h->err; return rc == AC_EINVAL ? AC_EINPUT : rc; }
+    if (verbose && max_unitigs == 0) fprintf(stderr, "Since --max_unitigs was set to 0, trimming is disabled.\n\n");
+    TrimStats ts;
+    trim_graph(h->graph, h->seqs, *h->pipe, min_identity, max_unitigs, mad, verbose != 0, ts);
+    h->graph.gfa_text(h->seqs, h->gfa);
+    FILE* f = fopen(out_gfa.c_str(), "wb");
+    if (!f || fwrite(h->gfa.data(), 1, h->gfa.size(), f) != h->gfa.size()) { if (f) fclose(f); return set_error(nullptr, AC_EIO, "cannot write " + out_gfa); }
+    fclose(f);
+    const std::string yaml = trimmed_metrics_yaml(h->seqs);
+    f = fopen(out_yaml.c_str(), "wb");
+    if (!f || fwrite(yaml.data(), 1, yaml.size(), f) != yaml.size()) { if (f) fclose(f); return set_error(nullptr, AC_EIO, "cannot write " + out_yaml); }
+    fclose(f);
+    if (verbose) fprintf(stderr, "\nFinished!\nUnitig graph of trimmed sequences: %s\n(%llu alignments, %llu DP cells, alignment kernels %.2f ms)\n\n", out_gfa.c_str(),
+                         (unsigned long long)ts.jobs, (unsigned long long)ts.cells, (double)ts.kernel_ms);
     return ok(h);
     AC_GUARD_END(nullptr)
 }

@@ -1,4 +1,4 @@
-// `autocycler compress` and `autocycler decompress` with the reference's flags (main.rs:126-162), messages and exit codes
+// `autocycler compress`, `autocycler decompress` and `autocycler trim` with the reference's flags (main.rs:126-162), messages and exit codes
 // (misc.rs:130-136: "Error: <text>" on stderr, exit 1), running the H100 path through the C ABI.
 #include <cstdio>
 #include <cstdlib>
@@ -43,8 +43,40 @@ static int decompress_main(int argc, char** argv) {
     return 0;
 }
 
+// `autocycler trim` (main.rs:301-322, trim.rs:36-101)
+static int trim_main(int argc, char** argv) {
+    static const char* trim_usage = "Usage: autocycler trim --cluster_dir <CLUSTER_DIR> [--min_identity 0.75] [--max_unitigs 5000] [--mad 5.0] [--threads 8] [--device N]\n";
+    std::string dir; double min_identity = 0.75, mad = 5.0; unsigned long max_unitigs = 5000, threads = 8; int device = 0;
+    for (int i = 2; i < argc; ++i) {
+        std::string a = argv[i];
+        auto value = [&]() -> const char* { if (i + 1 >= argc) { fprintf(stderr, "error: a value is required for '%s'\n", a.c_str()); exit(2); } return argv[++i]; };
+        auto number = [&](const char* v, bool integral) -> double {
+            char* end = nullptr; const double x = integral ? (double)strtoul(v, &end, 10) : strtod(v, &end);
+            if (!*v || *end || (integral && (*v == '-' || *v == '+'))) { fprintf(stderr, "error: invalid value '%s' for '%s'\n%s", v, a.c_str(), trim_usage); exit(2); }
+            return x;
+        };
+        if (a == "-c" || a == "--cluster_dir") dir = value();
+        else if (a == "--min_identity") min_identity = number(value(), false);
+        else if (a == "--max_unitigs") max_unitigs = (unsigned long)number(value(), true);
+        else if (a == "--mad") mad = number(value(), false);
+        else if (a == "-t" || a == "--threads") threads = (unsigned long)number(value(), true);
+        else if (a == "--device") device = atoi(value());
+        else if (a == "-h" || a == "--help") { fprintf(stderr, "%s", trim_usage); return 0; }
+        else { fprintf(stderr, "error: unexpected argument '%s'\n%s", a.c_str(), trim_usage); return 2; }
+    }
+    if (dir.empty()) { fprintf(stderr, "%s", trim_usage); return 2; }
+    if (max_unitigs > 0xFFFFFFFFul) max_unitigs = 0xFFFFFFFFul;
+    if (threads > 0xFFFFFFFFul) threads = 0xFFFFFFFFul;
+    fprintf(stderr, "\nStarting autocycler trim (%s)\n\nSettings:\n  --cluster_dir %s\n  --min_identity %g\n  --max_unitigs %lu\n  --mad %g\n  --threads %lu\n\n",
+            ac_version(), dir.c_str(), min_identity, max_unitigs, mad, threads);
+    const int rc = ac_trim_dir(dir.c_str(), min_identity, (uint32_t)max_unitigs, mad, (uint32_t)threads, device, 1);
+    if (rc != AC_OK) { fprintf(stderr, "\nError: %s\n", ac_last_error(nullptr)); return 1; }
+    return 0;
+}
+
 int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "decompress") == 0) return decompress_main(argc, argv);
+    if (argc >= 2 && strcmp(argv[1], "trim") == 0) return trim_main(argc, argv);
     if (argc < 2 || strcmp(argv[1], "compress") != 0) { usage(); return 2; }
     std::string in, out; unsigned k = 51, max_contigs = 25, threads = 8; int device = 0;
     std::vector<int32_t> devices;

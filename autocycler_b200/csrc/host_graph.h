@@ -72,6 +72,11 @@ public:
     // UnitigGraph::from_gfa_lines (unitig_graph.rs:55-174; host_gfa_load.cpp): replaces the graph by the one in `text`, returns its sequences
     void load_gfa(const char* text, size_t len, std::vector<HostSeq>& seqs);
     void merge_linear_paths(bool use_paths);  // graph_simplification.rs:315-371 (host_merge.cpp); use_paths=false is the reference's `seqs` = [] and drops the paths
+    // trim's graph edits (host_trim.cpp).  replace_paths: the sequence paths become `paths` (one per kept sequence, in order) — what
+    // remove_sequence_from_graph + create_sequence_and_positions (unitig_graph.rs:151-174, 566-573) do to the positions.
+    void replace_paths(const std::vector<std::vector<UStrand>>& paths);
+    void recalculate_depths();                // unitig_graph.rs:575-580: depth = forward_positions.len() = path steps through the unitig
+    void remove_zero_depth_unitigs();         // unitig_graph.rs:582-586, with delete_dangling_links (:547-564)
     void gfa_text(const std::vector<HostSeq>& seqs, std::string& out) const;   // unitig_graph.rs:317-360
     uint64_t total_length() const;
     uint64_t link_count_single() const;       // unitig_graph.rs:478-507 (.1)

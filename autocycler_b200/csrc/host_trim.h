@@ -1,0 +1,34 @@
+// `autocycler trim` (trim.rs:36-326) on the host graph, with the overlap alignments on the device (DevicePipeline::overlap_align).
+#pragma once
+#include <cstdint>
+#include <string>
+#include <vector>
+
+#include "host_graph.h"
+
+class DevicePipeline;
+
+enum TrimMode { TRIM_START_END = 0, TRIM_HAIRPIN_START = 1, TRIM_HAIRPIN_END = 2 };
+
+struct TrimStats {
+    float kernel_ms = 0;          // overlap_align kernels, CUDA events (0 under emulation)
+    uint32_t rounds = 0;          // overlap_align batches
+    uint64_t jobs = 0;            // alignments
+    uint64_t cells = 0;           // sum of k^2 over the alignments
+    uint32_t max_window = 0;      // largest k
+    uint64_t max_path = 0;        // longest path aligned
+};
+
+// trim_path_start_end / trim_path_hairpin_start / trim_path_hairpin_end (trim.rs:288-326) for every path of a batch, one device round.
+// weights[|unitig|] = unitig length.  trimmed[x] = 0: path x is not trimmed (out[x] is empty).
+void trim_paths(DevicePipeline& pipe, TrimMode mode, const std::vector<std::vector<int32_t>>& paths, const std::vector<uint32_t>& weights,
+                double min_identity, uint32_t max_unitigs, std::vector<uint8_t>& trimmed, std::vector<std::vector<int32_t>>& out, TrimStats& stats);
+
+// trim.rs:43-51 minus the file I/O: trims the sequences' paths, drops length outliers, cleans up the graph (recalculate_depths,
+// remove_zero_depth_unitigs, merge_linear_paths, renumber_unitigs).  `seqs` becomes the kept sequences in their order.  verbose: the
+// reference's stderr report.
+void trim_graph(HostGraph& g, std::vector<HostSeq>& seqs, DevicePipeline& pipe, double min_identity, uint32_t max_unitigs, double mad,
+                bool verbose, TrimStats& stats);
+
+// TrimmedClusterMetrics (metrics.rs:209-225) of the sequence lengths, as serde_yaml 0.9 writes it (2_trimmed.yaml)
+std::string trimmed_metrics_yaml(const std::vector<HostSeq>& seqs);

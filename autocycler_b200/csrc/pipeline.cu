@@ -1649,6 +1649,112 @@ template <int WH> struct LiteralScanBody {
     }
 };
 
+// ------------------------------------------------------------------------------------------------
+// trim: overlap alignment of unitig paths (trim.rs:366-479), see DESIGN.md §9
+// ------------------------------------------------------------------------------------------------
+// Every score is a sum of +w, -w and -(wi+wj)/2 with integral w < 2^32, so it is a multiple of 0.5 far below 2^52: f64 adds are exact
+// and the matrix is the same in any evaluation order (the CTA's anti-diagonal sweep, the emulation's row-major loop, the reference's).
+// The matrix itself is not kept: the traceback needs S[i-1][j] >= S[i][j-1] (:443) and path equality (:436), so the fill stores that
+// one comparison per cell, packed 32 cells to a word along anti-diagonals (d = i + j); each diagonal starts on a word boundary.
+#define AC_TRIM_GAP 0
+#define AC_TRIM_NONE (-1)
+AC_HD uint32_t trim_diag_lo(uint32_t d, uint32_t k) { return d > k ? d - k : 1u; }     // first row i of anti-diagonal d (2 <= d <= 2k)
+AC_HD uint32_t trim_diag_words(uint32_t d, uint32_t k) {                             // 32-bit words of diagonal d's bits (0 outside 2..2k)
+    if (d < 2 || d > 2 * k) return 0;
+    const uint32_t hi = d - 1 < k ? d - 1 : k;
+    return (hi - trim_diag_lo(d, k) + 1 + 31) / 32;
+}
+AC_HD uint64_t trim_bit_words(uint32_t k) { uint64_t w = 0; for (uint32_t d = 2; d <= 2 * k; ++d) w += trim_diag_words(d, k); return w; }
+// :396-405, one cell: the diagonal, up (i-1, j) and left (i, j-1) scores, the two unitigs and their weights
+AC_HD double trim_cell(double diag, double up, double left, int32_t a, int32_t b, double wa, double wb) {
+    const double match_score = diag + (a == b ? wa : -(wa + wb) / 2.0);
+    const double delete_score = up - wa, insert_score = left - wb;
+    const double m = match_score > delete_score ? match_score : delete_score;      // f64::max without NaNs
+    return m > insert_score ? m : insert_score;
+}
+// :413-419: the right edge S[i][k] is visited with i ascending and a strict > keeps the smallest i among ties
+AC_HD void trim_edge(double s, uint32_t i, double& best, uint32_t& best_i) { if (s > best) { best = s; best_i = i; } }
+// :431-461 from (max_i, k): writes the pieces in traceback order (last column first) and returns their count, or 0 when the walk ends
+// on the left edge (i > 0).  pa = path_a (its first k entries are rows 1..k), pb = path_b + n - k (columns 1..k), bits as above.
+AC_HD uint32_t trim_traceback(const int32_t* pa, const int32_t* pb, uint32_t n, uint32_t k, const uint32_t* bits, uint32_t max_i, AlignPiece* out) {
+    uint32_t i = max_i, j = k, cnt = 0;
+    uint64_t off = 0;
+    for (uint32_t d = 2; d < i + j; ++d) off += trim_diag_words(d, k);
+    while (i > 0 && j > 0) {
+        const uint32_t d = i + j;
+        const int32_t a = pa[i - 1], b = pb[j - 1];
+        const int32_t gi = (int32_t)(i - 1), gj = (int32_t)(n - k + j - 1);
+        if (a == b) {
+            out[cnt++] = AlignPiece{a, gi, b, gj};
+            --i; --j;
+            off -= trim_diag_words(d - 1, k) + trim_diag_words(d - 2, k);
+        } else {
+            const uint32_t t = i - trim_diag_lo(d, k);
+            if ((bits[off + t / 32] >> (t % 32)) & 1u) { out[cnt++] = AlignPiece{a, gi, AC_TRIM_GAP, AC_TRIM_NONE}; --i; }
+            else { out[cnt++] = AlignPiece{AC_TRIM_GAP, AC_TRIM_NONE, b, gj}; --j; }
+            off -= trim_diag_words(d - 1, k);
+        }
+    }
+    return i > 0 ? 0 : cnt;
+}
+// Per job: where its bit words, its traceback output (2k pieces), and, for windows beyond shared memory, its three diagonals (HBM) live.
+struct TrimLaunchJob { uint64_t a_off, b_off, bits_off, out_off, scratch_off; uint32_t n, k, skip, slot; };
+
+#ifndef AC_EMULATE
+// One CTA per job sweeps the 2k-1 anti-diagonals; the three live ones (d-2, d-1, d, indexed by row i) sit in shared memory, or in the
+// job's HBM scratch when 24 (k + 1) bytes exceed the CTA's shared memory (same code, another base pointer).  A thread owns a cell per
+// 1024 of its diagonal: the two path entries it reads are adjacent to its neighbours' (coalesced), and its warp packs the 32 traceback
+// bits with one ballot into one word.  Thread 0 then runs the O(k) traceback over those bits.
+__global__ void __launch_bounds__(1024) ac_overlap_align_kernel(const TrimLaunchJob* __restrict__ jobs, const int32_t* __restrict__ values,
+                                                                const uint32_t* __restrict__ weights, uint32_t* __restrict__ bits,
+                                                                double* scratch, AlignPiece* __restrict__ out, uint32_t* __restrict__ out_len, int use_shared) {
+    extern __shared__ double trim_smem[];
+    __shared__ double best;
+    __shared__ uint32_t best_i;
+    const TrimLaunchJob J = jobs[blockIdx.x];
+    const uint32_t k = J.k, tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    double* D = use_shared ? trim_smem : scratch + J.scratch_off;
+    const int32_t* pa = values + J.a_off;
+    const int32_t* pb = values + J.b_off + (J.n - k);
+    uint32_t* B = bits + J.bits_off;
+    const uint32_t diag_shift = J.n - k;             // global_i == global_j  <=>  i - 1 == n - k + j - 1
+    if (tid == 0) { best = -INFINITY; best_i = 0; }
+    uint64_t off = 0;
+    for (uint32_t d = 2; d <= 2 * k; ++d) {
+        double* cur = D + (size_t)(d % 3) * (k + 1);
+        const double* prev = D + (size_t)((d - 1) % 3) * (k + 1);
+        const double* prev2 = D + (size_t)((d - 2) % 3) * (k + 1);
+        const uint32_t lo = trim_diag_lo(d, k), hi = d - 1 < k ? d - 1 : k, len = hi - lo + 1;
+        for (uint32_t base = 0; base < len; base += blockDim.x) {      // the same trip count for every thread: all lanes reach the ballot
+            const uint32_t t = base + tid;
+            bool up_wins = false;
+            if (t < len) {
+                const uint32_t i = lo + t, j = d - i;
+                const double up = i == 1 ? 0.0 : prev[i - 1];
+                const double left = j == 1 ? 0.0 : prev[i];
+                up_wins = up >= left;
+                double s = -INFINITY;
+                if (!(J.skip && i == j + diag_shift)) {
+                    const double diag = (i == 1 || j == 1) ? 0.0 : prev2[i - 1];
+                    const int32_t a = pa[i - 1], b = pb[j - 1];
+                    s = trim_cell(diag, up, left, a, b, (double)__ldg(weights + (a < 0 ? -a : a)), (double)__ldg(weights + (b < 0 ? -b : b)));
+                }
+                cur[i] = s;
+                if (j == k) trim_edge(s, i, best, best_i);         // one cell per diagonal, rows in ascending order
+            }
+            const uint32_t word = __ballot_sync(0xFFFFFFFFu, up_wins);
+            if (lane == 0 && base + warp * 32 < len) B[off + base / 32 + warp] = word;
+        }
+        off += (len + 31) / 32;
+        __syncthreads();
+    }
+    if (tid == 0) {
+        AlignPiece* o = out + J.out_off;
+        out_len[J.slot] = best > 0.0 ? trim_traceback(pa, pb, J.n, k, B, best_i, o) : 0;      // :422 max_score <= 0: no alignment
+    }
+}
+#endif
+
 #ifndef AC_EMULATE
 // Product scan: tiles of 4096 values, coalesced loads, warp-shuffle block scans (the functor bodies above are the
 // host-emulation form of the same two phases).
@@ -1920,6 +2026,7 @@ struct DevicePipeline::Impl {
     void do_import_runs(const void* dev_ptr, uint64_t n);
     void do_import_runs_from(const void* const* ptrs, const uint64_t* counts, uint32_t n_ranks);
     DevBuf own_entries, own_runs;
+    DevBuf trim_jobs, trim_vals, trim_w, trim_bits, trim_scratch, trim_out, trim_len;      // overlap_align
 #ifdef AC_EMULATE
     // AC_EMU_POISON=1 (CPU suite): before every table build, every device buffer a kernel writes is filled with a pattern, so a kernel that
     // reads what THIS build has not written (on the GPU: leftovers of the previous build, whose slot numbers differ from run to run, while
@@ -2048,6 +2155,122 @@ void DevicePipeline::pair_shared_lengths(const UStrand* path, const uint64_t* pa
     ac_launch("pair_share", &m.stream, PairShareBody{m.dist_member.as<uint32_t>(), m.d_len.as<uint32_t>(), n, words, m.dist_shared.as<unsigned long long>()}, U);
     ac_d2h(shared, m.dist_shared.p, (size_t)n * n * 8, &m.stream);
     ac_sync(&m.stream);
+}
+
+uint32_t DevicePipeline::overlap_shared_k_max() {
+#ifndef AC_EMULATE
+    impl->set_device();
+    static int optin = -1;                           // one device model per process
+    if (optin < 0) { int dev = 0; AC_CUDA_CHECK(cudaGetDevice(&dev)); AC_CUDA_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev)); }
+    const int budget = optin - 64;                   // the kernel's own static shared variables
+#else
+    const int budget = 227 * 1024 - 64;              // what an H100 grants one CTA
+#endif
+    return (uint32_t)(budget / 24) - 1;
+}
+
+float DevicePipeline::overlap_align(const int32_t* values, uint64_t n_values, const uint32_t* weights, uint64_t n_weights,
+                                    const OverlapJob* jobs, uint32_t n_jobs, std::vector<std::vector<AlignPiece>>& out) {
+    Impl& m = *impl; m.set_device();
+    out.assign(n_jobs, {});
+    const uint32_t shared_k = overlap_shared_k_max();
+    // windows of k = 0 have no cell; the others are launched largest first (a CTA per job, the long ones start before the short ones)
+    std::vector<uint32_t> run;
+    for (uint32_t x = 0; x < n_jobs; ++x) {
+        if (jobs[x].k > jobs[x].n) throw std::runtime_error("overlap_align: window larger than the path");
+        if (jobs[x].k > 0) run.push_back(x);
+    }
+    if (run.empty()) return 0.f;
+    std::stable_sort(run.begin(), run.end(), [&](uint32_t a, uint32_t b) { return jobs[a].k > jobs[b].k; });
+    std::vector<TrimLaunchJob> lj(run.size());
+    uint64_t bits_words = 0, out_pieces = 0, scratch = 0;
+    uint32_t n_shared = 0, k_shared = 0;
+    for (size_t r = 0; r < run.size(); ++r) {
+        const OverlapJob& J = jobs[run[r]];
+        if (J.a_off + J.n > n_values || J.b_off + J.n > n_values) throw std::runtime_error("overlap_align: path outside the value array");
+        TrimLaunchJob& L = lj[r];
+        L.a_off = J.a_off; L.b_off = J.b_off; L.n = J.n; L.k = J.k; L.skip = J.skip_diagonal ? 1 : 0; L.slot = (uint32_t)r;
+        L.bits_off = bits_words; bits_words += trim_bit_words(J.k);
+        L.out_off = out_pieces; out_pieces += 2ull * J.k;
+        L.scratch_off = 0;
+        if (J.k <= shared_k) { ++n_shared; k_shared = std::max(k_shared, J.k); }
+        else { L.scratch_off = scratch; scratch += 3ull * (J.k + 1); }
+    }
+    // jobs with shared-memory diagonals first (largest first), then the ones whose diagonals live in HBM
+    std::stable_partition(lj.begin(), lj.end(), [&](const TrimLaunchJob& L) { return L.k <= shared_k; });
+    m.trim_jobs.ensure(lj.size() * sizeof(TrimLaunchJob)); m.trim_vals.ensure(n_values * 4 + 4); m.trim_w.ensure(n_weights * 4 + 4);
+    m.trim_bits.ensure(bits_words * 4 + 4); m.trim_out.ensure(out_pieces * sizeof(AlignPiece) + 16); m.trim_len.ensure(run.size() * 4);
+    m.trim_scratch.ensure(scratch * 8 + 8);
+    ac_h2d(m.trim_jobs.p, lj.data(), lj.size() * sizeof(TrimLaunchJob), &m.stream);
+    if (n_values) ac_h2d(m.trim_vals.p, values, n_values * 4, &m.stream);
+    if (n_weights) ac_h2d(m.trim_w.p, weights, n_weights * 4, &m.stream);
+    for (uint64_t v = 0; v < n_values; ++v) { const int64_t a = values[v] < 0 ? -(int64_t)values[v] : values[v]; if ((uint64_t)a >= n_weights) throw std::runtime_error("overlap_align: unitig without a weight"); }
+    std::vector<uint32_t> len(run.size());
+    float ms = 0.f;
+#ifndef AC_EMULATE
+    cudaEvent_t e0, e1;
+    AC_CUDA_CHECK(cudaEventCreate(&e0)); AC_CUDA_CHECK(cudaEventCreate(&e1));
+    AC_CUDA_CHECK(cudaEventRecord(e0, m.stream.s));
+    const size_t smem = (size_t)24 * (k_shared + 1);
+    if (n_shared) {
+        AC_CUDA_CHECK(cudaFuncSetAttribute(ac_overlap_align_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ac_overlap_align_kernel<<<n_shared, 1024, smem, m.stream.s>>>(m.trim_jobs.as<TrimLaunchJob>(), m.trim_vals.as<int32_t>(), m.trim_w.as<uint32_t>(),
+            m.trim_bits.as<uint32_t>(), m.trim_scratch.as<double>(), m.trim_out.as<AlignPiece>(), m.trim_len.as<uint32_t>(), 1);
+        AC_CUDA_CHECK(cudaGetLastError()); ++g_ac_kernel_launches; ac_debug_sync("overlap_align", &m.stream);
+    }
+    if (n_shared < lj.size()) {
+        ac_overlap_align_kernel<<<(unsigned)(lj.size() - n_shared), 1024, 0, m.stream.s>>>(m.trim_jobs.as<TrimLaunchJob>() + n_shared, m.trim_vals.as<int32_t>(),
+            m.trim_w.as<uint32_t>(), m.trim_bits.as<uint32_t>(), m.trim_scratch.as<double>(), m.trim_out.as<AlignPiece>(), m.trim_len.as<uint32_t>(), 0);
+        AC_CUDA_CHECK(cudaGetLastError()); ++g_ac_kernel_launches; ac_debug_sync("overlap_align_hbm", &m.stream);
+    }
+    AC_CUDA_CHECK(cudaEventRecord(e1, m.stream.s));
+    ac_d2h(len.data(), m.trim_len.p, run.size() * 4, &m.stream);
+    ac_sync(&m.stream);
+    AC_CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
+    cudaEventDestroy(e0); cudaEventDestroy(e1);
+#else
+    // the same per-cell recurrence, right-edge maximum and traceback, in row-major order (a topological order of the matrix)
+    (void)k_shared;
+    uint32_t* bits = m.trim_bits.as<uint32_t>();
+    memset(bits, 0, bits_words * 4);
+    for (const TrimLaunchJob& L : lj) {
+        const uint32_t k = L.k;
+        const int32_t* pa = m.trim_vals.as<int32_t>() + L.a_off;
+        const int32_t* pb = m.trim_vals.as<int32_t>() + L.b_off + (L.n - k);
+        const uint32_t* w = m.trim_w.as<uint32_t>();
+        std::vector<uint64_t> diag_off(2 * (size_t)k + 2, 0);
+        for (uint32_t d = 3; d <= 2 * k + 1; ++d) diag_off[d] = diag_off[d - 1] + trim_diag_words(d - 1, k);
+        std::vector<double> above(k + 1, 0.0), row(k + 1, 0.0);
+        double best = -INFINITY; uint32_t best_i = 0;
+        for (uint32_t i = 1; i <= k; ++i) {
+            row[0] = 0.0;
+            for (uint32_t j = 1; j <= k; ++j) {
+                const double up = above[j], left = row[j - 1];
+                const uint32_t d = i + j, t = i - trim_diag_lo(d, k);
+                if (up >= left) bits[L.bits_off + diag_off[d] + t / 32] |= 1u << (t % 32);
+                double s = -INFINITY;
+                if (!(L.skip && i == j + (L.n - k))) {
+                    const int32_t a = pa[i - 1], b = pb[j - 1];
+                    s = trim_cell(above[j - 1], up, left, a, b, (double)w[a < 0 ? -a : a], (double)w[b < 0 ? -b : b]);
+                }
+                row[j] = s;
+            }
+            trim_edge(row[k], i, best, best_i);
+            above.swap(row);
+        }
+        len[L.slot] = best > 0.0 ? trim_traceback(pa, pb, L.n, k, bits + L.bits_off, best_i, m.trim_out.as<AlignPiece>() + L.out_off) : 0;
+    }
+#endif
+    // the pieces of every job sit at the front of its 2k slots, last column first
+    for (const TrimLaunchJob& L : lj) {
+        if (!len[L.slot]) continue;
+        std::vector<AlignPiece>& o = out[run[L.slot]];
+        o.resize(len[L.slot]);
+        ac_d2h(o.data(), m.trim_out.as<AlignPiece>() + L.out_off, (size_t)len[L.slot] * sizeof(AlignPiece), &m.stream);
+    }
+    ac_sync(&m.stream);
+    for (auto& o : out) std::reverse(o.begin(), o.end());
+    return ms;
 }
 
 void DevicePipeline::find_literals(const uint8_t* ascii_host, uint64_t total_bytes, const SeqInfo* host_seq, uint32_t n, uint32_t h,

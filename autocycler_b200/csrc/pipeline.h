@@ -100,6 +100,13 @@ struct PipelineResult {
 // 2S repair patterns and their reverse complements) on the forward strands.
 struct LiteralHit { uint32_t needle; uint32_t pad; uint64_t gpos; };   // needle index, global coordinate of the matching window
 
+// One overlap alignment of `autocycler trim` (trim.rs:366-479): path_a's first k entries against path_b's last k, k = min(max_unitigs, n).
+// Both paths are n signed unitig numbers in the caller's value array.  skip_diagonal: the start-end form (path_a == path_b, cells with
+// global_i == global_j stay -inf, :395).
+struct OverlapJob { uint64_t a_off, b_off; uint32_t n, k, skip_diagonal, pad; };
+// One column of the traceback (trim.rs:329-335): GAP = 0 as a unitig, NONE = -1 as an index.
+struct AlignPiece { int32_t a_unitig, a_index, b_unitig, b_index; };
+
 class DevicePipeline {
 public:
     DevicePipeline(int device, void* stream);
@@ -153,6 +160,14 @@ public:
     // cluster.rs:132-151 pairwise_contig_distances, the integer part: shared[a * n_seqs + b] = total length of the unitigs that the
     // paths of sequences a and b have in common (the diagonal is the length of a's own unitig set).  Host arrays in, host array out.
     void pair_shared_lengths(const UStrand* path, const uint64_t* path_off, uint32_t n_seqs, const uint32_t* unitig_len, uint32_t n_unitigs, uint64_t* shared);
+    // trim.rs overlap_alignment up to the traceback, for a batch of jobs: fill, right-edge maximum and traceback on the device (one CTA per
+    // job, anti-diagonal sweep).  weights[|unitig|] = unitig length.  out[j] = the traceback's pieces in alignment order, empty when the
+    // best right-edge score is <= 0 or the traceback ends on the left edge; the identity test is the caller's.  Returns the kernels' time
+    // in milliseconds (CUDA events around the launches; 0 under emulation).
+    float overlap_align(const int32_t* values, uint64_t n_values, const uint32_t* weights, uint64_t n_weights,
+                        const OverlapJob* jobs, uint32_t n_jobs, std::vector<std::vector<AlignPiece>>& out);
+    // the largest k whose three live diagonals (24 * (k + 1) bytes) fit one CTA's shared memory; larger windows keep them in HBM
+    uint32_t overlap_shared_k_max();
     void find_literals(const uint8_t* ascii, uint64_t total, const SeqInfo* seqs, uint32_t n_seqs, uint32_t h,
                        const uint64_t* needle_words, uint32_t n_needles, std::vector<LiteralHit>& hits);
     unsigned long long kernel_launches() const;

@@ -13,6 +13,9 @@
  *   merge_linear_paths (downstream, 8f)     graph_simplification.rs:315-371 -> ac_merge_linear_paths
  *   UnitigGraph::save_gfa                   unitig_graph.rs:317-331  -> ac_gfa_size, ac_gfa_copy
  *   compress (the whole subcommand)         compress.rs:32-50        -> ac_compress_dir
+ *   trim_path_start_end / _hairpin_start / _hairpin_end   trim.rs:288-326 -> ac_trim_paths
+ *   trim.rs:43-51 on a loaded graph (trim minus the file I/O)     -> ac_trim
+ *   trim (the whole subcommand)             trim.rs:36-53            -> ac_trim_dir
  *
  * Conventions: every function returns 0 on success and a negative AC_E* code on failure; the message
  * is available from ac_last_error(handle) (or ac_last_error(NULL) when no handle exists).  No C++
@@ -81,7 +84,8 @@ typedef struct {            /* milliseconds */
     float h2d, pack, insert, adjacency, boundaries, runs, unitigs, links, seed_sort, emit, d2h, device_total;
     float host_graph, host_simplify, host_gfa;
     float sample, device_simplify, device_gfa;   /* sizing pass of the k-mer table; expand_repeats passes + renumbering and the GFA text when they run on the device */
-    float insert_kernel, reserved0;              /* the hash-insert kernel alone (CUDA events right around its launch; `insert` also holds the table initialisation and the counter read-back) */
+    float insert_kernel;                         /* the hash-insert kernel alone (CUDA events right around its launch; `insert` also holds the table initialisation and the counter read-back) */
+    float trim_kernel;                           /* ac_trim / ac_trim_paths: the overlap-alignment kernels alone (CUDA events around their launches), summed over the call's rounds */
     uint64_t insert_occurrences;   /* k-mer occurrences hashed by the insert kernel (forward windows; each feeds both strands) */
     uint64_t table_capacity, table_used;
     uint64_t kernel_launches;      /* cumulative launches of this library's kernels in the process */
@@ -200,6 +204,31 @@ int ac_decompress_gfa(const char* in_gfa, const char* out_dir, const char* out_f
 /* reconstruct_original_sequence (unitig_graph.rs:383-400; decompress.rs:83-105 writes these out): the sequence spelled by
  * the path of loaded/added sequence `index` through the current graph.  `out` may be null to query `length` only. */
 int ac_sequence_reconstruct(const ac_handle* h, uint64_t index, char* out, uint64_t cap, uint64_t* length);
+
+/* `autocycler trim`.  The overlap alignments (trim.rs:366-479: a dense (k+1)^2 f64 DP per alignment, k = min(max_unitigs, path
+ * length)) run on the GPU, one CTA per alignment, with the traceback on the device; the identity test, the midpoint and the hairpin
+ * walk run on the host.  There is no CPU path: the emulation build exists for the test-suite only. */
+#define AC_TRIM_START_END 0       /* trim_path_start_end (trim.rs:288-296) */
+#define AC_TRIM_HAIRPIN_START 1   /* trim_path_hairpin_start (trim.rs:320-326) */
+#define AC_TRIM_HAIRPIN_END 2     /* trim_path_hairpin_end (trim.rs:299-317) */
+/* One `mode` trim for each of n_paths paths: path x is paths[path_off[x] .. path_off[x+1]) (signed unitig numbers, negative = reverse
+ * strand); weights[u] = length of unitig u (n_weights entries, every |unitig| below n_weights).  trimmed[x] = 1 when path x was
+ * trimmed, and then out[out_off[x] .. out_off[x+1]) is the trimmed path; otherwise that range is empty.  out needs room for
+ * path_off[n_paths] values (a trimmed path is never longer than its input).  The reference's trim.rs unit tests run through this call. */
+int ac_trim_paths(ac_handle* h, int32_t mode, const int32_t* paths, const uint64_t* path_off, uint64_t n_paths,
+                  const uint32_t* weights, uint64_t n_weights, double min_identity, uint32_t max_unitigs,
+                  int32_t* out, uint64_t* out_off, uint8_t* trimmed);
+/* trim.rs:43-51 on the handle's graph (ac_load_gfa of a 1_untrimmed.gfa): start-end and hairpin trimming, choose_trim_type, length
+ * outliers (mad = 0 disables), clean-up (recalculate_depths, remove_zero_depth_unitigs, merge_linear_paths, renumber_unitigs).
+ * Afterwards ac_gfa_*, ac_counts_get, ac_path_copy and ac_sequence_get describe 2_trimmed.gfa and its sequences, ac_trim_yaml returns
+ * 2_trimmed.yaml (TrimmedClusterMetrics, metrics.rs:209-225) and ac_timings.trim_kernel the alignment kernels' time. */
+int ac_trim(ac_handle* h, double min_identity, uint32_t max_unitigs, double mad);
+int ac_trim_yaml(ac_handle* h, char* out, uint64_t cap, uint64_t* length);   /* `out` may be NULL to query the length */
+/* What the last ac_trim / ac_trim_paths aligned: alignments, DP cells (sum of k^2), the largest window k and the longest path. */
+int ac_trim_stats(const ac_handle* h, uint64_t* jobs, uint64_t* cells, uint32_t* max_window, uint64_t* max_path);
+/* `autocycler trim -c cluster_dir` (main.rs:302-322, trim.rs:36-67): reads 1_untrimmed.gfa, writes 2_trimmed.gfa and 2_trimmed.yaml.
+ * The reference's setting checks and messages (AC_EINPUT). */
+int ac_trim_dir(const char* cluster_dir, double min_identity, uint32_t max_unitigs, double mad, uint32_t threads, int32_t device, int32_t verbose);
 
 #ifdef __cplusplus
 }
