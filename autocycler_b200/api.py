@@ -64,7 +64,8 @@ EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_seq
            "ac_build_local", "ac_entries_count", "ac_entries_export", "ac_entries_merge", "ac_runs_local", "ac_runs_export",
            "ac_runs_import", "ac_runs_import_padded", "ac_build_finish", "ac_compress_finish", "ac_gfa_data",
            "ac_compress_finish_split", "ac_path_tokens_export", "ac_path_lines_render", "ac_path_lines_data", "ac_upload_shard", "ac_strand_block",
-           "ac_trim_paths", "ac_trim", "ac_trim_yaml", "ac_trim_stats", "ac_trim_dir"]
+           "ac_trim_paths", "ac_trim", "ac_trim_yaml", "ac_trim_stats", "ac_trim_dir",
+           "ac_cluster", "ac_cluster_text", "ac_cluster_assignments", "ac_cluster_stats", "ac_upgma", "ac_cluster_dir"]
 
 _libs = {}
 
@@ -129,6 +130,14 @@ def load_library(path=None):
     lib.ac_trim_yaml.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     lib.ac_trim_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]
     lib.ac_trim_dir.argtypes = [C.c_char_p, C.c_double, C.c_uint32, C.c_double, C.c_uint32, C.c_int32, C.c_int32]
+    lib.ac_cluster.argtypes = [C.c_void_p, C.c_double, C.c_int64, C.POINTER(C.c_uint16), C.c_uint64]
+    lib.ac_cluster_text.argtypes = [C.c_void_p, C.c_int32, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
+    lib.ac_cluster_assignments.argtypes = [C.c_void_p, C.POINTER(C.c_uint16), C.POINTER(C.c_uint8), C.c_uint64]
+    lib.ac_cluster_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_float),
+                                     C.POINTER(C.c_float), C.POINTER(C.c_double)]
+    lib.ac_upgma.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint32),
+                             C.POINTER(C.c_uint32), C.POINTER(C.c_double)]
+    lib.ac_cluster_dir.argtypes = [C.c_char_p, C.c_double, C.c_int64, C.c_uint32, C.c_char_p, C.c_int32, C.c_int32]
     _libs[path] = lib
     return lib
 
@@ -363,6 +372,34 @@ class UnitigGraph:
         self._h.check(self._h.lib.ac_trim_stats(self._h.ptr, C.byref(jobs), C.byref(cells), C.byref(window), C.byref(path)))
         return {"alignments": jobs.value, "dp_cells": cells.value, "max_window": window.value, "max_path": path.value}
 
+    def cluster(self, cutoff=0.2, min_assemblies=None, manual=None):   # cluster.rs:42-59 on this graph (loaded input_assemblies.gfa)
+        """Distances and UPGMA on the GPU, then clustering, QC and the output texts: cluster_text() returns them, cluster_assignments()
+        the per-sequence result and cluster_stats() the kernel times.  manual: node numbers of the tree (None: automatic)."""
+        man = sorted(manual or [])
+        arr = (C.c_uint16 * max(1, len(man)))(*man)
+        self._h.check(self._h.lib.ac_cluster(self._h.ptr, float(cutoff), -1 if min_assemblies is None else int(min_assemblies), arr, len(man)))
+
+    CLUSTER_TEXTS = {"phylip": 0, "newick": 1, "tsv": 2, "yaml": 3, "gfa": 4, "untrimmed_yaml": 5}
+
+    def cluster_text(self, what, cluster=0):   # "phylip", "newick", "tsv", "yaml"; per cluster: "gfa", "untrimmed_yaml"
+        n = C.c_uint64()
+        w = self.CLUSTER_TEXTS[what]
+        self._h.check(self._h.lib.ac_cluster_text(self._h.ptr, w, cluster, None, 0, C.byref(n)))
+        buf = C.create_string_buffer(max(1, n.value))
+        self._h.check(self._h.lib.ac_cluster_text(self._h.ptr, w, cluster, buf, n.value, C.byref(n)))
+        return buf.raw[:n.value].decode()
+
+    def cluster_assignments(self, n_seqs):   # -> [(cluster number, passed QC)] per sequence
+        cl = (C.c_uint16 * max(1, n_seqs))(); ps = (C.c_uint8 * max(1, n_seqs))()
+        self._h.check(self._h.lib.ac_cluster_assignments(self._h.ptr, cl, ps, n_seqs))
+        return [(cl[i], bool(ps[i])) for i in range(n_seqs)]
+
+    def cluster_stats(self):
+        n, p, f = C.c_uint32(), C.c_uint32(), C.c_uint32(); dm, um = C.c_float(), C.c_float(); gm = C.c_double()
+        self._h.check(self._h.lib.ac_cluster_stats(self._h.ptr, C.byref(n), C.byref(p), C.byref(f), C.byref(dm), C.byref(um), C.byref(gm)))
+        return {"sequences": n.value, "pass_clusters": p.value, "fail_clusters": f.value, "distance_ms": dm.value, "upgma_ms": um.value,
+                "cluster_gfa_ms": gm.value}
+
     def save_gfa(self, gfa_filename, sequences=None, use_other_colour=False):   # unitig_graph.rs:317-331
         with open(gfa_filename, "wb") as f:
             f.write(self.gfa_bytes())
@@ -458,5 +495,32 @@ def trim(cluster_dir, min_identity=0.75, max_unitigs=5000, mad=5.0, threads=8, d
     """trim.rs:36-53: reads <cluster_dir>/1_untrimmed.gfa, writes 2_trimmed.gfa and 2_trimmed.yaml."""
     lib = lib or load_library()
     rc = lib.ac_trim_dir(os.fsencode(cluster_dir), float(min_identity), max_unitigs, float(mad), threads, device, 1 if verbose else 0)
+    if rc != AC_OK:
+        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+
+
+def upgma(matrix, ids, lib=None, device=0, handle=None):
+    """UPGMA (cluster.rs:395-480) on the GPU: matrix is a symmetric n x n distance matrix (nested lists or an array) of the clusters `ids`
+    (strictly ascending).  -> ([(node, left, right, node distance)] in merge order, kernel milliseconds)."""
+    import numpy as np
+    lib = lib or load_library()
+    h = handle or _Handle(lib, 51, device)
+    m = np.ascontiguousarray(np.asarray(matrix, dtype=np.float64))
+    n = len(ids)
+    assert m.shape == (n, n)
+    k = max(1, n - 1)
+    node, left, right = (C.c_uint32 * k)(), (C.c_uint32 * k)(), (C.c_uint32 * k)()
+    dist = (C.c_double * k)()
+    h.check(lib.ac_upgma(h.ptr, m.ctypes.data_as(C.POINTER(C.c_double)), n, (C.c_uint32 * max(1, n))(*ids), node, left, right, dist))
+    ms = C.c_float()
+    h.check(lib.ac_cluster_stats(h.ptr, None, None, None, None, C.byref(ms), None))
+    return [(node[x], left[x], right[x], dist[x]) for x in range(n - 1)], ms.value
+
+
+def cluster(autocycler_dir, cutoff=0.2, min_assemblies=None, max_contigs=25, manual=None, device=0, verbose=False, lib=None):
+    """cluster.rs:30-64: reads <autocycler_dir>/input_assemblies.gfa and replaces <autocycler_dir>/clustering.  manual: "1,2,3"."""
+    lib = lib or load_library()
+    rc = lib.ac_cluster_dir(os.fsencode(autocycler_dir), float(cutoff), -1 if min_assemblies is None else int(min_assemblies), max_contigs,
+                            manual.encode() if manual is not None else None, device, 1 if verbose else 0)
     if rc != AC_OK:
         raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())

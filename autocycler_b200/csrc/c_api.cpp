@@ -2,10 +2,13 @@
 #include "../../include/autocycler_gpu.h"
 
 #include <sched.h>
+#include <dirent.h>
 #include <sys/stat.h>
+#include <unistd.h>
 #include <zlib.h>
 
 #include <algorithm>
+#include <cerrno>
 #include <chrono>
 #include <cstdio>
 #include <cstring>
@@ -16,6 +19,7 @@
 #include "backend.h"
 #include "host_graph.h"
 #include "host_io.h"
+#include "host_cluster.h"
 #include "host_trim.h"
 #include <immintrin.h>
 #include <functional>
@@ -68,6 +72,7 @@ struct ac_handle {
     uint64_t links_now = 0;
     std::string trim_yaml; bool trimmed = false;           // ac_trim: 2_trimmed.yaml
     TrimStats trim_stats;
+    ClusterResult cluster; ClusterStats cluster_stats; bool clustered = false;
 };
 
 static int set_error(const ac_handle* h, int code, const std::string& msg) {
@@ -557,6 +562,7 @@ int ac_load_gfa(ac_handle* h, const char* gfa_text, uint64_t length) {
     h->seqs.clear(); h->infos.clear(); h->ascii.clear(); h->loaded = LoadedInput(); h->res = PipelineResult(); h->t = ac_timings{};   // a loaded graph has no sequence bytes: ac_upload / ac_build need ac_add_sequence again
     h->graph.device_sort = nullptr;
     h->trimmed = false; h->trim_yaml.clear();
+    h->clustered = false; h->cluster = ClusterResult();
     h->graph.load_gfa(gfa_text, (size_t)length, h->seqs);
     h->cfg.k = h->graph.k;
     h->built = true; h->graph_ready = true;
@@ -596,36 +602,7 @@ int ac_distance_matrix_text(ac_handle* h, char* out, uint64_t cap, uint64_t* len
     std::vector<double> d(std::max<uint64_t>(1, S * S));
     const int rc = ac_pairwise_distances(h, d.data(), S * S);
     if (rc != AC_OK) return rc;
-    auto lower = [](std::string s) { for (char& c : s) if (c >= 'A' && c <= 'Z') c = (char)(c + 32); return s; };
-    auto weight = [&](const std::string& header, const std::string& key) -> uint64_t {   // sequence.rs:96-108
-        const std::string low = lower(header);
-        for (size_t a = 0; a < low.size();) {
-            while (a < low.size() && isspace((unsigned char)low[a])) ++a;
-            size_t b = a; while (b < low.size() && !isspace((unsigned char)low[b])) ++b;
-            if (b > a && low.compare(a, key.size(), key) == 0 && b - a > key.size()) {
-                const std::string v = low.substr(a + key.size(), b - a - key.size());
-                const size_t first = v[0] == '+' ? 1 : 0;
-                if (v.size() > first && v.find_first_not_of("0123456789", first) == std::string::npos) return strtoull(v.c_str(), nullptr, 10);
-            }
-            a = b;
-        }
-        return 1;
-    };
-    std::string text = std::to_string(S) + "\n";
-    for (uint64_t a = 0; a < S; ++a) {
-        const HostSeq& s = h->seqs[a];
-        const std::string low = lower(s.contig_header);
-        std::vector<std::string> extras;
-        if (low.find("autocycler_trusted") != std::string::npos) extras.push_back("trusted");
-        if (low.find("autocycler_ignore") != std::string::npos) extras.push_back("ignored");
-        const uint64_t cw = weight(s.contig_header, "autocycler_cluster_weight="), nw = weight(s.contig_header, "autocycler_consensus_weight=");
-        if (cw != 1) extras.push_back("cluster weight = " + std::to_string(cw));
-        if (nw != 1) extras.push_back("consensus weight = " + std::to_string(nw));
-        text += s.filename + " " + s.contig_header.substr(0, s.contig_header.find(' ')) + " (" + std::to_string(s.length) + " bp)";
-        if (!extras.empty()) { text += " ["; for (size_t i = 0; i < extras.size(); ++i) { if (i) text += ", "; text += extras[i]; } text += "]"; }
-        for (uint64_t b = 0; b < S; ++b) { char buf[64]; snprintf(buf, sizeof buf, "\t%.8f", d[a * S + b]); text += buf; }
-        text += "\n";
-    }
+    const std::string text = distance_matrix_text(h->seqs, d.data());
     *length = text.size();
     if (!out) return ok(h);
     if (cap < text.size()) return set_error(h, AC_ERANGE, "buffer too small");
@@ -1096,6 +1073,160 @@ int ac_trim_dir(const char* cluster_dir, double min_identity, uint32_t max_uniti
     fclose(f);
     if (verbose) fprintf(stderr, "\nFinished!\nUnitig graph of trimmed sequences: %s\n(%llu alignments, %llu DP cells, alignment kernels %.2f ms)\n\n", out_gfa.c_str(),
                          (unsigned long long)ts.jobs, (unsigned long long)ts.cells, (double)ts.kernel_ms);
+    return ok(h);
+    AC_GUARD_END(nullptr)
+}
+
+// UPGMA (cluster.rs:395-480) on a caller's symmetric matrix: the kernel that ac_cluster runs on the distances it leaves on the device
+int ac_upgma(ac_handle* h, const double* sym_dist, uint32_t n, const uint32_t* ids, uint32_t* node, uint32_t* left, uint32_t* right, double* dist) {
+    if (!h || (n && (!sym_dist || !ids)) || (n > 1 && (!node || !left || !right || !dist))) return set_error(h, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    for (uint64_t i = 0; i < n; ++i)          // a NaN distance can leave no pair to merge (the reference panics there)
+        for (uint64_t j = 0; j < n; ++j)
+            if (i != j && sym_dist[i * n + j] != sym_dist[i * n + j]) return set_error(h, AC_EINPUT, "the distance matrix holds a NaN off its diagonal");
+    std::vector<UpgmaMerge> m(n > 1 ? n - 1 : 0);
+    h->cluster_stats.upgma_ms = h->pipe->upgma(sym_dist, n, ids, m.data());
+    for (size_t x = 0; x < m.size(); ++x) { node[x] = m[x].node; left[x] = m[x].left; right[x] = m[x].right; dist[x] = m[x].dist; }
+    return ok(h);
+    AC_GUARD_END(h)
+}
+
+int ac_cluster(ac_handle* h, double cutoff, int64_t min_assemblies, const uint16_t* manual, uint64_t n_manual) {
+    if (!h || (n_manual && !manual)) return set_error(h, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    if (!h->built) return set_error(h, AC_EINVAL, "a graph must be built or loaded before ac_cluster");
+    if (cutoff <= 0.0 || cutoff >= 1.0) return set_error(h, AC_EINPUT, "--cutoff must be between 0 and 1 (exclusive)");
+    if (min_assemblies == 0) return set_error(h, AC_EINPUT, "--min_assemblies must be 1 or greater");
+    std::vector<uint16_t> man(manual, manual + n_manual);
+    std::sort(man.begin(), man.end());
+    ensure_graph(h);
+    h->clustered = false;
+    // the per-cluster graphs re-load the handle's graph as text, as the reference re-loads input_assemblies.gfa; the cluster numbers go
+    // to a copy of the sequences, so the handle's own GFA output is unchanged
+    std::string text;
+    h->graph.gfa_text(h->seqs, text);
+    std::vector<HostSeq> seqs = h->seqs;
+    cluster_graph(text, h->graph, seqs, *h->pipe, cutoff, min_assemblies < 0 ? -1 : min_assemblies, man, 0xFFFFFFFFu, "clustering", false, h->cluster, h->cluster_stats);
+    h->clustered = true;
+    return ok(h);
+    AC_GUARD_END(h)
+}
+
+int ac_cluster_text(ac_handle* h, int32_t what, uint32_t cluster, char* out, uint64_t cap, uint64_t* length) {
+    if (!h || !length) return set_error(h, AC_EINVAL, "null argument");
+    if (!h->clustered) return set_error(h, AC_EINVAL, "ac_cluster must precede ac_cluster_text");
+    const ClusterResult& r = h->cluster;
+    const bool per_cluster = what == AC_CLUSTER_GFA || what == AC_CLUSTER_UNTRIMMED_YAML;
+    if (per_cluster && (cluster < 1 || cluster > r.cluster_gfa.size())) return set_error(h, AC_ERANGE, "no cluster " + std::to_string(cluster));
+    const std::string* t = what == AC_CLUSTER_PHYLIP ? &r.phylip : what == AC_CLUSTER_NEWICK ? &r.newick : what == AC_CLUSTER_TSV ? &r.tsv :
+                           what == AC_CLUSTER_YAML ? &r.yaml : what == AC_CLUSTER_GFA ? &r.cluster_gfa[cluster - 1] :
+                           what == AC_CLUSTER_UNTRIMMED_YAML ? &r.cluster_yaml[cluster - 1] : nullptr;
+    if (!t) return set_error(h, AC_EINVAL, "unknown cluster text");
+    *length = t->size();
+    if (!out) return ok(h);
+    if (cap < t->size()) return set_error(h, AC_ERANGE, "buffer too small");
+    memcpy(out, t->data(), t->size());
+    return ok(h);
+}
+
+int ac_cluster_assignments(const ac_handle* h, uint16_t* cluster, uint8_t* pass, uint64_t cap) {
+    if (!h || !cluster || !pass) return set_error(h, AC_EINVAL, "null argument");
+    if (!h->clustered) return set_error(h, AC_EINVAL, "ac_cluster must precede ac_cluster_assignments");
+    const ClusterResult& r = h->cluster;
+    if (cap < r.seq_cluster.size()) return set_error(h, AC_ERANGE, "buffer too small");
+    for (size_t i = 0; i < r.seq_cluster.size(); ++i) { cluster[i] = r.seq_cluster[i]; pass[i] = r.cluster_pass[r.seq_cluster[i] - 1]; }
+    return ok(h);
+}
+
+int ac_cluster_stats(const ac_handle* h, uint32_t* n_seqs, uint32_t* pass_clusters, uint32_t* fail_clusters, float* distance_ms, float* upgma_ms, double* cluster_gfa_ms) {
+    if (!h) return set_error(nullptr, AC_EINVAL, "null handle");
+    const ClusterStats& s = h->cluster_stats;
+    if (n_seqs) *n_seqs = s.n_seqs;
+    if (pass_clusters) *pass_clusters = s.pass_clusters;
+    if (fail_clusters) *fail_clusters = s.fail_clusters;
+    if (distance_ms) *distance_ms = s.distance_ms;
+    if (upgma_ms) *upgma_ms = s.upgma_ms;
+    if (cluster_gfa_ms) *cluster_gfa_ms = s.cluster_gfa_ms;
+    return ok(h);
+}
+
+namespace {
+bool write_file(const std::string& path, const std::string& text) {
+    FILE* f = fopen(path.c_str(), "wb");
+    if (!f) return false;
+    const bool good = fwrite(text.data(), 1, text.size(), f) == text.size();
+    return fclose(f) == 0 && good;
+}
+int remove_tree(const std::string& path) {       // everything under a directory, and the directory
+    struct stat st;
+    if (lstat(path.c_str(), &st) != 0) return 0;
+    if (S_ISDIR(st.st_mode)) {
+        DIR* d = opendir(path.c_str());
+        if (!d) return -1;
+        std::vector<std::string> names;
+        while (dirent* e = readdir(d)) { const std::string n = e->d_name; if (n != "." && n != "..") names.push_back(n); }
+        closedir(d);
+        for (auto& n : names) if (remove_tree(path + "/" + n) != 0) return -1;
+        return rmdir(path.c_str());
+    }
+    return unlink(path.c_str());
+}
+}  // namespace
+
+int ac_cluster_dir(const char* autocycler_dir, double cutoff, int64_t min_assemblies, uint32_t max_contigs, const char* manual, int32_t device, int32_t verbose) {
+    if (!autocycler_dir) return set_error(nullptr, AC_EINVAL, "null argument");
+    ac_handle* h = nullptr;
+    AC_GUARD_BEGIN
+    // check_settings (cluster.rs:67-76)
+    const std::string dir = autocycler_dir, gfa = dir + "/input_assemblies.gfa", cdir = dir + "/clustering";
+    struct stat st;
+    if (stat(autocycler_dir, &st) != 0) return set_error(nullptr, AC_EINPUT, "directory does not exist: " + dir);
+    if (!S_ISDIR(st.st_mode)) return set_error(nullptr, AC_EINPUT, dir + " is not a directory");
+    if (stat(gfa.c_str(), &st) != 0) return set_error(nullptr, AC_EINPUT, "file does not exist: " + gfa);
+    if (!S_ISREG(st.st_mode)) return set_error(nullptr, AC_EINPUT, gfa + " is not a file");
+    if (cutoff <= 0.0 || cutoff >= 1.0) return set_error(nullptr, AC_EINPUT, "--cutoff must be between 0 and 1 (exclusive)");
+    if (min_assemblies == 0) return set_error(nullptr, AC_EINPUT, "--min_assemblies must be 1 or greater");
+    // delete_dir_if_exists (misc.rs:41-48): only a directory (or a link to one, which goes itself) is removed; anything else makes
+    // create_dir fail below
+    if (stat(cdir.c_str(), &st) == 0 && S_ISDIR(st.st_mode)) {
+        struct stat lst;
+        const int rc = lstat(cdir.c_str(), &lst) == 0 && S_ISLNK(lst.st_mode) ? unlink(cdir.c_str()) : remove_tree(cdir);
+        if (rc != 0) return set_error(nullptr, AC_EINPUT, "failed to delete directory " + cdir + "\n" + strerror(errno));
+    }
+    if (mkdir(cdir.c_str(), 0777) != 0) return set_error(nullptr, AC_EINPUT, "failed to create directory " + cdir + "\n" + strerror(errno));
+    if (verbose) fprintf(stderr, "\nStarting autocycler cluster\n    This command takes a unitig graph (made by autocycler compress) and clusters the sequences based on "
+                                 "their similarity. Ideally, each cluster will then contain sequences which can be combined into a consensus.\n\n");
+    std::string text;
+    {
+        FILE* f = fopen(gfa.c_str(), "rb");
+        if (!f) return set_error(nullptr, AC_EIO, "cannot read " + gfa);
+        char buf[1 << 16]; size_t n;
+        while ((n = fread(buf, 1, sizeof buf, f)) > 0) text.append(buf, n);
+        fclose(f);
+    }
+    ac_config cfg{}; cfg.k = 51; cfg.device = device; cfg.stream = nullptr; cfg.keep_positions = 0; cfg.n_devices = 1; cfg.devices = nullptr;
+    int rc = ac_create(&h, &cfg);
+    if (rc != AC_OK) return rc;
+    std::unique_ptr<ac_handle, void (*)(ac_handle*)> guard(h, ac_destroy);
+    if ((rc = ac_load_gfa(h, text.data(), text.size())) != AC_OK) { g_error = h->err; return rc == AC_EINVAL ? AC_EINPUT : rc; }
+    const std::vector<uint16_t> man = manual ? parse_manual_clusters(manual) : std::vector<uint16_t>();
+    if (verbose) fprintf(stderr, "Settings:\n  --autocycler_dir %s\n", dir.c_str());
+    cluster_graph(text, h->graph, h->seqs, *h->pipe, cutoff, min_assemblies < 0 ? -1 : min_assemblies, man, max_contigs, cdir, verbose != 0, h->cluster, h->cluster_stats);
+    const ClusterResult& r = h->cluster;
+    const std::string phylip = cdir + "/pairwise_distances.phylip", newick = cdir + "/clustering.newick", tsv = cdir + "/clustering.tsv";
+    bool good = write_file(phylip, r.phylip) && write_file(newick, r.newick);
+    for (size_t c = 0; good && c < r.cluster_gfa.size(); ++c) {
+        char name[32]; snprintf(name, sizeof name, "/cluster_%03zu", c + 1);
+        const std::string sub = cdir + (r.cluster_pass[c] ? "/qc_pass" : "/qc_fail"), cd = sub + name;
+        mkdir(sub.c_str(), 0777);
+        good = mkdir(cd.c_str(), 0777) == 0 && write_file(cd + "/1_untrimmed.gfa", r.cluster_gfa[c]) && write_file(cd + "/1_untrimmed.yaml", r.cluster_yaml[c]);
+    }
+    good = good && write_file(tsv, r.tsv) && write_file(cdir + "/clustering.yaml", r.yaml);
+    if (!good) return set_error(nullptr, AC_EIO, "cannot write the output files under " + cdir);
+    if (verbose) fprintf(stderr, "\nFinished!\n    You can now run autocycler trim on each cluster. If you want to manually inspect the clustering, you can "
+                                 "view the following files.\nPairwise distances:         %s\nClustering tree (Newick):   %s\nClustering tree (metadata): %s\n"
+                                 "\n(distance kernels %.2f ms, UPGMA kernel %.2f ms, per-cluster graphs %.1f ms)\n\n", phylip.c_str(), newick.c_str(), tsv.c_str(),
+                         (double)h->cluster_stats.distance_ms, (double)h->cluster_stats.upgma_ms, h->cluster_stats.cluster_gfa_ms);
     return ok(h);
     AC_GUARD_END(nullptr)
 }

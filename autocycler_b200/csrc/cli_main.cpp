@@ -1,4 +1,4 @@
-// `autocycler compress`, `autocycler decompress` and `autocycler trim` with the reference's flags (main.rs:126-162), messages and exit codes
+// `autocycler compress`, `autocycler decompress`, `autocycler cluster` and `autocycler trim` with the reference's flags (main.rs:126-162), messages and exit codes
 // (misc.rs:130-136: "Error: <text>" on stderr, exit 1), running the H100 path through the C ABI.
 #include <cstdio>
 #include <cstdlib>
@@ -74,8 +74,38 @@ static int trim_main(int argc, char** argv) {
     return 0;
 }
 
+// `autocycler cluster` (main.rs:92-113, cluster.rs:30-114)
+static int cluster_main(int argc, char** argv) {
+    static const char* cluster_usage = "Usage: autocycler cluster --autocycler_dir <AUTOCYCLER_DIR> [--cutoff 0.2] [--min_assemblies N] [--max_contigs 25] [--manual 1,2,3] [--device N]\n";
+    std::string dir, manual; bool has_manual = false; double cutoff = 0.2; long long min_assemblies = -1; unsigned long max_contigs = 25; int device = 0;
+    for (int i = 2; i < argc; ++i) {
+        std::string a = argv[i];
+        auto value = [&]() -> const char* { if (i + 1 >= argc) { fprintf(stderr, "error: a value is required for '%s'\n", a.c_str()); exit(2); } return argv[++i]; };
+        auto number = [&](const char* v, bool integral) -> double {
+            char* end = nullptr; const double x = integral ? (double)strtoul(v, &end, 10) : strtod(v, &end);
+            if (!*v || *end || (integral && (*v == '-' || *v == '+'))) { fprintf(stderr, "error: invalid value '%s' for '%s'\n%s", v, a.c_str(), cluster_usage); exit(2); }
+            return x;
+        };
+        if (a == "-a" || a == "--autocycler_dir") dir = value();
+        else if (a == "--cutoff") cutoff = number(value(), false);
+        else if (a == "--min_assemblies") min_assemblies = (long long)number(value(), true);
+        else if (a == "--max_contigs") max_contigs = (unsigned long)number(value(), true);
+        else if (a == "--manual") { manual = value(); has_manual = true; }
+        else if (a == "--device") device = atoi(value());
+        else if (a == "-h" || a == "--help") { fprintf(stderr, "%s", cluster_usage); return 0; }
+        else { fprintf(stderr, "error: unexpected argument '%s'\n%s", a.c_str(), cluster_usage); return 2; }
+    }
+    if (dir.empty()) { fprintf(stderr, "%s", cluster_usage); return 2; }
+    if (max_contigs > 0xFFFFFFFFul) max_contigs = 0xFFFFFFFFul;
+    fprintf(stderr, "\nStarting autocycler cluster (%s)\n\n", ac_version());
+    const int rc = ac_cluster_dir(dir.c_str(), cutoff, min_assemblies, (uint32_t)max_contigs, has_manual ? manual.c_str() : nullptr, device, 1);
+    if (rc != AC_OK) { fprintf(stderr, "\nError: %s\n", ac_last_error(nullptr)); return 1; }
+    return 0;
+}
+
 int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "decompress") == 0) return decompress_main(argc, argv);
+    if (argc >= 2 && strcmp(argv[1], "cluster") == 0) return cluster_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "trim") == 0) return trim_main(argc, argv);
     if (argc < 2 || strcmp(argv[1], "compress") != 0) { usage(); return 2; }
     std::string in, out; unsigned k = 51, max_contigs = 25, threads = 8; int device = 0;

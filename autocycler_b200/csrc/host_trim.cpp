@@ -116,6 +116,8 @@ bool finish_hairpin_end(const std::vector<int32_t>& path, Alignment al, std::vec
     return true;
 }
 
+}  // namespace
+
 // median_isize / mad_isize (misc.rs:399-423): integer halving of the two middle values for even counts
 int64_t median_i64(std::vector<int64_t> v) {
     if (v.empty()) return 0;
@@ -130,6 +132,8 @@ int64_t mad_i64(const std::vector<int64_t>& v) {
     for (size_t x = 0; x < v.size(); ++x) dev[x] = v[x] > m ? v[x] - m : m - v[x];
     return median_i64(dev);
 }
+
+namespace {
 uint64_t round_to_usize(double x) {   // (x).round() as usize: half away from zero, negatives and NaN saturate to 0
     const double r = std::round(x);
     if (!(r > 0)) return 0;

@@ -30,5 +30,9 @@ void trim_paths(DevicePipeline& pipe, TrimMode mode, const std::vector<std::vect
 void trim_graph(HostGraph& g, std::vector<HostSeq>& seqs, DevicePipeline& pipe, double min_identity, uint32_t max_unitigs, double mad,
                 bool verbose, TrimStats& stats);
 
+// median_isize / mad_isize (misc.rs:399-423), which median_usize / mad_usize equal on lengths
+int64_t median_i64(std::vector<int64_t> v);
+int64_t mad_i64(const std::vector<int64_t>& v);
+
 // TrimmedClusterMetrics (metrics.rs:209-225) of the sequence lengths, as serde_yaml 0.9 writes it (2_trimmed.yaml)
 std::string trimmed_metrics_yaml(const std::vector<HostSeq>& seqs);

@@ -106,6 +106,9 @@ struct LiteralHit { uint32_t needle; uint32_t pad; uint64_t gpos; };   // needle
 struct OverlapJob { uint64_t a_off, b_off; uint32_t n, k, skip_diagonal, pad; };
 // One column of the traceback (trim.rs:329-335): GAP = 0 as a unitig, NONE = -1 as an index.
 struct AlignPiece { int32_t a_unitig, a_index, b_unitig, b_index; };
+// One merge of `autocycler cluster`'s UPGMA (cluster.rs:410-430): the new node's number, its left child (the cluster with the smaller
+// id), its right child, and the node's distance to the tips (half the merged pair's mean distance).
+struct UpgmaMerge { uint32_t node, left, right, pad; double dist; };
 
 class DevicePipeline {
 public:
@@ -160,6 +163,13 @@ public:
     // cluster.rs:132-151 pairwise_contig_distances, the integer part: shared[a * n_seqs + b] = total length of the unitigs that the
     // paths of sequences a and b have in common (the diagonal is the length of a's own unitig set).  Host arrays in, host array out.
     void pair_shared_lengths(const UStrand* path, const uint64_t* path_off, uint32_t n_seqs, const uint32_t* unitig_len, uint32_t n_unitigs, uint64_t* shared);
+    // cluster.rs:132-192: the same shared lengths turned into the asymmetric distance matrix on the device (copied back into
+    // asym[n_seqs * n_seqs]) and its symmetric max, which stays in HBM for upgma(nullptr, ...).  Returns the kernels' time in ms.
+    float cluster_distances(const UStrand* path, const uint64_t* path_off, uint32_t n_seqs, const uint32_t* unitig_len, uint32_t n_unitigs, double* asym);
+    // UPGMA (cluster.rs:395-480) in one persistent CTA: n - 1 merges of the n clusters ids[0..n) (strictly ascending), new nodes numbered
+    // from ids[n-1] + 1.  sym: a symmetric n x n host matrix, or null for the one cluster_distances left on the device (used up).
+    // Returns the kernel's time in ms (CUDA events; 0 under emulation).
+    float upgma(const double* sym, uint32_t n, const uint32_t* ids, UpgmaMerge* merges);
     // trim.rs overlap_alignment up to the traceback, for a batch of jobs: fill, right-edge maximum and traceback on the device (one CTA per
     // job, anti-diagonal sweep).  weights[|unitig|] = unitig length.  out[j] = the traceback's pieces in alignment order, empty when the
     // best right-edge score is <= 0 or the traceback ends on the left edge; the identity test is the caller's.  Returns the kernels' time

@@ -230,6 +230,38 @@ int ac_trim_stats(const ac_handle* h, uint64_t* jobs, uint64_t* cells, uint32_t*
  * The reference's setting checks and messages (AC_EINPUT). */
 int ac_trim_dir(const char* cluster_dir, double min_identity, uint32_t max_unitigs, double mad, uint32_t threads, int32_t device, int32_t verbose);
 
+/* `autocycler cluster`.  The contig distances (cluster.rs:132-192) and UPGMA (:395-480) run on the GPU: the symmetric matrix stays in
+ * HBM and one persistent CTA performs all n - 1 merges; the tree, clustering, QC and the output files are built on the host.  Averages
+ * are kept as sums over member pairs (T(A u B, C) = T(A, C) + T(B, C)), see DESIGN.md section 12. */
+#define AC_CLUSTER_PHYLIP 0            /* pairwise_distances.phylip */
+#define AC_CLUSTER_NEWICK 1            /* clustering.newick */
+#define AC_CLUSTER_TSV 2               /* clustering.tsv */
+#define AC_CLUSTER_YAML 3              /* clustering.yaml (ClusteringMetrics) */
+#define AC_CLUSTER_GFA 4               /* one cluster's 1_untrimmed.gfa */
+#define AC_CLUSTER_UNTRIMMED_YAML 5    /* one cluster's 1_untrimmed.yaml (UntrimmedClusterMetrics) */
+/* cluster.rs:42-59 on the handle's graph as it is now (normally ac_load_gfa of an input_assemblies.gfa): the distances and the
+ * per-cluster graphs both come from it.  The handle's sequences and graph are not changed.  min_assemblies < 0: set automatically;
+ * manual: n_manual node numbers of the tree (none: automatic clustering refined by score).  The reference's setting checks (AC_EINPUT);
+ * two sequences whose paths have no length have a NaN distance and are refused (AC_EINPUT), where the reference would panic. */
+int ac_cluster(ac_handle* h, double cutoff, int64_t min_assemblies, const uint16_t* manual, uint64_t n_manual);
+/* One output of the last ac_cluster (`what` = AC_CLUSTER_*; `cluster` = 1-based number for the per-cluster texts).  `out` may be NULL
+ * to query the length. */
+int ac_cluster_text(ac_handle* h, int32_t what, uint32_t cluster, char* out, uint64_t cap, uint64_t* length);
+/* Per sequence of the handle: its cluster number and whether that cluster passed QC. */
+int ac_cluster_assignments(const ac_handle* h, uint16_t* cluster, uint8_t* pass, uint64_t cap);
+/* The last ac_cluster: sequences, passed and failed clusters, the distance and UPGMA kernels' times (CUDA events) and the host time of
+ * the per-cluster graphs. */
+int ac_cluster_stats(const ac_handle* h, uint32_t* n_seqs, uint32_t* pass_clusters, uint32_t* fail_clusters, float* distance_ms, float* upgma_ms,
+                     double* cluster_gfa_ms);
+/* The UPGMA kernel on a caller's symmetric n x n matrix (row-major) of the clusters ids[0..n), strictly ascending: n - 1 merges, each
+ * the new node's number (from ids[n-1] + 1), its left and right child and its distance to the tips.  A NaN off the diagonal is refused
+ * (AC_EINPUT).  The reference's UPGMA tests run through this call. */
+int ac_upgma(ac_handle* h, const double* sym_dist, uint32_t n, const uint32_t* ids, uint32_t* node, uint32_t* left, uint32_t* right, double* dist);
+/* `autocycler cluster -a autocycler_dir` (main.rs:92-113, cluster.rs:30-64): replaces autocycler_dir/clustering with
+ * pairwise_distances.phylip, clustering.newick, clustering.tsv, clustering.yaml and qc_pass|qc_fail/cluster_NNN/1_untrimmed.{gfa,yaml}.
+ * min_assemblies < 0: automatic; manual: "1,2,3" or NULL. */
+int ac_cluster_dir(const char* autocycler_dir, double cutoff, int64_t min_assemblies, uint32_t max_contigs, const char* manual, int32_t device, int32_t verbose);
+
 #ifdef __cplusplus
 }
 #endif
