@@ -2105,6 +2105,10 @@ struct DevicePipeline::Impl {
 #endif
     }
     template <int W> void local_w(uint32_t seq_lo, uint32_t seq_hi, bool multi);
+    template <int W> void insert_w();
+    uint64_t safe_cap = 0;          // 1.5 slots per window of every sequence (all ranks'): holds any input, the union of the ranks' k-mers included
+    int table_attempt = 0;          // of the current build: the initial size, the safe size, the side counts (AC_HOST_PROFILE prints each)
+    std::vector<std::pair<const void*, uint64_t>> merged;      // the (records, count) of every merge_entries since build_local
     template <int W> void merge_w(const void* dev_ptr, uint64_t n);
     template <int W> void runs_local_w();
     template <int W> void finish_w(PipelineResult& out, bool keep_positions, bool fused, bool split_paths);
@@ -2156,8 +2160,15 @@ struct DevicePipeline::Impl {
                          &claimed_cnt, &occ_list, &bloom, &count_big, &interior8, &d_small, &d_totals, &d_own_off, &d_own_last, &d_own_size, &own_entries, &own_runs, &d_due};
         for (DevBuf* b : all) if (b->p) memset(b->p, 0xA5, b->cap);
     }
+    void poison_table() {          // and before every attempt at the table: a retry must not read what the failed attempt left
+        static const bool on = getenv("AC_EMU_POISON") != nullptr;
+        if (!on) return;
+        DevBuf* all[] = {&slots, &pos_slot, &claimed, &claimed_cnt, &occ_list, &count_big, &counters};
+        for (DevBuf* b : all) if (b->p) memset(b->p, 0xA5, b->cap);
+    }
 #else
     void poison() {}
+    void poison_table() {}
 #endif
 };
 
@@ -2568,10 +2579,25 @@ template <int W> void DevicePipeline::Impl::local_w(uint32_t seq_lo, uint32_t se
         }
     }
     mark(15);
+    this->safe_cap = safe_cap;
+    table_attempt = 0;
+    merged.clear();
+    insert_w<W>();
+    mark(4);
+    stage = 1;
+}
 
+// The table over this rank's windows at `cap`, started again at the safe size if the probe limit trips and with the counts in the side
+// array if the count alarm rises.  Every attempt starts from an empty table, so nothing of a failed one is read.
+template <int W> void DevicePipeline::Impl::insert_w() {
+    const KParams p = make_kparams(k, W);
+    const uint64_t n_words = (total + 31) / 32;
+    unsigned long long hc[AC_N_COUNTERS] = {0, 0, 0, 0};
     pos_slot.ensure(total * sizeof(uint32_t));
-    for (int attempt = 0;; ++attempt) {
-        if (attempt > 3) throw std::runtime_error("k-mer table build did not settle");
+    for (;; ++table_attempt) {
+        if (table_attempt > 3) throw std::runtime_error("k-mer table build did not settle");
+        if (getenv("AC_HOST_PROFILE")) fprintf(stderr, "[device] k-mer table attempt %d: capacity %llu, side counts %d\n", table_attempt, (unsigned long long)cap, (int)big_counts);
+        poison_table();
         slots.ensure(cap * sizeof(Slot));
         // AC_L2_PERSIST=table | packed (comparison only): ask the L2 to keep the k-mer table, or the 2-bit sequence store every probe's
         // comparison reads at random, resident while the table is probed (inputs whose table is several times the L2)
@@ -2584,7 +2610,7 @@ template <int W> void DevicePipeline::Impl::local_w(uint32_t seq_lo, uint32_t se
         const TableView tv = table_view();
         const uint64_t g_first = g_begin & ~31ull;
         claimed.ensure((n_words + 8) * 4); ac_memset(claimed.p, 0, (n_words + 8) * 4, &stream);
-        const InsertBody<W> ins{tv, p, interior8.as<uint8_t>(), (uint32_t)g_first, (uint32_t)g_begin, (uint32_t)g_end, multi, pos_slot.as<uint32_t>(), counters.as<unsigned long long>(), false, claimed.as<uint32_t>()};
+        const InsertBody<W> ins{tv, p, interior8.as<uint8_t>(), (uint32_t)g_first, (uint32_t)g_begin, (uint32_t)g_end, is_multi, pos_slot.as<uint32_t>(), counters.as<unsigned long long>(), false, claimed.as<uint32_t>()};
         // (a software-pipelined form of this loop — the next unit's keys built and its home group in flight while the current one is probed —
         // needs 75 registers and was slower; it is not kept)
         mark(20);
@@ -2596,9 +2622,8 @@ template <int W> void DevicePipeline::Impl::local_w(uint32_t seq_lo, uint32_t se
         if (hc[3] && !big_counts) { big_counts = true; continue; }          // a k-mer with half a million occurrences: counts move to the 32-bit side array
         break;
     }
+    ++table_attempt;
     n_dotted = hc[1];
-    mark(4);
-    stage = 1;
 }
 
 // The list of distinct k-mers (their slots) from the claim bits; returns how many there are.
@@ -2627,22 +2652,34 @@ template <int W> void DevicePipeline::Impl::merge_w(const void* dev_ptr, uint64_
     if (stage < 1) throw std::runtime_error("build_local must precede merge_entries");
     const KParams p = make_kparams(k, W);
     ac_launch("merge", &stream, MergeBody<W>{table_view(), p, (const SlotRec*)dev_ptr, pos_slot.as<uint32_t>(), counters.as<unsigned long long>(), claimed.as<uint32_t>()}, n);
+    merged.emplace_back(dev_ptr, n);      // folded in again if the union overflows the table (runs_local_w)
 }
 
 // ---- stage 2: adjacency over the (now global) table, unitig occurrences along this rank's sequences ----
 template <int W> void DevicePipeline::Impl::runs_local_w() {
     if (stage < 1) throw std::runtime_error("build_local must precede runs_local");
     const KParams p = make_kparams(k, W);
-    const TableView tv = table_view();
     mark(13);
     if (is_multi) {      // the merges may have tripped the limits too
         unsigned long long hc[AC_N_COUNTERS];
         ac_d2h(hc, counters.p, sizeof hc, &stream); ac_sync(&stream);
+        if (hc[2] && cap != safe_cap) {
+            // This rank's own k-mers fitted the estimated size, the union with the other ranks' did not.  The safe size counts every rank's
+            // windows, so it holds the union: build the own table again at that size and fold the same records in again.  Exported entries
+            // do not depend on the table's size, so no rank has to export again (ac_entries_merge's buffers stay valid until this returns).
+            cap = safe_cap;
+            insert_w<W>();
+            const TableView tv = table_view();
+            for (const auto& e : merged)
+                ac_launch("merge", &stream, MergeBody<W>{tv, p, (const SlotRec*)e.first, pos_slot.as<uint32_t>(), counters.as<unsigned long long>(), claimed.as<uint32_t>()}, e.second);
+            ac_d2h(hc, counters.p, sizeof hc, &stream); ac_sync(&stream);
+        }
         if (hc[2]) throw std::runtime_error("k-mer table overflow while merging");
         if (hc[3] && !big_counts) throw std::runtime_error("a k-mer occurs more than 524287 times across the ranks: not supported by the multi-GPU exchange");
         n_dotted = hc[1];
     }
     any_dotted = n_dotted != 0;
+    const TableView tv = table_view();
 
     flags8.ensure(cap);
     n_slots_used = list_claimed();          // distinct canonical k-mers (with the other ranks' after a merge)

@@ -131,7 +131,9 @@ int ac_renumber_unitigs(ac_handle* h);
  *   -> ac_runs_local -> ac_runs_export -> [gather to rank 0] -> rank 0: ac_runs_import (all ranks, rank order) -> ac_build_finish
  * Records are opaque: 16 bytes per k-mer entry, 16 bytes per unitig occurrence.  ac_runs_import_padded reads the buffer a padded
  * gather leaves behind (rank r's counts[r] records start at record r * stride_records); ac_compress_finish is ac_compress for the
- * importing rank (simplify_structure and the GFA text on the device as well). */
+ * importing rank (simplify_structure and the GFA text on the device as well).
+ * The buffers passed to ac_entries_merge must stay valid, unchanged, until ac_runs_local returns: when the other ranks' k-mers overflow
+ * a table sized from the estimate, ac_runs_local builds this rank's table again at the safe size and folds the same records in again. */
 int ac_build_local(ac_handle* h, uint32_t seq_lo, uint32_t seq_hi, uint32_t multi);
 int ac_entries_count(ac_handle* h, uint64_t* n);
 int ac_entries_export(ac_handle* h, void* dst, uint64_t cap_records);

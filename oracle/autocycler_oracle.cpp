@@ -760,11 +760,23 @@ UnitigStrand UnitigGraph::find_starting_unitig(uint16_t seq_id) const {   // uni
 }
 
 bool UnitigGraph::get_next_unitig(uint16_t seq_id, bool seq_strand, const Unitig* u, bool strand, uint32_t pos,
-                                  UnitigStrand* next_out, uint32_t* next_pos_out) const {   // unitig_graph.rs:423-445
+                                  UnitigStrand* next_out, uint32_t* next_pos_out, PositionIndex* index) const {   // unitig_graph.rs:423-445
     uint32_t next_pos = pos + u->length();
     auto& next_edges = strand ? u->forward_next : u->reverse_next;
+    auto key = [](uint16_t id, bool s, uint32_t p) { return (uint64_t)id << 33 | (uint64_t)s << 32 | p; };
     for (auto& next : next_edges) {
         auto& positions = next.strand ? next.unitig->forward_positions : next.unitig->reverse_positions;
+        // The same answer as the scan below: the first edge whose list holds the position.  A walk through a run that repeats one unitig
+        // (a homopolymer) looks its list up once per step, and the scan alone makes that walk quadratic in the run's length.
+        if (index && positions.size() > 1024) {
+            auto it = index->find(&positions);
+            if (it == index->end()) {
+                it = index->emplace(&positions, std::unordered_set<uint64_t>()).first;
+                for (auto& p : positions) it->second.insert(key(p.seq_id(), p.strand(), p.pos));
+            }
+            if (it->second.count(key(seq_id, seq_strand, next_pos))) { *next_out = next; *next_pos_out = next_pos; return true; }
+            continue;
+        }
         for (auto& p : positions)
             if (p.seq_id() == seq_id && p.strand() == seq_strand && p.pos == next_pos) { *next_out = next; *next_pos_out = next_pos; return true; }
     }
@@ -775,10 +787,11 @@ std::vector<std::pair<uint32_t, bool>> UnitigGraph::get_unitig_path_for_sequence
     std::vector<std::pair<uint32_t, bool>> path;
     UnitigStrand u = find_starting_unitig(seq.id);
     uint32_t pos = 0;
+    PositionIndex index;      // the graph does not change during the walk
     for (;;) {
         path.emplace_back(u.number(), u.strand);
         UnitigStrand next; uint32_t next_pos;
-        if (!get_next_unitig(seq.id, strand::FORWARD, u.unitig, u.strand, pos, &next, &next_pos)) break;
+        if (!get_next_unitig(seq.id, strand::FORWARD, u.unitig, u.strand, pos, &next, &next_pos, &index)) break;
         u = next; pos = next_pos;
     }
     return path;

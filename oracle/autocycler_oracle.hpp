@@ -185,8 +185,10 @@ public:
     void trim_overlaps();
 private:
     UnitigStrand find_starting_unitig(uint16_t seq_id) const;
+    // (seq_id, strand, pos) of every entry of a long position list, built the first time one walk along a sequence looks the list up
+    typedef std::unordered_map<const std::vector<Position>*, std::unordered_set<uint64_t>> PositionIndex;
     bool get_next_unitig(uint16_t seq_id, bool seq_strand, const Unitig* u, bool strand, uint32_t pos,
-                         UnitigStrand* next, uint32_t* next_pos) const;
+                         UnitigStrand* next, uint32_t* next_pos, PositionIndex* index = nullptr) const;
 };
 
 // graph_simplification.rs:26-312

@@ -76,6 +76,53 @@ def random_case(seed, k):
     return files
 
 
+def _walk_steps(sampled_set):
+    """For every 6-mer (2 bits a base, first base most significant): the bases that extend it to an unsampled 7-mer whose own last six
+    bases can be extended the same way.  Iterated until no step leads to a dead end."""
+    ok = {c6: [b for b in range(4) if ((c6 << 2) | b) not in sampled_set] for c6 in range(1 << 12)}
+    while True:
+        dead = {c6 for c6, bs in ok.items() if not bs}
+        if not dead:
+            return ok
+        ok = {c6: [b for b in bs if (((c6 << 2) | b) & 0xFFF) not in dead] for c6, bs in ok.items()}
+
+
+_STEPS = None
+
+
+def sampled_walk(rng, n, rate=0.0):
+    """n bases of a random walk over 7-mers that avoids the 7-mers the table's sizing pass samples (tests/table_sizing.py), except that at
+    about `rate` of its steps it writes out a whole sampled 7-mer (the 7-mers across that seam are whatever they happen to be).  The sampled
+    set is closed under reverse complement, so at rate 0 neither strand holds a sampled 7-mer: every k-mer's centre is unsampled and the
+    size estimate sees nothing of this sequence."""
+    global _STEPS
+    import table_sizing
+    if _STEPS is None:
+        _STEPS = _walk_steps(table_sizing.SAMPLED_SET)
+    ok = _STEPS
+    jumps = [c7 for c7 in sorted(table_sizing.SAMPLED_SET) if ok[c7 & 0xFFF]]
+    c6 = rng.choice([c for c, bs in ok.items() if bs])
+    out = [(c6 >> (2 * (5 - i))) & 3 for i in range(6)]
+    while len(out) < n:
+        if rate and rng.random() < rate:
+            c7 = rng.choice(jumps)
+            out += [(c7 >> (2 * (6 - i))) & 3 for i in range(7)]
+            c6 = c7 & 0xFFF
+            continue
+        b = rng.choice(ok[c6])
+        out.append(b)
+        c6 = ((c6 << 2) | b) & 0xFFF
+    return "".join("ACGT"[b] for b in out[:n])
+
+
+def homopolymer_case(rng, occurrences, k, base="A", flank=300):
+    """One contig holding a run of `base` whose k-mer occurs `occurrences` times (a run of occurrences + k - 1 bases) between random
+    flanks (T: the occurrences land on the reverse strand of the canonical all-A k-mer)."""
+    stop = "G" if base in "AT" else "A"           # the flanks must not lengthen the run
+    a = rand_seq(rng, flank) + stop + base * (occurrences + k - 1) + stop + rand_seq(rng, flank)
+    return [("a.fasta", [("c1", a)])]
+
+
 def write_case(files, directory):
     import os
     os.makedirs(directory, exist_ok=True)

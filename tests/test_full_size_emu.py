@@ -19,7 +19,7 @@ from parity_common import run_library
 d = sys.argv[1]
 synth.write_assemblies(synth.make_assemblies("cfg2"), d)
 got = run_library(api.load_library(%(lib)r), d, 51)
-print("SHA", hashlib.sha256(got["gfa"].encode()).hexdigest(), got["before"].n_kmers, got["after"].n_unitigs, got["after"].n_links)
+print("SHA", hashlib.sha256(got["gfa"].encode()).hexdigest(), got["before"].n_kmers, got["after"].n_unitigs, got["after"].n_links, got["graph"].timings().table_capacity)
 """
 
 
@@ -35,6 +35,12 @@ def test_config2_golden_under_emulation(tmp_path, env):
     assert (int(line[3]), int(line[4])) == (g["unitigs_after"], g["links_after"])
     if "AC_DEVICE_SIMPLIFY" not in env:
         assert int(line[2]) == g["n_kmers"]
+    if not env:          # the size the sizing pass's exact restatement predicts (tests/table_sizing.py)
+        import oracle_lib as o
+        import table_sizing
+        count, oseqs = o.load_sequences(str(tmp_path / "cfg2"), 51)
+        pred = table_sizing.predict([s[4] for s in oseqs], 51, g["n_kmers"] // 2)
+        assert pred["capacity"] < pred["safe"] and int(line[5]) == pred["capacity"]
 
 
 MULTI_CODE = """

@@ -63,3 +63,24 @@ def test_several_devices_in_one_process(tmp_path, n_devices):
         kg2.add_sequences(seqs, count)
         graph = api.UnitigGraph.compress(kg2)
         assert hashlib.sha256(bytes(graph.gfa_view())).hexdigest() == g["sha256"]
+
+
+@pytest.mark.parametrize("n_devices", [2, 3])
+@pytest.mark.parametrize("big_first", [False, True])
+def test_several_devices_survive_a_low_estimate(tmp_path, n_devices, big_first):
+    """Imbalanced shards: a small file and a large walk the size estimate cannot see.  The rank holding only the small file overflows
+    its table while merging, builds it again at the safe size and merges the same records again: the oracle's bytes."""
+    n = _devices()
+    if n < n_devices:
+        pytest.skip(f"{n} CUDA device(s) visible, {n_devices} needed")
+    sys.path.insert(0, ROOT)
+    import cases
+    import oracle_lib as o
+    import table_routes
+    from autocycler_b200 import api
+    d = str(tmp_path / "in")
+    cases.write_case(table_routes.walk_case(77, 0.0, big_first=big_first), d)
+    expected, yaml, st = o.compress_dir(d, 51)
+    out = str(tmp_path / "out")
+    api.compress(d, out, k_size=51, devices=list(range(n_devices)))
+    assert open(os.path.join(out, "input_assemblies.gfa")).read() == expected

@@ -23,6 +23,9 @@ for seed, k in [(1, 9), (2, 31), (3, 51), (717, 9), (44, 5), (45, 65), (46, 91)]
     todo.append((cases.random_case(seed * 100 + k, k), k))
 big = synth.make_assemblies("x", n_assemblies=5, replicon_lengths=[40_000, 3_000], seed=77)
 todo.append(([(fn, [(h, s.tobytes().decode()) for h, s in recs]) for fn, recs in big], 51))
+import table_routes                  # a small file and a large walk the size estimate cannot see: the small file's rank overflows while merging
+for big_first in (False, True):
+    todo.append((table_routes.walk_case(77, 0.0, big_first=big_first), 51))
 for ci, (files, k) in enumerate(todo):
     d = os.path.join({tmp!r}, f"case{{ci}}")
     if rank == 0:
