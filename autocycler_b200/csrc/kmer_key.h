@@ -77,6 +77,33 @@ template <int W> AC_HD void key_push_left(Key<W>& key, uint64_t code, const KPar
     key.w[0] = (key.w[0] >> 2) | (code << (p.top_bits - 2));
 }
 
+// `c ? a : b` by value, word by word.  The same choice between two references takes their addresses, and the device compiler then
+// keeps both keys in local memory.
+template <int W> AC_HD Key<W> key_select(bool c, const Key<W>& a, const Key<W>& b) {
+    Key<W> r;
+#pragma unroll
+    for (int j = 0; j < W; ++j) r.w[j] = c ? a.w[j] : b.w[j];
+    r.d = c ? a.d : b.d;
+    return r;
+}
+
+// The two (k-1)-mers of a k-mer, right-aligned like a key and without dots (a dot at the dropped end goes with it): its first k-1
+// bases (the last one dropped) and its last k-1 bases (the first one dropped).
+template <int W> AC_HD Key<W> key_prefix(const Key<W>& key) {
+    Key<W> r;
+#pragma unroll
+    for (int j = W - 1; j > 0; --j) r.w[j] = (key.w[j] >> 2) | (key.w[j - 1] << 62);
+    r.w[0] = key.w[0] >> 2;
+    r.d = 0;
+    return r;
+}
+template <int W> AC_HD Key<W> key_suffix(const Key<W>& key, const KParams& p) {
+    Key<W> r = key;
+    r.w[0] &= p.top_mask >> 2;
+    r.d = 0;
+    return r;
+}
+
 // code of base at index i (0 = first base).
 template <int W> AC_HD uint32_t key_base(const Key<W>& key, uint32_t i, const KParams& p) {
     const uint32_t bit = 2 * (p.k - 1 - i), word = W - 1 - (bit >> 6);
@@ -130,8 +157,8 @@ template <int W> AC_HD Key<W> key_rc(const Key<W>& key, const KParams& p) {
     return r;
 }
 
-// One multiply-add per key word, then two multiply-xorshift rounds.  The slot index takes the top bits (umulhi), the fingerprint and the
-// Bloom bits the low ones.
+// One multiply-add per key word, then two multiply-xorshift rounds.  The slot index takes the top bits (umulhi), the fingerprint the
+// low ones.
 template <int W> AC_HD uint64_t key_hash(const Key<W>& key) {
     uint64_t h = key.w[0];
 #pragma unroll
