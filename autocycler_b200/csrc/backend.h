@@ -43,7 +43,6 @@ inline void ac_h2d(void* d, const void* h, size_t bytes, AcStream*) { memcpy(d, 
 inline void ac_d2h(void* h, const void* d, size_t bytes, AcStream*) { memcpy(h, d, bytes); }
 inline void ac_copy_dd(void* dst, const void* src, size_t bytes, AcStream*) { memcpy(dst, src, bytes); }
 inline void ac_sync(AcStream*) {}
-inline void ac_l2_keep(AcStream*, void*, size_t) {}
 inline void* ac_host_alloc(size_t bytes) { return malloc(bytes ? bytes : 1); }
 inline void ac_host_free(void* p) { free(p); }
 
@@ -109,28 +108,6 @@ inline void ac_h2d(void* d, const void* h, size_t bytes, AcStream* st) { AC_CUDA
 inline void ac_d2h(void* h, const void* d, size_t bytes, AcStream* st) { AC_CUDA_CHECK(cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, st->s)); }
 inline void ac_copy_dd(void* dst, const void* src, size_t bytes, AcStream* st) { AC_CUDA_CHECK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st->s)); }
 inline void ac_sync(AcStream* st) { AC_CUDA_CHECK(cudaStreamSynchronize(st->s)); }
-// Asks the L2 to keep [base, base + bytes) resident for the kernels that follow on the stream (the k-mer table while it is probed at
-// random): as much of it as the device lets a process pin, the rest of the range competes normally.  bytes == 0 ends the window.
-inline void ac_l2_keep(AcStream* st, void* base, size_t bytes) {
-    static int max_persist = -1, max_window = 0;
-    if (max_persist < 0) {
-        int dev = 0; cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, dev);
-        cudaDeviceGetAttribute(&max_window, cudaDevAttrMaxAccessPolicyWindowSize, dev);
-        if (max_persist > 0) cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, (size_t)max_persist);
-        if (getenv("AC_HOST_PROFILE")) fprintf(stderr, "[device] persisting L2 up to %d MB, window up to %d MB\n", max_persist >> 20, max_window >> 20);
-        cudaGetLastError();
-    }
-    if (max_persist <= 0 || max_window <= 0) return;
-    cudaStreamAttrValue v; memset(&v, 0, sizeof v);
-    const size_t win = bytes < (size_t)max_window ? bytes : (size_t)max_window;
-    v.accessPolicyWindow.base_ptr = base; v.accessPolicyWindow.num_bytes = win;
-    v.accessPolicyWindow.hitRatio = win == 0 ? 0.f : (win <= (size_t)max_persist ? 1.f : (float)((double)max_persist / (double)win));
-    v.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting; v.accessPolicyWindow.missProp = cudaAccessPropertyNormal;
-    cudaStreamSetAttribute(st->s, cudaStreamAttributeAccessPolicyWindow, &v);
-    if (bytes == 0) cudaCtxResetPersistingL2Cache();
-    cudaGetLastError();
-}
 // AC_SYNC_LAUNCHES=1 (debugging): wait for every kernel right after its launch and name the one that failed.
 inline void ac_debug_sync(const char* name, AcStream* st) {
     static const bool on = getenv("AC_SYNC_LAUNCHES") != nullptr;
@@ -208,9 +185,8 @@ template <class Body> inline void ac_launch_coop(const char* name, AcStream* st,
     }
     uint64_t want = (work + per_block - 1) / per_block;
     if (want < 1) want = 1;
-    static const int env_cap = getenv("AC_COOP_CTAS") ? atoi(getenv("AC_COOP_CTAS")) : 0;       // comparison only: fewer CTAs make a cheaper barrier and a longer walk
-    const int sms = (int)ac_sm_count(), limit = env_cap > 0 && env_cap < sms ? env_cap : sms;
-    const uint64_t cap = resident < limit ? (uint64_t)resident : (uint64_t)limit;     // one CTA per SM is plenty for these small steps, and keeps the barrier cheap
+    const int sms = (int)ac_sm_count();
+    const uint64_t cap = resident < sms ? (uint64_t)resident : (uint64_t)sms;     // one CTA per SM is plenty for these small steps, and keeps the barrier cheap
     const unsigned blocks = (unsigned)(want < cap ? want : cap);
     void* args[] = {(void*)&body};
     cudaError_t e = cudaLaunchCooperativeKernel((void*)ac_coop_kernel<Body>, dim3(blocks), dim3(256), args, 0, st->s);

@@ -64,7 +64,6 @@ struct ac_handle {
     HostGraph graph;
     std::string gfa;
     const char* gfa_ptr = nullptr; uint64_t gfa_len = 0;     // the finished file: h->gfa, or the pinned buffer the device wrote the S and L lines into
-    bool device_text_ok = false;                             // the device-written text describes the graph as it is now
     bool uploaded = false, built = false, gfa_ready = false;
     bool fused = false;                                      // built by ac_compress: simplified on the device; the host graph is adopted on first use
     bool graph_ready = false;                                // h->graph describes the current graph
@@ -254,8 +253,7 @@ void flush_lines(const char* p, size_t n) {
 struct ResultFlusher {
     std::vector<std::thread> threads;
     void start(const PipelineResult& r) {
-        static const bool off = getenv("AC_NO_RESULT_FLUSH") != nullptr;
-        if (off || !r.rec) return;
+        if (!r.rec) return;
         const size_t U = r.n_unitigs, strands = 2 * U + 1;
         std::vector<std::pair<const char*, size_t>> ranges = {
             {(const char*)r.rec, U * sizeof(UnitigRec)}, {(const char*)r.depth, U * 4}, {(const char*)r.order, U * 4}, {r.arena, (size_t)r.arena_cap},
@@ -299,11 +297,12 @@ static void record_timings(ac_handle* h) {
 static void adopt_result(ac_handle* h) {   // host graph over the device result + bookkeeping shared by ac_build / ac_build_finish / the first use after ac_compress
     const double t0 = now_ms();
     h->graph.build(h->res, h->seqs, h->cfg.k, h->cfg.keep_positions != 0);
-    if (!h->graph.device_sort) { DevicePipeline* pipe = h->pipe.get(); h->graph.device_sort = [pipe](const NumberKey* k, uint32_t n, uint32_t* out) { pipe->sort_number_keys(k, n, out); }; }
     const double ta = now_ms();
     h->graph.check_links();
     const double tb = now_ms();
-    if (!h->graph.adopt_candidates(h->res)) h->graph.prepare_simplify();   // the expand_repeats work list: made on the device, or (needing links and paths only) here while the sequences are still being copied
+    // a plain build: the expand_repeats work list, made on the device, or (needing links and paths only) here while the sequences are
+    // still being copied.  A fused build has run expand_repeats to its end: a later ac_simplify lists the candidates afresh.
+    if (!h->fused && !h->graph.adopt_candidates(h->res)) h->graph.prepare_simplify();
     const double tc = now_ms();
     h->pipe->complete(h->res);
     const double t1 = now_ms();
@@ -318,8 +317,7 @@ static void ensure_graph(const ac_handle* ch) {
     if (!h->built || h->graph_ready) return;
     if (!h->fused) throw std::runtime_error("no graph on this handle");
     h->pipe->fetch_graph(h->res, h->cfg.keep_positions != 0);
-    adopt_result(h);
-    h->graph.simplify_structure();           // everything was done on the device: this adopts its numbering (nothing is recomputed)
+    adopt_result(h);                         // simplified and renumbered on the device: the graph is taken as it is
 }
 
 int ac_build(ac_handle* h) {
@@ -335,7 +333,7 @@ int ac_build(ac_handle* h) {
     }
     h->fused = false; h->graph_ready = false;
     adopt_result(h);
-    h->built = true; h->gfa_ready = false; h->device_text_ok = false;
+    h->built = true; h->gfa_ready = false;
     return ok(h);
     AC_GUARD_END(h)
 }
@@ -346,12 +344,6 @@ int ac_compress(ac_handle* h) {
     if (!h) return set_error(nullptr, AC_EINVAL, "null handle");
     AC_GUARD_BEGIN
     if (!h->uploaded) return set_error(h, AC_EINVAL, "ac_upload must precede ac_compress");
-    static const bool host_tail = getenv("AC_HOST_SIMPLIFY") != nullptr;       // comparison only: device graph, then expand_repeats and the text on the host
-    if (host_tail) {
-        int rc = ac_build(h); if (rc != AC_OK) return rc;
-        if ((rc = ac_simplify(h)) != AC_OK) return rc;
-        uint64_t n = 0; return ac_gfa_size(h, &n);
-    }
     ResultFlusher flusher;
     if (h->built && h->graph_ready) flusher.start(h->res);                     // the host only ever writes to the graph arrays, and only once they were fetched
     {
@@ -361,7 +353,7 @@ int ac_compress(ac_handle* h) {
     }
     h->pipe->complete(h->res);
     h->fused = true; h->graph_ready = false; h->built = true;
-    h->gfa_ptr = h->res.gfa_text; h->gfa_len = h->res.gfa_bytes; h->gfa_ready = true; h->device_text_ok = true;
+    h->gfa_ptr = h->res.gfa_text; h->gfa_len = h->res.gfa_bytes; h->gfa_ready = true;
     record_timings(h);
     h->t.host_graph = h->t.host_simplify = h->t.host_gfa = 0;
     return ok(h);
@@ -432,12 +424,6 @@ int ac_runs_import_padded(ac_handle* h, const void* src, uint64_t stride_records
 static int compress_finish(ac_handle* h, bool split_paths) {
     if (!h) return set_error(nullptr, AC_EINVAL, "null handle");
     AC_GUARD_BEGIN
-    static const bool host_tail = getenv("AC_HOST_SIMPLIFY") != nullptr;
-    if (host_tail && !split_paths) {
-        int rc = ac_build_finish(h); if (rc != AC_OK) return rc;
-        if ((rc = ac_simplify(h)) != AC_OK) return rc;
-        uint64_t n = 0; return ac_gfa_size(h, &n);
-    }
     ResultFlusher flusher;
     if (h->built && h->graph_ready) flusher.start(h->res);
     {
@@ -446,7 +432,7 @@ static int compress_finish(ac_handle* h, bool split_paths) {
     }
     h->pipe->complete(h->res);
     h->fused = true; h->graph_ready = false; h->built = true;
-    h->gfa_ptr = h->res.gfa_text; h->gfa_len = h->res.gfa_bytes; h->gfa_ready = true; h->device_text_ok = true;
+    h->gfa_ptr = h->res.gfa_text; h->gfa_len = h->res.gfa_bytes; h->gfa_ready = true;
     record_timings(h);
     h->t.host_graph = h->t.host_simplify = h->t.host_gfa = 0;
     return ok(h);
@@ -485,7 +471,7 @@ int ac_build_finish(ac_handle* h) {
     }
     h->fused = false; h->graph_ready = false;
     adopt_result(h);
-    h->built = true; h->gfa_ready = false; h->device_text_ok = false;
+    h->built = true; h->gfa_ready = false;
     return ok(h);
     AC_GUARD_END(h)
 }
@@ -499,7 +485,6 @@ int ac_simplify(ac_handle* h) {
     h->graph.simplify_structure();
     h->t.host_simplify = (float)(now_ms() - t0);
     h->gfa_ready = false;
-    h->device_text_ok = !h->fused && h->res.gfa_text != nullptr && h->graph.last_simplify_on_device;
     return ok(h);
     AC_GUARD_END(h)
 }
@@ -510,7 +495,7 @@ int ac_merge_linear_paths(ac_handle* h, int use_paths) {
     if (!h->built) return set_error(h, AC_EINVAL, "ac_build must precede ac_merge_linear_paths");
     ensure_graph(h);
     h->graph.merge_linear_paths(use_paths != 0);
-    h->gfa_ready = false; h->device_text_ok = false;
+    h->gfa_ready = false;
     return ok(h);
     AC_GUARD_END(h)
 }
@@ -558,9 +543,8 @@ int ac_bind_host_to_device(int32_t device) {
 int ac_load_gfa(ac_handle* h, const char* gfa_text, uint64_t length) {
     if (!h || !gfa_text) return set_error(h, AC_EINVAL, "null argument");
     AC_GUARD_BEGIN
-    h->built = false; h->gfa_ready = false; h->uploaded = false; h->device_text_ok = false; h->fused = false; h->graph_ready = false;
+    h->built = false; h->gfa_ready = false; h->uploaded = false; h->fused = false; h->graph_ready = false;
     h->seqs.clear(); h->infos.clear(); h->ascii.clear(); h->loaded = LoadedInput(); h->res = PipelineResult(); h->t = ac_timings{};   // a loaded graph has no sequence bytes: ac_upload / ac_build need ac_add_sequence again
-    h->graph.device_sort = nullptr;
     h->trimmed = false; h->trim_yaml.clear();
     h->clustered = false; h->cluster = ClusterResult();
     h->graph.load_gfa(gfa_text, (size_t)length, h->seqs);
@@ -617,7 +601,7 @@ int ac_renumber_unitigs(ac_handle* h) {
     if (!h->built) return set_error(h, AC_EINVAL, "ac_build must precede ac_renumber_unitigs");
     ensure_graph(h);
     h->graph.renumber();
-    h->gfa_ready = false; h->device_text_ok = false;
+    h->gfa_ready = false;
     return ok(h);
     AC_GUARD_END(h)
 }
@@ -710,13 +694,9 @@ int ac_gfa_size(ac_handle* h, uint64_t* n_bytes) {
     if (!h->built) return set_error(h, AC_EINVAL, "ac_build must precede ac_gfa_size");
     if (!h->gfa_ready) {
         const double t0 = now_ms();
-        if (h->device_text_ok) {      // the whole file was rendered on the device (AC_DEVICE_SIMPLIFY + AC_DEVICE_GFA in a plain build)
-            h->gfa_ptr = h->res.gfa_text; h->gfa_len = h->res.gfa_bytes;
-        } else {
-            ensure_graph(h);
-            h->graph.gfa_text(h->seqs, h->gfa);
-            h->gfa_ptr = h->gfa.data(); h->gfa_len = h->gfa.size();
-        }
+        ensure_graph(h);
+        h->graph.gfa_text(h->seqs, h->gfa);
+        h->gfa_ptr = h->gfa.data(); h->gfa_len = h->gfa.size();
         h->t.host_gfa = (float)(now_ms() - t0);
         h->gfa_ready = true;
         if (getenv("AC_HOST_PROFILE")) {
@@ -758,8 +738,8 @@ int ac_load_sequences(ac_handle* h, const char* dir, uint32_t max_contigs, uint3
     if (!h || !dir) return set_error(h, AC_EINVAL, "null argument");
     AC_GUARD_BEGIN
     ac_clear_sequences(h);
-    // end repair runs on the device unless its k/2-base literals are longer than the scan kernel's two key words (k > 129) or AC_HOST_END_REPAIR is set
-    const bool device_repair = !getenv("AC_HOST_END_REPAIR") && h->cfg.k / 2 <= 64;
+    // end repair runs on the device unless its k/2-base literals are longer than the scan kernel's two key words (k > 129)
+    const bool device_repair = h->cfg.k / 2 <= 64;
     LoadedInput in = load_sequences(dir, h->cfg.k, max_contigs, threads ? threads : 1, false, device_repair ? h->pipe.get() : nullptr);
     for (size_t i = 0; i < in.seqs.size(); ++i) {
         int rc = ac_add_sequence(h, in.seqs[i].id, (const uint8_t*)in.padded[i].data(), in.padded[i].size(),
@@ -1008,7 +988,7 @@ int ac_trim(ac_handle* h, double min_identity, uint32_t max_unitigs, double mad)
     h->infos.clear(); h->ascii.clear();      // the sequences are trimmed paths now: no bytes
     h->trim_yaml = trimmed_metrics_yaml(h->seqs); h->trimmed = true;
     h->t.trim_kernel = st.kernel_ms; h->trim_stats = st;
-    h->gfa_ready = false; h->device_text_ok = false;
+    h->gfa_ready = false;
     return ok(h);
     AC_GUARD_END(h)
 }

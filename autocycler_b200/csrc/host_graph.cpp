@@ -160,9 +160,12 @@ void HostGraph::build(const PipelineResult& r, const std::vector<HostSeq>& seqs,
     prof.adopt = now_ms() - t0;
 
     order.resize(U);
-    if (r.order) {                            // sorted on the device while the sequences were still in HBM
+    // sorted on the device while the sequences were still in HBM: the numbering of the graph as built or, after a fused build, the one
+    // simplify_structure ends with (graph_simplification.rs:38)
+    const uint32_t* given = r.final_order ? r.final_order : r.order;
+    if (given) {
         const double t1 = now_ms();
-        memcpy(order.data(), r.order, (size_t)U * 4);
+        memcpy(order.data(), given, (size_t)U * 4);
         for (uint32_t n = 0; n < U; ++n) number[order[n]] = n + 1;
         prof.renumber += now_ms() - t1;
     } else {
@@ -200,32 +203,7 @@ void HostGraph::renumber() {   // unitig_graph.rs:295-315: stable sort by length
         }
     });
     const double t_keys = now_ms();
-    // Opt-in (AC_DEVICE_RENUMBER=1): the round trip (14 small launches, two copies, the tie pass) is no cheaper than the host
-    // sample sort for graphs of a hundred thousand unitigs, so the host sort is the default.
-    static const bool on_device = getenv("AC_DEVICE_RENUMBER") != nullptr;
-    static const uint32_t device_min = getenv("AC_DEVICE_SORT_MIN") ? (uint32_t)atoi(getenv("AC_DEVICE_SORT_MIN")) : 16384;   // tests lower it
-    if (device_sort && on_device && U >= device_min) {
-        // The device orders by (length, first 8 bases, current position); what 16 bytes cannot decide — equal length and prefix — is
-        // settled here, run by run, with the full comparison (rest of the sequence, depth, position).
-        std::vector<NumberKey> nk(U); std::vector<uint32_t> sorted(U);
-        parallel_tasks(T, [&](size_t t) { for (size_t n = bounds(t); n < bounds(t + 1); ++n) { nk[n].prefix = keys[n].prefix; nk[n].len = keys[n].len; nk[n].pad = 0; } });
-        device_sort(nk.data(), U, sorted.data());
-        std::vector<Key> arranged(U);
-        parallel_tasks(T, [&](size_t t) { for (size_t n = bounds(t); n < bounds(t + 1); ++n) arranged[n] = keys[sorted[n]]; });
-        keys.swap(arranged);
-        // run boundaries, then the runs of each piece (a run straddling a piece boundary belongs to the piece it starts in)
-        parallel_tasks(T, [&](size_t t) {
-            size_t n = bounds(t); const size_t stop = bounds(t + 1);
-            auto same = [&](size_t x, size_t y) { return keys[x].len == keys[y].len && keys[x].prefix == keys[y].prefix; };
-            while (n > 0 && n < stop && same(n - 1, n)) ++n;           // the run that began in the previous piece is theirs
-            while (n < stop) {
-                size_t e = n + 1;
-                while (e < U && same(n, e)) ++e;
-                if (e - n > 1) std::sort(keys.begin() + n, keys.begin() + e, less);
-                n = e;
-            }
-        });
-    } else if (T == 1) std::sort(keys.begin(), keys.end(), less);
+    if (T == 1) std::sort(keys.begin(), keys.end(), less);
     else {   // sample sort: splitters from a sample, every thread scatters its piece into the buckets, every bucket is sorted on its own
         const size_t B = T, per = 16;
         std::vector<Key> sample;
@@ -388,7 +366,7 @@ void HostGraph::compute_candidates() {
     exhausted.assign(cands.size(), 0);
     for (uint32_t u = 0; u < U; ++u) rec[u].flags = 0;
     first_pass = true;
-    cands_ready = true; spec_from_device = false; device_pass_total = (size_t)-1; final_order.clear();
+    cands_ready = true; spec_from_device = false;
 }
 
 namespace {
@@ -626,12 +604,12 @@ void HostGraph::prepare_simplify() {   // the structural part of expand_repeats:
 }
 
 // The lists compute_candidates() makes, taken from the device (pipeline.cu: CandidateFlagBody ... CommonLengthBody), which
-// listed them in the numbering order it had just sorted.  Only valid for the graph exactly as built.
+// listed them in the numbering order it had just sorted.  Only valid for the graph exactly as built (a plain build).
 bool HostGraph::adopt_candidates(const PipelineResult& r) {
     static const bool on_host = getenv("AC_HOST_CANDIDATES") != nullptr, cross_check = getenv("AC_CHECK_CANDIDATES") != nullptr;
     if (!r.cands || !r.deps || !r.fixed_start || on_host) return false;
     const double t0 = now_ms();
-    if (cross_check && !r.first_pass_done) {  // tests: the host listing of the same graph must agree field by field (not comparable once the device has applied passes)
+    if (cross_check) {                        // tests: the host listing of the same graph must agree field by field
         compute_candidates();
         bool same = cands.size() == r.n_cands && memcmp(fixed_start.data(), r.fixed_start, U) == 0 && memcmp(fixed_end.data(), r.fixed_end, U) == 0;
         for (size_t i = 0; same && i < cands.size(); ++i) {
@@ -654,30 +632,12 @@ bool HostGraph::adopt_candidates(const PipelineResult& r) {
     dirty.assign((n + 63) / 64, 0);
     exhausted.assign(n, 0);
     first_pass = true; cands_ready = true; spec_from_device = true;
-    device_pass_total = (size_t)-1;
-    if (r.first_pass_done) {                  // the device has applied pass 1 already: rec / arena hold its result, this is what it left for pass 2
-        if (n) {                              // (no candidates: nothing was listed and the vectors are empty)
-            memcpy(dirty.data(), r.dirty, dirty.size() * 8);
-            memcpy(exhausted.data(), r.exhausted, n);
-        }
-        first_pass = false; spec_from_device = false;
-        pass_id = 1;                          // the unitigs it changed carry flags == 1
-        device_pass_total = (size_t)r.first_pass_total;
-        if (r.final_order) final_order.assign(r.final_order, r.final_order + U);     // the whole loop ran there, and the renumbering after it
-    }
     prof.candidates = now_ms() - t0;
     return true;
 }
 
 size_t HostGraph::expand_repeats() {   // graph_simplification.rs:43-86
     const double t0 = now_ms();
-    if (cands_ready && device_pass_total != (size_t)-1) {   // pass 1 ran on the device: hand its count to the caller's `while expand_repeats() > 0`
-        const size_t moved = device_pass_total;
-        device_pass_total = (size_t)-1;
-        if (getenv("AC_HOST_PROFILE")) fprintf(stderr, "[host] pass 1 (on the device): %zu bases\n", moved);
-        prof.passes += 1;
-        return moved;
-    }
     if (!cands_ready) { compute_candidates(); prof.candidates = now_ms() - t0; }
     size_t total_shifted = 0;
     ++pass_id;                                      // unitigs modified during this pass carry it in rec[].flags
@@ -724,16 +684,8 @@ size_t HostGraph::expand_repeats() {   // graph_simplification.rs:43-86
 }
 
 void HostGraph::simplify_structure() {   // graph_simplification.rs:26-40
-    const bool on_device = cands_ready && device_pass_total == 0 && final_order.size() == U;    // nothing left to do but adopt the numbering
     while (expand_repeats() > 0) {}
-    last_simplify_on_device = on_device;
-    if (on_device) {
-        const double t0 = now_ms();
-        order = final_order;
-        for (uint32_t n = 0; n < U; ++n) number[order[n]] = n + 1;
-        prof.renumber += now_ms() - t0;
-    } else renumber();
-    final_order.clear();
+    renumber();
     cands_ready = false;      // the numbering order changed: a later call starts from the new order
 }
 

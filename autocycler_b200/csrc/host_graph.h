@@ -8,7 +8,6 @@
 // unitig so that repeat expansion moves bytes without reallocating.
 #pragma once
 #include <cstdint>
-#include <functional>
 #include <string>
 #include <vector>
 
@@ -61,14 +60,11 @@ public:
     // unitig_graph.rs:36-48 from the device result (build, simplify_seqs, create_links, trim_overlaps, renumber, check)
     void build(const PipelineResult& r, const std::vector<HostSeq>& seqs, uint32_t k, bool keep_positions);
     void renumber();                          // unitig_graph.rs:295-315
-    // optional: sorts NumberKeys on the device (DevicePipeline::sort_number_keys); unset = the host sample sort
-    std::function<void(const NumberKey*, uint32_t, uint32_t*)> device_sort;
     void check_links() const;                 // unitig_graph.rs:752-793
     void simplify_structure();                // graph_simplification.rs:26-40
     size_t expand_repeats();                  // graph_simplification.rs:43-86
-    bool last_simplify_on_device = false;     // simplify_structure found everything done by the device (then its GFA text, if any, describes this graph)
     void prepare_simplify();                  // lists the candidates of expand_repeats ahead of time (links and paths only, no sequence bytes)
-    bool adopt_candidates(const PipelineResult& r);   // ... or takes the same lists from the device result (graph as built only)
+    bool adopt_candidates(const PipelineResult& r);   // ... or takes the same lists from a plain build's device result (graph as built only)
     // UnitigGraph::from_gfa_lines (unitig_graph.rs:55-174; host_gfa_load.cpp): replaces the graph by the one in `text`, returns its sequences
     void load_gfa(const char* text, size_t len, std::vector<HostSeq>& seqs);
     void merge_linear_paths(bool use_paths);  // graph_simplification.rs:315-371 (host_merge.cpp); use_paths=false is the reference's `seqs` = [] and drops the paths
@@ -105,8 +101,6 @@ private:
     bool cands_ready = false, first_pass = true;
     void compute_candidates();
     bool spec_from_device = false;
-    std::vector<uint32_t> final_order;        // the numbering after simplify_structure when the device ran all of it (consumed by simplify_structure)
-    size_t device_pass_total = (size_t)-1;    // bases moved by a first pass the device already applied ((size_t)-1: none pending)
     uint32_t common_length(const Candidate& cand) const;
     // The sources of a candidate: its inline copy (at most 6; a graph built from k-mers has at most 5 neighbours per side), or, for
     // a loaded graph with more, the link list they were copied from (links never change during simplify_structure).

@@ -925,21 +925,6 @@ struct NumberKeyBody {
         prefix[s] = v;
     }
 };
-struct NumberKeyLess {      // sort_number_keys: the part of renumber_unitigs' order that 16 bytes per unitig can decide
-    const NumberKey* key;
-    typedef SortRec Key;
-    AC_D Key load(uint32_t id) const { Key k; k.id = id; k.pad = 0; k.a = key[id].prefix; k.b = 0; k.c = key[id].len; k.d = 0; return k; }
-    AC_D bool less_keys(const Key& x, const Key& y, uint32_t ia, uint32_t ib) const {
-        if (x.c != y.c) return x.c > y.c;
-        if (x.a != y.a) return x.a < y.a;
-        return ia < ib;
-    }
-    AC_D bool operator()(uint32_t a, uint32_t b) const {
-        if (key[a].len != key[b].len) return key[a].len > key[b].len;
-        if (key[a].prefix != key[b].prefix) return key[a].prefix < key[b].prefix;
-        return a < b;
-    }
-};
 struct InversePermBody { const uint32_t* order; uint32_t* pos; AC_D void operator()(uint64_t n) const { pos[order[n]] = (uint32_t)n; } };
 struct NumberLess {
     const UnitigRec* rec; const uint32_t* depth; const char* arena; const uint64_t* prefix;
@@ -1174,7 +1159,7 @@ struct CommonLengthBody {   // get_common_end_seq (:298-312) for side 0, get_com
     }
 };
 
-// ---- first pass of expand_repeats on the device (opt-in, AC_DEVICE_FIRST_PASS=1; host_graph.cpp apply_candidate is the model) ----
+// ---- expand_repeats on the device (fused builds; host_graph.cpp apply_candidate is the model) ----
 // Two candidates conflict when they share a unitig; level = 1 + the highest level of an earlier conflicting candidate.  The earlier
 // readers of a unitig are its deps entries, so the levels are the fixed point of "1 + max over predecessors" (longest path in a DAG
 // whose edges point to higher indices), reached in as many relaxation rounds as there are levels.
@@ -1288,9 +1273,9 @@ struct ApplyLevelBody {      // graph_simplification.rs:64-84 for the candidates
     // "somebody may be due"; the dirty bits stay the truth.
     uint32_t* due_cur = nullptr; uint32_t* due_next = nullptr;
     AC_D void count_mark(uint32_t cnd) const {
-        if (!due_cur) return;
         const uint32_t lv = level[cnd];
-        ac_atomic_add(!all_due && lv > this_level ? &due_cur[lv] : &due_next[lv], 1u);
+        uint32_t* counts = !all_due && lv > this_level ? due_cur : due_next;     // chosen by value: a choice between the two addresses spills
+        ac_atomic_add(counts + lv, 1u);
     }
     // strand s read from the end that candidate side `side` compares: its last bases backwards (inputs, side 0) or its first bases (outputs)
     AC_D StrandCursor cursor(UStrand s, uint32_t side) const {
@@ -1403,13 +1388,13 @@ struct ApplyLevelBody {      // graph_simplification.rs:64-84 for the candidates
 #define AC_PASS_WORDS (2 + 2 * AC_PASS_SET_WORDS)
 struct SimplifyCoopBody {
     ApplyLevelBody apply; RelocBoundBody next_bound; uint64_t n; const uint32_t* n_levels;
-    unsigned long long* c64; unsigned long long* res; uint64_t arena_cap; uint32_t first_set; bool first_is_pass_one, single_pass;
+    unsigned long long* c64; unsigned long long* res; uint64_t arena_cap; uint32_t first_set; bool first_is_pass_one;
     // Levels nobody is due on are stepped over without a barrier (later passes touch few of them: BASELINE config 2 walks 47 of its
     // 6 x 14 levels).  due: three sets of per-level mark counts (stride due_stride), used in rotation — the pass reads `cur`, marks for the
     // pass after it go to `next`, and the set the pass before read is cleared for re-use once everybody is past this pass's first barrier.
     // Every thread takes the same decision at a level: marks into cur[l] are only made while a level below l is worked on, and a barrier
     // lies between that and the first look at cur[l].  The last level is never skipped, so that every pass has a barrier.
-    uint32_t* due = nullptr; uint32_t due_stride = 0, first_due = 0;
+    uint32_t* due; uint32_t due_stride, first_due;
     template <class Sync> AC_D void operator()(uint64_t tid, uint64_t nt, Sync& sync) const {
         const uint32_t levels = *n_levels;
         ApplyLevelBody a = apply;
@@ -1419,11 +1404,11 @@ struct SimplifyCoopBody {
             unsigned long long* mine = c64 + AC_PASS_SET(q); unsigned long long* other = c64 + AC_PASS_SET(q ^ 1u);
             a.all_due = first_is_pass_one && pass == 0; a.total_shifted = mine;
             const uint32_t dq = (first_due + pass) % 3u;
-            uint32_t* due_old = nullptr;
-            if (due) { a.due_cur = due + (size_t)dq * due_stride; a.due_next = due + (size_t)((dq + 1u) % 3u) * due_stride; due_old = due + (size_t)((dq + 2u) % 3u) * due_stride; }
+            a.due_cur = due + (size_t)dq * due_stride; a.due_next = due + (size_t)((dq + 1u) % 3u) * due_stride;
+            uint32_t* due_old = due + (size_t)((dq + 2u) % 3u) * due_stride;
             bool fenced = false;
             for (uint32_t l = 1; l <= levels; ++l) {
-                if (due && !a.all_due && l < levels && ac_ld_volatile(&a.due_cur[l]) == 0) continue;
+                if (!a.all_due && l < levels && ac_ld_volatile(&a.due_cur[l]) == 0) continue;
                 a.this_level = l;
 #ifdef AC_EMULATE
                 if (getenv("AC_HOST_PROFILE")) {
@@ -1436,7 +1421,7 @@ struct SimplifyCoopBody {
                 sync();
                 if (!fenced && tid == 0) {
                     for (uint32_t x = 0; x < AC_PASS_SET_WORDS; ++x) other[x] = 0;
-                    if (due_old) for (uint32_t x = 0; x <= levels; ++x) due_old[x] = 0;
+                    for (uint32_t x = 0; x <= levels; ++x) due_old[x] = 0;
                 }
                 fenced = true;
                 if (l == levels && tid == 0) mine[2 + AC_BOUND_STRIPES] = ac_ld_volatile(c64);       // nothing is relocated after the last level: the same value for every thread's decision below
@@ -1451,14 +1436,14 @@ struct SimplifyCoopBody {
             const unsigned long long moved = ac_ld_volatile(mine), used = ac_ld_volatile(mine + 2 + AC_BOUND_STRIPES);
             unsigned long long bound = 0;
             for (uint32_t x = 0; x < AC_BOUND_STRIPES; ++x) bound += ac_ld_volatile(mine + 1 + x);
-            const bool go_on = moved != 0 && !single_pass && used + bound + 64 <= arena_cap && pass < 1000000u;
+            const bool go_on = moved != 0 && used + bound + 64 <= arena_cap && pass < 1000000u;
             if (tid == 0) { res[0] = moved; res[1] += moved; res[2] = pass + 1; res[3] = bound; res[4] = ac_ld_volatile(mine + 1 + AC_BOUND_STRIPES); res[5] = q ^ 1u; res[6] = used; res[7] = (dq + 1u) % 3u; }
             if (!go_on) return;
         }
     }
 };
 
-// ---- save_gfa on the device (opt-in with AC_DEVICE_SIMPLIFY + AC_DEVICE_GFA; unitig_graph.rs:317-360, unitig.rs:167-171) ----
+// ---- save_gfa on the device (fused builds; unitig_graph.rs:317-360, unitig.rs:167-171) ----
 // S and L lines are written straight from the simplified, renumbered graph in HBM; the P lines carry host strings (file names,
 // headers), so only their unitig lists are rendered here and the host wraps them.
 AC_D uint32_t ac_put_dec(char* p, uint32_t v) {            // decimal text of v, returns its length
@@ -2029,9 +2014,9 @@ struct DevicePipeline::Impl {
     DevBuf sort_a, sort_b, sort_ra, sort_rb, num_prefix, rank, d_len, d_depth, need, d_seq_off, d_arena, d_min_fpos, d_min_rpos;
     DevBuf strand_cnt, d_next_off, d_next, prev_cnt, d_prev_off, d_prev, d_path, d_path_off;
     DevBuf d_rec;
-    PinBuf h_cands, h_deps, h_spec, h_fixed, h_keys, h_sorted;
-    DevBuf d_keys, dist_member, dist_shared, d_pred, d_level, d_flagmax, d_counters64, d_dirty, d_exhausted, d_arena2, d_arena3, d_pos, sort_c, sort_d, d_pos2, gfa_s_size, gfa_l_size, gfa_p_size, gfa_pieces, d_text, d_ptext, d_last, d_pbound, d_due;
-    PinBuf h_dirty, h_exhausted, h_order2, h_text, h_ptext, h_pbound;
+    PinBuf h_cands, h_deps, h_spec, h_fixed;
+    DevBuf dist_member, dist_shared, d_pred, d_level, d_flagmax, d_counters64, d_dirty, d_exhausted, d_arena2, d_arena3, d_pos, sort_c, sort_d, d_pos2, gfa_s_size, gfa_l_size, gfa_p_size, gfa_pieces, d_text, d_ptext, d_last, d_pbound, d_due;
+    PinBuf h_order2, h_text, h_ptext, h_pbound;
     PinBuf h_rec, h_depth, h_order, h_arena, h_next_off, h_next, h_prev_off, h_prev, h_path, h_path_off, h_run_start, h_run_len;
 #ifndef AC_EMULATE
     cudaEvent_t ev[24];
@@ -2133,8 +2118,8 @@ struct DevicePipeline::Impl {
         uint32_t U = 0, n_strands = 0; uint64_t n_links = 0, n_cands = 0;
         uint32_t* order_built = nullptr; uint32_t* final_order = nullptr; uint8_t* fix_start = nullptr;
         DevBuf* arena_src = nullptr; uint64_t arena_final = 0;
-        bool first_pass_done = false, any_moved = false, gfa_on_device = false, hairpins_ready = false, paths_split = false;
-        uint64_t first_pass_total = 0, bases_removed = 0, gfa_bytes = 0;
+        bool any_moved = false, gfa_on_device = false, hairpins_ready = false, paths_split = false;
+        uint64_t bases_removed = 0, gfa_bytes = 0;
     } R;
     bool pending_keep_positions = false;
     void pull_graph(PipelineResult& out, bool keep_positions);
@@ -2263,21 +2248,6 @@ void DevicePipeline::set_path_line_texts(const char* blob, const uint32_t* prefi
     m.path_pre.assign(prefix_len, prefix_len + n); m.path_suf.assign(suffix_len, suffix_len + n);
     uint64_t bytes = 0; for (uint32_t i = 0; i < n; ++i) bytes += (uint64_t)prefix_len[i] + suffix_len[i];
     m.path_blob.assign(blob, blob + bytes);
-}
-
-void DevicePipeline::sort_number_keys(const NumberKey* keys, uint32_t n, uint32_t* sorted) {
-    Impl& m = *impl; m.set_device();
-    if (n == 0) return;
-    m.h_keys.ensure((size_t)n * sizeof(NumberKey));                 // pinned staging: the copy runs at link speed and the call stays asynchronous until the sync
-    memcpy(m.h_keys.p, keys, (size_t)n * sizeof(NumberKey));
-    m.d_keys.ensure((size_t)n * sizeof(NumberKey)); m.sort_a.ensure((size_t)n * 4); m.sort_b.ensure((size_t)n * 4); m.sort_ra.ensure((size_t)n * sizeof(SortRec)); m.sort_rb.ensure((size_t)n * sizeof(SortRec));
-    ac_h2d(m.d_keys.p, m.h_keys.p, (size_t)n * sizeof(NumberKey), &m.stream);
-    const NumberKeyLess less{m.d_keys.as<NumberKey>()};
-    uint32_t* in = sort_indices(&m.stream, less, n, m.sort_a.as<uint32_t>(), m.sort_b.as<uint32_t>(), m.sort_ra.as<SortRec>(), m.sort_rb.as<SortRec>());
-    m.h_sorted.ensure((size_t)n * 4);
-    ac_d2h(m.h_sorted.p, in, (size_t)n * 4, &m.stream);
-    ac_sync(&m.stream);
-    memcpy(sorted, m.h_sorted.p, (size_t)n * 4);
 }
 
 void DevicePipeline::Impl::upload_paths(const UStrand* path, const uint64_t* path_off, uint32_t n, const uint32_t* unitig_len, uint32_t U) {
@@ -2615,11 +2585,6 @@ template <int W> void DevicePipeline::Impl::insert_w() {
         if (getenv("AC_HOST_PROFILE")) fprintf(stderr, "[device] k-mer table attempt %d: capacity %llu, side counts %d\n", table_attempt, (unsigned long long)cap, (int)big_counts);
         poison_table();
         slots.ensure(cap * sizeof(Slot));
-        // AC_L2_PERSIST=table | packed (comparison only): ask the L2 to keep the k-mer table, or the 2-bit sequence store every probe's
-        // comparison reads at random, resident while the table is probed (inputs whose table is several times the L2)
-        static const char* l2_keep = getenv("AC_L2_PERSIST");
-        if (l2_keep && !strcmp(l2_keep, "packed")) ac_l2_keep(&stream, packed.p, n_words * sizeof(uint64_t));
-        else if (l2_keep) ac_l2_keep(&stream, slots.p, cap * sizeof(Slot));
         ac_memset(slots.p, 0xFF, cap * sizeof(Slot), &stream);               // AC_EMPTY_SLOT
         if (big_counts) { count_big.ensure(cap * 4); ac_memset(count_big.p, 0, cap * 4, &stream); }
         ac_memset(counters.p, 0, sizeof hc, &stream);
@@ -2798,7 +2763,6 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
     link_count.ensure((size_t)n_unitigs * 2 * 4); links.ensure((size_t)n_unitigs * 2 * AC_MAX_LINKS * 4);
     ac_launch("links", &stream, LinkBody<W>{tv, p, any_dotted, unitigs.as<DeviceUnitig>(), pos_slot.as<uint32_t>(), slot_unitig.as<uint32_t>(),
                                             link_count.as<uint32_t>(), links.as<uint32_t>()}, (uint64_t)n_unitigs * 2);
-    if (getenv("AC_L2_PERSIST")) ac_l2_keep(&stream, nullptr, 0);        // the table has had its last random access
     mark(9);
 
     // ---- seed order: stable LSD radix sort of the unitigs by their seed k-mer ----
@@ -2865,16 +2829,12 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
     ac_launch("dependents", &stream, DependentsBody{d_next_off.as<uint32_t>(), d_next.as<UStrand>(), d_prev_off.as<uint32_t>(), d_prev.as<UStrand>(), d_cand_at.as<int32_t>(),
                                                     d_deps.as<ExpandDeps>()}, U);
     ac_launch("common_length", &stream, CommonLengthBody{d_cands.as<ExpandCandidate>(), d_rec.as<UnitigRec>(), d_arena.as<char>(), d_spec.as<uint32_t>()}, n_cands);
-    // ---- simplify_structure and save_gfa on the device: always in a fused build; in a plain build only behind the switches
-    // AC_DEVICE_FIRST_PASS (first expand_repeats call), AC_DEVICE_SIMPLIFY (the whole loop + renumbering), AC_DEVICE_GFA (the text) ----
-    static const bool env_first = getenv("AC_DEVICE_FIRST_PASS") != nullptr, env_simplify = getenv("AC_DEVICE_SIMPLIFY") != nullptr, env_gfa = getenv("AC_DEVICE_GFA") != nullptr;
-    const bool device_simplify = fused || env_simplify, device_first_pass = device_simplify || env_first, device_gfa = fused || (env_simplify && env_gfa);
+    // ---- simplify_structure and save_gfa on the device: fused builds only (a plain build hands the host the graph as built) ----
     R = Pending();
     R.U = U; R.n_links = n_links; R.n_cands = n_cands; R.n_strands = n_strands; R.order_built = ord_in; R.fix_start = fix_start;
     R.arena_final = arena_bytes; R.arena_src = &d_arena;
     mark(11);
-    if (device_first_pass && n_cands == 0 && device_simplify) { R.first_pass_done = true; R.first_pass_total = 0; }     // nothing can shift: the loop ends at once
-    if (device_first_pass && n_cands > 0) {
+    if (fused && n_cands > 0) {
         d_pred.ensure(n_cands * 7 * 4); d_level.ensure(n_cands * 4); d_flagmax.ensure(32); d_counters64.ensure((AC_PASS_WORDS + 8) * 8);
         d_dirty.ensure(((n_cands + 63) / 64) * 8 + 8); d_exhausted.ensure(n_cands + 8);
         unsigned long long* c64 = d_counters64.as<unsigned long long>();         // SimplifyCoopBody's counters, then its eight result words
@@ -2897,26 +2857,24 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
         ac_h2d(c64, &start, 8, &stream);
         ac_memset(c64 + AC_PASS_SET(1), 0, AC_PASS_SET_WORDS * 8, &stream);
         ac_memset(d_dirty.p, 0, ((n_cands + 63) / 64) * 8 + 8, &stream); ac_memset(d_exhausted.p, 0, n_cands + 8, &stream);
-        // `while expand_repeats() > 0 {}` (only its first call without device_simplify): one launch for as many passes as the arena has room for
+        // `while expand_repeats() > 0 {}`: one launch for as many passes as the arena has room for
         static const bool always_grow = getenv("AC_DEVICE_TIGHT_ARENA") != nullptr;   // test hook: one pass per launch, the growth path before every pass
         uint32_t next_set = 0, next_due = 0; uint64_t passes = 0;
-        static const bool walk_all_levels = getenv("AC_SIMPLIFY_ALL_LEVELS") != nullptr;      // comparison only: every pass walks every level
         const uint32_t due_stride = fm[3] + 2;
-        if (!walk_all_levels) { d_due.ensure((size_t)3 * due_stride * 4); ac_memset(d_due.p, 0, (size_t)3 * due_stride * 4, &stream); }
+        d_due.ensure((size_t)3 * due_stride * 4); ac_memset(d_due.p, 0, (size_t)3 * due_stride * 4, &stream);
         for (bool first = true;; first = false) {
             const ApplyLevelBody apply{d_cands.as<ExpandCandidate>(), d_deps.as<ExpandDeps>(), d_level.as<uint32_t>(), 0, d_spec.as<uint32_t>(),
                                        d_rec.as<UnitigRec>(), d_arena2.as<char>(), c64, c64, d_dirty.as<uint64_t>(), d_exhausted.as<uint8_t>(), first, c64 + AC_PASS_REMOVED};
             const uint64_t room = always_grow ? 0 : d_arena2.cap;
-            ac_launch_coop("simplify", &stream, SimplifyCoopBody{apply, bound_body, n_cands, d_flagmax.as<uint32_t>() + 3, c64, res, room, next_set, first, !device_simplify,
-                                                                 walk_all_levels ? nullptr : d_due.as<uint32_t>(), due_stride, next_due}, n_cands, 64);
+            ac_launch_coop("simplify", &stream, SimplifyCoopBody{apply, bound_body, n_cands, d_flagmax.as<uint32_t>() + 3, c64, res, room, next_set, first,
+                                                                 d_due.as<uint32_t>(), due_stride, next_due}, n_cands, 64);
             ac_d2h(h64, c64, sizeof h64, &stream); ac_sync(&stream);
             const unsigned long long* r = h64 + AC_PASS_WORDS;
-            R.arena_final = h64[0]; R.first_pass_total = r[0]; R.first_pass_done = true;      // what the last expand_repeats() call returned
-            R.bases_removed = h64[AC_PASS_REMOVED]; R.any_moved = r[1] != 0;
+            R.arena_final = h64[0]; R.bases_removed = h64[AC_PASS_REMOVED]; R.any_moved = r[1] != 0;
             passes += r[2]; next_set = (uint32_t)r[5]; next_due = (uint32_t)r[7];
             if (getenv("AC_HOST_PROFILE")) fprintf(stderr, "[device] expand_repeats launch: %llu passes (%llu so far), %u levels, %llu candidates, %llu left on the work list, last pass moved %llu bases\n",
                                                    r[2], (unsigned long long)passes, fm[3], (unsigned long long)n_cands, r[4], r[0]);
-            if (!device_simplify || R.first_pass_total == 0) break;
+            if (r[0] == 0) break;                                                          // the last expand_repeats() call moved nothing
             if (passes > 1000000) throw std::runtime_error("repeat expansion did not settle");
             bound = r[3];                                                                  // the launch stopped for want of room: make it
             if (R.arena_final + bound >= 0xFFFFFFF0ull) throw std::runtime_error("unitig sequence arena would exceed 4 GB");
@@ -2927,8 +2885,7 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
         R.arena_src = &d_arena2;
     }
     mark(17);
-    const bool simplified = device_simplify && R.first_pass_done && R.first_pass_total == 0;
-    if (simplified) {      // simplify_structure ends with renumber_unitigs (:38): stable with respect to the numbering the passes ran in
+    if (fused) {      // simplify_structure ends with renumber_unitigs (:38): stable with respect to the numbering the passes ran in
         if (R.any_moved) {
             d_pos.ensure((size_t)U * 4); sort_c.ensure((size_t)U * 4); sort_d.ensure((size_t)U * 4);
             ac_launch("inverse_perm", &stream, InversePermBody{ord_in, d_pos.as<uint32_t>()}, U);
@@ -2936,7 +2893,7 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
             const NumberLess final_less{d_rec.as<UnitigRec>(), d_depth.as<uint32_t>(), R.arena_src->as<char>(), num_prefix.as<uint64_t>(), d_pos.as<uint32_t>()};
             R.final_order = sort_indices(&stream, final_less, U, sort_c.as<uint32_t>(), sort_d.as<uint32_t>(), sort_ra.as<SortRec>(), sort_rb.as<SortRec>());
         } else R.final_order = ord_in;     // nothing moved: the stable sort would change nothing
-        if (device_gfa && U < 100000000u) {          // save_gfa (unitig_graph.rs:317-360): H, S, L and P lines rendered here
+        if (U < 100000000u) {          // save_gfa (unitig_graph.rs:317-360): H, S, L and P lines rendered here
             uint32_t* fin = R.final_order;
             d_pos2.ensure((size_t)U * 4);
             ac_launch("inverse_perm", &stream, InversePermBody{fin, d_pos2.as<uint32_t>()}, U);
@@ -3007,8 +2964,8 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
     else { mark(16); mark(12); arena_pending = true; }
 }
 
-// The graph arrays (unitig records, sequences, links, paths, work list state) into pinned host memory: at once in a plain build,
-// on request after a fused one.
+// The graph arrays (unitig records, sequences, links, paths, and the numbering and expand_repeats work list of the graph as built, or
+// the final numbering after a fused build) into pinned host memory: at once in a plain build, on request after a fused one.
 void DevicePipeline::Impl::pull_graph(PipelineResult& out, bool keep_positions) {
     const uint32_t U = R.U; const uint64_t n_links = R.n_links, n_cands = R.n_cands; const uint32_t n_strands = R.n_strands;
     const uint64_t arena_cap = R.arena_final + R.arena_final / 4 + (1u << 20);     // head room for relocations during repeat expansion
@@ -3018,22 +2975,19 @@ void DevicePipeline::Impl::pull_graph(PipelineResult& out, bool keep_positions) 
     uint64_t d2h = 0;
     auto pull = [&](PinBuf& dst, DevBuf& src, size_t bytes) { if (bytes) ac_d2h(dst.p, src.p, bytes, &stream); d2h += bytes; };
     pull(h_rec, d_rec, (size_t)U * sizeof(UnitigRec)); pull(h_depth, d_depth, (size_t)U * 4);
-    h_order.ensure((size_t)U * 4 + 4);
-    if (U) { ac_d2h(h_order.p, R.order_built, (size_t)U * 4, &stream); d2h += (size_t)U * 4; }
+    const bool plain = !out.fused;
+    if (plain) { h_order.ensure((size_t)U * 4 + 4); if (U) { ac_d2h(h_order.p, R.order_built, (size_t)U * 4, &stream); d2h += (size_t)U * 4; } }
     pull(h_next_off, d_next_off, ((size_t)n_strands + 1) * 4); pull(h_prev_off, d_prev_off, ((size_t)n_strands + 1) * 4);
     pull(h_next, d_next, n_links * 4); pull(h_prev, d_prev, n_links * 4); pull(h_path, d_path, n_runs * 4); pull(h_path_off, d_path_off, ((size_t)n_seqs + 1) * 8);
     if (keep_positions) {
         h_run_start.ensure(n_runs * 8 + 8); h_run_len.ensure(n_runs * 4 + 4);
         pull(h_run_start, run_start, n_runs * 8); pull(h_run_len, run_len, n_runs * 4);
     }
-    h_cands.ensure((n_cands + 1) * sizeof(ExpandCandidate)); h_deps.ensure((size_t)U * sizeof(ExpandDeps) + 4); h_spec.ensure((n_cands + 1) * 4); h_fixed.ensure((size_t)U * 2 + 4);
-    pull(h_cands, d_cands, n_cands * sizeof(ExpandCandidate)); pull(h_deps, d_deps, (size_t)U * sizeof(ExpandDeps)); pull(h_spec, d_spec, n_cands * 4);
-    if (U) { ac_d2h(h_fixed.p, R.fix_start, (size_t)U * 2, &stream); d2h += (size_t)U * 2; }
-    if (R.final_order) { h_order2.ensure((size_t)U * 4 + 4); ac_d2h(h_order2.p, R.final_order, (size_t)U * 4, &stream); d2h += (size_t)U * 4; }
-    if (R.first_pass_done) {
-        h_dirty.ensure(((n_cands + 63) / 64) * 8 + 8); h_exhausted.ensure(n_cands + 8);
-        if (n_cands) { pull(h_dirty, d_dirty, ((n_cands + 63) / 64) * 8); pull(h_exhausted, d_exhausted, n_cands); }
-    }
+    if (plain) {
+        h_cands.ensure((n_cands + 1) * sizeof(ExpandCandidate)); h_deps.ensure((size_t)U * sizeof(ExpandDeps) + 4); h_spec.ensure((n_cands + 1) * 4); h_fixed.ensure((size_t)U * 2 + 4);
+        pull(h_cands, d_cands, n_cands * sizeof(ExpandCandidate)); pull(h_deps, d_deps, (size_t)U * sizeof(ExpandDeps)); pull(h_spec, d_spec, n_cands * 4);
+        if (U) { ac_d2h(h_fixed.p, R.fix_start, (size_t)U * 2, &stream); d2h += (size_t)U * 2; }
+    } else { h_order2.ensure((size_t)U * 4 + 4); if (U) { ac_d2h(h_order2.p, R.final_order, (size_t)U * 4, &stream); d2h += (size_t)U * 4; } }
     // The sequences (most of the bytes) go last: the caller gets the graph structure as soon as everything else has
     // landed and lists the repeat-expansion candidates while the arena is still on its way (complete() waits for it).
     mark(16);
@@ -3042,12 +2996,12 @@ void DevicePipeline::Impl::pull_graph(PipelineResult& out, bool keep_positions) 
     mark(12);
     wait_mark(16);
     out.graph_fetched = true;
-    out.rec = h_rec.as<UnitigRec>(); out.depth = h_depth.as<uint32_t>(); out.order = h_order.as<uint32_t>();
-    out.n_cands = n_cands; out.cands = h_cands.as<ExpandCandidate>(); out.deps = h_deps.as<ExpandDeps>(); out.spec_len = h_spec.as<uint32_t>();
-    out.fixed_start = h_fixed.as<uint8_t>(); out.fixed_end = h_fixed.as<uint8_t>() + U;
+    out.rec = h_rec.as<UnitigRec>(); out.depth = h_depth.as<uint32_t>();
+    out.order = plain ? h_order.as<uint32_t>() : nullptr; out.final_order = plain ? nullptr : h_order2.as<uint32_t>();
+    out.n_cands = plain ? n_cands : 0; out.cands = plain ? h_cands.as<ExpandCandidate>() : nullptr; out.deps = plain ? h_deps.as<ExpandDeps>() : nullptr;
+    out.spec_len = plain ? h_spec.as<uint32_t>() : nullptr;
+    out.fixed_start = plain ? h_fixed.as<uint8_t>() : nullptr; out.fixed_end = plain ? h_fixed.as<uint8_t>() + U : nullptr;
     out.arena = h_arena.as<char>(); out.arena_used = R.arena_final; out.arena_cap = arena_cap;
-    out.first_pass_done = R.first_pass_done; out.first_pass_total = R.first_pass_total; out.final_order = R.final_order ? h_order2.as<uint32_t>() : nullptr;
-    out.dirty = R.first_pass_done ? h_dirty.as<uint64_t>() : nullptr; out.exhausted = R.first_pass_done ? h_exhausted.as<uint8_t>() : nullptr;
     out.next_off = h_next_off.as<uint32_t>(); out.next = h_next.as<UStrand>(); out.prev_off = h_prev_off.as<uint32_t>(); out.prev = h_prev.as<UStrand>();
     out.path_off = h_path_off.as<uint64_t>(); out.path = h_path.as<UStrand>();
     out.run_start = keep_positions ? h_run_start.as<uint64_t>() : nullptr; out.run_len = keep_positions ? h_run_len.as<uint32_t>() : nullptr;

@@ -46,8 +46,6 @@ struct UnitigRec {
 struct ExpandCandidate { uint32_t idx; uint16_t side, gn; uint32_t src[6]; };   // 32 B: destination, side (0 inputs / 1 outputs), its sources (UStrand)
 struct ExpandDeps { int32_t c[6]; };          // candidates that read unitig u: its own two, and those it exclusively feeds / is fed by
 
-struct NumberKey { uint64_t prefix; uint32_t len; uint32_t pad; };   // first 8 bases (big-endian) and length of one unitig
-
 // A unitig strand: (seed index << 1) | reverse.  The seed index is the position the unitig would have had in the
 // reference's `unitigs` vector straight after build_unitigs_from_kmer_graph (unitig_graph.rs:179-225).
 typedef uint32_t UStrand;
@@ -72,11 +70,8 @@ struct PipelineResult {
     uint32_t* spec_len = nullptr;              // [n_cands] length of the common piece of each candidate's sources on the untouched graph
     ExpandDeps* deps = nullptr;                // [U]
     uint8_t* fixed_start = nullptr; uint8_t* fixed_end = nullptr;   // [U] get_fixed_unitig_starts_and_ends (graph_simplification.rs:190-230)
-    // set when the device has already applied the first pass of expand_repeats (AC_DEVICE_FIRST_PASS): rec / arena hold its result
-    bool first_pass_done = false; uint64_t first_pass_total = 0;    // bases it moved = the first expand_repeats() return value
-    uint64_t* dirty = nullptr; uint8_t* exhausted = nullptr;        // the work list and the per-candidate state it left for pass 2
-    uint32_t* final_order = nullptr;                                // [U] AC_DEVICE_SIMPLIFY: the numbering simplify_structure ends with (:38)
-    // The finished file as the device rendered it (fused builds, or AC_DEVICE_SIMPLIFY + AC_DEVICE_GFA): H, S, L and P lines, pinned
+    uint32_t* final_order = nullptr;                                // [U] fused builds: the numbering simplify_structure ends with (:38)
+    // The finished file as the device rendered it (fused builds): H, S, L and P lines, pinned
     char* gfa_text = nullptr; uint64_t gfa_bytes = 0;
     // Fused build (DevicePipeline::build(..., fused = true)): simplify_structure and save_gfa ran on the device and only the text and
     // these counts came back; the graph arrays below stay in HBM until fetch_graph() is asked for them.
@@ -156,10 +151,6 @@ public:
     void finish(PipelineResult& out, bool keep_positions, bool fused = false, bool split_paths = false);
     void export_path_tokens(void* dst, uint64_t stride, const uint64_t* counts, uint32_t n_ranks);
     void render_path_lines(const void* tokens_dev, uint64_t n_tokens, const char** text, uint64_t* bytes);
-    // needles: n_needles keys of h bases each (2 words per key, kmer_key.h layout for k = h), pairwise distinct.
-    // renumber_unitigs for a graph the host has edited: sorts n keys by (length descending, first 8 bases ascending, index
-    // ascending) and writes the sorted indices; the host settles the rare ties beyond the prefix.  `keys` may be any host memory.
-    void sort_number_keys(const NumberKey* keys, uint32_t n, uint32_t* sorted);
     // cluster.rs:132-151 pairwise_contig_distances, the integer part: shared[a * n_seqs + b] = total length of the unitigs that the
     // paths of sequences a and b have in common (the diagonal is the length of a's own unitig set).  Host arrays in, host array out.
     void pair_shared_lengths(const UStrand* path, const uint64_t* path_off, uint32_t n_seqs, const uint32_t* unitig_len, uint32_t n_unitigs, uint64_t* shared);
@@ -178,6 +169,7 @@ public:
                         const OverlapJob* jobs, uint32_t n_jobs, std::vector<std::vector<AlignPiece>>& out);
     // the largest k whose three live diagonals (24 * (k + 1) bytes) fit one CTA's shared memory; larger windows keep them in HBM
     uint32_t overlap_shared_k_max();
+    // needles: n_needles keys of h bases each (2 words per key, kmer_key.h layout for k = h), pairwise distinct.
     void find_literals(const uint8_t* ascii, uint64_t total, const SeqInfo* seqs, uint32_t n_seqs, uint32_t h,
                        const uint64_t* needle_words, uint32_t n_needles, std::vector<LiteralHit>& hits);
     unsigned long long kernel_launches() const;

@@ -1,6 +1,5 @@
 """Shared body of the parity tests: run one case through a C-ABI library (the CUDA build on the GPU box, or
 the host-emulation build of the same device bodies on CPU) and compare with the oracle."""
-import os
 import tempfile
 
 import cases
@@ -43,6 +42,8 @@ def check_fused(kg, expected, st, seqs, k):
     assert g.gfa_bytes().decode() == expected
     api.merge_linear_paths(g, seqs)
     assert g.gfa_bytes().decode() == o.gfa_merge_linear_paths(expected)
+    g.renumber_unitigs()
+    assert g.gfa_bytes().decode() == o.gfa_merge_linear_paths(expected, renumber=True)
     return g
 
 
@@ -63,9 +64,8 @@ def check_case(lib, files, k, tmpdir=None):
         assert [(s.id, s.filename, s.contig_header, s.length, s.forward_seq) for s in got["seqs"]] == oseqs, "load/end-repair differs"
         assert got["count"] == count
         assert got["before"].n_kmers == st.n_kmers
-        if not (os.environ.get("AC_DEVICE_FIRST_PASS") or os.environ.get("AC_DEVICE_SIMPLIFY")):      # with those switches ac_build already returns the graph after the first expansion pass
-            assert (got["before"].n_unitigs, got["before"].n_links, got["before"].total_length) == \
-                   (st.unitigs_before, st.links_before, st.length_before)
+        assert (got["before"].n_unitigs, got["before"].n_links, got["before"].total_length) == \
+               (st.unitigs_before, st.links_before, st.length_before)
         assert (got["after"].n_unitigs, got["after"].n_links, got["after"].total_length) == \
                (st.unitigs_after, st.links_after, st.length_after)
         assert got["gfa"] == expected, "GFA differs from the oracle"

@@ -18,24 +18,32 @@ from autocycler_b200 import api, synth
 from parity_common import run_library
 d = sys.argv[1]
 synth.write_assemblies(synth.make_assemblies("cfg2"), d)
-got = run_library(api.load_library(%(lib)r), d, 51)
-print("SHA", hashlib.sha256(got["gfa"].encode()).hexdigest(), got["before"].n_kmers, got["after"].n_unitigs, got["after"].n_links, got["graph"].timings().table_capacity)
+lib = api.load_library(%(lib)r)
+if sys.argv[2] == "fused":           # ac_compress: simplify_structure and the GFA text by the device bodies
+    kg, seqs, count = api.load_sequences(d, 51, lib=lib)
+    kg.upload()
+    g = api.UnitigGraph.compress(kg)
+    gfa, before, after = bytes(g.gfa_view()), g.counts(), g.counts()
+else:
+    got = run_library(lib, d, 51)
+    g, gfa, before, after = got["graph"], got["gfa"].encode(), got["before"], got["after"]
+print("SHA", hashlib.sha256(gfa).hexdigest(), before.n_kmers, after.n_unitigs, after.n_links, g.timings().table_capacity)
 """
 
 
-@pytest.mark.parametrize("env", [{}, {"AC_DEVICE_SIMPLIFY": "1", "AC_DEVICE_GFA": "1"}, {"AC_EXPAND_SERIAL": "1", "AC_HOST_CANDIDATES": "1"}], ids=["default", "device_simplify_and_gfa", "serial_host"])
-def test_config2_golden_under_emulation(tmp_path, env):
+@pytest.mark.parametrize("mode,env", [("plain", {}), ("fused", {}), ("plain", {"AC_EXPAND_SERIAL": "1", "AC_HOST_CANDIDATES": "1"})],
+                         ids=["default", "device_simplify_and_gfa", "serial_host"])
+def test_config2_golden_under_emulation(tmp_path, mode, env):
     subprocess.run(["make", "-s", "-C", os.path.join(ROOT, "autocycler_b200", "csrc"), "emu"], check=True)
     g = json.load(open(os.path.join(ROOT, "tests", "golden", "config_goldens.json")))["cfg2_k51"]
     code = CODE % {"tests": os.path.join(ROOT, "tests"), "root": ROOT, "lib": os.path.join(ROOT, "tests", "emu", "libautocycler_emu.so")}
-    r = subprocess.run([sys.executable, "-c", code, str(tmp_path / "cfg2")], env={**os.environ, **env}, capture_output=True, text=True, timeout=900)
+    r = subprocess.run([sys.executable, "-c", code, str(tmp_path / "cfg2"), mode], env={**os.environ, **env}, capture_output=True, text=True, timeout=900)
     assert r.returncode == 0, r.stderr[-2000:]
     line = [l for l in r.stdout.splitlines() if l.startswith("SHA")][0].split()
     assert line[1] == g["sha256"]
     assert (int(line[3]), int(line[4])) == (g["unitigs_after"], g["links_after"])
-    if "AC_DEVICE_SIMPLIFY" not in env:
-        assert int(line[2]) == g["n_kmers"]
-    if not env:          # the size the sizing pass's exact restatement predicts (tests/table_sizing.py)
+    assert int(line[2]) == g["n_kmers"]
+    if mode == "plain" and not env:          # the size the sizing pass's exact restatement predicts (tests/table_sizing.py)
         import oracle_lib as o
         import table_sizing
         count, oseqs = o.load_sequences(str(tmp_path / "cfg2"), 51)

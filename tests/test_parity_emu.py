@@ -123,10 +123,7 @@ def test_cli_yaml_and_gfa_files(emu, tmp_path):
 
 @pytest.mark.parametrize("env", [{"AC_EXPAND_MIN_DUE": "1"}, {"AC_EXPAND_MIN_DUE": "1", "AC_EXPAND_TIGHT_ARENA": "1"}, {"AC_EXPAND_SERIAL": "1"},
                                  {"AC_HOST_POOL": "0", "AC_HOST_THREADS": "3"}, {"AC_CHECK_CANDIDATES": "1"}, {"AC_HOST_CANDIDATES": "1"},
-                                 {"AC_DEVICE_RENUMBER": "1", "AC_DEVICE_SORT_MIN": "1", "AC_HOST_THREADS": "3"},
-                                 {"AC_DEVICE_FIRST_PASS": "1"}, {"AC_DEVICE_FIRST_PASS": "1", "AC_EXPAND_MIN_DUE": "1"},
-                                 {"AC_DEVICE_SIMPLIFY": "1"}, {"AC_DEVICE_SIMPLIFY": "1", "AC_DEVICE_TIGHT_ARENA": "1"},
-                                 {"AC_DEVICE_SIMPLIFY": "1", "AC_DEVICE_GFA": "1"}])
+                                 {"AC_DEVICE_TIGHT_ARENA": "1"}])
 def test_repeat_expansion_schedules_agree(emu, env):
     """simplify_structure has three schedules (serial sweep; conflict levels on several threads; the same with every
     relocation handed back to the barrier) and two sources of its work list (device kernels; the host listing, which

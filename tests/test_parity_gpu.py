@@ -166,18 +166,20 @@ def test_loaded_graphs_and_reference_kats(lib, golden_dir, tmp_path):
         assert open(os.path.join(out, fn), "rb").read() == open(os.path.join(d, fn), "rb").read()
 
 
-@pytest.mark.parametrize("switch", ["AC_DEVICE_FIRST_PASS", "AC_DEVICE_SIMPLIFY", "AC_DEVICE_SIMPLIFY,AC_DEVICE_GFA", "AC_DEVICE_SIMPLIFY,AC_DEVICE_TIGHT_ARENA"])
-def test_device_expansion_switches_match_the_oracle(lib, tmp_path, switch):
-    """expand_repeats applied by device kernels (pipeline.cu ApplyLevelBody), alone and with the device GFA writer: same bytes as the oracle
-    on a medium graph.  The switches are read once per process, so the build runs in a child."""
+@pytest.mark.parametrize("env", [{}, {"AC_DEVICE_TIGHT_ARENA": "1"}], ids=["fused", "fused_tight_arena"])
+def test_device_expansion_switches_match_the_oracle(lib, tmp_path, env):
+    """The fused build (ac_compress: expand_repeats applied by device kernels, pipeline.cu ApplyLevelBody, then the device GFA writer), as it
+    runs and with the arena regrown before every pass: same bytes as the oracle on a medium graph.  The switch is read once per process, so
+    the build runs in a child."""
     import subprocess
     import sys
     d = str(tmp_path / "m")
     synth.write_assemblies(synth.make_assemblies("m", n_assemblies=6, replicon_lengths=[400_000, 22_000, 8_000, 3_000], seed=99), d)
     expected, yaml, st = o.compress_dir(d, 51)
     code = ("import sys; sys.path.insert(0, %r); sys.path.insert(0, %r)\n"
-            "from autocycler_b200 import api\nfrom parity_common import run_library\n"
-            "got = run_library(api.load_library(), %r, 51)\nopen(%r, 'w').write(got['gfa'])\n") % (os.path.join(ROOT, "tests"), ROOT, d, str(tmp_path / "out.gfa"))
-    r = subprocess.run([sys.executable, "-c", code], env={**os.environ, **{name: "1" for name in switch.split(",")}}, capture_output=True, text=True, timeout=120)
+            "from autocycler_b200 import api\n"
+            "kg, seqs, count = api.load_sequences(%r, 51)\nkg.upload()\n"
+            "open(%r, 'wb').write(bytes(api.UnitigGraph.compress(kg).gfa_view()))\n") % (os.path.join(ROOT, "tests"), ROOT, d, str(tmp_path / "out.gfa"))
+    r = subprocess.run([sys.executable, "-c", code], env={**os.environ, **env}, capture_output=True, text=True, timeout=120)
     assert r.returncode == 0, r.stderr[-2000:]
     assert open(tmp_path / "out.gfa").read() == expected
