@@ -143,8 +143,8 @@ template <class Body> __global__ void __launch_bounds__(256) ac_body_kernel(cons
     }
 }
 
-// The same loop compiled for a given number of resident 256-thread CTAs per SM (a register budget): latency-bound bodies
-// trade a few spills for more loads in flight.
+// The same loop compiled for a given number of resident 256-thread CTAs per SM (a register budget).  For the insert, a budget
+// without spills beats more resident CTAs with spills (DESIGN.md §4).
 template <class Body, int CTAS> __global__ void __launch_bounds__(256, CTAS) ac_body_kernel_occ(const Body body, uint64_t n) {
     const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
     const uint32_t lane = threadIdx.x & 31u;
@@ -159,7 +159,7 @@ template <class Body> inline void ac_launch_occ(const char* name, AcStream* st, 
     const int threads = 256;
     const uint64_t want = (n + threads - 1) / threads, max_blocks = ac_sm_count() * (uint64_t)ctas_per_sm * 2;   // two waves of resident CTAs, grid-stride beyond
     const unsigned blocks = (unsigned)(want < max_blocks ? want : max_blocks);
-    ac_body_kernel_occ<Body, 6><<<blocks, threads, 0, st->s>>>(body, n);      // one register budget is compiled (6 resident CTAs per SM: 40 registers for the insert body)
+    ac_body_kernel_occ<Body, 4><<<blocks, threads, 0, st->s>>>(body, n);      // one register budget is compiled (4 resident CTAs per SM: 64 registers for the insert body)
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) throw std::runtime_error(std::string("launch ") + name + ": " + cudaGetErrorString(e));
     ++g_ac_kernel_launches;

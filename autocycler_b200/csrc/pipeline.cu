@@ -2009,7 +2009,7 @@ struct DevicePipeline::Impl {
     DevBuf ascii, packed, seqs, slots, pos_slot, flags8, bmask, bcount, boff, counters, uid_rep, slot_unitig;
     DevBuf run_start, run_len, run_uk, run_dir, is_rep, rep_idx, run_unitig, unitigs, nchunks, chunk_off, partial, link_count, links;
     DevBuf scan_tmp[4];
-    int insert_occupancy = 6;   // resident CTAs per SM the insert kernel is compiled for (40 registers: a latency-bound body trades a few spills for more loads in flight)
+    int insert_occupancy = 4;   // resident CTAs per SM the insert kernel is compiled for: 64 registers, no spills up to W = 5 (at 6 CTAs, 40 registers spilled at every W and the kernel was 1.3x slower on the H100, DESIGN.md §4)
     DevBuf d_fixed, cand_flag, cand_index, d_cands, d_cand_at, d_deps, d_spec;
     DevBuf sort_a, sort_b, sort_ra, sort_rb, num_prefix, rank, d_len, d_depth, need, d_seq_off, d_arena, d_min_fpos, d_min_rpos;
     DevBuf strand_cnt, d_next_off, d_next, prev_cnt, d_prev_off, d_prev, d_path, d_path_off;
