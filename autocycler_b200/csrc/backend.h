@@ -47,7 +47,7 @@ inline void* ac_host_alloc(size_t bytes) { return malloc(bytes ? bytes : 1); }
 inline void ac_host_free(void* p) { free(p); }
 
 template <class Body> inline void ac_launch(const char*, AcStream*, const Body& body, uint64_t n);
-template <class Body> inline void ac_launch_occ(const char* name, AcStream* st, const Body& body, uint64_t n, int) { ac_launch(name, st, body, n); }
+template <int CTAS, class Body> inline void ac_launch_occ(const char* name, AcStream* st, const Body& body, uint64_t n) { ac_launch(name, st, body, n); }
 template <class Body> inline void ac_launch(const char*, AcStream*, const Body& body, uint64_t n) {
     for (uint64_t i = 0; i < n; ++i) body(i);
 }
@@ -154,12 +154,12 @@ template <class Body, int CTAS> __global__ void __launch_bounds__(256, CTAS) ac_
         __syncwarp();
     }
 }
-template <class Body> inline void ac_launch_occ(const char* name, AcStream* st, const Body& body, uint64_t n, int ctas_per_sm) {
+template <int CTAS, class Body> inline void ac_launch_occ(const char* name, AcStream* st, const Body& body, uint64_t n) {
     if (n == 0) return;
     const int threads = 256;
-    const uint64_t want = (n + threads - 1) / threads, max_blocks = ac_sm_count() * (uint64_t)ctas_per_sm * 2;   // two waves of resident CTAs, grid-stride beyond
+    const uint64_t want = (n + threads - 1) / threads, max_blocks = ac_sm_count() * (uint64_t)CTAS * 2;   // two waves of resident CTAs, grid-stride beyond
     const unsigned blocks = (unsigned)(want < max_blocks ? want : max_blocks);
-    ac_body_kernel_occ<Body, 4><<<blocks, threads, 0, st->s>>>(body, n);      // one register budget is compiled (4 resident CTAs per SM: 64 registers for the insert body)
+    ac_body_kernel_occ<Body, CTAS><<<blocks, threads, 0, st->s>>>(body, n);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) throw std::runtime_error(std::string("launch ") + name + ": " + cudaGetErrorString(e));
     ++g_ac_kernel_launches;

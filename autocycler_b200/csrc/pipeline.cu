@@ -26,6 +26,11 @@ static unsigned long long g_ac_kernel_launches = 0;
 #define AC_MINCHUNK 128        // windows per thread in the seed-k-mer kernel
 #define AC_MAX_RANKS 16         // ranks of one multi-GPU build (one box)
 #define AC_BOUND_STRIPES 64     // power of two: accumulators that every candidate adds to are striped
+// Resident 256-thread CTAs per SM the insert kernel is compiled for, i.e. its register budget (65536 / (256 x CTAS) registers per
+// thread).  profiles/insert_budget_sweep.py builds the library at other values and times the insert; DESIGN.md §4 has the numbers.
+#ifndef AC_INSERT_CTAS
+#define AC_INSERT_CTAS 2
+#endif
 
 // ------------------------------------------------------------------------------------------------
 // small device helpers
@@ -138,48 +143,50 @@ struct PackBody {
 };
 
 // kmer_graph.rs:92-134 add_sequence, both strands at once: one canonical entry per k-mer, count = depth.
-// One window per thread; a warp takes the 32 windows that start in one 32-base word of the packed store (units are aligned to 32
-// coordinates), so the W+2 packed words its keys, their left and their right neighbour bases are cut from sit at the same addresses
-// for all of its lanes (one transaction each) and the slot-id stores coalesce.  Almost every such block lies in the interior of one
-// sequence: no dots, no first or last window, every window has both neighbours — that case is decided once per block and skips the
-// per-window bookkeeping.  The table is probed a 32-byte group of four slots at a time (one sector, one 256-bit load; the home slot
-// of a k-mer is the first of a group and the probe order is plain linear probing from there), in two phases: a cheap scan to the
-// first slot that is empty (claimed at once, count and flags in the same CAS) or carries the k-mer's 6-bit tag, then — lanes
-// together again — the comparison with the occurrence that slot points at.
+// A warp takes the 64 windows that start in two consecutive 32-base words of the packed store (units are aligned to 64 coordinates),
+// and lane l owns two of them, g0 + l and g0 + 32 + l: the W+3 packed words both keys, their left and their right neighbour bases are
+// cut from sit at the same addresses for all of its lanes (one transaction each), and the slot-id stores coalesce (one 128-byte store
+// per half).  Almost every 32-window half lies in the interior of one sequence: no dots, no first or last window, every window has
+// both neighbours — that case is decided once per half and skips the per-window bookkeeping.  The table is probed a 32-byte group of
+// four slots at a time (one sector, one 256-bit load; the home slot of a k-mer is the first of a group and the probe order is plain
+// linear probing from there), in two phases: a cheap scan to the first slot that is empty (claimed at once, count and flags in the
+// same CAS) or carries the k-mer's 6-bit tag, then — lanes together again — the comparison with the occurrence that slot points at.
+// Each probe is a chain of dependent loads; a lane runs the chains of its two windows side by side, so that twice as many loads are in
+// flight per warp (DESIGN.md §4).
 template <int W> struct InsertBody {
     TableView t; KParams p;
     const uint8_t* interior;            // [total / 32] PackBody's flag per block of 32 coordinates
-    uint32_t g_first;                   // coordinate of unit 0, a multiple of 32 (inputs are limited to 2^32 - 2 padded bytes: coordinates fit 32 bits)
+    uint32_t g_first;                   // coordinate of unit 0, a multiple of 64 (inputs are limited to 2^32 - 2 padded bytes: coordinates fit 32 bits)
     uint32_t g_begin, g_end;            // coordinates of the sequences this rank owns
     bool track_min;                     // multi-GPU: the slot must end up pointing at the SMALLEST occurrence
     uint32_t* pos_slot;                 // [total] slot of the window starting at each global coordinate (null in the sizing pass)
     unsigned long long* counters;       // [0] slots claimed (sizing pass only), [1] dotted k-mers claimed, [2] probe-limit flag, [3] count alarm
     bool sizing;                        // the sizing pass: the caller has picked the windows (SampleBody), only distinct k-mers are counted
     uint32_t* claimed_bits;             // [total / 32] bit j of word w: the window at coordinate 32w + j claimed its slot, i.e. it is the first occurrence of a distinct k-mer (the list of distinct k-mers is made from these); null in the sizing pass
-    // a window of an interior block: keys and neighbour bases from the block's W+2 words
-    AC_D void interior_unit(uint32_t g, Key<W>& fwd, Key<W>& rc, uint64_t& h, uint32_t& flags) const {
-        const uint32_t l = g & 31u, i0 = g >> 5;
-        uint64_t x[W + 1];
+    struct Unit { Key<W> fwd, rc; uint64_t h; uint32_t flags, g; bool valid; };
+    // window l of an interior block: x = the packed word before the block, then the block's own W+1 words
+    AC_D void interior_unit(uint32_t l, const uint64_t (&x)[W + 2], Unit& u) const {
+        uint64_t xs[W + 1];
 #pragma unroll
-        for (int j = 0; j <= W; ++j) x[j] = t.packed[i0 + j];
-        const uint64_t xp = t.packed[i0 - 1];
+        for (int j = 0; j <= W; ++j) xs[j] = x[j + 1];
         const uint32_t sh = 2 * l;
         uint64_t y[W];
-        ac_stream_window<W>(x, sh, y);       // y = the 64W bits of the base stream that start at bit `sh` of x[0]
+        ac_stream_window<W>(xs, sh, y);      // y = the 64W bits of the base stream that start at bit `sh` of the block's first word
         const uint32_t al = 64 - p.top_bits;
 #pragma unroll
-        for (int j = W - 1; j >= 0; --j) { uint64_t v = y[j] >> al; if (al && j > 0) v |= y[j - 1] << (64 - al); fwd.w[j] = v; }
-        fwd.d = 0;
-        rc = key_rc(fwd, p);
-        const bool canon_fwd = key_is_canonical(fwd, p);
+        for (int j = W - 1; j >= 0; --j) { uint64_t v = y[j] >> al; if (al && j > 0) v |= y[j - 1] << (64 - al); u.fwd.w[j] = v; }
+        u.fwd.d = 0;
+        u.rc = key_rc(u.fwd, p);
+        const bool canon_fwd = key_is_canonical(u.fwd, p);
         // the base after the window is base k of the stream that starts at the window: 32(W-1) < k < 32W, so it lies in y[W-1]
         const uint32_t nb = (uint32_t)(y[W - 1] >> (62 - 2 * (p.k & 31u))) & 3u;
-        const uint32_t pb = l ? (uint32_t)(x[0] >> (64 - sh)) & 3u : (uint32_t)xp & 3u;
+        const uint32_t pb = l ? (uint32_t)(xs[0] >> (64 - sh)) & 3u : (uint32_t)x[0] & 3u;
         const uint32_t out_b = canon_fwd ? nb : 3u - pb, in_b = canon_fwd ? pb : 3u - nb;
-        flags = (1u << (AC_AUX_OBS_OUT_SHIFT + out_b)) | (1u << (AC_AUX_OBS_IN_SHIFT + in_b));
-        h = key_hash(canon_fwd ? fwd : rc);
+        u.flags = (1u << (AC_AUX_OBS_OUT_SHIFT + out_b)) | (1u << (AC_AUX_OBS_IN_SHIFT + in_b));
+        u.h = key_hash(key_select(canon_fwd, u.fwd, u.rc));     // by value: a choice between the two references would keep the units in local memory
+        u.valid = true;
     }
-    // a block at the end of a sequence, between two sequences or at the edge of the shard; false: no window starts at g
+    // a window of a block at the end of a sequence, between two sequences or at the edge of the shard; false: no window starts at g
     AC_D bool edge_unit(uint32_t g, Key<W>& fwd, Key<W>& rc, uint64_t& h, uint32_t& flags) const {
         const SeqInfo s = t.seqs[find_seq(t.seqs, t.n_seqs, g)];
         const uint64_t fs = g - s.start;
@@ -203,104 +210,149 @@ template <int W> struct InsertBody {
                 flags |= canon_fwd ? (1u << (AC_AUX_OBS_IN_SHIFT + b)) : (1u << (AC_AUX_OBS_OUT_SHIFT + 3 - b));
             }
         }
-        h = key_hash(canon_fwd ? fwd : rc);
+        h = key_hash(key_select(canon_fwd, fwd, rc));
         return true;
     }
-    // Enters the k-mer (or finds it) and counts the occurrence.  All lanes of the warp call this together.
-    AC_D void upsert(bool valid, const Key<W>& fwd, const Key<W>& rc, uint64_t h, uint32_t flags, uint32_t g, const Slot* home_group = nullptr) const {
-        const bool dotted = valid && fwd.d != 0;
-        const uint32_t tag = make_tag(dotted, h, t.gb);
-        const Slot mine = make_slot(g, tag, t.count_big ? 0u : 1u, flags, t.gb);
+    // Enters the k-mers of the lane's N windows (or finds them) and counts the occurrences.  All lanes of the warp call this together.
+    // The windows are probed side by side: every round loads the next group of each window still scanning before it looks at any of
+    // them, and fetches the stored occurrences of all windows that met their tag before it compares any.  `home_group`, when given,
+    // is window 0's home group, already in registers.
+    template <int N> AC_D void upsert(const Unit (&u)[N], const Slot* home_group = nullptr) const {
         const uint32_t tag_mask = (1u << AC_SLOT_TAG_BITS(t.gb)) - 1u;
         // An empty slot is all ones and no window starts at coordinate 2^gb - 1, so "empty" is a test of the occurrence pointer alone: the
         // high word at or above this value.  The tag sits at bits 30.. of the slot; slot_tag_word() brings it down with one funnel shift.
         const uint32_t empty_hi = 0xFFFFFFFFu << (32u - t.gb);
-        uint64_t slot = table_home(t, h);
-        bool done = !valid, failed = false;
+        bool dotted[N], done[N], failed[N];
+        uint32_t tag[N], probes[N], fresh[N];      // fresh: lanes of this warp whose window claimed a slot
+        uint64_t slot[N];
+#pragma unroll
+        for (int w = 0; w < N; ++w) {
+            dotted[w] = u[w].valid && u[w].fwd.d != 0;
+            tag[w] = make_tag(dotted[w], u[w].h, t.gb);
+            slot[w] = table_home(t, u[w].h);
+            done[w] = !u[w].valid; failed[w] = false; probes[w] = 0; fresh[w] = 0;
+        }
         bool fetched = home_group != nullptr;      // the home group is in registers already: good for the first look at it only
-        uint32_t fresh = 0;                 // lanes of this warp whose window claimed a slot
-        for (uint32_t probes = 0;;) {
-            bool claimed = false; Slot q = 0;
-            if (!done) {
-                for (;; fetched = false) {
-                    Slot grp[4];
-                    const uint64_t base = slot & ~3ull;
-                    if (fetched) { fetched = false; grp[0] = home_group[0]; grp[1] = home_group[1]; grp[2] = home_group[2]; grp[3] = home_group[3]; }      // loaded while the previous unit was probed; may lag the table, as any load may (see slot_add_occurrence)
-                    else ac_ld_group(t.slots + base, grp);
+        for (;;) {
+            bool claimed[N], scanning[N]; Slot q[N];
+#pragma unroll
+            for (int w = 0; w < N; ++w) { claimed[w] = false; q[w] = 0; scanning[w] = !done[w]; }
+            for (;;) {
+                Slot grp[N][4];
+#pragma unroll
+                for (int w = 0; w < N; ++w) {
+                    if (!scanning[w]) continue;
+                    if (w == 0 && fetched) { grp[0][0] = home_group[0]; grp[0][1] = home_group[1]; grp[0][2] = home_group[2]; grp[0][3] = home_group[3]; }      // may lag the table, as any load may (see slot_add_occurrence)
+                    else ac_ld_group(t.slots + (slot[w] & ~3ull), grp[w]);
+                }
+                fetched = false;
+                bool more = false;
+#pragma unroll
+                for (int w = 0; w < N; ++w) {
+                    if (!scanning[w]) continue;
                     // the first slot of the group, from `slot` on, that is empty or carries the tag
+                    const uint64_t base = slot[w] & ~3ull;
                     uint32_t cand = 0;
 #pragma unroll
                     for (uint32_t j = 0; j < 4; ++j) {
-                        const bool is_empty = (uint32_t)(grp[j] >> 32) >= empty_hi;
-                        const bool has_tag = ((slot_tag_word(grp[j]) ^ tag) & tag_mask) == 0;
+                        const bool is_empty = (uint32_t)(grp[w][j] >> 32) >= empty_hi;
+                        const bool has_tag = ((slot_tag_word(grp[w][j]) ^ tag[w]) & tag_mask) == 0;
                         cand |= (is_empty || has_tag) ? 1u << j : 0u;
                     }
-                    cand &= 0xFu << (slot & 3u);
+                    cand &= 0xFu << (slot[w] & 3u);
                     if (cand == 0) {
-                        slot = base + 4; if (slot >= t.cap) slot = 0;
-                        if (++probes > 2048) { counters[2] = 1; failed = true; done = true; break; }    // the table was sized too small: the host retries with the safe size
+                        slot[w] = base + 4; if (slot[w] >= t.cap) slot[w] = 0;
+                        if (++probes[w] > 2048) { counters[2] = 1; failed[w] = true; done[w] = true; scanning[w] = false; }    // the table was sized too small: the host retries with the safe size
+                        else more = true;
                         continue;
                     }
                     const uint32_t j = (uint32_t)ac_ctz(cand);
-                    slot = base + j;
-                    q = j == 0 ? grp[0] : j == 1 ? grp[1] : j == 2 ? grp[2] : grp[3];
-                    if ((uint32_t)(q >> 32) >= empty_hi) {
-                        q = ac_atomic_cas(&t.slots[slot], (Slot)AC_EMPTY_SLOT, mine);
-                        if (q == AC_EMPTY_SLOT) { claimed = true; break; }
-                        if (slot_tag(q, t.gb) != tag) { ++slot; if (slot >= t.cap) slot = 0; continue; }      // somebody else's k-mer got there first: on to the next slot
+                    slot[w] = base + j;
+                    q[w] = j == 0 ? grp[w][0] : j == 1 ? grp[w][1] : j == 2 ? grp[w][2] : grp[w][3];
+                    if ((uint32_t)(q[w] >> 32) >= empty_hi) {
+                        q[w] = ac_atomic_cas(&t.slots[slot[w]], (Slot)AC_EMPTY_SLOT, make_slot(u[w].g, tag[w], t.count_big ? 0u : 1u, u[w].flags, t.gb));
+                        if (q[w] == AC_EMPTY_SLOT) { claimed[w] = true; scanning[w] = false; continue; }
+                        if (slot_tag(q[w], t.gb) != tag[w]) { ++slot[w]; if (slot[w] >= t.cap) slot[w] = 0; more = true; continue; }      // somebody else's k-mer got there first: on to the next slot
                     }
-                    break;
+                    scanning[w] = false;
                 }
+                if (!more) break;
             }
 #ifdef __CUDA_ARCH__
             __syncwarp();
-#endif
-#ifdef __CUDA_ARCH__
-            fresh |= __ballot_sync(0xFFFFFFFFu, !done && claimed);          // a claimed slot is a new distinct k-mer
+#pragma unroll
+            for (int w = 0; w < N; ++w) fresh[w] |= __ballot_sync(0xFFFFFFFFu, !done[w] && claimed[w]);          // a claimed slot is a new distinct k-mer
 #else
-            if (!done && claimed) fresh = 1;
+            for (int w = 0; w < N; ++w) if (!done[w] && claimed[w]) fresh[w] = 1;
 #endif
-            if (!done) {
-                if (claimed) {
-                    if (t.count_big) ac_atomic_add(&t.count_big[slot], 1u);
+            Key<W> rep[N] = {};
+#pragma unroll
+            for (int w = 0; w < N; ++w) if (!done[w] && !claimed[w]) rep[w] = window_key<W>(t, slot_gpos(q[w], t.gb), dotted[w], p);
+#pragma unroll
+            for (int w = 0; w < N; ++w) {
+                if (done[w]) continue;
+                if (claimed[w]) {
+                    if (t.count_big) ac_atomic_add(&t.count_big[slot[w]], 1u);
                     if (sizing) ac_atomic_add(&counters[0], 1ull);
-                    if (dotted) ac_atomic_add(&counters[1], 1ull);
-                    done = true;
-                } else {
-                    const Key<W> rep = window_key<W>(t, slot_gpos(q, t.gb), dotted, p);
-                    if (key_eq(rep, fwd) || key_eq(rep, rc)) { if (!sizing) slot_add_occurrence(t, slot, q, g, 1u, flags, track_min, counters); done = true; }
-                    else if (++slot == t.cap) slot = 0;
-                }
+                    if (dotted[w]) ac_atomic_add(&counters[1], 1ull);
+                    done[w] = true;
+                } else if (key_eq(rep[w], u[w].fwd) || key_eq(rep[w], u[w].rc)) {
+                    if (!sizing) slot_add_occurrence(t, slot[w], q[w], u[w].g, 1u, u[w].flags, track_min, counters);
+                    done[w] = true;
+                } else if (++slot[w] == t.cap) slot[w] = 0;
             }
+            bool all_done = true;
+#pragma unroll
+            for (int w = 0; w < N; ++w) all_done = all_done && done[w];
 #ifdef __CUDA_ARCH__
-            if (__all_sync(0xFFFFFFFFu, done)) break;
+            if (__all_sync(0xFFFFFFFFu, all_done)) break;
 #else
-            if (done) break;
+            if (all_done) break;
 #endif
         }
-        if (valid && !failed && pos_slot) ac_st_stream(&pos_slot[g], (uint32_t)slot);
-        if (claimed_bits) {
+#pragma unroll
+        for (int w = 0; w < N; ++w) {
+            if (u[w].valid && !failed[w] && pos_slot) ac_st_stream(&pos_slot[u[w].g], (uint32_t)slot[w]);
+            if (!claimed_bits) continue;
 #ifdef __CUDA_ARCH__
-            if ((threadIdx.x & 31u) == 0) claimed_bits[g >> 5] = fresh;      // the warp's 32 windows start in one word of coordinates
+            if ((threadIdx.x & 31u) == 0) claimed_bits[u[w].g >> 5] = fresh[w];      // each half's 32 windows start in one word of coordinates
 #else
-            if (fresh) claimed_bits[g >> 5] |= 1u << (g & 31u);
+            if (fresh[w]) claimed_bits[u[w].g >> 5] |= 1u << (u[w].g & 31u);
 #endif
         }
     }
-    struct Unit { Key<W> fwd, rc; uint64_t h; uint32_t flags, g; bool valid; };
-    AC_D void prepare(uint64_t i, Unit& u) const {
-        u.g = g_first + (uint32_t)i; u.fwd = Key<W>(); u.rc = Key<W>(); u.h = 0; u.flags = 0; u.valid = true;
-        const uint32_t g0 = u.g & ~31u;
-        if (interior[g0 >> 5] && g0 >= g_begin && g0 + 32 <= g_end) interior_unit(u.g, u.fwd, u.rc, u.h, u.flags);
-        else u.valid = edge_unit(u.g, u.fwd, u.rc, u.h, u.flags);
+    AC_D void prepare(uint64_t i, Unit (&u)[2]) const {
+        const uint32_t g0 = g_first + (uint32_t)(i >> 5) * 64u, l = (uint32_t)i & 31u, i0 = g0 >> 5;
+        bool inner[2];
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+            const uint64_t b = (uint64_t)g0 + 32u * s;
+            inner[s] = b >= g_begin && b + 32 <= g_end && interior[i0 + s];
+        }
+        uint64_t x[W + 3] = {};              // the word before the unit, then the W+2 words from the unit's first on
+        if (inner[0] || inner[1]) {
+            if (inner[0]) x[0] = t.packed[i0 - 1];
+#pragma unroll
+            for (int j = 0; j <= W + 1; ++j) x[j + 1] = t.packed[i0 + j];
+        }
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+            u[s].g = g0 + 32u * s + l; u[s].fwd = Key<W>(); u[s].rc = Key<W>(); u[s].h = 0; u[s].flags = 0;
+            if (inner[s]) {
+                uint64_t xs[W + 2];
+#pragma unroll
+                for (int j = 0; j <= W + 1; ++j) xs[j] = x[s + j];
+                interior_unit(l, xs, u[s]);
+            } else u[s].valid = edge_unit(u[s].g, u[s].fwd, u[s].rc, u[s].h, u[s].flags);
+        }
     }
     AC_D void operator()(uint64_t i) const {
-        Unit u; prepare(i, u);
+        Unit u[2]; prepare(i, u);
 #ifdef AC_EMULATE
-        Slot grp[4] = {0, 0, 0, 0};          // the CPU suite also takes the route with the home group handed in by the caller
-        if (u.valid && !sizing) { ac_ld_group(t.slots + table_home(t, u.h), grp); upsert(u.valid, u.fwd, u.rc, u.h, u.flags, u.g, grp); return; }
+        Slot grp[4] = {0, 0, 0, 0};          // the CPU suite also takes the route with window 0's home group handed in by the caller
+        if (u[0].valid && !sizing) { ac_ld_group(t.slots + table_home(t, u[0].h), grp); upsert<2>(u, grp); return; }
 #endif
-        upsert(u.valid, u.fwd, u.rc, u.h, u.flags, u.g);
+        upsert<2>(u);
     }
 };
 
@@ -352,20 +404,22 @@ template <int W> struct SampleBody {
         for (;;) {
             const bool have = hits != 0;
             if (!__any_sync(0xFFFFFFFFu, have)) break;
-            Key<W> fwd = Key<W>(), rc = Key<W>(); uint64_t hh = 0;
-            uint32_t g = g0;
+            typename InsertBody<W>::Unit u[1];
+            u[0].fwd = Key<W>(); u[0].rc = Key<W>(); u[0].h = 0; u[0].flags = 0; u[0].g = g0; u[0].valid = have;
             if (have) {
-                const uint32_t l = (uint32_t)ac_ctz(hits); hits &= hits - 1; g = g0 + l;
-                fwd = fetch_codes<W>(ins.t.packed, g, ins.p); fwd.d = 0; rc = key_rc(fwd, ins.p);
-                hh = key_hash(key_is_canonical(fwd, ins.p) ? fwd : rc);
+                const uint32_t l = (uint32_t)ac_ctz(hits); hits &= hits - 1; u[0].g = g0 + l;
+                u[0].fwd = fetch_codes<W>(ins.t.packed, u[0].g, ins.p); u[0].rc = key_rc(u[0].fwd, ins.p);
+                u[0].h = key_hash(key_select(key_is_canonical(u[0].fwd, ins.p), u[0].fwd, u[0].rc));
             }
-            ins.upsert(have, fwd, rc, hh, 0u, g);
+            ins.template upsert<1>(u);
         }
 #else
         for (; hits; hits &= hits - 1) {
-            const uint32_t g = g0 + (uint32_t)ac_ctz(hits);
-            Key<W> fwd = fetch_codes<W>(ins.t.packed, g, ins.p); fwd.d = 0; const Key<W> rc = key_rc(fwd, ins.p);
-            ins.upsert(true, fwd, rc, key_hash(key_is_canonical(fwd, ins.p) ? fwd : rc), 0u, g);
+            typename InsertBody<W>::Unit u[1];
+            u[0].g = g0 + (uint32_t)ac_ctz(hits); u[0].flags = 0; u[0].valid = true;
+            u[0].fwd = fetch_codes<W>(ins.t.packed, u[0].g, ins.p); u[0].rc = key_rc(u[0].fwd, ins.p);
+            u[0].h = key_hash(key_select(key_is_canonical(u[0].fwd, ins.p), u[0].fwd, u[0].rc));
+            ins.template upsert<1>(u);
         }
 #endif
     }
@@ -2009,7 +2063,6 @@ struct DevicePipeline::Impl {
     DevBuf ascii, packed, seqs, slots, pos_slot, flags8, bmask, bcount, boff, counters, uid_rep, slot_unitig;
     DevBuf run_start, run_len, run_uk, run_dir, is_rep, rep_idx, run_unitig, unitigs, nchunks, chunk_off, partial, link_count, links;
     DevBuf scan_tmp[4];
-    int insert_occupancy = 4;   // resident CTAs per SM the insert kernel is compiled for: 64 registers, no spills up to W = 5 (at 6 CTAs, 40 registers spilled at every W and the kernel was 1.3x slower on the H100, DESIGN.md §4)
     DevBuf d_fixed, cand_flag, cand_index, d_cands, d_cand_at, d_deps, d_spec;
     DevBuf sort_a, sort_b, sort_ra, sort_rb, num_prefix, rank, d_len, d_depth, need, d_seq_off, d_arena, d_min_fpos, d_min_rpos;
     DevBuf strand_cnt, d_next_off, d_next, prev_cnt, d_prev_off, d_prev, d_path, d_path_off;
@@ -2589,13 +2642,13 @@ template <int W> void DevicePipeline::Impl::insert_w() {
         if (big_counts) { count_big.ensure(cap * 4); ac_memset(count_big.p, 0, cap * 4, &stream); }
         ac_memset(counters.p, 0, sizeof hc, &stream);
         const TableView tv = table_view();
-        const uint64_t g_first = g_begin & ~31ull;
+        const uint64_t g_first = g_begin & ~63ull;     // the first unit may start up to 63 coordinates before the shard: edge_unit rejects those windows
         claimed.ensure((n_words + 8) * 4); ac_memset(claimed.p, 0, (n_words + 8) * 4, &stream);
         const InsertBody<W> ins{tv, p, interior8.as<uint8_t>(), (uint32_t)g_first, (uint32_t)g_begin, (uint32_t)g_end, is_multi, pos_slot.as<uint32_t>(), counters.as<unsigned long long>(), false, claimed.as<uint32_t>()};
-        // (a software-pipelined form of this loop — the next unit's keys built and its home group in flight while the current one is probed —
-        // needs 75 registers and was slower; it is not kept)
+        // (a software-pipelined form of the one-window loop — the next unit's keys built and its home group in flight while the current one is
+        // probed — needed 75 registers and was slower; it is not kept)
         mark(20);
-        ac_launch_occ("insert", &stream, ins, (g_end - g_first + 31) / 32 * 32, insert_occupancy);
+        ac_launch_occ<AC_INSERT_CTAS>("insert", &stream, ins, (g_end - g_first + 63) / 64 * 32);     // one warp per 64 windows
         mark(21);
         ac_d2h(hc, counters.p, sizeof hc, &stream); ac_sync(&stream);
         if (hc[2] && cap != safe_cap) { cap = safe_cap; continue; }         // the estimate was off (it is an estimate): start again with the safe size
