@@ -11,6 +11,9 @@ Names and argument meaning follow the reference (rrwick/Autocycler v0.6.1):
     trim_path_start_end / _hairpin_start / _hairpin_end         trim.rs:288-326 (batch forms over lists of paths)
     unitig_graph.trim(min_identity, max_unitigs, mad)          trim.rs:43-51 (trim minus the file I/O)
     trim(cluster_dir, min_identity, max_unitigs, mad, ...)     trim.rs:36-53
+    bridge_best_paths(groups, weights)                         resolve.rs:430-462 (Bridge::new for a batch of bridges)
+    unitig_graph.resolve() / resolve_text() / resolve_stats()   resolve.rs:41-67 (resolve minus the file I/O)
+    resolve(cluster_dir), combine(autocycler_dir, in_gfas)      resolve.rs:31-69, combine.rs:25-49
 
 There is no CPU path here: if the CUDA library is missing, or no device is present, every entry
 point raises.
@@ -58,6 +61,15 @@ class AcTimings(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class AcResolveInfo(C.Structure):
+    _fields_ = [("anchors", C.c_uint32), ("unique_bridges", C.c_uint32), ("conflicting_bridges", C.c_uint32), ("culled_bridges", C.c_uint32),
+                ("jobs", C.c_uint64), ("cells", C.c_uint64), ("longest_path", C.c_uint64), ("shared_jobs", C.c_uint32), ("hbm_jobs", C.c_uint32),
+                ("kernel_ms", C.c_float)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_sequence", "ac_clear_sequences", "ac_upload",
            "ac_build", "ac_compress", "ac_simplify", "ac_merge_linear_paths", "ac_renumber_unitigs", "ac_load_gfa", "ac_bind_host_to_device", "ac_decompress_gfa", "ac_pairwise_distances", "ac_distance_matrix_text", "ac_sequence_reconstruct", "ac_counts_get", "ac_unitigs_copy", "ac_path_copy", "ac_gfa_size", "ac_gfa_copy",
            "ac_timings_get", "ac_compress_dir", "ac_compress_dir_devices", "ac_load_sequences", "ac_sequence_get",
@@ -65,7 +77,8 @@ EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_seq
            "ac_runs_import", "ac_runs_import_padded", "ac_build_finish", "ac_compress_finish", "ac_gfa_data",
            "ac_compress_finish_split", "ac_path_tokens_export", "ac_path_lines_render", "ac_path_lines_data", "ac_upload_shard", "ac_strand_block",
            "ac_trim_paths", "ac_trim", "ac_trim_yaml", "ac_trim_stats", "ac_trim_dir",
-           "ac_cluster", "ac_cluster_text", "ac_cluster_assignments", "ac_cluster_stats", "ac_upgma", "ac_cluster_dir"]
+           "ac_cluster", "ac_cluster_text", "ac_cluster_assignments", "ac_cluster_stats", "ac_upgma", "ac_cluster_dir",
+           "ac_bridge_best_paths", "ac_resolve", "ac_resolve_text", "ac_resolve_stats", "ac_resolve_dir", "ac_combine_dir"]
 
 _libs = {}
 
@@ -138,6 +151,13 @@ def load_library(path=None):
     lib.ac_upgma.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint32),
                              C.POINTER(C.c_uint32), C.POINTER(C.c_double)]
     lib.ac_cluster_dir.argtypes = [C.c_char_p, C.c_double, C.c_int64, C.c_uint32, C.c_char_p, C.c_int32, C.c_int32]
+    lib.ac_bridge_best_paths.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_uint64), C.c_uint64, C.POINTER(C.c_uint64), C.c_uint64,
+                                         C.POINTER(C.c_uint32), C.c_uint64, C.POINTER(C.c_uint32), C.POINTER(C.c_int32), C.POINTER(C.c_uint64)]
+    lib.ac_resolve.argtypes = [C.c_void_p, C.c_int32]
+    lib.ac_resolve_text.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
+    lib.ac_resolve_stats.argtypes = [C.c_void_p, C.POINTER(AcResolveInfo)]
+    lib.ac_resolve_dir.argtypes = [C.c_char_p, C.c_int32, C.c_int32]
+    lib.ac_combine_dir.argtypes = [C.c_char_p, C.POINTER(C.c_char_p), C.c_uint32, C.c_int32]
     _libs[path] = lib
     return lib
 
@@ -400,6 +420,26 @@ class UnitigGraph:
         return {"sequences": n.value, "pass_clusters": p.value, "fail_clusters": f.value, "distance_ms": dm.value, "upgma_ms": um.value,
                 "cluster_gfa_ms": gm.value}
 
+    def resolve(self, verbose=False):   # resolve.rs:41-67 on this graph (a loaded 2_trimmed.gfa)
+        """Anchors, bridges (their path distances on the GPU), the unique bridges applied, culling and the final bridges: resolve_text()
+        returns 3_bridged.gfa, 4_merged.gfa and 5_final.gfa, resolve_stats() the counts and the kernel time.  The graph is unchanged."""
+        self._h.check(self._h.lib.ac_resolve(self._h.ptr, 1 if verbose else 0))
+
+    RESOLVE_TEXTS = {"bridged": 0, "merged": 1, "final": 2}
+
+    def resolve_text(self, what):   # "bridged", "merged" or "final"
+        n = C.c_uint64()
+        w = self.RESOLVE_TEXTS[what]
+        self._h.check(self._h.lib.ac_resolve_text(self._h.ptr, w, None, 0, C.byref(n)))
+        buf = C.create_string_buffer(max(1, n.value))
+        self._h.check(self._h.lib.ac_resolve_text(self._h.ptr, w, buf, n.value, C.byref(n)))
+        return buf.raw[:n.value].decode()
+
+    def resolve_stats(self):
+        info = AcResolveInfo()
+        self._h.check(self._h.lib.ac_resolve_stats(self._h.ptr, C.byref(info)))
+        return info.as_dict()
+
     def save_gfa(self, gfa_filename, sequences=None, use_other_colour=False):   # unitig_graph.rs:317-331
         with open(gfa_filename, "wb") as f:
             f.write(self.gfa_bytes())
@@ -522,5 +562,49 @@ def cluster(autocycler_dir, cutoff=0.2, min_assemblies=None, max_contigs=25, man
     lib = lib or load_library()
     rc = lib.ac_cluster_dir(os.fsencode(autocycler_dir), float(cutoff), -1 if min_assemblies is None else int(min_assemblies), max_contigs,
                             manual.encode() if manual is not None else None, device, 1 if verbose else 0)
+    if rc != AC_OK:
+        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+
+
+def bridge_best_paths(groups, weights, lib=None, device=0, handle=None):
+    """Bridge::new (resolve.rs:430-462) for every group of trimmed paths (lists of signed unitig numbers, start and end removed), with the
+    distances on the GPU; weights: {unitig: length} or a list indexed by unitig number.  -> ([[u32 total per path]], [best path])"""
+    lib = lib or load_library()
+    h = handle or _Handle(lib, 51, device)
+    if isinstance(weights, dict):
+        w = [0] * (max(weights) + 1 if weights else 1)
+        for u, ln in weights.items():
+            w[u] = ln
+    else:
+        w = list(weights)
+    paths = [p for g in groups for p in g]
+    flat = [u for p in paths for u in p]
+    off, goff = [0], [0]
+    for p in paths:
+        off.append(off[-1] + len(p))
+    for g in groups:
+        goff.append(goff[-1] + len(g))
+    n, G = len(paths), len(groups)
+    totals = (C.c_uint32 * max(1, n))()
+    best = (C.c_int32 * max(1, len(flat)))()
+    best_off = (C.c_uint64 * (G + 1))()
+    h.check(lib.ac_bridge_best_paths(h.ptr, (C.c_int32 * max(1, len(flat)))(*flat), (C.c_uint64 * (n + 1))(*off), n, (C.c_uint64 * (G + 1))(*goff), G,
+                                     (C.c_uint32 * max(1, len(w)))(*w), len(w), totals, best, best_off))
+    return ([list(totals[goff[g]:goff[g + 1]]) for g in range(G)], [list(best[best_off[g]:best_off[g + 1]]) for g in range(G)])
+
+
+def resolve(cluster_dir, verbose=False, device=0, lib=None):
+    """resolve.rs:31-69: reads <cluster_dir>/2_trimmed.gfa, writes 3_bridged.gfa, 4_merged.gfa and 5_final.gfa."""
+    lib = lib or load_library()
+    rc = lib.ac_resolve_dir(os.fsencode(cluster_dir), 1 if verbose else 0, device)
+    if rc != AC_OK:
+        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+
+
+def combine(autocycler_dir, in_gfas, verbose=False, lib=None):
+    """combine.rs:25-49: writes <autocycler_dir>/consensus_assembly.gfa, .fasta and .yaml from the GFAs in order."""
+    lib = lib or load_library()
+    names = [os.fsencode(g) for g in in_gfas]
+    rc = lib.ac_combine_dir(os.fsencode(autocycler_dir), (C.c_char_p * max(1, len(names)))(*names), len(names), 1 if verbose else 0)
     if rc != AC_OK:
         raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())

@@ -21,6 +21,7 @@
 #include "host_io.h"
 #include "host_cluster.h"
 #include "host_trim.h"
+#include "host_resolve.h"
 #include <immintrin.h>
 #include <functional>
 #include <thread>
@@ -72,6 +73,7 @@ struct ac_handle {
     std::string trim_yaml; bool trimmed = false;           // ac_trim: 2_trimmed.yaml
     TrimStats trim_stats;
     ClusterResult cluster; ClusterStats cluster_stats; bool clustered = false;
+    ResolveResult resolve; ResolveStats resolve_stats; bool resolved = false;
 };
 
 static int set_error(const ac_handle* h, int code, const std::string& msg) {
@@ -547,6 +549,7 @@ int ac_load_gfa(ac_handle* h, const char* gfa_text, uint64_t length) {
     h->seqs.clear(); h->infos.clear(); h->ascii.clear(); h->loaded = LoadedInput(); h->res = PipelineResult(); h->t = ac_timings{};   // a loaded graph has no sequence bytes: ac_upload / ac_build need ac_add_sequence again
     h->trimmed = false; h->trim_yaml.clear();
     h->clustered = false; h->cluster = ClusterResult();
+    h->resolved = false; h->resolve = ResolveResult();
     h->graph.load_gfa(gfa_text, (size_t)length, h->seqs);
     h->cfg.k = h->graph.k;
     h->built = true; h->graph_ready = true;
@@ -1208,6 +1211,162 @@ int ac_cluster_dir(const char* autocycler_dir, double cutoff, int64_t min_assemb
                                  "\n(distance kernels %.2f ms, UPGMA kernel %.2f ms, per-cluster graphs %.1f ms)\n\n", phylip.c_str(), newick.c_str(), tsv.c_str(),
                          (double)h->cluster_stats.distance_ms, (double)h->cluster_stats.upgma_ms, h->cluster_stats.cluster_gfa_ms);
     return ok(h);
+    AC_GUARD_END(nullptr)
+}
+
+// Bridge::new (resolve.rs:430-462) for caller groups of paths, one device round of distances
+int ac_bridge_best_paths(ac_handle* h, const int32_t* paths, const uint64_t* path_off, uint64_t n_paths, const uint64_t* group_off, uint64_t n_groups,
+                         const uint32_t* weights, uint64_t n_weights, uint32_t* totals, int32_t* best, uint64_t* best_off) {
+    if (!h || !path_off || !group_off || !best_off || (n_weights && !weights) || (n_paths && !totals) || (n_paths && path_off[n_paths] && (!paths || !best)))
+        return set_error(h, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    if (group_off[0] != 0 || group_off[n_groups] != n_paths) return set_error(h, AC_EINVAL, "the groups must cover the paths in order");
+    std::vector<std::vector<std::vector<int32_t>>> groups(n_groups);
+    for (uint64_t g = 0; g < n_groups; ++g) {
+        if (group_off[g + 1] < group_off[g]) return set_error(h, AC_EINVAL, "group offsets must not decrease");
+        for (uint64_t x = group_off[g]; x < group_off[g + 1]; ++x) {
+            if (path_off[x + 1] < path_off[x]) return set_error(h, AC_EINVAL, "path offsets must not decrease");
+            groups[g].emplace_back(paths + path_off[x], paths + path_off[x + 1]);
+            for (int32_t u : groups[g].back()) {
+                const int64_t a = u < 0 ? -(int64_t)u : u;
+                if (u == 0 || (uint64_t)a >= n_weights) return set_error(h, AC_EINVAL, "path entry " + std::to_string(u) + " has no weight");
+            }
+        }
+    }
+    std::vector<uint32_t> w(weights, weights + n_weights);
+    std::vector<std::vector<uint32_t>> tot;
+    std::vector<std::vector<int32_t>> bp;
+    ResolveStats st;
+    bridge_best_paths(*h->pipe, groups, w, tot, bp, st);
+    uint64_t at = 0;
+    best_off[0] = 0;
+    for (uint64_t g = 0; g < n_groups; ++g) {
+        std::copy(tot[g].begin(), tot[g].end(), totals + group_off[g]);
+        std::copy(bp[g].begin(), bp[g].end(), best + at); at += bp[g].size();
+        best_off[g + 1] = at;
+    }
+    h->resolve_stats = st;
+    return ok(h);
+    AC_GUARD_END(h)
+}
+
+int ac_resolve(ac_handle* h, int32_t verbose) {
+    if (!h) return set_error(nullptr, AC_EINVAL, "null handle");
+    AC_GUARD_BEGIN
+    if (!h->built) return set_error(h, AC_EINVAL, "a graph must be loaded before ac_resolve");
+    ensure_graph(h);
+    h->resolved = false;
+    std::string text;                      // the graph as a 2_trimmed.gfa: resolve re-loads it for its second pass (resolve.rs:59)
+    h->graph.gfa_text(h->seqs, text);
+    resolve_text(text, *h->pipe, verbose != 0, h->resolve, h->resolve_stats);
+    h->resolved = true;
+    return ok(h);
+    AC_GUARD_END(h)
+}
+
+int ac_resolve_text(ac_handle* h, int32_t what, char* out, uint64_t cap, uint64_t* length) {
+    if (!h || !length) return set_error(h, AC_EINVAL, "null argument");
+    if (!h->resolved) return set_error(h, AC_EINVAL, "ac_resolve must precede ac_resolve_text");
+    const std::string* t = what == AC_RESOLVE_BRIDGED ? &h->resolve.bridged : what == AC_RESOLVE_MERGED ? &h->resolve.merged :
+                           what == AC_RESOLVE_FINAL ? &h->resolve.final_gfa : nullptr;
+    if (!t) return set_error(h, AC_EINVAL, "unknown resolve text");
+    *length = t->size();
+    if (!out) return ok(h);
+    if (cap < t->size()) return set_error(h, AC_ERANGE, "buffer too small");
+    memcpy(out, t->data(), t->size());
+    return ok(h);
+}
+
+int ac_resolve_stats(const ac_handle* h, ac_resolve_info* out) {
+    if (!h || !out) return set_error(h, AC_EINVAL, "null argument");
+    const ResolveStats& s = h->resolve_stats;
+    out->anchors = s.anchors; out->unique_bridges = s.unique_bridges; out->conflicting_bridges = s.conflicting_bridges; out->culled_bridges = s.culled_bridges;
+    out->jobs = s.jobs; out->cells = s.cells; out->longest_path = s.longest_path; out->shared_jobs = s.shared_jobs; out->hbm_jobs = s.hbm_jobs;
+    out->kernel_ms = s.kernel_ms;
+    return ok(h);
+}
+
+namespace {
+bool read_file(const std::string& path, std::string& text) {
+    FILE* f = fopen(path.c_str(), "rb");
+    if (!f) return false;
+    char buf[1 << 16]; size_t n;
+    text.clear();
+    while ((n = fread(buf, 1, sizeof buf, f)) > 0) text.append(buf, n);
+    fclose(f);
+    return true;
+}
+bool check_file(const std::string& path) {      // check_if_file_exists (misc.rs:98-107)
+    struct stat st;
+    if (stat(path.c_str(), &st) != 0) { set_error(nullptr, AC_EINPUT, "file does not exist: " + path); return false; }
+    if (!S_ISREG(st.st_mode)) { set_error(nullptr, AC_EINPUT, path + " is not a file"); return false; }
+    return true;
+}
+bool make_dirs(const std::string& path) {       // create_dir_all
+    struct stat st;
+    if (path.empty() || stat(path.c_str(), &st) == 0) return path.empty() || S_ISDIR(st.st_mode);
+    const size_t slash = path.find_last_of('/', path.size() > 1 ? path.size() - 2 : 0);
+    if (slash != std::string::npos && slash > 0 && !make_dirs(path.substr(0, slash))) return false;
+    return mkdir(path.c_str(), 0777) == 0 || (stat(path.c_str(), &st) == 0 && S_ISDIR(st.st_mode));
+}
+}  // namespace
+
+int ac_resolve_dir(const char* cluster_dir, int32_t verbose, int32_t device) {
+    if (!cluster_dir) return set_error(nullptr, AC_EINVAL, "null argument");
+    ac_handle* h = nullptr;
+    AC_GUARD_BEGIN
+    // check_settings, resolve.rs:72-75 (misc.rs:98-119)
+    const std::string dir = cluster_dir, trimmed = dir + "/2_trimmed.gfa";
+    struct stat st;
+    if (stat(cluster_dir, &st) != 0) return set_error(nullptr, AC_EINPUT, "directory does not exist: " + dir);
+    if (!S_ISDIR(st.st_mode)) return set_error(nullptr, AC_EINPUT, dir + " is not a directory");
+    if (!check_file(trimmed)) return AC_EINPUT;
+    std::string text;
+    if (!read_file(trimmed, text)) return set_error(nullptr, AC_EIO, "cannot read " + trimmed);
+    ac_config cfg{}; cfg.k = 51; cfg.device = device; cfg.stream = nullptr; cfg.keep_positions = 0; cfg.n_devices = 1; cfg.devices = nullptr;
+    int rc = ac_create(&h, &cfg);
+    if (rc != AC_OK) return rc;
+    std::unique_ptr<ac_handle, void (*)(ac_handle*)> guard(h, ac_destroy);
+    if (verbose) fprintf(stderr, "\nStarting autocycler resolve\n    This command resolves repeats in the unitig graph.\n\nSettings:\n  --cluster_dir %s\n\n", dir.c_str());
+    {   // the loader's own errors (a malformed 2_trimmed.gfa) are input errors
+        HostGraph check; std::vector<HostSeq> seqs;
+        try { check.load_gfa(text.data(), text.size(), seqs); }
+        catch (const std::runtime_error& e) { return set_error(nullptr, AC_EINPUT, e.what()); }
+    }
+    ResolveResult r; ResolveStats rs;
+    resolve_text(text, *h->pipe, verbose != 0, r, rs);
+    const std::string bridged = dir + "/3_bridged.gfa", merged = dir + "/4_merged.gfa", final_gfa = dir + "/5_final.gfa";
+    if (!write_file(bridged, r.bridged) || !write_file(merged, r.merged) || !write_file(final_gfa, r.final_gfa))
+        return set_error(nullptr, AC_EIO, "cannot write the output files under " + dir);
+    if (verbose) fprintf(stderr, "\nFinished!\nFinal consensus graph: %s\n(%llu distance jobs, %llu DP cells, distance kernels %.2f ms)\n\n", final_gfa.c_str(),
+                         (unsigned long long)rs.jobs, (unsigned long long)rs.cells, (double)rs.kernel_ms);
+    return ok(h);
+    AC_GUARD_END(nullptr)
+}
+
+int ac_combine_dir(const char* autocycler_dir, const char* const* in_gfas, uint32_t n_gfas, int32_t verbose) {
+    if (!autocycler_dir || (n_gfas && !in_gfas)) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    if (n_gfas == 0) return set_error(nullptr, AC_EINPUT, "at least one input GFA is required");
+    std::vector<std::string> names, texts(n_gfas);
+    for (uint32_t i = 0; i < n_gfas; ++i) { if (!in_gfas[i]) return set_error(nullptr, AC_EINVAL, "null argument"); names.push_back(in_gfas[i]); }
+    for (const std::string& n : names) if (!check_file(n)) return AC_EINPUT;     // check_settings (combine.rs:52-56)
+    const std::string dir = autocycler_dir;
+    if (!make_dirs(dir)) return set_error(nullptr, AC_EINPUT, "failed to create directory " + dir + "\n" + strerror(errno));
+    if (verbose) {
+        fprintf(stderr, "\nStarting autocycler combine\n    This command combines different clusters into a single assembly file.\n\nSettings:\n  --autocycler_dir %s\n  --in_gfas %s\n",
+                dir.c_str(), names[0].c_str());
+        for (size_t i = 1; i < names.size(); ++i) fprintf(stderr, "            %s\n", names[i].c_str());
+        fprintf(stderr, "\n");
+    }
+    for (uint32_t i = 0; i < n_gfas; ++i) if (!read_file(names[i], texts[i])) return set_error(nullptr, AC_EIO, "cannot read " + names[i]);
+    std::string gfa, fasta, yaml;
+    combine_texts(texts, names, verbose != 0, gfa, fasta, yaml);
+    const std::string out_gfa = dir + "/consensus_assembly.gfa", out_fasta = dir + "/consensus_assembly.fasta", out_yaml = dir + "/consensus_assembly.yaml";
+    if (!write_file(out_gfa, gfa) || !write_file(out_fasta, fasta) || !write_file(out_yaml, yaml)) return set_error(nullptr, AC_EIO, "cannot write the output files under " + dir);
+    if (verbose) fprintf(stderr, "\nFinished!\nCombined graph: %s\nCombined fasta: %s\n\n%s\n\n", out_gfa.c_str(), out_fasta.c_str(),
+                         yaml.find("fully_resolved: true") != std::string::npos ? "Consensus assembly is fully resolved" : "One or more clusters failed to fully resolve");
+    return ok(nullptr);
     AC_GUARD_END(nullptr)
 }
 

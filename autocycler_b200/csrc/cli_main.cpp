@@ -1,4 +1,4 @@
-// `autocycler compress`, `autocycler decompress`, `autocycler cluster` and `autocycler trim` with the reference's flags (main.rs:126-162), messages and exit codes
+// `autocycler compress`, `autocycler decompress`, `autocycler cluster`, `autocycler trim`, `autocycler resolve` and `autocycler combine` with the reference's flags (main.rs:126-162), messages and exit codes
 // (misc.rs:130-136: "Error: <text>" on stderr, exit 1), running the H100 path through the C ABI.
 #include <cstdio>
 #include <cstdlib>
@@ -103,7 +103,50 @@ static int cluster_main(int argc, char** argv) {
     return 0;
 }
 
+// `autocycler resolve` (main.rs:238-247, resolve.rs:31-111)
+static int resolve_main(int argc, char** argv) {
+    static const char* resolve_usage = "Usage: autocycler resolve --cluster_dir <CLUSTER_DIR> [--verbose] [--device N]\n";
+    std::string dir; bool verbose = false; int device = 0;
+    for (int i = 2; i < argc; ++i) {
+        std::string a = argv[i];
+        auto value = [&]() -> const char* { if (i + 1 >= argc) { fprintf(stderr, "error: a value is required for '%s'\n", a.c_str()); exit(2); } return argv[++i]; };
+        if (a == "-c" || a == "--cluster_dir") dir = value();
+        else if (a == "--verbose") verbose = true;
+        else if (a == "--device") device = atoi(value());
+        else if (a == "-h" || a == "--help") { fprintf(stderr, "%s", resolve_usage); return 0; }
+        else { fprintf(stderr, "error: unexpected argument '%s'\n%s", a.c_str(), resolve_usage); return 2; }
+    }
+    if (dir.empty()) { fprintf(stderr, "%s", resolve_usage); return 2; }
+    fprintf(stderr, "\nStarting autocycler resolve (%s)\n\n", ac_version());
+    const int rc = ac_resolve_dir(dir.c_str(), verbose ? 1 : 0, device);
+    if (rc != AC_OK) { fprintf(stderr, "\nError: %s\n", ac_last_error(nullptr)); return 1; }
+    return 0;
+}
+
+// `autocycler combine` (main.rs:115-124, combine.rs:25-87): -i takes one or more GFAs, up to the next flag
+static int combine_main(int argc, char** argv) {
+    static const char* combine_usage = "Usage: autocycler combine --autocycler_dir <AUTOCYCLER_DIR> --in_gfas <IN_GFAS>...\n";
+    std::string dir; std::vector<std::string> gfas;
+    for (int i = 2; i < argc; ++i) {
+        std::string a = argv[i];
+        auto value = [&]() -> const char* { if (i + 1 >= argc) { fprintf(stderr, "error: a value is required for '%s'\n", a.c_str()); exit(2); } return argv[++i]; };
+        if (a == "-a" || a == "--autocycler_dir") dir = value();
+        else if (a == "-i" || a == "--in_gfas") { gfas.push_back(value()); while (i + 1 < argc && argv[i + 1][0] != '-') gfas.push_back(argv[++i]); }
+        else if (a == "-h" || a == "--help") { fprintf(stderr, "%s", combine_usage); return 0; }
+        else { fprintf(stderr, "error: unexpected argument '%s'\n%s", a.c_str(), combine_usage); return 2; }
+    }
+    if (dir.empty() || gfas.empty()) { fprintf(stderr, "%s", combine_usage); return 2; }
+    std::vector<const char*> ptrs;
+    for (const std::string& g : gfas) ptrs.push_back(g.c_str());
+    fprintf(stderr, "\nStarting autocycler combine (%s)\n\n", ac_version());
+    const int rc = ac_combine_dir(dir.c_str(), ptrs.data(), (uint32_t)ptrs.size(), 1);
+    if (rc != AC_OK) { fprintf(stderr, "\nError: %s\n", ac_last_error(nullptr)); return 1; }
+    return 0;
+}
+
 int main(int argc, char** argv) {
+    if (argc >= 2 && strcmp(argv[1], "resolve") == 0) return resolve_main(argc, argv);
+    if (argc >= 2 && strcmp(argv[1], "combine") == 0) return combine_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "decompress") == 0) return decompress_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "cluster") == 0) return cluster_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "trim") == 0) return trim_main(argc, argv);

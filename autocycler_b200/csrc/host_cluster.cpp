@@ -279,6 +279,8 @@ std::string filter_paths(const std::string& gfa, const std::vector<uint8_t>& dro
 }
 }  // namespace
 
+uint64_t sequence_consensus_weight(const HostSeq& s) { return consensus_weight(s); }
+
 std::string rust_display_f64(double v) {
     if (std::isnan(v)) return "NaN";
     if (std::isinf(v)) return v > 0 ? "inf" : "-inf";

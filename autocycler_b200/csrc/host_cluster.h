@@ -31,6 +31,9 @@ struct ClusterResult {
 void cluster_graph(const std::string& gfa, const HostGraph& g, std::vector<HostSeq>& seqs, DevicePipeline& pipe, double cutoff, int64_t min_assemblies,
                    const std::vector<uint16_t>& manual, uint32_t max_contigs, const std::string& out_dir, bool verbose, ClusterResult& out, ClusterStats& stats);
 
+// Sequence::consensus_weight (sequence.rs:104-109): the autocycler_consensus_weight= value of the header, 1 when absent or unparsable
+uint64_t sequence_consensus_weight(const HostSeq& s);
+
 // parse_manual_clusters (:664-671): "1, 2,3" -> sorted node numbers
 std::vector<uint16_t> parse_manual_clusters(const std::string& text);
 

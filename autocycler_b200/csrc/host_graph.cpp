@@ -704,9 +704,13 @@ inline uint32_t put_depth(char* p, double d) {
     return (uint32_t)snprintf(p, 400, "%.2f", d);
 }
 const char* const COLOUR_TAG[4] = {"", "\tCL:Z:forestgreen", "\tCL:Z:pink", "\tCL:Z:steelblue"};   // unitig.rs:23-26, colour_tag :173-181 with use_other_colour = false
+const char* const OTHER_COLOUR_TAG = "\tCL:Z:orangered";                                              // unitig.rs:27, use_other_colour = true
 }  // namespace
 
-void HostGraph::gfa_text(const std::vector<HostSeq>& seqs, std::string& out) const {
+uint32_t gfa_depth_text(char* p, double d) { return put_depth(p, d); }
+
+void HostGraph::gfa_text(const std::vector<HostSeq>& seqs, std::string& out, bool other_colour) const {
+    auto colour = [&](uint32_t idx) { const uint8_t t = type_of(idx); return t == 0 && other_colour ? OTHER_COLOUR_TAG : COLOUR_TAG[t]; };
     // Decimal text of every unitig number, by seed index, so that the hot loops copy bytes instead of dividing.
     std::vector<uint64_t> num_txt(U); std::vector<uint8_t> num_len(U);
     const size_t TU = std::max<size_t>(1, std::min<size_t>(host_threads() * 4, (size_t)U / 2048));
@@ -733,7 +737,7 @@ void HostGraph::gfa_text(const std::vector<HostSeq>& seqs, std::string& out) con
         for (uint32_t n = ub(t); n < ub(t + 1); ++n) {
             const uint32_t idx = order[n];
             if (!depth_f) ss += 2 + num_len[idx] + 1 + rec[idx].len + 6 + digits10(depth[idx]) + 4;            // "S\t" num "\t" seq "\tDP:f:" depth ".00\n"
-            else { char tmp[400]; ss += 2 + num_len[idx] + 1 + rec[idx].len + 6 + put_depth(tmp, depth_f[idx]) + strlen(COLOUR_TAG[type_of(idx)]) + 1; }
+            else { char tmp[400]; ss += 2 + num_len[idx] + 1 + rec[idx].len + 6 + put_depth(tmp, depth_f[idx]) + strlen(colour(idx)) + 1; }
             for (uint32_t rev = 0; rev < 2; ++rev) {
                 const UStrand from = us_make(idx, rev != 0);
                 for (uint32_t x = next_off[from]; x < next_off[from + 1]; ++x)
@@ -775,7 +779,7 @@ void HostGraph::gfa_text(const std::vector<HostSeq>& seqs, std::string& out) con
                 p = put_str(p, seq_ptr(idx), rec[idx].len);
                 p = put_str(p, "\tDP:f:", 6);
                 if (!depth_f) { p = put_uint(p, depth[idx]); p = put_str(p, ".00\n", 4); }
-                else { char tmp[400]; const uint32_t dn = put_depth(tmp, depth_f[idx]); p = put_str(p, tmp, dn); const char* ct = COLOUR_TAG[type_of(idx)]; p = put_str(p, ct, strlen(ct)); *p++ = '\n'; }
+                else { char tmp[400]; const uint32_t dn = put_depth(tmp, depth_f[idx]); p = put_str(p, tmp, dn); const char* ct = colour(idx); p = put_str(p, ct, strlen(ct)); *p++ = '\n'; }
             }
             if ((uint64_t)(p - base) != s_at[task] + s_size[task]) throw std::runtime_error("GFA S-line size mismatch");
         } else if (task < 2 * TU) {                             // L lines, get_links_for_gfa :333-350: forward_next then reverse_next

@@ -27,6 +27,9 @@ static inline bool us_reverse(UStrand s) { return s & 1; }
 static inline UStrand us_make(uint32_t idx, bool reverse) { return (idx << 1) | (reverse ? 1u : 0u); }
 static inline UStrand us_flip(UStrand s) { return s ^ 1u; }
 
+// "{:.2}" of an f64 depth as the S lines print it (unitig.rs:169); p needs room for 400 bytes.  Returns the length.
+uint32_t gfa_depth_text(char* p, double d);
+
 struct HostProfile { double adopt = 0, renumber = 0, candidates = 0, compare = 0, pass1 = 0, expand = 0; int passes = 0; };   // milliseconds (AC_HOST_PROFILE=1 prints them)
 
 class HostGraph {
@@ -73,7 +76,12 @@ public:
     void replace_paths(const std::vector<std::vector<UStrand>>& paths);
     void recalculate_depths();                // unitig_graph.rs:575-580: depth = forward_positions.len() = path steps through the unitig
     void remove_zero_depth_unitigs();         // unitig_graph.rs:582-586, with delete_dangling_links (:547-564)
-    void gfa_text(const std::vector<HostSeq>& seqs, std::string& out) const;   // unitig_graph.rs:317-360
+    // resolve's graph edits (host_resolve.cpp): the graph becomes these unitigs in this order, with these link lists (index 2 * i + reverse,
+    // entries UStrand over the same indices), f64 depths, unitig types and no sequence paths
+    void replace_unitigs(const std::vector<uint32_t>& numbers, const std::vector<std::string>& seqs, const std::vector<double>& depths,
+                         const std::vector<uint8_t>& types, const std::vector<std::vector<UStrand>>& next_lists, const std::vector<std::vector<UStrand>>& prev_lists);
+    // unitig_graph.rs:317-360; other_colour: colour_tag(true) (unitig.rs:173-181), Other unitigs get CL:Z:orangered
+    void gfa_text(const std::vector<HostSeq>& seqs, std::string& out, bool other_colour = false) const;
     uint64_t total_length() const;
     uint64_t link_count_single() const;       // unitig_graph.rs:478-507 (.1)
     const char* seq_ptr(uint32_t idx) const { return arena + rec[idx].seq_off; }

@@ -1920,6 +1920,61 @@ __global__ void __launch_bounds__(1024) ac_overlap_align_kernel(const TrimLaunch
 }
 #endif
 
+// ------------------------------------------------------------------------------------------------
+// resolve: all-pairs path distances of a bridge (global_alignment_distance, resolve.rs:387-418), see DESIGN.md §13
+// ------------------------------------------------------------------------------------------------
+// D[i][j] over rows i (the shorter path a) and columns j (path b), in u32 with wraparound as the reference's release build computes it.
+// The sweep goes by anti-diagonals d = i + j; the three live ones (d-2, d-1, d) are indexed by row i, n + 1 words each.  Swapping the
+// two paths transposes the recurrence and applies the same adds and mins to the same operands, so D(a, b) == D(b, a) bit for bit.
+#define AC_BRIDGE_THREADS 256
+AC_HD uint32_t bridge_weight(const uint32_t* w, int32_t u) { return w[u < 0 ? (uint32_t)(-(int64_t)u) : (uint32_t)u]; }
+// One cell (i, j = d - i) of diagonal d from the two diagonals before it: the top edge (gaps in a), the left edge (gaps in b), or the
+// min of match/mismatch, delete and insert (:404-411).
+AC_HD void bridge_cell(uint32_t* cur, const uint32_t* prev, const uint32_t* prev2, uint32_t i, uint32_t j, const int32_t* pa, const int32_t* pb,
+                       const uint32_t* w) {
+    if (i == 0) { cur[0] = prev[0] + bridge_weight(w, pb[j - 1]); return; }
+    const int32_t a = pa[i - 1];
+    const uint32_t wa = bridge_weight(w, a);
+    if (j == 0) { cur[i] = prev[i - 1] + wa; return; }
+    const int32_t b = pb[j - 1];
+    const uint32_t wb = bridge_weight(w, b);
+    const uint32_t match_or_mismatch = prev2[i - 1] + (a == b ? 0u : (wa > wb ? wa : wb));
+    const uint32_t delete_cost = prev[i - 1] + wa, insert_cost = prev[i] + wb;
+    const uint32_t m = match_or_mismatch < delete_cost ? match_or_mismatch : delete_cost;
+    cur[i] = m < insert_cost ? m : insert_cost;
+}
+AC_HD uint32_t bridge_diag_lo(uint32_t d, uint32_t m) { return d > m ? d - m : 0u; }
+AC_HD uint32_t bridge_diag_hi(uint32_t d, uint32_t n) { return d < n ? d : n; }
+// Per job: its two paths, where its diagonals live when they exceed shared memory, and its output slot.
+struct BridgeLaunchJob { uint64_t a_off, b_off, scratch_off; uint32_t n, m, slot, pad; };
+
+#ifndef AC_EMULATE
+// One CTA per job.  The diagonals sit in dynamic shared memory, or in the job's HBM scratch when 12 (n + 1) bytes exceed the CTA's
+// shared memory (same code, another base pointer).  Thread t owns rows t, t + 256, ... of every diagonal: neighbouring threads read
+// neighbouring path entries and diagonal words.
+__global__ void __launch_bounds__(AC_BRIDGE_THREADS) ac_bridge_distance_kernel(const BridgeLaunchJob* __restrict__ jobs, const int32_t* __restrict__ values,
+                                                                               const uint32_t* __restrict__ weights, uint32_t* scratch,
+                                                                               uint32_t* __restrict__ dist, int use_shared) {
+    extern __shared__ uint32_t bridge_smem[];
+    const BridgeLaunchJob J = jobs[blockIdx.x];
+    const uint32_t n = J.n, m = J.m, stride = n + 1;
+    uint32_t* D = use_shared ? bridge_smem : scratch + J.scratch_off;
+    const int32_t* pa = values + J.a_off;
+    const int32_t* pb = values + J.b_off;
+    if (threadIdx.x == 0) D[0] = 0;                   // d = 0: D[0][0]
+    __syncthreads();
+    for (uint32_t d = 1; d <= n + m; ++d) {
+        uint32_t* cur = D + (size_t)(d % 3) * stride;
+        const uint32_t* prev = D + (size_t)((d - 1) % 3) * stride;
+        const uint32_t* prev2 = D + (size_t)((d + 1) % 3) * stride;     // d - 2 (mod 3); not read on d = 1
+        const uint32_t hi = bridge_diag_hi(d, n);
+        for (uint32_t i = bridge_diag_lo(d, m) + threadIdx.x; i <= hi; i += AC_BRIDGE_THREADS) bridge_cell(cur, prev, prev2, i, d - i, pa, pb, weights);
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) dist[J.slot] = D[(size_t)((n + m) % 3) * stride + n];
+}
+#endif
+
 #ifndef AC_EMULATE
 // Product scan: tiles of 4096 values, coalesced loads, warp-shuffle block scans (the functor bodies above are the
 // host-emulation form of the same two phases).
@@ -2195,6 +2250,7 @@ struct DevicePipeline::Impl {
     void do_import_runs_from(const void* const* ptrs, const uint64_t* counts, uint32_t n_ranks);
     DevBuf own_entries, own_runs;
     DevBuf trim_jobs, trim_vals, trim_w, trim_bits, trim_scratch, trim_out, trim_len;      // overlap_align
+    DevBuf br_jobs, br_vals, br_w, br_scratch, br_dist;                                      // bridge_distances
     DevBuf dist_asym, upgma_m, upgma_alive, upgma_cnt, upgma_node, upgma_rd, upgma_rj, upgma_list, upgma_out, upgma_done;   // cluster_distances / upgma
     uint32_t sym_n = 0;                                      // upgma_m holds cluster_distances' symmetric matrix of this many sequences (0: none)
     void upload_paths(const UStrand* path, const uint64_t* path_off, uint32_t n, const uint32_t* unitig_len, uint32_t U);   // and clears the outputs
@@ -2525,6 +2581,93 @@ float DevicePipeline::overlap_align(const int32_t* values, uint64_t n_values, co
     }
     ac_sync(&m.stream);
     for (auto& o : out) std::reverse(o.begin(), o.end());
+    return ms;
+}
+
+uint32_t DevicePipeline::bridge_shared_n_max() {
+#ifndef AC_EMULATE
+    impl->set_device();
+    static int optin = -1;                           // one device model per process
+    if (optin < 0) { int dev = 0; AC_CUDA_CHECK(cudaGetDevice(&dev)); AC_CUDA_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev)); }
+    const int budget = optin;                        // the kernel has no static shared variables
+#else
+    const int budget = 227 * 1024;                   // what an H100 grants one CTA
+#endif
+    return (uint32_t)(budget / 12) - 1;
+}
+
+float DevicePipeline::bridge_distances(const int32_t* values, uint64_t n_values, const uint32_t* weights, uint64_t n_weights,
+                                       const BridgeJob* jobs, uint32_t n_jobs, uint32_t* dist, BridgeRun* run_info) {
+    Impl& m = *impl; m.set_device();
+    if (run_info) *run_info = BridgeRun();
+    if (n_jobs == 0) return 0.f;
+    for (uint64_t v = 0; v < n_values; ++v) { const int64_t a = values[v] < 0 ? -(int64_t)values[v] : values[v]; if ((uint64_t)a >= n_weights) throw std::runtime_error("bridge_distances: unitig without a weight"); }
+    const uint32_t shared_n = bridge_shared_n_max();
+    // largest first (a CTA per job: the long ones start before the short ones); jobs with shared-memory diagonals, then the HBM ones
+    std::vector<BridgeLaunchJob> lj(n_jobs);
+    for (uint32_t x = 0; x < n_jobs; ++x) {
+        const BridgeJob& J = jobs[x];
+        if (J.n > J.m) throw std::runtime_error("bridge_distances: the rows must be the shorter path");
+        if (J.a_off + J.n > n_values || J.b_off + J.m > n_values) throw std::runtime_error("bridge_distances: path outside the value array");
+        lj[x] = BridgeLaunchJob{J.a_off, J.b_off, 0, J.n, J.m, x, 0};
+    }
+    std::stable_sort(lj.begin(), lj.end(), [](const BridgeLaunchJob& a, const BridgeLaunchJob& b) { return (uint64_t)a.n * a.m > (uint64_t)b.n * b.m; });
+    std::stable_partition(lj.begin(), lj.end(), [&](const BridgeLaunchJob& L) { return L.n <= shared_n; });
+    uint32_t n_shared = 0, n_max_shared = 0;
+    uint64_t scratch = 0;
+    for (BridgeLaunchJob& L : lj) {
+        if (L.n <= shared_n) { ++n_shared; n_max_shared = std::max(n_max_shared, L.n); }
+        else { L.scratch_off = scratch; scratch += 3ull * (L.n + 1); }
+    }
+    if (run_info) { run_info->shared_jobs = n_shared; run_info->hbm_jobs = n_jobs - n_shared; }
+    m.br_jobs.ensure(lj.size() * sizeof(BridgeLaunchJob)); m.br_vals.ensure(n_values * 4 + 4); m.br_w.ensure(n_weights * 4 + 4);
+    m.br_scratch.ensure(scratch * 4 + 4); m.br_dist.ensure((size_t)n_jobs * 4);
+    ac_h2d(m.br_jobs.p, lj.data(), lj.size() * sizeof(BridgeLaunchJob), &m.stream);
+    if (n_values) ac_h2d(m.br_vals.p, values, n_values * 4, &m.stream);
+    if (n_weights) ac_h2d(m.br_w.p, weights, n_weights * 4, &m.stream);
+    float ms = 0.f;
+#ifndef AC_EMULATE
+    cudaEvent_t e0, e1;
+    AC_CUDA_CHECK(cudaEventCreate(&e0)); AC_CUDA_CHECK(cudaEventCreate(&e1));
+    AC_CUDA_CHECK(cudaEventRecord(e0, m.stream.s));
+    if (n_shared) {
+        const size_t smem = (size_t)12 * (n_max_shared + 1);
+        AC_CUDA_CHECK(cudaFuncSetAttribute(ac_bridge_distance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ac_bridge_distance_kernel<<<n_shared, AC_BRIDGE_THREADS, smem, m.stream.s>>>(m.br_jobs.as<BridgeLaunchJob>(), m.br_vals.as<int32_t>(), m.br_w.as<uint32_t>(),
+            m.br_scratch.as<uint32_t>(), m.br_dist.as<uint32_t>(), 1);
+        AC_CUDA_CHECK(cudaGetLastError()); ++g_ac_kernel_launches; ac_debug_sync("bridge_distance", &m.stream);
+    }
+    if (n_shared < n_jobs) {
+        ac_bridge_distance_kernel<<<n_jobs - n_shared, AC_BRIDGE_THREADS, 0, m.stream.s>>>(m.br_jobs.as<BridgeLaunchJob>() + n_shared, m.br_vals.as<int32_t>(),
+            m.br_w.as<uint32_t>(), m.br_scratch.as<uint32_t>(), m.br_dist.as<uint32_t>(), 0);
+        AC_CUDA_CHECK(cudaGetLastError()); ++g_ac_kernel_launches; ac_debug_sync("bridge_distance_hbm", &m.stream);
+    }
+    AC_CUDA_CHECK(cudaEventRecord(e1, m.stream.s));
+    ac_d2h(dist, m.br_dist.p, (size_t)n_jobs * 4, &m.stream);
+    ac_sync(&m.stream);
+    AC_CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
+    cudaEventDestroy(e0); cudaEventDestroy(e1);
+#else
+    // the same diagonals and per-cell body, one job and one cell at a time
+    const int32_t* vals = m.br_vals.as<int32_t>();
+    const uint32_t* w = m.br_w.as<uint32_t>();
+    std::vector<uint32_t> own;
+    for (const BridgeLaunchJob& L : lj) {
+        const uint32_t stride = L.n + 1;
+        uint32_t* D;
+        if (L.n <= shared_n) { own.assign(3 * (size_t)stride, 0xA5A5A5A5u); D = own.data(); }
+        else D = m.br_scratch.as<uint32_t>() + L.scratch_off;
+        D[0] = 0;
+        for (uint32_t d = 1; d <= L.n + L.m; ++d) {
+            uint32_t* cur = D + (size_t)(d % 3) * stride;
+            const uint32_t* prev = D + (size_t)((d - 1) % 3) * stride;
+            const uint32_t* prev2 = D + (size_t)((d + 1) % 3) * stride;
+            for (uint32_t i = bridge_diag_lo(d, L.m); i <= bridge_diag_hi(d, L.n); ++i) bridge_cell(cur, prev, prev2, i, d - i, vals + L.a_off, vals + L.b_off, w);
+        }
+        m.br_dist.as<uint32_t>()[L.slot] = D[(size_t)((L.n + L.m) % 3) * stride + L.n];
+    }
+    ac_d2h(dist, m.br_dist.p, (size_t)n_jobs * 4, &m.stream);
+#endif
     return ms;
 }
 

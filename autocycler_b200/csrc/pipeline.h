@@ -101,6 +101,11 @@ struct LiteralHit { uint32_t needle; uint32_t pad; uint64_t gpos; };   // needle
 struct OverlapJob { uint64_t a_off, b_off; uint32_t n, k, skip_diagonal, pad; };
 // One column of the traceback (trim.rs:329-335): GAP = 0 as a unitig, NONE = -1 as an index.
 struct AlignPiece { int32_t a_unitig, a_index, b_unitig, b_index; };
+// One path distance of `autocycler resolve` (global_alignment_distance, resolve.rs:387-418): the n values at a_off (rows, the shorter
+// path) against the m values at b_off, signed unitig numbers in the caller's value array.
+struct BridgeJob { uint64_t a_off, b_off; uint32_t n, m; };
+// What one bridge_distances call ran: jobs whose three diagonals sat in shared memory, jobs whose diagonals sat in HBM scratch.
+struct BridgeRun { uint32_t shared_jobs = 0, hbm_jobs = 0; };
 // One merge of `autocycler cluster`'s UPGMA (cluster.rs:410-430): the new node's number, its left child (the cluster with the smaller
 // id), its right child, and the node's distance to the tips (half the merged pair's mean distance).
 struct UpgmaMerge { uint32_t node, left, right, pad; double dist; };
@@ -169,6 +174,13 @@ public:
                         const OverlapJob* jobs, uint32_t n_jobs, std::vector<std::vector<AlignPiece>>& out);
     // the largest k whose three live diagonals (24 * (k + 1) bytes) fit one CTA's shared memory; larger windows keep them in HBM
     uint32_t overlap_shared_k_max();
+    // resolve.rs:387-418 for a batch of path pairs: dist[x] = the u32 (wrapping) edit distance of job x, weights[|unitig|] = unitig
+    // length.  One CTA per job sweeps the anti-diagonals, largest job first.  Returns the kernels' time in ms (CUDA events; 0 under
+    // emulation).
+    float bridge_distances(const int32_t* values, uint64_t n_values, const uint32_t* weights, uint64_t n_weights,
+                           const BridgeJob* jobs, uint32_t n_jobs, uint32_t* dist, BridgeRun* run);
+    // the largest row count n whose three live diagonals (12 * (n + 1) bytes) fit one CTA's shared memory; longer rows keep them in HBM
+    uint32_t bridge_shared_n_max();
     // needles: n_needles keys of h bases each (2 words per key, kmer_key.h layout for k = h), pairwise distinct.
     void find_literals(const uint8_t* ascii, uint64_t total, const SeqInfo* seqs, uint32_t n_seqs, uint32_t h,
                        const uint64_t* needle_words, uint32_t n_needles, std::vector<LiteralHit>& hits);

@@ -16,6 +16,9 @@
  *   trim_path_start_end / _hairpin_start / _hairpin_end   trim.rs:288-326 -> ac_trim_paths
  *   trim.rs:43-51 on a loaded graph (trim minus the file I/O)     -> ac_trim
  *   trim (the whole subcommand)             trim.rs:36-53            -> ac_trim_dir
+ *   Bridge::new (best path of a bridge)     resolve.rs:430-462       -> ac_bridge_best_paths
+ *   resolve.rs:41-67 on a loaded graph                               -> ac_resolve, ac_resolve_text, ac_resolve_stats
+ *   resolve / combine (the whole subcommands)  resolve.rs:31-69, combine.rs:25-49 -> ac_resolve_dir, ac_combine_dir
  *
  * Conventions: every function returns 0 on success and a negative AC_E* code on failure; the message
  * is available from ac_last_error(handle) (or ac_last_error(NULL) when no handle exists).  No C++
@@ -263,6 +266,44 @@ int ac_upgma(ac_handle* h, const double* sym_dist, uint32_t n, const uint32_t* i
  * pairwise_distances.phylip, clustering.newick, clustering.tsv, clustering.yaml and qc_pass|qc_fail/cluster_NNN/1_untrimmed.{gfa,yaml}.
  * min_assemblies < 0: automatic; manual: "1,2,3" or NULL. */
 int ac_cluster_dir(const char* autocycler_dir, double cutoff, int64_t min_assemblies, uint32_t max_contigs, const char* manual, int32_t device, int32_t verbose);
+
+/* `autocycler resolve` and `autocycler combine`.  The one step of resolve whose cost grows quadratically — global_alignment_distance
+ * (resolve.rs:387-418) between every pair of a bridge's paths (Bridge::new, :430-462) — runs on the GPU: identical paths are aligned
+ * once, each pair of distinct paths is one CTA sweeping the anti-diagonals of a u32 DP (shared memory, or HBM scratch for paths beyond
+ * it), all bridges in one launch per storage form.  Anchors, bridges, ambiguity, culling and the graph edits run on the host
+ * (DESIGN.md section 13).  combine needs no device. */
+#define AC_RESOLVE_BRIDGED 0           /* 3_bridged.gfa */
+#define AC_RESOLVE_MERGED 1            /* 4_merged.gfa */
+#define AC_RESOLVE_FINAL 2             /* 5_final.gfa */
+typedef struct {
+    uint32_t anchors;                  /* anchor unitigs */
+    uint32_t unique_bridges, conflicting_bridges, culled_bridges;
+    uint64_t jobs;                     /* distance jobs: pairs of distinct trimmed paths of one bridge */
+    uint64_t cells;                    /* sum of n * m over the jobs */
+    uint64_t longest_path;             /* longest trimmed bridge path (unitigs) */
+    uint32_t shared_jobs, hbm_jobs;    /* jobs whose three diagonals sat in shared memory / in HBM scratch */
+    float kernel_ms;                   /* the distance kernels alone (CUDA events around their launches; 0 under emulation) */
+} ac_resolve_info;
+/* Bridge::new for n_groups bridges at once: group g holds paths group_off[g] .. group_off[g+1] (indices into the path list), path x is
+ * paths[path_off[x] .. path_off[x+1]) (signed unitig numbers: a bridge's paths with the start and end anchors already removed);
+ * weights[u] = length of unitig u (every |unitig| below n_weights).  totals[x] = path x's u32 (wrapping) sum of distances to the other
+ * paths of its group; best[best_off[g] .. best_off[g+1]) = the path the reference selects for group g (least total, ties to the
+ * lexicographically smaller path; empty when every total is u32::MAX).  best needs room for path_off[n_paths] values.  The reference's
+ * resolve.rs unit tests run through this call. */
+int ac_bridge_best_paths(ac_handle* h, const int32_t* paths, const uint64_t* path_off, uint64_t n_paths, const uint64_t* group_off, uint64_t n_groups,
+                         const uint32_t* weights, uint64_t n_weights, uint32_t* totals, int32_t* best, uint64_t* best_off);
+/* resolve.rs:41-67 on the handle's graph (ac_load_gfa of a 2_trimmed.gfa): anchors, bridges, the unique bridges applied, culling and,
+ * when anything was culled, the final bridges applied to the graph as loaded.  The handle's graph is not changed; the three files are
+ * available from ac_resolve_text, the counts and the kernel time from ac_resolve_stats.  verbose: a report on stderr. */
+int ac_resolve(ac_handle* h, int32_t verbose);
+int ac_resolve_text(ac_handle* h, int32_t what, char* out, uint64_t cap, uint64_t* length);   /* `out` may be NULL to query the length */
+int ac_resolve_stats(const ac_handle* h, ac_resolve_info* out);
+/* `autocycler resolve -c cluster_dir` (main.rs:238-247, resolve.rs:31-75): reads 2_trimmed.gfa, writes 3_bridged.gfa, 4_merged.gfa and
+ * 5_final.gfa.  The reference's checks (AC_EINPUT). */
+int ac_resolve_dir(const char* cluster_dir, int32_t verbose, int32_t device);
+/* `autocycler combine -a autocycler_dir -i gfa [gfa ...]` (main.rs:115-124, combine.rs:25-137): writes consensus_assembly.gfa, .fasta and
+ * .yaml under autocycler_dir (created if needed) from the n_gfas GFAs in argument order.  Host only. */
+int ac_combine_dir(const char* autocycler_dir, const char* const* in_gfas, uint32_t n_gfas, int32_t verbose);
 
 #ifdef __cplusplus
 }
