@@ -14,6 +14,7 @@ Names and argument meaning follow the reference (rrwick/Autocycler v0.6.1):
     bridge_best_paths(groups, weights)                         resolve.rs:430-462 (Bridge::new for a batch of bridges)
     unitig_graph.resolve() / resolve_text() / resolve_stats()   resolve.rs:41-67 (resolve minus the file I/O)
     resolve(cluster_dir), combine(autocycler_dir, in_gfas)      resolve.rs:31-69, combine.rs:25-49
+    dotplot_rgb(seqs, res, kmer) / dotplot(input, out_png)      dotplot.rs:179-221 / dotplot.rs:44-52
 
 There is no CPU path here: if the CUDA library is missing, or no device is present, every entry
 point raises.
@@ -70,6 +71,14 @@ class AcResolveInfo(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class AcDotplotInfo(C.Structure):
+    _fields_ = [("windows", C.c_uint64), ("groups", C.c_uint64), ("dots", C.c_uint64), ("host_windows", C.c_uint64),
+                ("bp_per_pixel", C.c_double), ("text_height", C.c_float), ("kernel_ms", C.c_float)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_sequence", "ac_clear_sequences", "ac_upload",
            "ac_build", "ac_compress", "ac_simplify", "ac_merge_linear_paths", "ac_renumber_unitigs", "ac_load_gfa", "ac_bind_host_to_device", "ac_decompress_gfa", "ac_pairwise_distances", "ac_distance_matrix_text", "ac_sequence_reconstruct", "ac_counts_get", "ac_unitigs_copy", "ac_path_copy", "ac_gfa_size", "ac_gfa_copy",
            "ac_timings_get", "ac_compress_dir", "ac_compress_dir_devices", "ac_load_sequences", "ac_sequence_get",
@@ -78,7 +87,8 @@ EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_seq
            "ac_compress_finish_split", "ac_path_tokens_export", "ac_path_lines_render", "ac_path_lines_data", "ac_upload_shard", "ac_strand_block",
            "ac_trim_paths", "ac_trim", "ac_trim_yaml", "ac_trim_stats", "ac_trim_dir",
            "ac_cluster", "ac_cluster_text", "ac_cluster_assignments", "ac_cluster_stats", "ac_upgma", "ac_cluster_dir",
-           "ac_bridge_best_paths", "ac_resolve", "ac_resolve_text", "ac_resolve_stats", "ac_resolve_dir", "ac_combine_dir"]
+           "ac_bridge_best_paths", "ac_resolve", "ac_resolve_text", "ac_resolve_stats", "ac_resolve_dir", "ac_combine_dir",
+           "ac_dotplot_rgb", "ac_dotplot_dir", "ac_png_write"]
 
 _libs = {}
 
@@ -158,6 +168,10 @@ def load_library(path=None):
     lib.ac_resolve_stats.argtypes = [C.c_void_p, C.POINTER(AcResolveInfo)]
     lib.ac_resolve_dir.argtypes = [C.c_char_p, C.c_int32, C.c_int32]
     lib.ac_combine_dir.argtypes = [C.c_char_p, C.POINTER(C.c_char_p), C.c_uint32, C.c_int32]
+    lib.ac_dotplot_rgb.argtypes = [C.POINTER(C.c_char_p), C.POINTER(C.c_uint64), C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_uint32,
+                                   C.c_uint32, C.c_uint32, C.c_char_p, C.c_int32, C.c_void_p, C.POINTER(AcDotplotInfo)]
+    lib.ac_dotplot_dir.argtypes = [C.c_char_p, C.c_char_p, C.c_uint32, C.c_uint32, C.c_char_p, C.c_int32, C.c_int32, C.POINTER(AcDotplotInfo)]
+    lib.ac_png_write.argtypes = [C.c_char_p, C.c_void_p, C.c_uint32, C.c_uint32]
     _libs[path] = lib
     return lib
 
@@ -606,5 +620,48 @@ def combine(autocycler_dir, in_gfas, verbose=False, lib=None):
     lib = lib or load_library()
     names = [os.fsencode(g) for g in in_gfas]
     rc = lib.ac_combine_dir(os.fsencode(autocycler_dir), (C.c_char_p * max(1, len(names)))(*names), len(names), 1 if verbose else 0)
+    if rc != AC_OK:
+        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+
+
+def _font_arg(font):
+    return None if font is None else os.fsencode(font)
+
+
+def dotplot_rgb(seqs, res=2000, kmer=32, font=None, device=0, lib=None):
+    """create_dotplot (dotplot.rs:179-221) without the file.  seqs: [(filename, name, bytes)], in box order.  font: a TrueType file for
+    the labels, "" for none, None for the first standard DejaVuSans.ttf found.  -> ((res, res, 3) uint8 array, info dict: windows,
+    groups, dots, host_windows, bp_per_pixel, text_height, kernel_ms)."""
+    import numpy as np
+    lib = lib or load_library()
+    n = len(seqs)
+    data = [bytes(s) if not isinstance(s, str) else s.encode() for _, _, s in seqs]
+    img = np.empty((res, res, 3), dtype=np.uint8) if 500 <= res <= 10000 else np.empty((1, 1, 3), dtype=np.uint8)
+    info = AcDotplotInfo()
+    rc = lib.ac_dotplot_rgb((C.c_char_p * max(1, n))(*data), (C.c_uint64 * max(1, n))(*[len(d) for d in data]),
+                            (C.c_char_p * max(1, n))(*[f.encode() for f, _, _ in seqs]), (C.c_char_p * max(1, n))(*[m.encode() for _, m, _ in seqs]),
+                            n, res, kmer, _font_arg(font), device, img.ctypes.data, C.byref(info))
+    if rc != AC_OK:
+        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+    return img, info.as_dict()
+
+
+def dotplot(input, out_png, res=2000, kmer=32, font=None, device=0, verbose=False, lib=None):
+    """dotplot.rs:44-52: input is a directory of assemblies, a FASTA file or an Autocycler GFA; writes out_png.  font as for
+    dotplot_rgb.  -> the info dict."""
+    lib = lib or load_library()
+    info = AcDotplotInfo()
+    rc = lib.ac_dotplot_dir(os.fsencode(input), os.fsencode(out_png), res, kmer, _font_arg(font), device, 1 if verbose else 0, C.byref(info))
+    if rc != AC_OK:
+        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+    return info.as_dict()
+
+
+def png_write(path, rgb, lib=None):
+    """An (h, w, 3) uint8 array as an RGB PNG (the encoder `dotplot` uses)."""
+    import numpy as np
+    lib = lib or load_library()
+    rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
+    rc = lib.ac_png_write(os.fsencode(path), rgb.ctypes.data, rgb.shape[1], rgb.shape[0])
     if rc != AC_OK:
         raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())

@@ -83,6 +83,7 @@ AC_D uint32_t ac_atomic_or(uint32_t* p, uint32_t v) { return atomicOr(p, v); }
 AC_D uint32_t ac_atomic_min(uint32_t* p, uint32_t v) { return atomicMin(p, v); }
 AC_D uint32_t ac_atomic_max(uint32_t* p, uint32_t v) { return atomicMax(p, v); }
 AC_D uint64_t ac_atomic_min(uint64_t* p, uint64_t v) { return (uint64_t)atomicMin((unsigned long long*)p, (unsigned long long)v); }
+AC_D uint64_t ac_atomic_max(uint64_t* p, uint64_t v) { return (uint64_t)atomicMax((unsigned long long*)p, (unsigned long long)v); }
 template <class T> AC_D T ac_ld_volatile(const T* p) { return *(const volatile T*)p; }
 AC_D uint64_t ac_ld_cg(const uint64_t* p) { return (uint64_t)__ldcg(reinterpret_cast<const unsigned long long*>(p)); }   // L2 (cache-global) load: sees other threads' atomics
 // four consecutive 8-byte records (one 32-byte sector) in two 128-bit L2 loads (sm_90 has no 256-bit load); every record is read

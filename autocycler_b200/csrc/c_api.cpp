@@ -13,6 +13,7 @@
 #include <cstdio>
 #include <cstring>
 #include <memory>
+#include <set>
 #include <string>
 #include <vector>
 
@@ -22,6 +23,8 @@
 #include "host_cluster.h"
 #include "host_trim.h"
 #include "host_resolve.h"
+#include "host_dotplot.h"
+#include <mutex>
 #include <immintrin.h>
 #include <functional>
 #include <thread>
@@ -1370,4 +1373,93 @@ int ac_combine_dir(const char* autocycler_dir, const char* const* in_gfas, uint3
     AC_GUARD_END(nullptr)
 }
 
+// ---- `autocycler dotplot` (dotplot.rs) ------------------------------------------------------------------------------------------
+namespace {
+// One pipeline per device for the dotplot calls, kept for the process so that its device buffers are reused by the next call.  The
+// lock is held for the whole call: calls on one device run one at a time.
+std::mutex g_dotplot_mu;
+DevicePipeline& dotplot_pipeline(int32_t device) {        // with g_dotplot_mu held
+    static std::vector<std::pair<int32_t, DevicePipeline*>> pipes;
+    for (auto& p : pipes) if (p.first == device) return *p.second;
+    pipes.emplace_back(device, new DevicePipeline(device, nullptr));
+    return *pipes.back().second;
+}
+void fill_info(const DotplotStats& st, ac_dotplot_info* info) {
+    if (!info) return;
+    info->windows = st.windows; info->groups = st.groups; info->dots = st.dots; info->host_windows = st.host_windows;
+    info->bp_per_pixel = st.bp_per_pixel; info->text_height = st.text_height; info->kernel_ms = st.kernel_ms;
+}
+// font: a TrueType file, "" for no labels, NULL for the first standard DejaVuSans.ttf that exists (none: no labels, and a warning)
+std::shared_ptr<DotplotFont> dotplot_font(const char* font, bool warn) {
+    if (font && *font) return dotplot_font_load(font);
+    if (font) return nullptr;
+    std::shared_ptr<DotplotFont> f = dotplot_font_default(nullptr);
+    if (!f && warn) fprintf(stderr, "Warning: no font found (DejaVuSans.ttf; give one with --font), so the sequence labels are not drawn\n");
+    return f;
+}
+}  // namespace
+
+int ac_dotplot_rgb(const char* const* seqs, const uint64_t* lengths, const char* const* filenames, const char* const* names, uint32_t n,
+                   uint32_t res, uint32_t kmer, const char* font, int32_t device, uint8_t* rgb, ac_dotplot_info* info) {
+    if ((n && (!seqs || !lengths || !names)) || !rgb) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    dotplot_check_settings(res, kmer);
+    std::vector<DotplotInput> in(n);
+    for (uint32_t i = 0; i < n; ++i) {
+        if ((lengths[i] && !seqs[i]) || !names[i]) return set_error(nullptr, AC_EINVAL, "null argument");
+        in[i].filename = filenames && filenames[i] ? filenames[i] : "";
+        in[i].name = names[i];
+        in[i].seq.assign(seqs[i] ? seqs[i] : "", lengths[i]);
+        for (char& c : in[i].seq) if (c >= 'a' && c <= 'z') c = (char)(c - 32);
+    }
+    if (n == 0) return set_error(nullptr, AC_EINPUT, "no sequences were loaded");
+    std::set<std::pair<std::string, std::string>> seen;
+    for (const DotplotInput& d : in) if (!seen.insert({d.filename, d.name}).second) return set_error(nullptr, AC_EINPUT, "two sequences are named " + (d.filename.empty() ? d.name : d.filename + " " + d.name));
+    const std::shared_ptr<DotplotFont> f = dotplot_font(font, false);
+    std::vector<uint8_t> img;
+    DotplotStats st;
+    {
+        std::lock_guard<std::mutex> lock(g_dotplot_mu);
+        dotplot_image(dotplot_pipeline(device), in, res, kmer, f.get(), img, st);
+    }
+    memcpy(rgb, img.data(), img.size());
+    fill_info(st, info);
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
+int ac_dotplot_dir(const char* input, const char* out_png, uint32_t res, uint32_t kmer, const char* font, int32_t device, int32_t verbose,
+                   ac_dotplot_info* info) {
+    if (!input || !out_png) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    dotplot_check_settings(res, kmer);                                                  // dotplot.rs:44-52
+    const std::vector<DotplotInput> seqs = dotplot_load(input, verbose != 0);
+    const std::shared_ptr<DotplotFont> f = dotplot_font(font, true);
+    if (verbose) fprintf(stderr, "Creating dotplot\n    K-mers common between sequences are now used to build the dotplot image.\n\n");
+    std::vector<uint8_t> img;
+    DotplotStats st;
+    {
+        std::lock_guard<std::mutex> lock(g_dotplot_mu);
+        dotplot_image(dotplot_pipeline(device), seqs, res, kmer, f.get(), img, st);
+    }
+    if (!png_write(out_png, img.data(), res, res)) return set_error(nullptr, AC_EIO, std::string("cannot write ") + out_png);
+    fill_info(st, info);
+    if (verbose) {
+        const uint64_t count = (uint64_t)seqs.size() * seqs.size();
+        fprintf(stderr, "%llu pairwise dotplot%s drawn to image\n\nFinished!\nPairwise dotplots: %s\n(%llu windows, %llu dots, kernels %.2f ms)\n\n",
+                (unsigned long long)count, count == 1 ? "" : "s", out_png, (unsigned long long)st.windows, (unsigned long long)st.dots, (double)st.kernel_ms);
+    }
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
+int ac_png_write(const char* path, const uint8_t* rgb, uint32_t width, uint32_t height) {
+    if (!path || !rgb) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    if (!png_write(path, rgb, width, height)) return set_error(nullptr, AC_EIO, std::string("cannot write ") + path);
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
 }  // extern "C"
+

@@ -1,4 +1,4 @@
-// `autocycler compress`, `autocycler decompress`, `autocycler cluster`, `autocycler trim`, `autocycler resolve` and `autocycler combine` with the reference's flags (main.rs:126-162), messages and exit codes
+// `autocycler compress`, `autocycler decompress`, `autocycler cluster`, `autocycler trim`, `autocycler resolve`, `autocycler combine` and `autocycler dotplot` with the reference's flags (main.rs:126-162), messages and exit codes
 // (misc.rs:130-136: "Error: <text>" on stderr, exit 1), running the H100 path through the C ABI.
 #include <cstdio>
 #include <cstdlib>
@@ -144,7 +144,38 @@ static int combine_main(int argc, char** argv) {
     return 0;
 }
 
+// `autocycler dotplot` (main.rs:164-181, dotplot.rs:44-52)
+static int dotplot_main(int argc, char** argv) {
+    static const char* dotplot_usage = "Usage: autocycler dotplot --input <INPUT> --out_png <OUT_PNG> [--res <RES>] [--kmer <KMER>] [--font <TTF>] [--device N]\n";
+    std::string in, out, font; bool have_font = false; unsigned long res = 2000, kmer = 32; int device = 0;
+    for (int i = 2; i < argc; ++i) {
+        std::string a = argv[i];
+        auto value = [&]() -> const char* { if (i + 1 >= argc) { fprintf(stderr, "error: a value is required for '%s'\n", a.c_str()); exit(2); } return argv[++i]; };
+        auto number = [&](const char* v) -> unsigned long {
+            char* end = nullptr; const unsigned long x = strtoul(v, &end, 10);
+            if (!*v || *end || *v == '-' || x > 0xFFFFFFFFul) { fprintf(stderr, "error: invalid value '%s' for '%s'\n", v, a.c_str()); exit(2); }
+            return x;
+        };
+        if (a == "-i" || a == "--input") in = value();
+        else if (a == "-o" || a == "--out_png") out = value();
+        else if (a == "--res") res = number(value());
+        else if (a == "--kmer") kmer = number(value());
+        else if (a == "--font") { font = value(); have_font = true; }
+        else if (a == "--device") device = atoi(value());
+        else if (a == "-h" || a == "--help") { fprintf(stderr, "%s", dotplot_usage); return 0; }
+        else { fprintf(stderr, "error: unexpected argument '%s'\n%s", a.c_str(), dotplot_usage); return 2; }
+    }
+    if (in.empty() || out.empty()) { fprintf(stderr, "%s", dotplot_usage); return 2; }
+    fprintf(stderr, "\nStarting autocycler dotplot (%s)\n    This command will take a unitig graph (either before or after trimming) and generate a dotplot image "
+                    "containing all pairwise comparisons of the sequences.\n\nSettings:\n  --input %s\n  --res %lu\n  --kmer %lu\n\n",
+            ac_version(), in.c_str(), res, kmer);
+    const int rc = ac_dotplot_dir(in.c_str(), out.c_str(), (uint32_t)res, (uint32_t)kmer, have_font ? font.c_str() : nullptr, device, 1, nullptr);
+    if (rc != AC_OK) { fprintf(stderr, "\nError: %s\n", ac_last_error(nullptr)); return 1; }
+    return 0;
+}
+
 int main(int argc, char** argv) {
+    if (argc >= 2 && strcmp(argv[1], "dotplot") == 0) return dotplot_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "resolve") == 0) return resolve_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "combine") == 0) return combine_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "decompress") == 0) return decompress_main(argc, argv);

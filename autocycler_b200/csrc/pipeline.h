@@ -110,6 +110,18 @@ struct BridgeRun { uint32_t shared_jobs = 0, hbm_jobs = 0; };
 // id), its right child, and the node's distance to the tips (half the merged pair's mean distance).
 struct UpgmaMerge { uint32_t node, left, right, pad; double dist; };
 
+// One sequence of `autocycler dotplot` (dotplot.rs:394-450): its bytes at off in the caller's byte array, its first window's global
+// index (ascending; a sequence shorter than k has no windows) and the pixel its box starts at.
+struct DotplotSeq { uint64_t off, window_base; uint32_t len, start_px; };
+// What one dotplot call ran: windows with only ACGT (the device's), their distinct canonical k-mers, dots (sum of the groups' squared
+// sizes) and the kernels' time in ms (CUDA events; 0 under emulation).
+struct DotplotRun { uint64_t windows = 0, groups = 0, dots = 0; float kernel_ms = 0.f; };
+
+// A dot's key (dotplot.rs:202-211 loop order, last writer wins): the pixel shows the dot with the largest (a * n + b, j, forward), so
+// the key packs the pair of sequences above bit 34, b's window j in bits 2-33, forward in bit 1, and bit 0 set (0 is "no dot").
+inline uint64_t dotplot_key(uint64_t pair, uint32_t j, bool forward) { return (pair << 34) | ((uint64_t)j << 2) | ((uint64_t)forward << 1) | 1u; }
+#define AC_DOTPLOT_MAX_SEQS 32768u    // n * n pairs fit the key's 30 pair bits
+
 class DevicePipeline {
 public:
     DevicePipeline(int device, void* stream);
@@ -181,6 +193,13 @@ public:
                            const BridgeJob* jobs, uint32_t n_jobs, uint32_t* dist, BridgeRun* run);
     // the largest row count n whose three live diagonals (12 * (n + 1) bytes) fit one CTA's shared memory; longer rows keep them in HBM
     uint32_t bridge_shared_n_max();
+    // dotplot.rs:202-211 for every ordered pair of sequences at once: each window of only ACGT is grouped with the windows that share its
+    // canonical k-mer, and each ordered pair of windows in a group is one dot at (pixel of the first, pixel of the second), pixel =
+    // start_px + round(position / bpp).  Every pixel keeps the largest dot key (dotplot_key); host_idx / host_key add the dots the host
+    // found for the windows that hold other bytes.  rgb (res x res x 3) holds the base image on entry and the image with the dots on
+    // return.  bytes: the sequences, uppercased, at seqs[s].off.
+    void dotplot(const uint8_t* bytes, uint64_t n_bytes, const DotplotSeq* seqs, uint32_t n_seqs, uint32_t k, double bpp, uint32_t res,
+                 const uint64_t* host_idx, const uint64_t* host_key, uint64_t n_host, uint8_t* rgb, DotplotRun* run);
     // needles: n_needles keys of h bases each (2 words per key, kmer_key.h layout for k = h), pairwise distinct.
     void find_literals(const uint8_t* ascii, uint64_t total, const SeqInfo* seqs, uint32_t n_seqs, uint32_t h,
                        const uint64_t* needle_words, uint32_t n_needles, std::vector<LiteralHit>& hits);

@@ -19,6 +19,8 @@
  *   Bridge::new (best path of a bridge)     resolve.rs:430-462       -> ac_bridge_best_paths
  *   resolve.rs:41-67 on a loaded graph                               -> ac_resolve, ac_resolve_text, ac_resolve_stats
  *   resolve / combine (the whole subcommands)  resolve.rs:31-69, combine.rs:25-49 -> ac_resolve_dir, ac_combine_dir
+ *   create_dotplot without the file         dotplot.rs:179-221       -> ac_dotplot_rgb
+ *   dotplot (the whole subcommand)          dotplot.rs:44-52         -> ac_dotplot_dir, ac_png_write
  *
  * Conventions: every function returns 0 on success and a negative AC_E* code on failure; the message
  * is available from ac_last_error(handle) (or ac_last_error(NULL) when no handle exists).  No C++
@@ -304,6 +306,40 @@ int ac_resolve_dir(const char* cluster_dir, int32_t verbose, int32_t device);
 /* `autocycler combine -a autocycler_dir -i gfa [gfa ...]` (main.rs:115-124, combine.rs:25-137): writes consensus_assembly.gfa, .fasta and
  * .yaml under autocycler_dir (created if needed) from the n_gfas GFAs in argument order.  Host only. */
 int ac_combine_dir(const char* autocycler_dir, const char* const* in_gfas, uint32_t n_gfas, int32_t verbose);
+
+/* `autocycler dotplot`.  The all-vs-all k-mer dots (dotplot.rs:202-211, 394-450) run on the GPU: every window of only ACGT gets its
+ * canonical k-mer, the windows are grouped by it, and each ordered pair of windows in a group is one dot whose 64-bit key (pair of
+ * sequences, window, forward) goes into a per-pixel maximum, which fixes the colour the reference's loop order leaves.  Windows with
+ * other bytes are matched on the host by the reference's literal rules and merged into the same maxima.  The layout, the boxes, the
+ * labels (a TrueType font read at run time) and the PNG are host work (DESIGN.md section 14).
+ *
+ * font: a TrueType file for the labels; "" draws no labels; NULL takes the first of a fixed list of standard DejaVuSans.ttf paths that
+ * exists (none: no labels, and ac_dotplot_dir prints one warning line).  Without labels the layout is the one the reference uses when
+ * its labels fit at the largest font size.
+ *
+ * Calls on one device run one at a time (a lock around the device work).  The device buffers of a call stay allocated for the next
+ * call on that device until the process ends: about 70 to 80 bytes per window and 8 bytes per pixel (res * res). */
+typedef struct {
+    uint64_t windows;                  /* k-mer windows over every sequence (len - k + 1 each) */
+    uint64_t groups;                   /* distinct canonical k-mers among the windows of only ACGT */
+    uint64_t dots;                     /* dots, including those that fall outside the image: the groups' squared sizes plus the host's */
+    uint64_t host_windows;             /* windows holding a byte other than ACGT, matched on the host */
+    double bp_per_pixel;               /* get_positions (dotplot.rs:268-269) */
+    float text_height;                 /* reduce_scale's font size (dotplot.rs:308-327) */
+    float kernel_ms;                   /* CUDA events from the first to the last dot kernel (0 under emulation); the span includes two
+                                          blocking reads of a count by the host (the group count and the dot count) */
+} ac_dotplot_info;
+/* create_dotplot (dotplot.rs:179-221) for n sequences: seqs[i] holds lengths[i] bytes (uppercased here; bytes other than ACGT are kept),
+ * labelled (filenames[i] or "" when filenames is NULL, names[i]); no two labels may be equal (AC_EINPUT).  rgb: res * res * 3 bytes,
+ * row-major RGB.  The reference's --res and --kmer checks apply (AC_EINPUT).  info may be NULL. */
+int ac_dotplot_rgb(const char* const* seqs, const uint64_t* lengths, const char* const* filenames, const char* const* names, uint32_t n,
+                   uint32_t res, uint32_t kmer, const char* font, int32_t device, uint8_t* rgb, ac_dotplot_info* info);
+/* `autocycler dotplot -i input -o out_png --res R --kmer K [--font F]` (main.rs:164-181, dotplot.rs:44-52): input is a directory of
+ * assemblies, a FASTA file or an Autocycler GFA (gzipped or not).  The reference's checks and messages (AC_EINPUT).  info may be NULL. */
+int ac_dotplot_dir(const char* input, const char* out_png, uint32_t res, uint32_t kmer, const char* font, int32_t device, int32_t verbose,
+                   ac_dotplot_info* info);
+/* rgb (width * height * 3 bytes, row-major) as an 8-bit RGB PNG at path.  Host only. */
+int ac_png_write(const char* path, const uint8_t* rgb, uint32_t width, uint32_t height);
 
 #ifdef __cplusplus
 }
