@@ -34,7 +34,40 @@ def global_alignment_distance(a, b, weights):   # resolve.rs:387-418
         if key not in _dp_cache:
             _dp_cache[key] = global_alignment_distance_rows(a, b, weights)
         return _dp_cache[key]
+    if WRAP_DP:
+        key = min((tuple(a), tuple(b)), (tuple(b), tuple(a)))      # D(a, b) == D(b, a): checked against the cell form in the tests
+        if key not in _wrap_cache:
+            _wrap_cache[key] = global_alignment_distance_diagonals(a, b, weights)
+        return _wrap_cache[key]
     return global_alignment_distance_cells(a, b, weights)
+
+
+WRAP_DP = False          # tests only: the anti-diagonal form below, exact with wraparound, for bridges of hundreds of unitigs
+_wrap_cache = {}
+
+
+def global_alignment_distance_diagonals(a, b, weights):
+    """The cell form one anti-diagonal (i + j = d) at a time: a cell needs only the two diagonals before it, so each diagonal is a few
+    uint32 vector adds and mins on the same operands as the cell form, wrapping as it does."""
+    n, m = len(a), len(b)
+    wa = np.array([weights[abs(u)] for u in a], dtype=np.uint32)
+    wb = np.array([weights[abs(u)] for u in b], dtype=np.uint32)
+    av, bv = np.array(a, dtype=np.int64), np.array(b, dtype=np.int64)
+    diags = [np.zeros(n + 1, dtype=np.uint32) for _ in range(3)]       # diagonal d lives in diags[d % 3], indexed by row i
+    for d in range(1, n + m + 1):
+        cur, prev, prev2 = diags[d % 3], diags[(d - 1) % 3], diags[(d - 2) % 3]
+        if d <= m:
+            cur[0] = (int(prev[0]) + int(wb[d - 1])) & U32                # top edge: gaps in a
+        if d <= n:
+            cur[d] = (int(prev[d - 1]) + int(wa[d - 1])) & U32            # left edge: gaps in b
+        lo, hi = max(1, d - m), min(d - 1, n)
+        if lo <= hi:
+            i = np.arange(lo, hi + 1)
+            j = d - i
+            wi, wj = wa[i - 1], wb[j - 1]
+            sub = np.where(av[i - 1] == bv[j - 1], np.uint32(0), np.maximum(wi, wj))
+            cur[lo:hi + 1] = np.minimum(np.minimum(prev2[i - 1] + sub, prev[i - 1] + wi), prev[i] + wj)
+    return int(diags[(n + m) % 3][n])
 
 
 def global_alignment_distance_cells(a, b, weights):

@@ -66,10 +66,10 @@ def distinct_canonical(padded, k):
     return len({canonical(s[i:i + k]) for s in padded for i in range(len(s) - k + 1)})
 
 
-def predict(padded, k, n_distinct=None):
+def predict(padded, k, n_distinct=None, load=0.5):
     """-> dict(capacity, safe, estimate_cap, sampled, distinct, retry).  `padded`: the oracle's padded forward strands (oracle_lib.load_sequences);
-    `n_distinct`: distinct canonical k-mers if known (the oracle's n_kmers / 2), else counted here.  Raises when the input's load on the
-    estimated table lies in the band where the route is not certain."""
+    `n_distinct`: distinct canonical k-mers if known (the oracle's n_kmers / 2), else counted here; `load`: the table load the estimate is
+    sized for (AC_TABLE_LOAD).  Raises when the input's load on the estimated table lies in the band where the route is not certain."""
     n = sum(len(s) - (k - 1) for s in padded)
     safe = (n + n // 2 + 64 + 3) & ~3
     distinct = distinct_canonical(padded, k) if n_distinct is None else n_distinct
@@ -84,7 +84,7 @@ def predict(padded, k, n_distinct=None):
     if PROBE_LIMIT_LOAD[0] * sample_cap <= s:
         raise ValueError(f"sample table load {s / sample_cap:.3f}: whether the sizing pass overflows is not certain")
     est = (s + 3 * math.isqrt(s) + 16) * 64 + len(padded) * 2 * k
-    cap = min(safe, (2 * est + 4096 + 3) & ~3)
+    cap = min(safe, (int(est / load) + 4096 + 3) & ~3)             # (uint64_t)((double)est / load): est < 2^53, so est / 0.5 == 2 * est
     out["estimate_cap"] = cap
     if distinct > cap:
         out["retry"] = cap != safe
