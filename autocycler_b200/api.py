@@ -93,6 +93,22 @@ EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_seq
 _libs = {}
 
 
+def _raise_unless_ok(lib, rc):
+    """Raises the library's error for a call without a handle."""
+    if rc != AC_OK:
+        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+
+
+def _weight_list(weights):
+    """{unitig: length} or a list indexed by unitig number -> the list the C ABI takes."""
+    if not isinstance(weights, dict):
+        return list(weights)
+    w = [0] * (max(weights) + 1 if weights else 1)
+    for u, ln in weights.items():
+        w[u] = ln
+    return w
+
+
 def load_library(path=None):
     """Loads the C-ABI library (default: the in-tree CUDA build) and declares its prototypes."""
     path = os.path.abspath(path or DEFAULT_LIB)
@@ -204,9 +220,7 @@ class _Handle:
         self.ptr = C.c_void_p()
         devs = (C.c_int32 * len(devices))(*devices) if devices else None      # several GPUs driven by this one process (ac_config.n_devices)
         cfg = AcConfig(k, device, stream_handle(stream), 1 if keep_positions else 0, len(devices) if devices else 0, devs)
-        rc = lib.ac_create(C.byref(self.ptr), C.byref(cfg))
-        if rc != AC_OK:
-            raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+        _raise_unless_ok(lib, lib.ac_create(C.byref(self.ptr), C.byref(cfg)))
 
     def check(self, rc):
         if rc != AC_OK:
@@ -372,22 +386,21 @@ class UnitigGraph:
         self._h.check(self._h.lib.ac_pairwise_distances(self._h.ptr, buf, S * S))
         return [[buf[a * S + b] for b in range(S)] for a in range(S)]
 
-    def distance_matrix_text(self):   # cluster.rs:160-176
+    def _text(self, fn, *args):   # a two-call getter fn(handle, *args, out, cap, length): the length, then the text
         n = C.c_uint64()
-        self._h.check(self._h.lib.ac_distance_matrix_text(self._h.ptr, None, 0, C.byref(n)))
+        self._h.check(fn(self._h.ptr, *args, None, 0, C.byref(n)))
         buf = C.create_string_buffer(max(1, n.value))
-        self._h.check(self._h.lib.ac_distance_matrix_text(self._h.ptr, buf, n.value, C.byref(n)))
+        self._h.check(fn(self._h.ptr, *args, buf, n.value, C.byref(n)))
         return buf.raw[:n.value].decode()
+
+    def distance_matrix_text(self):   # cluster.rs:160-176
+        return self._text(self._h.lib.ac_distance_matrix_text)
 
     def renumber_unitigs(self):   # unitig_graph.rs:295-315
         self._h.check(self._h.lib.ac_renumber_unitigs(self._h.ptr))
 
     def reconstruct_original_sequence(self, index):   # unitig_graph.rs:383-388, by position in the sequence list
-        n = C.c_uint64()
-        self._h.check(self._h.lib.ac_sequence_reconstruct(self._h.ptr, index, None, 0, C.byref(n)))
-        buf = C.create_string_buffer(max(1, n.value))
-        self._h.check(self._h.lib.ac_sequence_reconstruct(self._h.ptr, index, buf, n.value, C.byref(n)))
-        return buf.raw[:n.value].decode()
+        return self._text(self._h.lib.ac_sequence_reconstruct, index)
 
     def trim(self, min_identity=0.75, max_unitigs=5000, mad=5.0):   # trim.rs:43-51 on this (loaded) graph
         """Start-end and hairpin trimming (alignments on the GPU), length outliers, clean-up: afterwards the graph and its sequences are
@@ -395,11 +408,7 @@ class UnitigGraph:
         self._h.check(self._h.lib.ac_trim(self._h.ptr, min_identity, max_unitigs, mad))
 
     def trimmed_yaml(self):   # TrimmedClusterMetrics (metrics.rs:209-225) after trim()
-        n = C.c_uint64()
-        self._h.check(self._h.lib.ac_trim_yaml(self._h.ptr, None, 0, C.byref(n)))
-        buf = C.create_string_buffer(max(1, n.value))
-        self._h.check(self._h.lib.ac_trim_yaml(self._h.ptr, buf, n.value, C.byref(n)))
-        return buf.raw[:n.value].decode()
+        return self._text(self._h.lib.ac_trim_yaml)
 
     def trim_stats(self):   # what the last trim aligned
         jobs, cells, path = C.c_uint64(), C.c_uint64(), C.c_uint64(); window = C.c_uint32()
@@ -416,12 +425,7 @@ class UnitigGraph:
     CLUSTER_TEXTS = {"phylip": 0, "newick": 1, "tsv": 2, "yaml": 3, "gfa": 4, "untrimmed_yaml": 5}
 
     def cluster_text(self, what, cluster=0):   # "phylip", "newick", "tsv", "yaml"; per cluster: "gfa", "untrimmed_yaml"
-        n = C.c_uint64()
-        w = self.CLUSTER_TEXTS[what]
-        self._h.check(self._h.lib.ac_cluster_text(self._h.ptr, w, cluster, None, 0, C.byref(n)))
-        buf = C.create_string_buffer(max(1, n.value))
-        self._h.check(self._h.lib.ac_cluster_text(self._h.ptr, w, cluster, buf, n.value, C.byref(n)))
-        return buf.raw[:n.value].decode()
+        return self._text(self._h.lib.ac_cluster_text, self.CLUSTER_TEXTS[what], cluster)
 
     def cluster_assignments(self, n_seqs):   # -> [(cluster number, passed QC)] per sequence
         cl = (C.c_uint16 * max(1, n_seqs))(); ps = (C.c_uint8 * max(1, n_seqs))()
@@ -442,12 +446,7 @@ class UnitigGraph:
     RESOLVE_TEXTS = {"bridged": 0, "merged": 1, "final": 2}
 
     def resolve_text(self, what):   # "bridged", "merged" or "final"
-        n = C.c_uint64()
-        w = self.RESOLVE_TEXTS[what]
-        self._h.check(self._h.lib.ac_resolve_text(self._h.ptr, w, None, 0, C.byref(n)))
-        buf = C.create_string_buffer(max(1, n.value))
-        self._h.check(self._h.lib.ac_resolve_text(self._h.ptr, w, buf, n.value, C.byref(n)))
-        return buf.raw[:n.value].decode()
+        return self._text(self._h.lib.ac_resolve_text, self.RESOLVE_TEXTS[what])
 
     def resolve_stats(self):
         info = AcResolveInfo()
@@ -465,9 +464,8 @@ def simplify_structure(graph, seqs=None):   # graph_simplification.rs:26-40
 
 def decompress(in_gfa, out_dir=None, out_file=None, lib=None, device=0):   # decompress.rs:27-38
     lib = lib or load_library()
-    rc = lib.ac_decompress_gfa(os.fsencode(in_gfa), os.fsencode(out_dir) if out_dir else None, os.fsencode(out_file) if out_file else None, device, 0)
-    if rc != AC_OK:
-        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+    _raise_unless_ok(lib, lib.ac_decompress_gfa(os.fsencode(in_gfa), os.fsencode(out_dir) if out_dir else None,
+                                                os.fsencode(out_file) if out_file else None, device, 0))
 
 
 def merge_linear_paths(graph, seqs=()):   # graph_simplification.rs:315-371; seqs=None/[] merges without regard to the paths
@@ -499,10 +497,8 @@ def compress(assemblies_dir, autocycler_dir, k_size=51, max_contigs=25, threads=
     """compress.rs:32-50: writes <autocycler_dir>/input_assemblies.gfa and .yaml.  devices=[...]: sharded by file over several GPUs."""
     lib = lib or load_library()
     devs = list(devices) if devices else [device]
-    rc = lib.ac_compress_dir_devices(os.fsencode(assemblies_dir), os.fsencode(autocycler_dir), k_size, max_contigs, threads,
-                                     (C.c_int32 * len(devs))(*devs), len(devs), 1 if verbose else 0)
-    if rc != AC_OK:
-        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+    _raise_unless_ok(lib, lib.ac_compress_dir_devices(os.fsencode(assemblies_dir), os.fsencode(autocycler_dir), k_size, max_contigs, threads,
+                                                      (C.c_int32 * len(devs))(*devs), len(devs), 1 if verbose else 0))
 
 
 TRIM_START_END, TRIM_HAIRPIN_START, TRIM_HAIRPIN_END = 0, 1, 2
@@ -513,12 +509,7 @@ def _trim_paths(mode, paths, weights, min_identity, max_unitigs, lib=None, devic
     by unitig number.  -> [trimmed path or None]"""
     lib = lib or load_library()
     h = handle or _Handle(lib, 51, device)
-    if isinstance(weights, dict):
-        w = [0] * (max(weights) + 1 if weights else 1)
-        for u, ln in weights.items():
-            w[u] = ln
-    else:
-        w = list(weights)
+    w = _weight_list(weights)
     flat = [u for p in paths for u in p]
     off = [0]
     for p in paths:
@@ -548,9 +539,7 @@ def trim_path_hairpin_end(paths, weights, min_identity, max_unitigs, **kw):    #
 def trim(cluster_dir, min_identity=0.75, max_unitigs=5000, mad=5.0, threads=8, device=0, verbose=False, lib=None):
     """trim.rs:36-53: reads <cluster_dir>/1_untrimmed.gfa, writes 2_trimmed.gfa and 2_trimmed.yaml."""
     lib = lib or load_library()
-    rc = lib.ac_trim_dir(os.fsencode(cluster_dir), float(min_identity), max_unitigs, float(mad), threads, device, 1 if verbose else 0)
-    if rc != AC_OK:
-        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+    _raise_unless_ok(lib, lib.ac_trim_dir(os.fsencode(cluster_dir), float(min_identity), max_unitigs, float(mad), threads, device, 1 if verbose else 0))
 
 
 def upgma(matrix, ids, lib=None, device=0, handle=None):
@@ -574,10 +563,8 @@ def upgma(matrix, ids, lib=None, device=0, handle=None):
 def cluster(autocycler_dir, cutoff=0.2, min_assemblies=None, max_contigs=25, manual=None, device=0, verbose=False, lib=None):
     """cluster.rs:30-64: reads <autocycler_dir>/input_assemblies.gfa and replaces <autocycler_dir>/clustering.  manual: "1,2,3"."""
     lib = lib or load_library()
-    rc = lib.ac_cluster_dir(os.fsencode(autocycler_dir), float(cutoff), -1 if min_assemblies is None else int(min_assemblies), max_contigs,
-                            manual.encode() if manual is not None else None, device, 1 if verbose else 0)
-    if rc != AC_OK:
-        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+    _raise_unless_ok(lib, lib.ac_cluster_dir(os.fsencode(autocycler_dir), float(cutoff), -1 if min_assemblies is None else int(min_assemblies), max_contigs,
+                                             manual.encode() if manual is not None else None, device, 1 if verbose else 0))
 
 
 def bridge_best_paths(groups, weights, lib=None, device=0, handle=None):
@@ -585,12 +572,7 @@ def bridge_best_paths(groups, weights, lib=None, device=0, handle=None):
     distances on the GPU; weights: {unitig: length} or a list indexed by unitig number.  -> ([[u32 total per path]], [best path])"""
     lib = lib or load_library()
     h = handle or _Handle(lib, 51, device)
-    if isinstance(weights, dict):
-        w = [0] * (max(weights) + 1 if weights else 1)
-        for u, ln in weights.items():
-            w[u] = ln
-    else:
-        w = list(weights)
+    w = _weight_list(weights)
     paths = [p for g in groups for p in g]
     flat = [u for p in paths for u in p]
     off, goff = [0], [0]
@@ -610,18 +592,14 @@ def bridge_best_paths(groups, weights, lib=None, device=0, handle=None):
 def resolve(cluster_dir, verbose=False, device=0, lib=None):
     """resolve.rs:31-69: reads <cluster_dir>/2_trimmed.gfa, writes 3_bridged.gfa, 4_merged.gfa and 5_final.gfa."""
     lib = lib or load_library()
-    rc = lib.ac_resolve_dir(os.fsencode(cluster_dir), 1 if verbose else 0, device)
-    if rc != AC_OK:
-        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+    _raise_unless_ok(lib, lib.ac_resolve_dir(os.fsencode(cluster_dir), 1 if verbose else 0, device))
 
 
 def combine(autocycler_dir, in_gfas, verbose=False, lib=None):
     """combine.rs:25-49: writes <autocycler_dir>/consensus_assembly.gfa, .fasta and .yaml from the GFAs in order."""
     lib = lib or load_library()
     names = [os.fsencode(g) for g in in_gfas]
-    rc = lib.ac_combine_dir(os.fsencode(autocycler_dir), (C.c_char_p * max(1, len(names)))(*names), len(names), 1 if verbose else 0)
-    if rc != AC_OK:
-        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+    _raise_unless_ok(lib, lib.ac_combine_dir(os.fsencode(autocycler_dir), (C.c_char_p * max(1, len(names)))(*names), len(names), 1 if verbose else 0))
 
 
 def _font_arg(font):
@@ -638,11 +616,9 @@ def dotplot_rgb(seqs, res=2000, kmer=32, font=None, device=0, lib=None):
     data = [bytes(s) if not isinstance(s, str) else s.encode() for _, _, s in seqs]
     img = np.empty((res, res, 3), dtype=np.uint8) if 500 <= res <= 10000 else np.empty((1, 1, 3), dtype=np.uint8)
     info = AcDotplotInfo()
-    rc = lib.ac_dotplot_rgb((C.c_char_p * max(1, n))(*data), (C.c_uint64 * max(1, n))(*[len(d) for d in data]),
-                            (C.c_char_p * max(1, n))(*[f.encode() for f, _, _ in seqs]), (C.c_char_p * max(1, n))(*[m.encode() for _, m, _ in seqs]),
-                            n, res, kmer, _font_arg(font), device, img.ctypes.data, C.byref(info))
-    if rc != AC_OK:
-        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+    _raise_unless_ok(lib, lib.ac_dotplot_rgb((C.c_char_p * max(1, n))(*data), (C.c_uint64 * max(1, n))(*[len(d) for d in data]),
+                                             (C.c_char_p * max(1, n))(*[f.encode() for f, _, _ in seqs]), (C.c_char_p * max(1, n))(*[m.encode() for _, m, _ in seqs]),
+                                             n, res, kmer, _font_arg(font), device, img.ctypes.data, C.byref(info)))
     return img, info.as_dict()
 
 
@@ -651,9 +627,7 @@ def dotplot(input, out_png, res=2000, kmer=32, font=None, device=0, verbose=Fals
     dotplot_rgb.  -> the info dict."""
     lib = lib or load_library()
     info = AcDotplotInfo()
-    rc = lib.ac_dotplot_dir(os.fsencode(input), os.fsencode(out_png), res, kmer, _font_arg(font), device, 1 if verbose else 0, C.byref(info))
-    if rc != AC_OK:
-        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+    _raise_unless_ok(lib, lib.ac_dotplot_dir(os.fsencode(input), os.fsencode(out_png), res, kmer, _font_arg(font), device, 1 if verbose else 0, C.byref(info)))
     return info.as_dict()
 
 
@@ -662,6 +636,4 @@ def png_write(path, rgb, lib=None):
     import numpy as np
     lib = lib or load_library()
     rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
-    rc = lib.ac_png_write(os.fsencode(path), rgb.ctypes.data, rgb.shape[1], rgb.shape[0])
-    if rc != AC_OK:
-        raise AutocyclerGpuError(rc, lib.ac_last_error(None).decode())
+    _raise_unless_ok(lib, lib.ac_png_write(os.fsencode(path), rgb.ctypes.data, rgb.shape[1], rgb.shape[0]))

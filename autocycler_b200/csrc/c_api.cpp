@@ -15,6 +15,7 @@
 #include <memory>
 #include <set>
 #include <string>
+#include <string_view>
 #include <vector>
 
 #include "backend.h"
@@ -90,6 +91,93 @@ static int ok(const ac_handle* h) {      // a call that succeeded leaves no stal
     g_error.clear();
     return AC_OK;
 }
+
+// ---- what the commands (the ac_*_dir calls) and the getters share ----
+namespace {
+int check_dir(const std::string& path) {        // check_if_dir_exists (misc.rs:110-119)
+    struct stat st;
+    if (stat(path.c_str(), &st) != 0) return set_error(nullptr, AC_EINPUT, "directory does not exist: " + path);
+    if (!S_ISDIR(st.st_mode)) return set_error(nullptr, AC_EINPUT, path + " is not a directory");
+    return AC_OK;
+}
+int check_file(const std::string& path) {       // check_if_file_exists (misc.rs:98-107)
+    struct stat st;
+    if (stat(path.c_str(), &st) != 0) return set_error(nullptr, AC_EINPUT, "file does not exist: " + path);
+    if (!S_ISREG(st.st_mode)) return set_error(nullptr, AC_EINPUT, path + " is not a file");
+    return AC_OK;
+}
+int read_file(const std::string& path, std::string& text) {
+    FILE* f = fopen(path.c_str(), "rb");
+    if (!f) return set_error(nullptr, AC_EIO, "cannot read " + path);
+    char buf[1 << 16]; size_t n;
+    text.clear();
+    while ((n = fread(buf, 1, sizeof buf, f)) > 0) text.append(buf, n);
+    const bool good = !ferror(f);
+    fclose(f);
+    return good ? AC_OK : set_error(nullptr, AC_EIO, "cannot read " + path);
+}
+bool write_file(const std::string& path, std::string_view text) {      // false when the file cannot be opened, written or closed
+    FILE* f = fopen(path.c_str(), "wb");
+    if (!f) return false;
+    const bool good = fwrite(text.data(), 1, text.size(), f) == text.size();
+    return fclose(f) == 0 && good;
+}
+bool make_dirs(const std::string& path) {       // create_dir_all
+    struct stat st;
+    if (path.empty() || stat(path.c_str(), &st) == 0) return path.empty() || S_ISDIR(st.st_mode);
+    const size_t slash = path.find_last_of('/', path.size() > 1 ? path.size() - 2 : 0);
+    if (slash != std::string::npos && slash > 0 && !make_dirs(path.substr(0, slash))) return false;
+    return mkdir(path.c_str(), 0777) == 0 || (stat(path.c_str(), &st) == 0 && S_ISDIR(st.st_mode));
+}
+int remove_tree(const std::string& path) {       // everything under a directory, and the directory
+    struct stat st;
+    if (lstat(path.c_str(), &st) != 0) return 0;
+    if (S_ISDIR(st.st_mode)) {
+        DIR* d = opendir(path.c_str());
+        if (!d) return -1;
+        std::vector<std::string> names;
+        while (dirent* e = readdir(d)) { const std::string n = e->d_name; if (n != "." && n != "..") names.push_back(n); }
+        closedir(d);
+        for (auto& n : names) if (remove_tree(path + "/" + n) != 0) return -1;
+        return rmdir(path.c_str());
+    }
+    return unlink(path.c_str());
+}
+
+struct HandleDeleter { void operator()(ac_handle* h) const { ac_destroy(h); } };
+using Handle = std::unique_ptr<ac_handle, HandleDeleter>;
+int make_handle(int32_t device, Handle& h) {     // the handle a command makes for one device; a loaded GFA replaces its k
+    ac_config cfg{}; cfg.k = 51; cfg.device = device;
+    ac_handle* p = nullptr;
+    const int rc = ac_create(&p, &cfg);
+    h.reset(p);
+    return rc;
+}
+int load_input_gfa(ac_handle* h, const std::string& text) {      // a malformed input GFA is one of the reference's input errors
+    const int rc = ac_load_gfa(h, text.data(), text.size());
+    return rc == AC_EINVAL ? AC_EINPUT : rc;
+}
+
+// A text getter: `out` NULL asks for the length only; otherwise the text is copied when `cap` holds it
+int copy_text(const ac_handle* h, const std::string& text, char* out, uint64_t cap, uint64_t* length) {
+    *length = text.size();
+    if (!out) return ok(h);
+    if (cap < text.size()) return set_error(h, AC_ERANGE, "buffer too small");
+    memcpy(out, text.data(), text.size());
+    return ok(h);
+}
+
+// Path x of the caller paths of ac_trim_paths / ac_bridge_best_paths: its offsets must not decrease, and every entry needs a weight
+int check_path(const ac_handle* h, const int32_t* paths, const uint64_t* path_off, uint64_t x, uint64_t n_weights) {
+    if (path_off[x + 1] < path_off[x]) return set_error(h, AC_EINVAL, "path offsets must not decrease");
+    for (uint64_t i = path_off[x]; i < path_off[x + 1]; ++i) {
+        const int32_t u = paths[i];
+        const int64_t a = u < 0 ? -(int64_t)u : u;
+        if (u == 0 || (uint64_t)a >= n_weights) return set_error(h, AC_EINVAL, "path entry " + std::to_string(u) + " has no weight");
+    }
+    return AC_OK;
+}
+}  // namespace
 
 #define AC_GUARD_BEGIN try {
 #define AC_GUARD_END(h) } catch (const InputError& e) { return set_error(h, AC_EINPUT, e.msg); } \
@@ -325,20 +413,37 @@ static void ensure_graph(const ac_handle* ch) {
     adopt_result(h);                         // simplified and renumbered on the device: the graph is taken as it is
 }
 
+// What ac_build, ac_build_finish, ac_compress and ac_compress_finish share around their device work.  A plain build adopts the result
+// on the host; a fused one (simplified and written as GFA text on the device) takes only the text and the counts.
+static void build_graph(ac_handle* h, bool fused, const std::function<void()>& device_work) {
+    ResultFlusher flusher;
+    // a fused build's graph arrays are only ever written by the host once they were fetched
+    if (h->built && (!fused || h->graph_ready)) flusher.start(h->res);
+    {
+        CallbackScope scope(h->pipe.get(), [&flusher] { flusher.join(); });      // cleared again on every way out, exceptions included
+        device_work();
+    }
+    if (fused) {
+        h->pipe->complete(h->res);
+        h->fused = true; h->graph_ready = false; h->built = true;
+        h->gfa_ptr = h->res.gfa_text; h->gfa_len = h->res.gfa_bytes; h->gfa_ready = true;
+        record_timings(h);
+        h->t.host_graph = h->t.host_simplify = h->t.host_gfa = 0;
+    } else {
+        h->fused = false; h->graph_ready = false;
+        adopt_result(h);
+        h->built = true; h->gfa_ready = false;
+    }
+}
+
 int ac_build(ac_handle* h) {
     if (!h) return set_error(nullptr, AC_EINVAL, "null handle");
     AC_GUARD_BEGIN
     if (!h->uploaded) return set_error(h, AC_EINVAL, "ac_upload must precede ac_build");
-    ResultFlusher flusher;
-    if (h->built) flusher.start(h->res);
-    {
-        CallbackScope scope(h->pipe.get(), [&flusher] { flusher.join(); });      // cleared again on every way out, exceptions included
-        if (h->peers.empty()) h->pipe->build(h->res, h->cfg.keep_positions != 0);
+    build_graph(h, false, [h] {
+        if (h->peers.empty()) h->pipe->build(h->res, h->cfg.keep_positions != 0, false);
         else build_on_devices(h, false);
-    }
-    h->fused = false; h->graph_ready = false;
-    adopt_result(h);
-    h->built = true; h->gfa_ready = false;
+    });
     return ok(h);
     AC_GUARD_END(h)
 }
@@ -349,18 +454,10 @@ int ac_compress(ac_handle* h) {
     if (!h) return set_error(nullptr, AC_EINVAL, "null handle");
     AC_GUARD_BEGIN
     if (!h->uploaded) return set_error(h, AC_EINVAL, "ac_upload must precede ac_compress");
-    ResultFlusher flusher;
-    if (h->built && h->graph_ready) flusher.start(h->res);                     // the host only ever writes to the graph arrays, and only once they were fetched
-    {
-        CallbackScope scope(h->pipe.get(), [&flusher] { flusher.join(); });
+    build_graph(h, true, [h] {
         if (h->peers.empty()) h->pipe->build(h->res, h->cfg.keep_positions != 0, true);
         else build_on_devices(h, true);
-    }
-    h->pipe->complete(h->res);
-    h->fused = true; h->graph_ready = false; h->built = true;
-    h->gfa_ptr = h->res.gfa_text; h->gfa_len = h->res.gfa_bytes; h->gfa_ready = true;
-    record_timings(h);
-    h->t.host_graph = h->t.host_simplify = h->t.host_gfa = 0;
+    });
     return ok(h);
     AC_GUARD_END(h)
 }
@@ -429,17 +526,7 @@ int ac_runs_import_padded(ac_handle* h, const void* src, uint64_t stride_records
 static int compress_finish(ac_handle* h, bool split_paths) {
     if (!h) return set_error(nullptr, AC_EINVAL, "null handle");
     AC_GUARD_BEGIN
-    ResultFlusher flusher;
-    if (h->built && h->graph_ready) flusher.start(h->res);
-    {
-        CallbackScope scope(h->pipe.get(), [&flusher] { flusher.join(); });
-        h->pipe->finish(h->res, h->cfg.keep_positions != 0, true, split_paths);
-    }
-    h->pipe->complete(h->res);
-    h->fused = true; h->graph_ready = false; h->built = true;
-    h->gfa_ptr = h->res.gfa_text; h->gfa_len = h->res.gfa_bytes; h->gfa_ready = true;
-    record_timings(h);
-    h->t.host_graph = h->t.host_simplify = h->t.host_gfa = 0;
+    build_graph(h, true, [h, split_paths] { h->pipe->finish(h->res, h->cfg.keep_positions != 0, true, split_paths); });
     return ok(h);
     AC_GUARD_END(h)
 }
@@ -468,15 +555,7 @@ int ac_path_lines_data(ac_handle* h, const char** data, uint64_t* n_bytes) {
 int ac_build_finish(ac_handle* h) {
     if (!h) return set_error(nullptr, AC_EINVAL, "null handle");
     AC_GUARD_BEGIN
-    ResultFlusher flusher;
-    if (h->built) flusher.start(h->res);
-    {
-        CallbackScope scope(h->pipe.get(), [&flusher] { flusher.join(); });
-        h->pipe->finish(h->res, h->cfg.keep_positions != 0);
-    }
-    h->fused = false; h->graph_ready = false;
-    adopt_result(h);
-    h->built = true; h->gfa_ready = false;
+    build_graph(h, false, [h] { h->pipe->finish(h->res, h->cfg.keep_positions != 0); });
     return ok(h);
     AC_GUARD_END(h)
 }
@@ -592,12 +671,7 @@ int ac_distance_matrix_text(ac_handle* h, char* out, uint64_t cap, uint64_t* len
     std::vector<double> d(std::max<uint64_t>(1, S * S));
     const int rc = ac_pairwise_distances(h, d.data(), S * S);
     if (rc != AC_OK) return rc;
-    const std::string text = distance_matrix_text(h->seqs, d.data());
-    *length = text.size();
-    if (!out) return ok(h);
-    if (cap < text.size()) return set_error(h, AC_ERANGE, "buffer too small");
-    memcpy(out, text.data(), text.size());
-    return ok(h);
+    return copy_text(h, distance_matrix_text(h->seqs, d.data()), out, cap, length);
     AC_GUARD_END(h)
 }
 
@@ -810,12 +884,11 @@ int ac_compress_dir(const char* assemblies_dir, const char* autocycler_dir, uint
 int ac_compress_dir_devices(const char* assemblies_dir, const char* autocycler_dir, uint32_t k, uint32_t max_contigs, uint32_t threads,
                             const int32_t* devices, int32_t n_devices, int32_t verbose) {
     if (!assemblies_dir || !autocycler_dir || !devices || n_devices < 1) return set_error(nullptr, AC_EINVAL, "null argument");
-    ac_handle* h = nullptr;
     AC_GUARD_BEGIN
     // check_settings, compress.rs:53-62
+    int rc = check_dir(assemblies_dir);
+    if (rc != AC_OK) return rc;
     struct stat st;
-    if (stat(assemblies_dir, &st) != 0) return set_error(nullptr, AC_EINPUT, std::string("directory does not exist: ") + assemblies_dir);
-    if (!S_ISDIR(st.st_mode)) return set_error(nullptr, AC_EINPUT, std::string(assemblies_dir) + " is not a directory");
     if (stat(autocycler_dir, &st) == 0 && !S_ISDIR(st.st_mode)) return set_error(nullptr, AC_EINPUT, std::string(autocycler_dir) + " exists but is not a directory");
     if (k < 11) return set_error(nullptr, AC_EINPUT, "--kmer cannot be less than 11");
     if (k > 501) return set_error(nullptr, AC_EINPUT, "--kmer cannot be greater than 501");
@@ -824,19 +897,19 @@ int ac_compress_dir_devices(const char* assemblies_dir, const char* autocycler_d
     if (threads > 100) return set_error(nullptr, AC_EINPUT, "--threads cannot be greater than 100");
     if (k > AC_MAX_K) return set_error(nullptr, AC_EINPUT, "--kmer above " + std::to_string(AC_MAX_K) + " is not supported by this build of the GPU path (there is no CPU fallback)");
     ac_config cfg{}; cfg.k = k; cfg.device = devices[0]; cfg.stream = nullptr; cfg.keep_positions = 0; cfg.n_devices = n_devices; cfg.devices = devices;
-    int rc = ac_create(&h, &cfg);
-    if (rc != AC_OK) return rc;
-    std::unique_ptr<ac_handle, void (*)(ac_handle*)> guard(h, ac_destroy);
-    { std::string d = autocycler_dir; for (size_t i = 1; i <= d.size(); ++i) if (i == d.size() || d[i] == '/') mkdir(d.substr(0, i).c_str(), 0777); }   // create_dir_all
+    ac_handle* p = nullptr;
+    if ((rc = ac_create(&p, &cfg)) != AC_OK) return rc;
+    Handle h(p);
+    make_dirs(autocycler_dir);           // a directory that cannot be made shows as "cannot write" below
     uint64_t assemblies = 0;
     const double t0 = now_ms();
-    if ((rc = ac_load_sequences(h, assemblies_dir, max_contigs, threads, &assemblies)) != AC_OK) { g_error = h->err; return rc; }
+    if ((rc = ac_load_sequences(h.get(), assemblies_dir, max_contigs, threads, &assemblies)) != AC_OK) return rc;
     const double t1 = now_ms();
     if (verbose) fprintf(stderr, "%zu sequence%s loaded from %llu assembl%s\n\n", h->seqs.size(), h->seqs.size() == 1 ? "" : "s",
                          (unsigned long long)assemblies, assemblies == 1 ? "y" : "ies");
-    if ((rc = ac_upload(h)) != AC_OK || (rc = ac_compress(h)) != AC_OK) { g_error = h->err; return rc; }
+    if ((rc = ac_upload(h.get())) != AC_OK || (rc = ac_compress(h.get())) != AC_OK) return rc;
     ac_counts c{};
-    ac_counts_get(h, &c);
+    ac_counts_get(h.get(), &c);
     // simplify_structure moves bases between unitigs: the counts stay, the total length shrinks (print_basic_graph_info, unitig_graph.rs:509-516)
     if (verbose) fprintf(stderr, "Graph contains %llu k-mers\n\n%llu unitig%s, %llu link%s\ntotal length: %llu bp\n\n", (unsigned long long)c.n_kmers,
                          (unsigned long long)c.n_unitigs, c.n_unitigs == 1 ? "" : "s", (unsigned long long)c.n_links, c.n_links == 1 ? "" : "s",
@@ -844,15 +917,10 @@ int ac_compress_dir_devices(const char* assemblies_dir, const char* autocycler_d
     if (verbose) fprintf(stderr, "%llu unitig%s, %llu link%s\ntotal length: %llu bp\n\n", (unsigned long long)c.n_unitigs, c.n_unitigs == 1 ? "" : "s",
                          (unsigned long long)c.n_links, c.n_links == 1 ? "" : "s", (unsigned long long)c.total_length);
     uint64_t n = 0;
-    if ((rc = ac_gfa_size(h, &n)) != AC_OK) { g_error = h->err; return rc; }
+    if ((rc = ac_gfa_size(h.get(), &n)) != AC_OK) return rc;
     const std::string out_gfa = std::string(autocycler_dir) + "/input_assemblies.gfa", out_yaml = std::string(autocycler_dir) + "/input_assemblies.yaml";
-    FILE* f = fopen(out_gfa.c_str(), "wb");
-    if (!f || fwrite(h->gfa_ptr, 1, h->gfa_len, f) != h->gfa_len) { if (f) fclose(f); return set_error(nullptr, AC_EIO, "cannot write " + out_gfa); }
-    fclose(f);
-    const std::string yaml = metrics_yaml(h->loaded, c.n_unitigs, c.total_length);
-    f = fopen(out_yaml.c_str(), "wb");
-    if (!f || fwrite(yaml.data(), 1, yaml.size(), f) != yaml.size()) { if (f) fclose(f); return set_error(nullptr, AC_EIO, "cannot write " + out_yaml); }
-    fclose(f);
+    if (!write_file(out_gfa, std::string_view(h->gfa_ptr, h->gfa_len))) return set_error(nullptr, AC_EIO, "cannot write " + out_gfa);
+    if (!write_file(out_yaml, metrics_yaml(h->loaded, c.n_unitigs, c.total_length))) return set_error(nullptr, AC_EIO, "cannot write " + out_yaml);
     if (verbose) {
         const ac_timings& t = h->t;
         fprintf(stderr, "Compressed unitig graph: %s\nInput assembly stats:    %s\n", out_gfa.c_str(), out_yaml.c_str());
@@ -860,7 +928,7 @@ int ac_compress_dir_devices(const char* assemblies_dir, const char* autocycler_d
                         " simplify %.2f gfa %.2f | host graph %.1f simplify %.1f gfa %.1f ms | total %.1f ms\n\n",
                 t1 - t0, t.h2d, t.pack, t.insert, t.adjacency, t.boundaries, t.runs, t.unitigs, t.links, t.d2h, t.device_simplify, t.device_gfa, t.host_graph, t.host_simplify, t.host_gfa, now_ms() - t0);
     }
-    return ok(h);
+    return ok(h.get());
     AC_GUARD_END(nullptr)
 }
 
@@ -868,30 +936,17 @@ int ac_compress_dir_devices(const char* assemblies_dir, const char* autocycler_d
 // original file (FASTA, gzip when the name ends in .gz) and/or into one FASTA file.
 int ac_decompress_gfa(const char* in_gfa, const char* out_dir, const char* out_file, int32_t device, int32_t verbose) {
     if (!in_gfa) return set_error(nullptr, AC_EINVAL, "null argument");
-    ac_handle* h = nullptr;
     AC_GUARD_BEGIN
+    int rc = check_file(in_gfa);
+    if (rc != AC_OK) return rc;
     struct stat st;
-    if (stat(in_gfa, &st) != 0) return set_error(nullptr, AC_EINPUT, std::string("file does not exist: ") + in_gfa);            // misc.rs:98-107
-    if (!S_ISREG(st.st_mode)) return set_error(nullptr, AC_EINPUT, std::string(in_gfa) + " is not a file");
     const bool to_dir = out_dir && *out_dir, to_file = out_file && *out_file;
     if (!to_dir && !to_file) return set_error(nullptr, AC_EINPUT, "either --out_dir or --out_file is required");                  // decompress.rs:45-47
     if (to_dir && stat(out_dir, &st) == 0 && !S_ISDIR(st.st_mode)) return set_error(nullptr, AC_EINPUT, std::string(out_dir) + " exists but is not a directory");
-    std::string text;
-    {
-        FILE* f = fopen(in_gfa, "rb");
-        if (!f) return set_error(nullptr, AC_EIO, std::string("cannot read ") + in_gfa);
-        text.resize((size_t)st.st_size);
-        const size_t got = text.empty() ? 0 : fread(&text[0], 1, text.size(), f);
-        fclose(f);
-        if (got != text.size()) return set_error(nullptr, AC_EIO, std::string("cannot read ") + in_gfa);
-    }
-    ac_config cfg{}; cfg.k = 51; cfg.device = device;
-    int rc = ac_create(&h, &cfg);
-    if (rc != AC_OK) return rc;
-    std::unique_ptr<ac_handle, void (*)(ac_handle*)> guard(h, ac_destroy);
-    if ((rc = ac_load_gfa(h, text.data(), text.size())) != AC_OK) { g_error = h->err; return rc; }
+    std::string text; Handle h;
+    if ((rc = read_file(in_gfa, text)) != AC_OK || (rc = make_handle(device, h)) != AC_OK || (rc = load_input_gfa(h.get(), text)) != AC_OK) return rc;
     if (verbose) {
-        ac_counts c{}; ac_counts_get(h, &c);
+        ac_counts c{}; ac_counts_get(h.get(), &c);
         fprintf(stderr, "%llu unitig%s, %llu link%s\ntotal length: %llu bp\n\n", (unsigned long long)c.n_unitigs, c.n_unitigs == 1 ? "" : "s",
                 (unsigned long long)c.n_links, c.n_links == 1 ? "" : "s", (unsigned long long)c.total_length);
     }
@@ -899,17 +954,17 @@ int ac_decompress_gfa(const char* in_gfa, const char* out_dir, const char* out_f
     std::vector<std::string> seqs(h->seqs.size());
     for (size_t i = 0; i < h->seqs.size(); ++i) {
         uint64_t n = 0;
-        if ((rc = ac_sequence_reconstruct(h, i, nullptr, 0, &n)) != AC_OK) { g_error = h->err; return rc; }
+        if ((rc = ac_sequence_reconstruct(h.get(), i, nullptr, 0, &n)) != AC_OK) return rc;
         if (n != h->seqs[i].length) return set_error(nullptr, AC_EINPUT, "reconstructed sequence does not have expected length");   // unitig_graph.rs:386
         seqs[i].resize(n);
-        if (n && (rc = ac_sequence_reconstruct(h, i, &seqs[i][0], n, &n)) != AC_OK) { g_error = h->err; return rc; }
+        if (n && (rc = ac_sequence_reconstruct(h.get(), i, &seqs[i][0], n, &n)) != AC_OK) return rc;
     }
     std::vector<std::string> names;
     for (auto& s : h->seqs) names.push_back(s.filename);
     std::sort(names.begin(), names.end()); names.erase(std::unique(names.begin(), names.end()), names.end());
     auto first_word = [](const std::string& hd) { return hd.substr(0, hd.find(' ')); };
     if (to_dir) {
-        { std::string d = out_dir; for (size_t i = 1; i <= d.size(); ++i) if (i == d.size() || d[i] == '/') mkdir(d.substr(0, i).c_str(), 0777); }
+        make_dirs(out_dir);              // as in compress: a failure shows as "cannot write"
         for (const std::string& name : names) {
             const std::string path = std::string(out_dir) + "/" + name;
             if (verbose) fprintf(stderr, "%s:\n", path.c_str());
@@ -924,10 +979,8 @@ int ac_decompress_gfa(const char* in_gfa, const char* out_dir, const char* out_f
                 gzFile g = gzopen(path.c_str(), "wb");
                 if (!g || (body.size() && gzwrite(g, body.data(), (unsigned)body.size()) != (int)body.size())) { if (g) gzclose(g); return set_error(nullptr, AC_EIO, "cannot write " + path); }
                 gzclose(g);
-            } else {
-                FILE* f = fopen(path.c_str(), "wb");
-                if (!f || fwrite(body.data(), 1, body.size(), f) != body.size()) { if (f) fclose(f); return set_error(nullptr, AC_EIO, "cannot write " + path); }
-                fclose(f);
+            } else if (!write_file(path, body)) {
+                return set_error(nullptr, AC_EIO, "cannot write " + path);
             }
             if (verbose) fprintf(stderr, "\n");
         }
@@ -943,12 +996,10 @@ int ac_decompress_gfa(const char* in_gfa, const char* out_dir, const char* out_f
                     body += ">" + clean + "__" + h->seqs[i].contig_header + "\n" + seqs[i] + "\n";
                 }
         }
-        FILE* f = fopen(out_file, "wb");
-        if (!f || fwrite(body.data(), 1, body.size(), f) != body.size()) { if (f) fclose(f); return set_error(nullptr, AC_EIO, std::string("cannot write ") + out_file); }
-        fclose(f);
+        if (!write_file(out_file, body)) return set_error(nullptr, AC_EIO, std::string("cannot write ") + out_file);
         if (verbose) fprintf(stderr, "\n");
     }
-    return ok(h);
+    return ok(h.get());
     AC_GUARD_END(nullptr)
 }
 
@@ -961,12 +1012,9 @@ int ac_trim_paths(ac_handle* h, int32_t mode, const int32_t* paths, const uint64
     if (mode != AC_TRIM_START_END && mode != AC_TRIM_HAIRPIN_START && mode != AC_TRIM_HAIRPIN_END) return set_error(h, AC_EINVAL, "unknown trim mode");
     std::vector<std::vector<int32_t>> in(n_paths), res;
     for (uint64_t x = 0; x < n_paths; ++x) {
-        if (path_off[x + 1] < path_off[x]) return set_error(h, AC_EINVAL, "path offsets must not decrease");
+        const int rc = check_path(h, paths, path_off, x, n_weights);
+        if (rc != AC_OK) return rc;
         in[x].assign(paths + path_off[x], paths + path_off[x + 1]);
-        for (int32_t u : in[x]) {
-            const int64_t a = u < 0 ? -(int64_t)u : u;
-            if (u == 0 || (uint64_t)a >= n_weights) return set_error(h, AC_EINVAL, "path entry " + std::to_string(u) + " has no weight");
-        }
     }
     std::vector<uint32_t> w(weights, weights + n_weights);
     std::vector<uint8_t> ok_flags;
@@ -1002,11 +1050,7 @@ int ac_trim(ac_handle* h, double min_identity, uint32_t max_unitigs, double mad)
 int ac_trim_yaml(ac_handle* h, char* out, uint64_t cap, uint64_t* length) {
     if (!h || !length) return set_error(h, AC_EINVAL, "null argument");
     if (!h->trimmed) return set_error(h, AC_EINVAL, "ac_trim must precede ac_trim_yaml");
-    *length = h->trim_yaml.size();
-    if (!out) return ok(h);
-    if (cap < h->trim_yaml.size()) return set_error(h, AC_ERANGE, "buffer too small");
-    memcpy(out, h->trim_yaml.data(), h->trim_yaml.size());
-    return ok(h);
+    return copy_text(h, h->trim_yaml, out, cap, length);
 }
 
 int ac_trim_stats(const ac_handle* h, uint64_t* jobs, uint64_t* cells, uint32_t* max_window, uint64_t* max_path) {
@@ -1020,46 +1064,26 @@ int ac_trim_stats(const ac_handle* h, uint64_t* jobs, uint64_t* cells, uint32_t*
 
 int ac_trim_dir(const char* cluster_dir, double min_identity, uint32_t max_unitigs, double mad, uint32_t threads, int32_t device, int32_t verbose) {
     if (!cluster_dir) return set_error(nullptr, AC_EINVAL, "null argument");
-    ac_handle* h = nullptr;
     AC_GUARD_BEGIN
     // check_settings, trim.rs:56-67 (misc.rs:98-119)
     const std::string dir = cluster_dir, in_gfa = dir + "/1_untrimmed.gfa", out_gfa = dir + "/2_trimmed.gfa", out_yaml = dir + "/2_trimmed.yaml";
-    struct stat st;
-    if (stat(cluster_dir, &st) != 0) return set_error(nullptr, AC_EINPUT, "directory does not exist: " + dir);
-    if (!S_ISDIR(st.st_mode)) return set_error(nullptr, AC_EINPUT, dir + " is not a directory");
-    if (stat(in_gfa.c_str(), &st) != 0) return set_error(nullptr, AC_EINPUT, "file does not exist: " + in_gfa);
-    if (!S_ISREG(st.st_mode)) return set_error(nullptr, AC_EINPUT, in_gfa + " is not a file");
+    int rc;
+    if ((rc = check_dir(dir)) != AC_OK || (rc = check_file(in_gfa)) != AC_OK) return rc;
     if (!(min_identity >= 0.0 && min_identity <= 1.0)) return set_error(nullptr, AC_EINPUT, "--min_identity must be between 0.0 and 1 (inclusive)");
     if (threads < 1) return set_error(nullptr, AC_EINPUT, "--threads cannot be less than 1");
     if (threads > 100) return set_error(nullptr, AC_EINPUT, "--threads cannot be greater than 100");
     if (mad < 0.0) return set_error(nullptr, AC_EINPUT, "--mad cannot be less than 0");
-    std::string text;
-    {
-        FILE* f = fopen(in_gfa.c_str(), "rb");
-        if (!f) return set_error(nullptr, AC_EIO, "cannot read " + in_gfa);
-        char buf[1 << 16]; size_t n;
-        while ((n = fread(buf, 1, sizeof buf, f)) > 0) text.append(buf, n);
-        fclose(f);
-    }
-    ac_config cfg{}; cfg.k = 51; cfg.device = device; cfg.stream = nullptr; cfg.keep_positions = 0; cfg.n_devices = 1; cfg.devices = nullptr;
-    int rc = ac_create(&h, &cfg);
-    if (rc != AC_OK) return rc;
-    std::unique_ptr<ac_handle, void (*)(ac_handle*)> guard(h, ac_destroy);
-    if ((rc = ac_load_gfa(h, text.data(), text.size())) != AC_OK) { g_error = h->err; return rc == AC_EINVAL ? AC_EINPUT : rc; }
+    std::string text; Handle h;
+    if ((rc = read_file(in_gfa, text)) != AC_OK || (rc = make_handle(device, h)) != AC_OK || (rc = load_input_gfa(h.get(), text)) != AC_OK) return rc;
     if (verbose && max_unitigs == 0) fprintf(stderr, "Since --max_unitigs was set to 0, trimming is disabled.\n\n");
     TrimStats ts;
     trim_graph(h->graph, h->seqs, *h->pipe, min_identity, max_unitigs, mad, verbose != 0, ts);
     h->graph.gfa_text(h->seqs, h->gfa);
-    FILE* f = fopen(out_gfa.c_str(), "wb");
-    if (!f || fwrite(h->gfa.data(), 1, h->gfa.size(), f) != h->gfa.size()) { if (f) fclose(f); return set_error(nullptr, AC_EIO, "cannot write " + out_gfa); }
-    fclose(f);
-    const std::string yaml = trimmed_metrics_yaml(h->seqs);
-    f = fopen(out_yaml.c_str(), "wb");
-    if (!f || fwrite(yaml.data(), 1, yaml.size(), f) != yaml.size()) { if (f) fclose(f); return set_error(nullptr, AC_EIO, "cannot write " + out_yaml); }
-    fclose(f);
+    if (!write_file(out_gfa, h->gfa)) return set_error(nullptr, AC_EIO, "cannot write " + out_gfa);
+    if (!write_file(out_yaml, trimmed_metrics_yaml(h->seqs))) return set_error(nullptr, AC_EIO, "cannot write " + out_yaml);
     if (verbose) fprintf(stderr, "\nFinished!\nUnitig graph of trimmed sequences: %s\n(%llu alignments, %llu DP cells, alignment kernels %.2f ms)\n\n", out_gfa.c_str(),
                          (unsigned long long)ts.jobs, (unsigned long long)ts.cells, (double)ts.kernel_ms);
-    return ok(h);
+    return ok(h.get());
     AC_GUARD_END(nullptr)
 }
 
@@ -1108,11 +1132,7 @@ int ac_cluster_text(ac_handle* h, int32_t what, uint32_t cluster, char* out, uin
                            what == AC_CLUSTER_YAML ? &r.yaml : what == AC_CLUSTER_GFA ? &r.cluster_gfa[cluster - 1] :
                            what == AC_CLUSTER_UNTRIMMED_YAML ? &r.cluster_yaml[cluster - 1] : nullptr;
     if (!t) return set_error(h, AC_EINVAL, "unknown cluster text");
-    *length = t->size();
-    if (!out) return ok(h);
-    if (cap < t->size()) return set_error(h, AC_ERANGE, "buffer too small");
-    memcpy(out, t->data(), t->size());
-    return ok(h);
+    return copy_text(h, *t, out, cap, length);
 }
 
 int ac_cluster_assignments(const ac_handle* h, uint16_t* cluster, uint8_t* pass, uint64_t cap) {
@@ -1136,65 +1156,28 @@ int ac_cluster_stats(const ac_handle* h, uint32_t* n_seqs, uint32_t* pass_cluste
     return ok(h);
 }
 
-namespace {
-bool write_file(const std::string& path, const std::string& text) {
-    FILE* f = fopen(path.c_str(), "wb");
-    if (!f) return false;
-    const bool good = fwrite(text.data(), 1, text.size(), f) == text.size();
-    return fclose(f) == 0 && good;
-}
-int remove_tree(const std::string& path) {       // everything under a directory, and the directory
-    struct stat st;
-    if (lstat(path.c_str(), &st) != 0) return 0;
-    if (S_ISDIR(st.st_mode)) {
-        DIR* d = opendir(path.c_str());
-        if (!d) return -1;
-        std::vector<std::string> names;
-        while (dirent* e = readdir(d)) { const std::string n = e->d_name; if (n != "." && n != "..") names.push_back(n); }
-        closedir(d);
-        for (auto& n : names) if (remove_tree(path + "/" + n) != 0) return -1;
-        return rmdir(path.c_str());
-    }
-    return unlink(path.c_str());
-}
-}  // namespace
-
 int ac_cluster_dir(const char* autocycler_dir, double cutoff, int64_t min_assemblies, uint32_t max_contigs, const char* manual, int32_t device, int32_t verbose) {
     if (!autocycler_dir) return set_error(nullptr, AC_EINVAL, "null argument");
-    ac_handle* h = nullptr;
     AC_GUARD_BEGIN
     // check_settings (cluster.rs:67-76)
     const std::string dir = autocycler_dir, gfa = dir + "/input_assemblies.gfa", cdir = dir + "/clustering";
-    struct stat st;
-    if (stat(autocycler_dir, &st) != 0) return set_error(nullptr, AC_EINPUT, "directory does not exist: " + dir);
-    if (!S_ISDIR(st.st_mode)) return set_error(nullptr, AC_EINPUT, dir + " is not a directory");
-    if (stat(gfa.c_str(), &st) != 0) return set_error(nullptr, AC_EINPUT, "file does not exist: " + gfa);
-    if (!S_ISREG(st.st_mode)) return set_error(nullptr, AC_EINPUT, gfa + " is not a file");
+    int rc;
+    if ((rc = check_dir(dir)) != AC_OK || (rc = check_file(gfa)) != AC_OK) return rc;
     if (cutoff <= 0.0 || cutoff >= 1.0) return set_error(nullptr, AC_EINPUT, "--cutoff must be between 0 and 1 (exclusive)");
     if (min_assemblies == 0) return set_error(nullptr, AC_EINPUT, "--min_assemblies must be 1 or greater");
     // delete_dir_if_exists (misc.rs:41-48): only a directory (or a link to one, which goes itself) is removed; anything else makes
     // create_dir fail below
+    struct stat st;
     if (stat(cdir.c_str(), &st) == 0 && S_ISDIR(st.st_mode)) {
         struct stat lst;
-        const int rc = lstat(cdir.c_str(), &lst) == 0 && S_ISLNK(lst.st_mode) ? unlink(cdir.c_str()) : remove_tree(cdir);
-        if (rc != 0) return set_error(nullptr, AC_EINPUT, "failed to delete directory " + cdir + "\n" + strerror(errno));
+        const int removed = lstat(cdir.c_str(), &lst) == 0 && S_ISLNK(lst.st_mode) ? unlink(cdir.c_str()) : remove_tree(cdir);
+        if (removed != 0) return set_error(nullptr, AC_EINPUT, "failed to delete directory " + cdir + "\n" + strerror(errno));
     }
     if (mkdir(cdir.c_str(), 0777) != 0) return set_error(nullptr, AC_EINPUT, "failed to create directory " + cdir + "\n" + strerror(errno));
     if (verbose) fprintf(stderr, "\nStarting autocycler cluster\n    This command takes a unitig graph (made by autocycler compress) and clusters the sequences based on "
                                  "their similarity. Ideally, each cluster will then contain sequences which can be combined into a consensus.\n\n");
-    std::string text;
-    {
-        FILE* f = fopen(gfa.c_str(), "rb");
-        if (!f) return set_error(nullptr, AC_EIO, "cannot read " + gfa);
-        char buf[1 << 16]; size_t n;
-        while ((n = fread(buf, 1, sizeof buf, f)) > 0) text.append(buf, n);
-        fclose(f);
-    }
-    ac_config cfg{}; cfg.k = 51; cfg.device = device; cfg.stream = nullptr; cfg.keep_positions = 0; cfg.n_devices = 1; cfg.devices = nullptr;
-    int rc = ac_create(&h, &cfg);
-    if (rc != AC_OK) return rc;
-    std::unique_ptr<ac_handle, void (*)(ac_handle*)> guard(h, ac_destroy);
-    if ((rc = ac_load_gfa(h, text.data(), text.size())) != AC_OK) { g_error = h->err; return rc == AC_EINVAL ? AC_EINPUT : rc; }
+    std::string text; Handle h;
+    if ((rc = read_file(gfa, text)) != AC_OK || (rc = make_handle(device, h)) != AC_OK || (rc = load_input_gfa(h.get(), text)) != AC_OK) return rc;
     const std::vector<uint16_t> man = manual ? parse_manual_clusters(manual) : std::vector<uint16_t>();
     if (verbose) fprintf(stderr, "Settings:\n  --autocycler_dir %s\n", dir.c_str());
     cluster_graph(text, h->graph, h->seqs, *h->pipe, cutoff, min_assemblies < 0 ? -1 : min_assemblies, man, max_contigs, cdir, verbose != 0, h->cluster, h->cluster_stats);
@@ -1213,7 +1196,7 @@ int ac_cluster_dir(const char* autocycler_dir, double cutoff, int64_t min_assemb
                                  "view the following files.\nPairwise distances:         %s\nClustering tree (Newick):   %s\nClustering tree (metadata): %s\n"
                                  "\n(distance kernels %.2f ms, UPGMA kernel %.2f ms, per-cluster graphs %.1f ms)\n\n", phylip.c_str(), newick.c_str(), tsv.c_str(),
                          (double)h->cluster_stats.distance_ms, (double)h->cluster_stats.upgma_ms, h->cluster_stats.cluster_gfa_ms);
-    return ok(h);
+    return ok(h.get());
     AC_GUARD_END(nullptr)
 }
 
@@ -1228,12 +1211,9 @@ int ac_bridge_best_paths(ac_handle* h, const int32_t* paths, const uint64_t* pat
     for (uint64_t g = 0; g < n_groups; ++g) {
         if (group_off[g + 1] < group_off[g]) return set_error(h, AC_EINVAL, "group offsets must not decrease");
         for (uint64_t x = group_off[g]; x < group_off[g + 1]; ++x) {
-            if (path_off[x + 1] < path_off[x]) return set_error(h, AC_EINVAL, "path offsets must not decrease");
+            const int rc = check_path(h, paths, path_off, x, n_weights);
+            if (rc != AC_OK) return rc;
             groups[g].emplace_back(paths + path_off[x], paths + path_off[x + 1]);
-            for (int32_t u : groups[g].back()) {
-                const int64_t a = u < 0 ? -(int64_t)u : u;
-                if (u == 0 || (uint64_t)a >= n_weights) return set_error(h, AC_EINVAL, "path entry " + std::to_string(u) + " has no weight");
-            }
         }
     }
     std::vector<uint32_t> w(weights, weights + n_weights);
@@ -1273,11 +1253,7 @@ int ac_resolve_text(ac_handle* h, int32_t what, char* out, uint64_t cap, uint64_
     const std::string* t = what == AC_RESOLVE_BRIDGED ? &h->resolve.bridged : what == AC_RESOLVE_MERGED ? &h->resolve.merged :
                            what == AC_RESOLVE_FINAL ? &h->resolve.final_gfa : nullptr;
     if (!t) return set_error(h, AC_EINVAL, "unknown resolve text");
-    *length = t->size();
-    if (!out) return ok(h);
-    if (cap < t->size()) return set_error(h, AC_ERANGE, "buffer too small");
-    memcpy(out, t->data(), t->size());
-    return ok(h);
+    return copy_text(h, *t, out, cap, length);
 }
 
 int ac_resolve_stats(const ac_handle* h, ac_resolve_info* out) {
@@ -1289,61 +1265,25 @@ int ac_resolve_stats(const ac_handle* h, ac_resolve_info* out) {
     return ok(h);
 }
 
-namespace {
-bool read_file(const std::string& path, std::string& text) {
-    FILE* f = fopen(path.c_str(), "rb");
-    if (!f) return false;
-    char buf[1 << 16]; size_t n;
-    text.clear();
-    while ((n = fread(buf, 1, sizeof buf, f)) > 0) text.append(buf, n);
-    fclose(f);
-    return true;
-}
-bool check_file(const std::string& path) {      // check_if_file_exists (misc.rs:98-107)
-    struct stat st;
-    if (stat(path.c_str(), &st) != 0) { set_error(nullptr, AC_EINPUT, "file does not exist: " + path); return false; }
-    if (!S_ISREG(st.st_mode)) { set_error(nullptr, AC_EINPUT, path + " is not a file"); return false; }
-    return true;
-}
-bool make_dirs(const std::string& path) {       // create_dir_all
-    struct stat st;
-    if (path.empty() || stat(path.c_str(), &st) == 0) return path.empty() || S_ISDIR(st.st_mode);
-    const size_t slash = path.find_last_of('/', path.size() > 1 ? path.size() - 2 : 0);
-    if (slash != std::string::npos && slash > 0 && !make_dirs(path.substr(0, slash))) return false;
-    return mkdir(path.c_str(), 0777) == 0 || (stat(path.c_str(), &st) == 0 && S_ISDIR(st.st_mode));
-}
-}  // namespace
-
 int ac_resolve_dir(const char* cluster_dir, int32_t verbose, int32_t device) {
     if (!cluster_dir) return set_error(nullptr, AC_EINVAL, "null argument");
-    ac_handle* h = nullptr;
     AC_GUARD_BEGIN
     // check_settings, resolve.rs:72-75 (misc.rs:98-119)
     const std::string dir = cluster_dir, trimmed = dir + "/2_trimmed.gfa";
-    struct stat st;
-    if (stat(cluster_dir, &st) != 0) return set_error(nullptr, AC_EINPUT, "directory does not exist: " + dir);
-    if (!S_ISDIR(st.st_mode)) return set_error(nullptr, AC_EINPUT, dir + " is not a directory");
-    if (!check_file(trimmed)) return AC_EINPUT;
-    std::string text;
-    if (!read_file(trimmed, text)) return set_error(nullptr, AC_EIO, "cannot read " + trimmed);
-    ac_config cfg{}; cfg.k = 51; cfg.device = device; cfg.stream = nullptr; cfg.keep_positions = 0; cfg.n_devices = 1; cfg.devices = nullptr;
-    int rc = ac_create(&h, &cfg);
-    if (rc != AC_OK) return rc;
-    std::unique_ptr<ac_handle, void (*)(ac_handle*)> guard(h, ac_destroy);
+    int rc;
+    if ((rc = check_dir(dir)) != AC_OK || (rc = check_file(trimmed)) != AC_OK) return rc;
+    std::string text; Handle h;
+    if ((rc = read_file(trimmed, text)) != AC_OK || (rc = make_handle(device, h)) != AC_OK) return rc;
     if (verbose) fprintf(stderr, "\nStarting autocycler resolve\n    This command resolves repeats in the unitig graph.\n\nSettings:\n  --cluster_dir %s\n\n", dir.c_str());
-    {   // the loader's own errors (a malformed 2_trimmed.gfa) are input errors
-        HostGraph check; std::vector<HostSeq> seqs;
-        try { check.load_gfa(text.data(), text.size(), seqs); }
-        catch (const std::runtime_error& e) { return set_error(nullptr, AC_EINPUT, e.what()); }
-    }
+    if ((rc = load_input_gfa(h.get(), text)) != AC_OK) return rc;
     ResolveResult r; ResolveStats rs;
-    resolve_text(text, *h->pipe, verbose != 0, r, rs);
+    resolve_text(text, *h->pipe, verbose != 0, r, rs);     // the file's own text, as the reference re-reads it (resolve.rs:59)
     const std::string bridged = dir + "/3_bridged.gfa", merged = dir + "/4_merged.gfa", final_gfa = dir + "/5_final.gfa";
     if (!write_file(bridged, r.bridged) || !write_file(merged, r.merged) || !write_file(final_gfa, r.final_gfa))
         return set_error(nullptr, AC_EIO, "cannot write the output files under " + dir);
     if (verbose) fprintf(stderr, "\nFinished!\nFinal consensus graph: %s\n(%llu distance jobs, %llu DP cells, distance kernels %.2f ms)\n\n", final_gfa.c_str(),
                          (unsigned long long)rs.jobs, (unsigned long long)rs.cells, (double)rs.kernel_ms);
-    return ok(h);
+    return ok(h.get());
     AC_GUARD_END(nullptr)
 }
 
@@ -1353,7 +1293,7 @@ int ac_combine_dir(const char* autocycler_dir, const char* const* in_gfas, uint3
     if (n_gfas == 0) return set_error(nullptr, AC_EINPUT, "at least one input GFA is required");
     std::vector<std::string> names, texts(n_gfas);
     for (uint32_t i = 0; i < n_gfas; ++i) { if (!in_gfas[i]) return set_error(nullptr, AC_EINVAL, "null argument"); names.push_back(in_gfas[i]); }
-    for (const std::string& n : names) if (!check_file(n)) return AC_EINPUT;     // check_settings (combine.rs:52-56)
+    for (const std::string& n : names) if (check_file(n) != AC_OK) return AC_EINPUT;     // check_settings (combine.rs:52-56)
     const std::string dir = autocycler_dir;
     if (!make_dirs(dir)) return set_error(nullptr, AC_EINPUT, "failed to create directory " + dir + "\n" + strerror(errno));
     if (verbose) {
@@ -1362,7 +1302,7 @@ int ac_combine_dir(const char* autocycler_dir, const char* const* in_gfas, uint3
         for (size_t i = 1; i < names.size(); ++i) fprintf(stderr, "            %s\n", names[i].c_str());
         fprintf(stderr, "\n");
     }
-    for (uint32_t i = 0; i < n_gfas; ++i) if (!read_file(names[i], texts[i])) return set_error(nullptr, AC_EIO, "cannot read " + names[i]);
+    for (uint32_t i = 0; i < n_gfas; ++i) if (read_file(names[i], texts[i]) != AC_OK) return AC_EIO;
     std::string gfa, fasta, yaml;
     combine_texts(texts, names, verbose != 0, gfa, fasta, yaml);
     const std::string out_gfa = dir + "/consensus_assembly.gfa", out_fasta = dir + "/consensus_assembly.fasta", out_yaml = dir + "/consensus_assembly.yaml";

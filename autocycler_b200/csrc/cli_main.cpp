@@ -8,170 +8,186 @@
 
 #include "../../include/autocycler_gpu.h"
 
-static void usage() {
-    fprintf(stderr,
-            "Usage: autocycler compress --assemblies_dir <ASSEMBLIES_DIR> --autocycler_dir <AUTOCYCLER_DIR> [OPTIONS]\n\n"
-            "Options:\n"
-            "  -i, --assemblies_dir <DIR>   Directory containing input assemblies (required)\n"
-            "  -a, --autocycler_dir <DIR>   Autocycler directory to be created (required)\n"
-            "      --kmer <KMER>            K-mer size for De Bruijn graph [default: 51]\n"
-            "      --max_contigs <N>        refuse to run if mean contigs per assembly exceeds this value [default: 25]\n"
-            "  -t, --threads <THREADS>      Number of CPU threads (end repair) [default: 8]\n"
-            "      --device <ORDINAL>       CUDA device [default: 0]\n"
-            "      --devices <A,B,...>      several CUDA devices of this box: the assemblies are sharded by file over them\n");
+static const char* compress_usage =
+    "Usage: autocycler compress --assemblies_dir <ASSEMBLIES_DIR> --autocycler_dir <AUTOCYCLER_DIR> [OPTIONS]\n\n"
+    "Options:\n"
+    "  -i, --assemblies_dir <DIR>   Directory containing input assemblies (required)\n"
+    "  -a, --autocycler_dir <DIR>   Autocycler directory to be created (required)\n"
+    "      --kmer <KMER>            K-mer size for De Bruijn graph [default: 51]\n"
+    "      --max_contigs <N>        refuse to run if mean contigs per assembly exceeds this value [default: 25]\n"
+    "  -t, --threads <THREADS>      Number of CPU threads (end repair) [default: 8]\n"
+    "      --device <ORDINAL>       CUDA device [default: 0]\n"
+    "      --devices <A,B,...>      several CUDA devices of this box: the assemblies are sharded by file over them\n";
+
+// A subcommand's arguments, read one flag at a time (argv[1] is the subcommand).  Errors in them exit with 2.
+struct Args {
+    int argc; char** argv; const char* usage;
+    int i = 1; std::string flag;
+    bool next() { if (++i >= argc) return false; flag = argv[i]; return true; }
+    bool is(const char* a, const char* b = nullptr) const { return flag == a || (b && flag == b); }
+    const char* value() {
+        if (i + 1 >= argc) { fprintf(stderr, "error: a value is required for '%s'\n", flag.c_str()); exit(2); }
+        return argv[++i];
+    }
+    // The value as a number: all of it must parse, and an integer takes no sign.  u32: dotplot's options, which accept a '+' and
+    // check the range instead, and print no usage after "invalid value".
+    double number(bool integral, bool u32 = false) {
+        const char* v = value();
+        char* end = nullptr;
+        const double x = integral ? (double)strtoul(v, &end, 10) : strtod(v, &end);
+        const bool bad = u32 ? (*v == '-' || x > 0xFFFFFFFFul) : (integral && (*v == '-' || *v == '+'));
+        if (!*v || *end || bad) { fprintf(stderr, "error: invalid value '%s' for '%s'\n%s", v, flag.c_str(), u32 ? "" : usage); exit(2); }
+        return x;
+    }
+    int help() const { fprintf(stderr, "%s", usage); return 0; }
+    int missing() const { fprintf(stderr, "%s", usage); return 2; }
+    int unexpected() const { fprintf(stderr, "error: unexpected argument '%s'\n%s", flag.c_str(), usage); return 2; }
+};
+
+static int finish(int rc) {
+    if (rc == AC_OK) return 0;
+    fprintf(stderr, "\nError: %s\n", ac_last_error(nullptr));
+    return 1;
 }
 
-// `autocycler decompress` (main.rs:150-162, decompress.rs:27-57)
-static int decompress_main(int argc, char** argv) {
-    std::string in, out_dir, out_file; int device = 0;
-    for (int i = 2; i < argc; ++i) {
-        std::string a = argv[i];
-        auto value = [&]() -> const char* { if (i + 1 >= argc) { fprintf(stderr, "error: a value is required for '%s'\n", a.c_str()); exit(2); } return argv[++i]; };
-        if (a == "-i" || a == "--in_gfa") in = value();
-        else if (a == "-o" || a == "--out_dir") out_dir = value();
-        else if (a == "-f" || a == "--out_file") out_file = value();
-        else if (a == "--device") device = atoi(value());
-        else { fprintf(stderr, "error: unexpected argument '%s'\nUsage: autocycler decompress --in_gfa <IN_GFA> [--out_dir <DIR>] [--out_file <FASTA>]\n", a.c_str()); return 2; }
+// `autocycler compress` (main.rs:126-148, compress.rs:32-62)
+static int compress_main(int argc, char** argv) {
+    Args a{argc, argv, compress_usage};
+    std::string in, out; unsigned k = 51, max_contigs = 25, threads = 8; int device = 0;
+    std::vector<int32_t> devices;
+    while (a.next()) {
+        if (a.is("-i", "--assemblies_dir")) in = a.value();
+        else if (a.is("-a", "--autocycler_dir")) out = a.value();
+        else if (a.is("--kmer")) k = (unsigned)strtoul(a.value(), nullptr, 10);
+        else if (a.is("--max_contigs")) max_contigs = (unsigned)strtoul(a.value(), nullptr, 10);
+        else if (a.is("-t", "--threads")) threads = (unsigned)strtoul(a.value(), nullptr, 10);
+        else if (a.is("--device")) device = atoi(a.value());
+        else if (a.is("--devices")) { devices.clear(); for (const char* q = a.value(); *q;) { devices.push_back((int32_t)strtol(q, (char**)&q, 10)); if (*q == ',') ++q; else if (*q) { fprintf(stderr, "error: --devices wants a comma-separated list of ordinals\n"); return 2; } } }
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
     }
-    if (in.empty()) { fprintf(stderr, "Usage: autocycler decompress --in_gfa <IN_GFA> [--out_dir <DIR>] [--out_file <FASTA>]\n"); return 2; }
+    if (in.empty() || out.empty()) return a.missing();
+    fprintf(stderr, "\nStarting autocycler compress (%s)\n\nSettings:\n  --assemblies_dir %s\n  --autocycler_dir %s\n  --kmer %u\n  --threads %u\n\n",
+            ac_version(), in.c_str(), out.c_str(), k, threads);
+    if (devices.empty()) devices.push_back(device);
+    const int node = ac_bind_host_to_device(devices[0]);   // stay on the socket of the GPU that finishes the graph; harmless when the topology cannot be read
+    if (node >= 0) fprintf(stderr, "host threads bound to NUMA node %d (device %d)\n\n", node, devices[0]);
+    return finish(ac_compress_dir_devices(in.c_str(), out.c_str(), k, max_contigs, threads, devices.data(), (int32_t)devices.size(), 1));
+}
+
+// `autocycler decompress` (main.rs:150-162, decompress.rs:27-57); it has no -h
+static int decompress_main(int argc, char** argv) {
+    Args a{argc, argv, "Usage: autocycler decompress --in_gfa <IN_GFA> [--out_dir <DIR>] [--out_file <FASTA>]\n"};
+    std::string in, out_dir, out_file; int device = 0;
+    while (a.next()) {
+        if (a.is("-i", "--in_gfa")) in = a.value();
+        else if (a.is("-o", "--out_dir")) out_dir = a.value();
+        else if (a.is("-f", "--out_file")) out_file = a.value();
+        else if (a.is("--device")) device = atoi(a.value());
+        else return a.unexpected();
+    }
+    if (in.empty()) return a.missing();
     fprintf(stderr, "\nStarting autocycler decompress (%s)\n\nSettings:\n  --in_gfa %s\n", ac_version(), in.c_str());
     if (!out_dir.empty()) fprintf(stderr, "  --out_dir %s\n", out_dir.c_str());
     if (!out_file.empty()) fprintf(stderr, "  --out_file %s\n", out_file.c_str());
     fprintf(stderr, "\n");
-    const int rc = ac_decompress_gfa(in.c_str(), out_dir.empty() ? nullptr : out_dir.c_str(), out_file.empty() ? nullptr : out_file.c_str(), device, 1);
-    if (rc != AC_OK) { fprintf(stderr, "\nError: %s\n", ac_last_error(nullptr)); return 1; }
-    return 0;
+    return finish(ac_decompress_gfa(in.c_str(), out_dir.empty() ? nullptr : out_dir.c_str(), out_file.empty() ? nullptr : out_file.c_str(), device, 1));
 }
 
 // `autocycler trim` (main.rs:301-322, trim.rs:36-101)
 static int trim_main(int argc, char** argv) {
-    static const char* trim_usage = "Usage: autocycler trim --cluster_dir <CLUSTER_DIR> [--min_identity 0.75] [--max_unitigs 5000] [--mad 5.0] [--threads 8] [--device N]\n";
+    Args a{argc, argv, "Usage: autocycler trim --cluster_dir <CLUSTER_DIR> [--min_identity 0.75] [--max_unitigs 5000] [--mad 5.0] [--threads 8] [--device N]\n"};
     std::string dir; double min_identity = 0.75, mad = 5.0; unsigned long max_unitigs = 5000, threads = 8; int device = 0;
-    for (int i = 2; i < argc; ++i) {
-        std::string a = argv[i];
-        auto value = [&]() -> const char* { if (i + 1 >= argc) { fprintf(stderr, "error: a value is required for '%s'\n", a.c_str()); exit(2); } return argv[++i]; };
-        auto number = [&](const char* v, bool integral) -> double {
-            char* end = nullptr; const double x = integral ? (double)strtoul(v, &end, 10) : strtod(v, &end);
-            if (!*v || *end || (integral && (*v == '-' || *v == '+'))) { fprintf(stderr, "error: invalid value '%s' for '%s'\n%s", v, a.c_str(), trim_usage); exit(2); }
-            return x;
-        };
-        if (a == "-c" || a == "--cluster_dir") dir = value();
-        else if (a == "--min_identity") min_identity = number(value(), false);
-        else if (a == "--max_unitigs") max_unitigs = (unsigned long)number(value(), true);
-        else if (a == "--mad") mad = number(value(), false);
-        else if (a == "-t" || a == "--threads") threads = (unsigned long)number(value(), true);
-        else if (a == "--device") device = atoi(value());
-        else if (a == "-h" || a == "--help") { fprintf(stderr, "%s", trim_usage); return 0; }
-        else { fprintf(stderr, "error: unexpected argument '%s'\n%s", a.c_str(), trim_usage); return 2; }
+    while (a.next()) {
+        if (a.is("-c", "--cluster_dir")) dir = a.value();
+        else if (a.is("--min_identity")) min_identity = a.number(false);
+        else if (a.is("--max_unitigs")) max_unitigs = (unsigned long)a.number(true);
+        else if (a.is("--mad")) mad = a.number(false);
+        else if (a.is("-t", "--threads")) threads = (unsigned long)a.number(true);
+        else if (a.is("--device")) device = atoi(a.value());
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
     }
-    if (dir.empty()) { fprintf(stderr, "%s", trim_usage); return 2; }
+    if (dir.empty()) return a.missing();
     if (max_unitigs > 0xFFFFFFFFul) max_unitigs = 0xFFFFFFFFul;
     if (threads > 0xFFFFFFFFul) threads = 0xFFFFFFFFul;
     fprintf(stderr, "\nStarting autocycler trim (%s)\n\nSettings:\n  --cluster_dir %s\n  --min_identity %g\n  --max_unitigs %lu\n  --mad %g\n  --threads %lu\n\n",
             ac_version(), dir.c_str(), min_identity, max_unitigs, mad, threads);
-    const int rc = ac_trim_dir(dir.c_str(), min_identity, (uint32_t)max_unitigs, mad, (uint32_t)threads, device, 1);
-    if (rc != AC_OK) { fprintf(stderr, "\nError: %s\n", ac_last_error(nullptr)); return 1; }
-    return 0;
+    return finish(ac_trim_dir(dir.c_str(), min_identity, (uint32_t)max_unitigs, mad, (uint32_t)threads, device, 1));
 }
 
 // `autocycler cluster` (main.rs:92-113, cluster.rs:30-114)
 static int cluster_main(int argc, char** argv) {
-    static const char* cluster_usage = "Usage: autocycler cluster --autocycler_dir <AUTOCYCLER_DIR> [--cutoff 0.2] [--min_assemblies N] [--max_contigs 25] [--manual 1,2,3] [--device N]\n";
+    Args a{argc, argv, "Usage: autocycler cluster --autocycler_dir <AUTOCYCLER_DIR> [--cutoff 0.2] [--min_assemblies N] [--max_contigs 25] [--manual 1,2,3] [--device N]\n"};
     std::string dir, manual; bool has_manual = false; double cutoff = 0.2; long long min_assemblies = -1; unsigned long max_contigs = 25; int device = 0;
-    for (int i = 2; i < argc; ++i) {
-        std::string a = argv[i];
-        auto value = [&]() -> const char* { if (i + 1 >= argc) { fprintf(stderr, "error: a value is required for '%s'\n", a.c_str()); exit(2); } return argv[++i]; };
-        auto number = [&](const char* v, bool integral) -> double {
-            char* end = nullptr; const double x = integral ? (double)strtoul(v, &end, 10) : strtod(v, &end);
-            if (!*v || *end || (integral && (*v == '-' || *v == '+'))) { fprintf(stderr, "error: invalid value '%s' for '%s'\n%s", v, a.c_str(), cluster_usage); exit(2); }
-            return x;
-        };
-        if (a == "-a" || a == "--autocycler_dir") dir = value();
-        else if (a == "--cutoff") cutoff = number(value(), false);
-        else if (a == "--min_assemblies") min_assemblies = (long long)number(value(), true);
-        else if (a == "--max_contigs") max_contigs = (unsigned long)number(value(), true);
-        else if (a == "--manual") { manual = value(); has_manual = true; }
-        else if (a == "--device") device = atoi(value());
-        else if (a == "-h" || a == "--help") { fprintf(stderr, "%s", cluster_usage); return 0; }
-        else { fprintf(stderr, "error: unexpected argument '%s'\n%s", a.c_str(), cluster_usage); return 2; }
+    while (a.next()) {
+        if (a.is("-a", "--autocycler_dir")) dir = a.value();
+        else if (a.is("--cutoff")) cutoff = a.number(false);
+        else if (a.is("--min_assemblies")) min_assemblies = (long long)a.number(true);
+        else if (a.is("--max_contigs")) max_contigs = (unsigned long)a.number(true);
+        else if (a.is("--manual")) { manual = a.value(); has_manual = true; }
+        else if (a.is("--device")) device = atoi(a.value());
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
     }
-    if (dir.empty()) { fprintf(stderr, "%s", cluster_usage); return 2; }
+    if (dir.empty()) return a.missing();
     if (max_contigs > 0xFFFFFFFFul) max_contigs = 0xFFFFFFFFul;
     fprintf(stderr, "\nStarting autocycler cluster (%s)\n\n", ac_version());
-    const int rc = ac_cluster_dir(dir.c_str(), cutoff, min_assemblies, (uint32_t)max_contigs, has_manual ? manual.c_str() : nullptr, device, 1);
-    if (rc != AC_OK) { fprintf(stderr, "\nError: %s\n", ac_last_error(nullptr)); return 1; }
-    return 0;
+    return finish(ac_cluster_dir(dir.c_str(), cutoff, min_assemblies, (uint32_t)max_contigs, has_manual ? manual.c_str() : nullptr, device, 1));
 }
 
 // `autocycler resolve` (main.rs:238-247, resolve.rs:31-111)
 static int resolve_main(int argc, char** argv) {
-    static const char* resolve_usage = "Usage: autocycler resolve --cluster_dir <CLUSTER_DIR> [--verbose] [--device N]\n";
+    Args a{argc, argv, "Usage: autocycler resolve --cluster_dir <CLUSTER_DIR> [--verbose] [--device N]\n"};
     std::string dir; bool verbose = false; int device = 0;
-    for (int i = 2; i < argc; ++i) {
-        std::string a = argv[i];
-        auto value = [&]() -> const char* { if (i + 1 >= argc) { fprintf(stderr, "error: a value is required for '%s'\n", a.c_str()); exit(2); } return argv[++i]; };
-        if (a == "-c" || a == "--cluster_dir") dir = value();
-        else if (a == "--verbose") verbose = true;
-        else if (a == "--device") device = atoi(value());
-        else if (a == "-h" || a == "--help") { fprintf(stderr, "%s", resolve_usage); return 0; }
-        else { fprintf(stderr, "error: unexpected argument '%s'\n%s", a.c_str(), resolve_usage); return 2; }
+    while (a.next()) {
+        if (a.is("-c", "--cluster_dir")) dir = a.value();
+        else if (a.is("--verbose")) verbose = true;
+        else if (a.is("--device")) device = atoi(a.value());
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
     }
-    if (dir.empty()) { fprintf(stderr, "%s", resolve_usage); return 2; }
+    if (dir.empty()) return a.missing();
     fprintf(stderr, "\nStarting autocycler resolve (%s)\n\n", ac_version());
-    const int rc = ac_resolve_dir(dir.c_str(), verbose ? 1 : 0, device);
-    if (rc != AC_OK) { fprintf(stderr, "\nError: %s\n", ac_last_error(nullptr)); return 1; }
-    return 0;
+    return finish(ac_resolve_dir(dir.c_str(), verbose ? 1 : 0, device));
 }
 
 // `autocycler combine` (main.rs:115-124, combine.rs:25-87): -i takes one or more GFAs, up to the next flag
 static int combine_main(int argc, char** argv) {
-    static const char* combine_usage = "Usage: autocycler combine --autocycler_dir <AUTOCYCLER_DIR> --in_gfas <IN_GFAS>...\n";
+    Args a{argc, argv, "Usage: autocycler combine --autocycler_dir <AUTOCYCLER_DIR> --in_gfas <IN_GFAS>...\n"};
     std::string dir; std::vector<std::string> gfas;
-    for (int i = 2; i < argc; ++i) {
-        std::string a = argv[i];
-        auto value = [&]() -> const char* { if (i + 1 >= argc) { fprintf(stderr, "error: a value is required for '%s'\n", a.c_str()); exit(2); } return argv[++i]; };
-        if (a == "-a" || a == "--autocycler_dir") dir = value();
-        else if (a == "-i" || a == "--in_gfas") { gfas.push_back(value()); while (i + 1 < argc && argv[i + 1][0] != '-') gfas.push_back(argv[++i]); }
-        else if (a == "-h" || a == "--help") { fprintf(stderr, "%s", combine_usage); return 0; }
-        else { fprintf(stderr, "error: unexpected argument '%s'\n%s", a.c_str(), combine_usage); return 2; }
+    while (a.next()) {
+        if (a.is("-a", "--autocycler_dir")) dir = a.value();
+        else if (a.is("-i", "--in_gfas")) { gfas.push_back(a.value()); while (a.i + 1 < argc && argv[a.i + 1][0] != '-') gfas.push_back(argv[++a.i]); }
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
     }
-    if (dir.empty() || gfas.empty()) { fprintf(stderr, "%s", combine_usage); return 2; }
+    if (dir.empty() || gfas.empty()) return a.missing();
     std::vector<const char*> ptrs;
     for (const std::string& g : gfas) ptrs.push_back(g.c_str());
     fprintf(stderr, "\nStarting autocycler combine (%s)\n\n", ac_version());
-    const int rc = ac_combine_dir(dir.c_str(), ptrs.data(), (uint32_t)ptrs.size(), 1);
-    if (rc != AC_OK) { fprintf(stderr, "\nError: %s\n", ac_last_error(nullptr)); return 1; }
-    return 0;
+    return finish(ac_combine_dir(dir.c_str(), ptrs.data(), (uint32_t)ptrs.size(), 1));
 }
 
 // `autocycler dotplot` (main.rs:164-181, dotplot.rs:44-52)
 static int dotplot_main(int argc, char** argv) {
-    static const char* dotplot_usage = "Usage: autocycler dotplot --input <INPUT> --out_png <OUT_PNG> [--res <RES>] [--kmer <KMER>] [--font <TTF>] [--device N]\n";
+    Args a{argc, argv, "Usage: autocycler dotplot --input <INPUT> --out_png <OUT_PNG> [--res <RES>] [--kmer <KMER>] [--font <TTF>] [--device N]\n"};
     std::string in, out, font; bool have_font = false; unsigned long res = 2000, kmer = 32; int device = 0;
-    for (int i = 2; i < argc; ++i) {
-        std::string a = argv[i];
-        auto value = [&]() -> const char* { if (i + 1 >= argc) { fprintf(stderr, "error: a value is required for '%s'\n", a.c_str()); exit(2); } return argv[++i]; };
-        auto number = [&](const char* v) -> unsigned long {
-            char* end = nullptr; const unsigned long x = strtoul(v, &end, 10);
-            if (!*v || *end || *v == '-' || x > 0xFFFFFFFFul) { fprintf(stderr, "error: invalid value '%s' for '%s'\n", v, a.c_str()); exit(2); }
-            return x;
-        };
-        if (a == "-i" || a == "--input") in = value();
-        else if (a == "-o" || a == "--out_png") out = value();
-        else if (a == "--res") res = number(value());
-        else if (a == "--kmer") kmer = number(value());
-        else if (a == "--font") { font = value(); have_font = true; }
-        else if (a == "--device") device = atoi(value());
-        else if (a == "-h" || a == "--help") { fprintf(stderr, "%s", dotplot_usage); return 0; }
-        else { fprintf(stderr, "error: unexpected argument '%s'\n%s", a.c_str(), dotplot_usage); return 2; }
+    while (a.next()) {
+        if (a.is("-i", "--input")) in = a.value();
+        else if (a.is("-o", "--out_png")) out = a.value();
+        else if (a.is("--res")) res = (unsigned long)a.number(true, true);
+        else if (a.is("--kmer")) kmer = (unsigned long)a.number(true, true);
+        else if (a.is("--font")) { font = a.value(); have_font = true; }
+        else if (a.is("--device")) device = atoi(a.value());
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
     }
-    if (in.empty() || out.empty()) { fprintf(stderr, "%s", dotplot_usage); return 2; }
+    if (in.empty() || out.empty()) return a.missing();
     fprintf(stderr, "\nStarting autocycler dotplot (%s)\n    This command will take a unitig graph (either before or after trimming) and generate a dotplot image "
                     "containing all pairwise comparisons of the sequences.\n\nSettings:\n  --input %s\n  --res %lu\n  --kmer %lu\n\n",
             ac_version(), in.c_str(), res, kmer);
-    const int rc = ac_dotplot_dir(in.c_str(), out.c_str(), (uint32_t)res, (uint32_t)kmer, have_font ? font.c_str() : nullptr, device, 1, nullptr);
-    if (rc != AC_OK) { fprintf(stderr, "\nError: %s\n", ac_last_error(nullptr)); return 1; }
-    return 0;
+    return finish(ac_dotplot_dir(in.c_str(), out.c_str(), (uint32_t)res, (uint32_t)kmer, have_font ? font.c_str() : nullptr, device, 1, nullptr));
 }
 
 int main(int argc, char** argv) {
@@ -181,29 +197,7 @@ int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "decompress") == 0) return decompress_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "cluster") == 0) return cluster_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "trim") == 0) return trim_main(argc, argv);
-    if (argc < 2 || strcmp(argv[1], "compress") != 0) { usage(); return 2; }
-    std::string in, out; unsigned k = 51, max_contigs = 25, threads = 8; int device = 0;
-    std::vector<int32_t> devices;
-    for (int i = 2; i < argc; ++i) {
-        std::string a = argv[i];
-        auto value = [&]() -> const char* { if (i + 1 >= argc) { fprintf(stderr, "error: a value is required for '%s'\n", a.c_str()); exit(2); } return argv[++i]; };
-        if (a == "-i" || a == "--assemblies_dir") in = value();
-        else if (a == "-a" || a == "--autocycler_dir") out = value();
-        else if (a == "--kmer") k = (unsigned)strtoul(value(), nullptr, 10);
-        else if (a == "--max_contigs") max_contigs = (unsigned)strtoul(value(), nullptr, 10);
-        else if (a == "-t" || a == "--threads") threads = (unsigned)strtoul(value(), nullptr, 10);
-        else if (a == "--device") device = atoi(value());
-        else if (a == "--devices") { devices.clear(); for (const char* q = value(); *q;) { devices.push_back((int32_t)strtol(q, (char**)&q, 10)); if (*q == ',') ++q; else if (*q) { fprintf(stderr, "error: --devices wants a comma-separated list of ordinals\n"); return 2; } } }
-        else if (a == "-h" || a == "--help") { usage(); return 0; }
-        else { fprintf(stderr, "error: unexpected argument '%s'\n", a.c_str()); usage(); return 2; }
-    }
-    if (in.empty() || out.empty()) { usage(); return 2; }
-    fprintf(stderr, "\nStarting autocycler compress (%s)\n\nSettings:\n  --assemblies_dir %s\n  --autocycler_dir %s\n  --kmer %u\n  --threads %u\n\n",
-            ac_version(), in.c_str(), out.c_str(), k, threads);
-    if (devices.empty()) devices.push_back(device);
-    const int node = ac_bind_host_to_device(devices[0]);   // stay on the socket of the GPU that finishes the graph; harmless when the topology cannot be read
-    if (node >= 0) fprintf(stderr, "host threads bound to NUMA node %d (device %d)\n\n", node, devices[0]);
-    int rc = ac_compress_dir_devices(in.c_str(), out.c_str(), k, max_contigs, threads, devices.data(), (int32_t)devices.size(), 1);
-    if (rc != AC_OK) { fprintf(stderr, "\nError: %s\n", ac_last_error(nullptr)); return 1; }
-    return 0;
+    if (argc >= 2 && strcmp(argv[1], "compress") == 0) return compress_main(argc, argv);
+    fprintf(stderr, "%s", compress_usage);
+    return 2;
 }

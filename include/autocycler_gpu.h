@@ -43,7 +43,7 @@ extern "C" {
 #define AC_ENODEVICE (-2)   /* no usable CUDA device */
 #define AC_ECUDA (-3)       /* CUDA runtime error */
 #define AC_ERANGE (-4)      /* buffer too small / input too large */
-#define AC_EIO (-5)         /* file system error (ac_compress_dir) */
+#define AC_EIO (-5)         /* file system error: an input that cannot be read, an output that cannot be written (the commands) */
 #define AC_EINPUT (-6)      /* the reference's own input errors (misc.rs:130-136 quit_with_error) */
 
 typedef struct ac_handle ac_handle;
@@ -205,7 +205,7 @@ int ac_pairwise_distances(ac_handle* h, double* out, uint64_t cap);
 int ac_distance_matrix_text(ac_handle* h, char* out, uint64_t cap, uint64_t* length);
 
 /* `autocycler decompress` (decompress.rs:27-137): every contig of the GFA's paths written back per original file under out_dir
- * (gzip when the name ends in .gz) and/or as one FASTA (out_file); either may be NULL, not both. */
+ * (gzip when the name ends in .gz) and/or as one FASTA (out_file); either may be NULL, not both.  A malformed GFA is AC_EINPUT. */
 int ac_decompress_gfa(const char* in_gfa, const char* out_dir, const char* out_file, int32_t device, int32_t verbose);
 
 /* reconstruct_original_sequence (unitig_graph.rs:383-400; decompress.rs:83-105 writes these out): the sequence spelled by
