@@ -88,7 +88,8 @@ EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_seq
            "ac_trim_paths", "ac_trim", "ac_trim_yaml", "ac_trim_stats", "ac_trim_dir",
            "ac_cluster", "ac_cluster_text", "ac_cluster_assignments", "ac_cluster_stats", "ac_upgma", "ac_cluster_dir",
            "ac_bridge_best_paths", "ac_resolve", "ac_resolve_text", "ac_resolve_stats", "ac_resolve_dir", "ac_combine_dir",
-           "ac_dotplot_rgb", "ac_dotplot_dir", "ac_png_write"]
+           "ac_dotplot_rgb", "ac_dotplot_dir", "ac_png_write",
+           "ac_clean_gfa", "ac_clean_text", "ac_gfa_to_fasta", "ac_gfa_fasta_text", "ac_table_text"]
 
 _libs = {}
 
@@ -188,6 +189,12 @@ def load_library(path=None):
                                    C.c_uint32, C.c_uint32, C.c_char_p, C.c_int32, C.c_void_p, C.POINTER(AcDotplotInfo)]
     lib.ac_dotplot_dir.argtypes = [C.c_char_p, C.c_char_p, C.c_uint32, C.c_uint32, C.c_char_p, C.c_int32, C.c_int32, C.POINTER(AcDotplotInfo)]
     lib.ac_png_write.argtypes = [C.c_char_p, C.c_void_p, C.c_uint32, C.c_uint32]
+    lib.ac_clean_gfa.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.POINTER(C.c_double), C.c_int32]
+    lib.ac_clean_text.argtypes = [C.c_char_p, C.c_uint64, C.POINTER(C.c_uint32), C.c_uint64, C.POINTER(C.c_uint32), C.c_uint64,
+                                  C.POINTER(C.c_double), C.c_int32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
+    lib.ac_gfa_to_fasta.argtypes = [C.c_char_p, C.c_char_p, C.c_int32]
+    lib.ac_gfa_fasta_text.argtypes = [C.c_char_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
+    lib.ac_table_text.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint64, C.c_int32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     _libs[path] = lib
     return lib
 
@@ -637,3 +644,51 @@ def png_write(path, rgb, lib=None):
     lib = lib or load_library()
     rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
     _raise_unless_ok(lib, lib.ac_png_write(os.fsencode(path), rgb.ctypes.data, rgb.shape[1], rgb.shape[0]))
+
+
+def _host_text(lib, fn, *args):
+    """A host-only two-call getter fn(*args, out, cap, length): the length, then the text."""
+    n = C.c_uint64()
+    _raise_unless_ok(lib, fn(*args, None, 0, C.byref(n)))
+    buf = C.create_string_buffer(max(1, n.value))
+    _raise_unless_ok(lib, fn(*args, buf, n.value, C.byref(n)))
+    return buf.raw[:n.value].decode()
+
+
+def _depth_arg(min_depth):
+    return None if min_depth is None else C.byref(C.c_double(min_depth))
+
+
+def clean(in_gfa, out_gfa, remove=None, duplicate=None, min_depth=None, verbose=False, lib=None):
+    """clean.rs:23-45: remove and duplicate are the CLI's comma-separated tig lists (or None); writes out_gfa.  Host only."""
+    lib = lib or load_library()
+    _raise_unless_ok(lib, lib.ac_clean_gfa(os.fsencode(in_gfa), os.fsencode(out_gfa), None if remove is None else remove.encode(),
+                                           None if duplicate is None else duplicate.encode(), _depth_arg(min_depth), 1 if verbose else 0))
+
+
+def clean_text(gfa_text, remove=(), duplicate=(), min_depth=None, merge=True, lib=None):
+    """clean.rs:26-45 on a GFA text -> the cleaned GFA text.  merge=False stops before merge_linear_paths and renumbering."""
+    lib = lib or load_library()
+    data = gfa_text.encode() if isinstance(gfa_text, str) else bytes(gfa_text)
+    rm, dup = (C.c_uint32 * max(1, len(remove)))(*remove), (C.c_uint32 * max(1, len(duplicate)))(*duplicate)
+    return _host_text(lib, lib.ac_clean_text, data, len(data), rm, len(remove), dup, len(duplicate), _depth_arg(min_depth), 1 if merge else 0)
+
+
+def gfa2fasta(in_gfa, out_fasta, verbose=False, lib=None):
+    """gfa2fasta.rs:23-29: writes out_fasta.  Host only."""
+    lib = lib or load_library()
+    _raise_unless_ok(lib, lib.ac_gfa_to_fasta(os.fsencode(in_gfa), os.fsencode(out_fasta), 1 if verbose else 0))
+
+
+def gfa_fasta_text(gfa_text, lib=None):
+    """save_graph_to_fasta (gfa2fasta.rs:55-82) of a GFA text -> the FASTA text."""
+    lib = lib or load_library()
+    data = gfa_text.encode() if isinstance(gfa_text, str) else bytes(gfa_text)
+    return _host_text(lib, lib.ac_gfa_fasta_text, data, len(data))
+
+
+def table(autocycler_dir=None, name="", fields=None, sigfigs=3, verbose=False, lib=None):
+    """table.rs:24-32 -> the line `autocycler table` prints, newline included: the header without autocycler_dir, else the values."""
+    lib = lib or load_library()
+    return _host_text(lib, lib.ac_table_text, None if autocycler_dir is None else os.fsencode(autocycler_dir), name.encode(),
+                      None if fields is None else fields.encode(), sigfigs, 1 if verbose else 0)

@@ -24,6 +24,7 @@
 #include "host_cluster.h"
 #include "host_trim.h"
 #include "host_resolve.h"
+#include "host_clean.h"
 #include "host_dotplot.h"
 #include <mutex>
 #include <immintrin.h>
@@ -1310,6 +1311,100 @@ int ac_combine_dir(const char* autocycler_dir, const char* const* in_gfas, uint3
     if (verbose) fprintf(stderr, "\nFinished!\nCombined graph: %s\nCombined fasta: %s\n\n%s\n\n", out_gfa.c_str(), out_fasta.c_str(),
                          yaml.find("fully_resolved: true") != std::string::npos ? "Consensus assembly is fully resolved" : "One or more clusters failed to fully resolve");
     return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
+// ---- `autocycler clean`, `autocycler gfa2fasta` and `autocycler table` (host only) ----------------------------------------------
+int ac_clean_gfa(const char* in_gfa, const char* out_gfa, const char* remove, const char* duplicate, const double* min_depth, int32_t verbose) {
+    if (!in_gfa || !out_gfa) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    const std::string in = in_gfa, out = out_gfa;
+    int rc;
+    if ((rc = check_file(in)) != AC_OK) return rc;        // check_settings (clean.rs:47-49)
+    if (verbose) fprintf(stderr, "\nStarting autocycler clean\n    This command removes user-specified tigs from a combined Autocycler graph and then merges "
+                                 "all linear paths to produce a clean output graph.\n\n");
+    const std::vector<uint32_t> rm = remove ? parse_tig_numbers(remove) : std::vector<uint32_t>(),
+                                dup = duplicate ? parse_tig_numbers(duplicate) : std::vector<uint32_t>();
+    auto joined = [](const std::vector<uint32_t>& v) { std::string s; for (uint32_t n : v) s += (s.empty() ? "" : ",") + std::to_string(n); return s; };
+    if (verbose) {
+        fprintf(stderr, "Settings:\n  --in_gfa %s\n  --out_gfa %s\n", in.c_str(), out.c_str());
+        if (!rm.empty()) fprintf(stderr, "  --remove %s\n", joined(rm).c_str());
+        if (!dup.empty()) fprintf(stderr, "  --duplicate %s\n", joined(dup).c_str());
+        fprintf(stderr, "\n\nLoading graph\n    The unitig graph is now loaded into memory.\n\n");
+    }
+    std::string text, gfa;
+    if ((rc = read_file(in, text)) != AC_OK) return rc;
+    HostGraph g;
+    load_user_gfa(text, g);
+    if (verbose) fprintf(stderr, "%u unitig%s, %llu link%s\ntotal length: %llu bp\n\n", g.U, g.U == 1 ? "" : "s", (unsigned long long)g.link_count_single(),
+                         g.link_count_single() == 1 ? "" : "s", (unsigned long long)g.total_length());
+    clean_graph(g, in, rm, dup, min_depth, true, verbose != 0, gfa);
+    if (!write_file(out, gfa)) return set_error(nullptr, AC_EIO, "cannot write " + out);
+    if (verbose) fprintf(stderr, "\nFinished!\nCleaned graph: %s\n\n", out.c_str());
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
+int ac_clean_text(const char* gfa_text, uint64_t length, const uint32_t* remove, uint64_t n_remove, const uint32_t* duplicate, uint64_t n_duplicate,
+                  const double* min_depth, int32_t merge, char* out, uint64_t cap, uint64_t* out_length) {
+    if (!gfa_text || !out_length || (n_remove && !remove) || (n_duplicate && !duplicate)) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    HostGraph g;
+    load_user_gfa(std::string(gfa_text, length), g);
+    std::string gfa;
+    clean_graph(g, "the GFA", std::vector<uint32_t>(remove, remove + n_remove), std::vector<uint32_t>(duplicate, duplicate + n_duplicate),
+                min_depth, merge != 0, false, gfa);
+    return copy_text(nullptr, gfa, out, cap, out_length);
+    AC_GUARD_END(nullptr)
+}
+
+int ac_gfa_to_fasta(const char* in_gfa, const char* out_fasta, int32_t verbose) {
+    if (!in_gfa || !out_fasta) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    const std::string in = in_gfa, out = out_fasta;
+    int rc;
+    if ((rc = check_file(in)) != AC_OK) return rc;
+    if (verbose) fprintf(stderr, "\nStarting autocycler gfa2fasta\n    This command loads an Autocycler graph and saves it as a FASTA file with topological "
+                                 "information in the sequence headers.\n\nSettings:\n  --in_gfa %s\n  --out_fasta %s\n\n\nLoading graph\n    The unitig graph "
+                                 "is now loaded into memory.\n\n", in.c_str(), out.c_str());
+    std::string text;
+    if ((rc = read_file(in, text)) != AC_OK) return rc;
+    HostGraph g;
+    load_user_gfa(text, g);
+    if (verbose) fprintf(stderr, "%u unitig%s, %llu link%s\ntotal length: %llu bp\n\n\nSaving to FASTA\n    The unitig graph is now saved to a FASTA file.\n\n",
+                         g.U, g.U == 1 ? "" : "s", (unsigned long long)g.link_count_single(), g.link_count_single() == 1 ? "" : "s",
+                         (unsigned long long)g.total_length());
+    uint64_t counts[3];
+    const std::string fasta = gfa_fasta_text(g, counts);
+    if (!write_file(out, fasta)) return set_error(nullptr, AC_EIO, "cannot write " + out);
+    if (verbose) {
+        const char* what[3] = {"circular", "linear", "other"};
+        for (int i = 0; i < 3; ++i) fprintf(stderr, "%llu %s sequence%s\n", (unsigned long long)counts[i], what[i], counts[i] == 1 ? "" : "s");
+        fprintf(stderr, "\n");
+    }
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
+int ac_gfa_fasta_text(const char* gfa_text, uint64_t length, char* out, uint64_t cap, uint64_t* out_length) {
+    if (!gfa_text || !out_length) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    HostGraph g;
+    load_user_gfa(std::string(gfa_text, length), g);
+    uint64_t counts[3];
+    return copy_text(nullptr, gfa_fasta_text(g, counts), out, cap, out_length);
+    AC_GUARD_END(nullptr)
+}
+
+int ac_table_text(const char* autocycler_dir, const char* name, const char* fields, uint64_t sigfigs, int32_t verbose, char* out, uint64_t cap,
+                  uint64_t* length) {
+    if (!length) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    int rc;
+    if (autocycler_dir && (rc = check_dir(autocycler_dir)) != AC_OK) return rc;     // check_settings (table.rs:34-41)
+    const std::string line = table_text(autocycler_dir ? autocycler_dir : "", autocycler_dir != nullptr, name ? name : "",
+                                        fields ? fields : TABLE_DEFAULT_FIELDS, sigfigs, verbose != 0);
+    return copy_text(nullptr, line, out, cap, length);
     AC_GUARD_END(nullptr)
 }
 

@@ -1,4 +1,5 @@
-// `autocycler compress`, `autocycler decompress`, `autocycler cluster`, `autocycler trim`, `autocycler resolve`, `autocycler combine` and `autocycler dotplot` with the reference's flags (main.rs:126-162), messages and exit codes
+// `autocycler compress`, `autocycler decompress`, `autocycler cluster`, `autocycler trim`, `autocycler resolve`, `autocycler combine`, `autocycler dotplot`,
+// `autocycler clean`, `autocycler gfa2fasta` and `autocycler table` with the reference's flags (main.rs:126-162), messages and exit codes
 // (misc.rs:130-136: "Error: <text>" on stderr, exit 1), running the H100 path through the C ABI.
 #include <cstdio>
 #include <cstdlib>
@@ -190,6 +191,59 @@ static int dotplot_main(int argc, char** argv) {
     return finish(ac_dotplot_dir(in.c_str(), out.c_str(), (uint32_t)res, (uint32_t)kmer, have_font ? font.c_str() : nullptr, device, 1, nullptr));
 }
 
+// `autocycler clean` (main.rs:69-90, clean.rs:23-45); no device
+static int clean_main(int argc, char** argv) {
+    Args a{argc, argv, "Usage: autocycler clean --in_gfa <IN_GFA> --out_gfa <OUT_GFA> [--remove 1,2,3] [--duplicate 4,5] [--min_depth D]\n"};
+    std::string in, out, remove, duplicate; bool has_remove = false, has_duplicate = false, has_min_depth = false; double min_depth = 0;
+    while (a.next()) {
+        if (a.is("-i", "--in_gfa")) in = a.value();
+        else if (a.is("-o", "--out_gfa")) out = a.value();
+        else if (a.is("-r", "--remove")) { remove = a.value(); has_remove = true; }
+        else if (a.is("-d", "--duplicate")) { duplicate = a.value(); has_duplicate = true; }
+        else if (a.is("-m", "--min_depth")) { min_depth = a.number(false); has_min_depth = true; }
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
+    }
+    if (in.empty() || out.empty()) return a.missing();
+    return finish(ac_clean_gfa(in.c_str(), out.c_str(), has_remove ? remove.c_str() : nullptr, has_duplicate ? duplicate.c_str() : nullptr,
+                               has_min_depth ? &min_depth : nullptr, 1));
+}
+
+// `autocycler gfa2fasta` (main.rs:183-192, gfa2fasta.rs:23-29); no device
+static int gfa2fasta_main(int argc, char** argv) {
+    Args a{argc, argv, "Usage: autocycler gfa2fasta --in_gfa <IN_GFA> --out_fasta <OUT_FASTA>\n"};
+    std::string in, out;
+    while (a.next()) {
+        if (a.is("-i", "--in_gfa")) in = a.value();
+        else if (a.is("-o", "--out_fasta")) out = a.value();
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
+    }
+    if (in.empty() || out.empty()) return a.missing();
+    return finish(ac_gfa_to_fasta(in.c_str(), out.c_str(), 1));
+}
+
+// `autocycler table` (main.rs:276-299, table.rs:24-32): the line goes to stdout; no device
+static int table_main(int argc, char** argv) {
+    Args a{argc, argv, "Usage: autocycler table [--autocycler_dir <AUTOCYCLER_DIR>] [--name <NAME>] [--fields <FIELDS>] [--sigfigs 3]\n"};
+    std::string dir, name, fields; bool has_dir = false, has_fields = false; unsigned long long sigfigs = 3;
+    while (a.next()) {
+        if (a.is("-a", "--autocycler_dir")) { dir = a.value(); has_dir = true; }
+        else if (a.is("-n", "--name")) name = a.value();
+        else if (a.is("-f", "--fields")) { fields = a.value(); has_fields = true; }
+        else if (a.is("-s", "--sigfigs")) sigfigs = (unsigned long long)a.number(true);
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
+    }
+    uint64_t n = 0;
+    const char* d = has_dir ? dir.c_str() : nullptr, *f = has_fields ? fields.c_str() : nullptr;
+    int rc = ac_table_text(d, name.c_str(), f, sigfigs, 1, nullptr, 0, &n);
+    std::string line(n, '\0');
+    if (rc == AC_OK) rc = ac_table_text(d, name.c_str(), f, sigfigs, 0, &line[0], n, &n);
+    if (rc == AC_OK) fwrite(line.data(), 1, line.size(), stdout);
+    return finish(rc);
+}
+
 int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "dotplot") == 0) return dotplot_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "resolve") == 0) return resolve_main(argc, argv);
@@ -198,6 +252,9 @@ int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "cluster") == 0) return cluster_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "trim") == 0) return trim_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "compress") == 0) return compress_main(argc, argv);
+    if (argc >= 2 && strcmp(argv[1], "clean") == 0) return clean_main(argc, argv);
+    if (argc >= 2 && strcmp(argv[1], "gfa2fasta") == 0) return gfa2fasta_main(argc, argv);
+    if (argc >= 2 && strcmp(argv[1], "table") == 0) return table_main(argc, argv);
     fprintf(stderr, "%s", compress_usage);
     return 2;
 }

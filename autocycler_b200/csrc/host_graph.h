@@ -80,6 +80,16 @@ public:
     // entries UStrand over the same indices), f64 depths, unitig types and no sequence paths
     void replace_unitigs(const std::vector<uint32_t>& numbers, const std::vector<std::string>& seqs, const std::vector<double>& depths,
                          const std::vector<uint8_t>& types, const std::vector<std::vector<UStrand>>& next_lists, const std::vector<std::vector<UStrand>>& prev_lists);
+    // clean's graph edits (host_clean.cpp), on the unitigs in list order; each keeps only the position counts (set_position_counts).
+    // Errors: InputError.
+    void remove_unitigs(const std::vector<uint32_t>& numbers);   // remove_unitigs_by_number (unitig_graph.rs:588-592)
+    void duplicate_unitig(uint32_t num);                         // duplicate_unitig_by_number (:594-668)
+    void remove_low_depth_unitigs(double min_depth);             // :670-721
+    // what a loaded graph's positions tell merge_linear_paths once clean has edited the graph: counts[i] = forward_positions.len() of
+    // unitig i (index order), carried as paths of single steps (the sequences themselves are not kept)
+    void set_position_counts(const std::vector<uint32_t>& counts);
+    bool is_isolated_and_circular(uint32_t idx) const;           // unitig.rs:275-281: one circularising link and no other
+    bool is_isolated_and_linear(uint32_t idx) const;             // :283-292: no links but hairpins
     // unitig_graph.rs:317-360; other_colour: colour_tag(true) (unitig.rs:173-181), Other unitigs get CL:Z:orangered
     void gfa_text(const std::vector<HostSeq>& seqs, std::string& out, bool other_colour = false) const;
     uint64_t total_length() const;

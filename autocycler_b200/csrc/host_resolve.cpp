@@ -16,6 +16,7 @@
 #include <unordered_map>
 
 #include "host_cluster.h"
+#include "host_edit.h"
 #include "pipeline.h"
 
 namespace {
@@ -105,93 +106,6 @@ void bridge_best_paths(DevicePipeline& pipe, const std::vector<std::vector<Path>
 // the graph resolve edits
 // ------------------------------------------------------------------------------------------------
 namespace {
-struct EditGraph {
-    std::vector<uint32_t> number;
-    std::vector<std::string> seq;
-    std::vector<double> depth;
-    std::vector<uint8_t> type;                        // 0 Other, 1 Anchor, 2 Bridge, 3 Consentig
-    std::vector<std::vector<UStrand>> nx, pv;         // [2 i + reverse]: forward_next / reverse_next, forward_prev / reverse_prev
-    std::unordered_map<uint32_t, uint32_t> index;     // unitig_index: number -> position
-    uint32_t max_number = 0;
-
-    void from(const HostGraph& g) {
-        const uint32_t U = g.U;
-        std::vector<uint32_t> pos(U);
-        for (uint32_t n = 0; n < U; ++n) pos[g.order[n]] = n;
-        number.resize(U); seq.resize(U); depth.resize(U); type.resize(U); nx.assign(2 * (size_t)U, {}); pv.assign(2 * (size_t)U, {});
-        index.clear(); max_number = 0;
-        auto map = [&](UStrand s) { return us_make(pos[us_index(s)], us_reverse(s)); };
-        for (uint32_t n = 0; n < U; ++n) {
-            const uint32_t u = g.order[n];
-            number[n] = g.number[u]; seq[n].assign(g.seq_ptr(u), g.rec[u].len); depth[n] = g.depth_of(u); type[n] = g.type_of(u);
-            for (uint32_t r = 0; r < 2; ++r) {
-                const UStrand s = us_make(u, r != 0);
-                for (uint32_t x = 0; x < g.next_size(s); ++x) nx[2 * (size_t)n + r].push_back(map(g.next_begin(s)[x]));
-                for (uint32_t x = 0; x < g.prev_size(s); ++x) pv[2 * (size_t)n + r].push_back(map(g.prev_begin(s)[x]));
-            }
-            index[number[n]] = n;                     // build_unitig_index: the last unitig with a number wins
-            max_number = std::max(max_number, number[n]);
-        }
-    }
-    UStrand strand(int32_t s) const {
-        const auto it = index.find(abs_u32(s));
-        if (it == index.end()) throw std::runtime_error("unitig " + std::to_string(abs_u32(s)) + " not found in unitig index");
-        return us_make(it->second, s < 0);
-    }
-    void delete_one_way(UStrand s, UStrand e) {       // unitig_graph.rs:826-865: every matching entry, the others keep their order
-        std::vector<UStrand>& a = nx[s]; a.erase(std::remove(a.begin(), a.end(), e), a.end());
-        std::vector<UStrand>& b = pv[e]; b.erase(std::remove(b.begin(), b.end(), s), b.end());
-    }
-    void delete_link(UStrand s, UStrand e) { delete_one_way(s, e); delete_one_way(us_flip(e), us_flip(s)); }
-    void delete_outgoing_links(UStrand s) { const std::vector<UStrand> snap = nx[s]; for (UStrand e : snap) delete_link(s, e); }
-    void delete_incoming_links(UStrand e) { const std::vector<UStrand> snap = pv[e]; for (UStrand s : snap) delete_link(s, e); }
-    void create_one_way(UStrand s, UStrand e) { nx[s].push_back(e); pv[e].push_back(s); }
-    void create_link(UStrand s, UStrand e) { create_one_way(s, e); if (s != us_flip(e)) create_one_way(us_flip(e), us_flip(s)); }   // :867-872
-    uint32_t add_unitig(uint32_t num, std::string&& s, double d, uint8_t t) {
-        const uint32_t i = (uint32_t)number.size();
-        number.push_back(num); seq.push_back(std::move(s)); depth.push_back(d); type.push_back(t);
-        nx.resize(nx.size() + 2); pv.resize(pv.size() + 2);
-        index[num] = i; max_number = std::max(max_number, num);
-        return i;
-    }
-    // connected_components (:905-919) without an anchor, then remove_zero_depth_unitigs (depth > 0.0), both with delete_dangling_links
-    void prune() {
-        const uint32_t U = (uint32_t)number.size(), NONE = 0xFFFFFFFFu;
-        std::vector<uint32_t> comp(U, NONE), stack;
-        std::vector<uint8_t> comp_has_anchor;
-        for (uint32_t s = 0; s < U; ++s) {
-            if (comp[s] != NONE) continue;
-            const uint32_t c = (uint32_t)comp_has_anchor.size();
-            comp_has_anchor.push_back(0);
-            comp[s] = c; stack.assign(1, s);
-            while (!stack.empty()) {
-                const uint32_t u = stack.back(); stack.pop_back();
-                if (type[u] == 1) comp_has_anchor[c] = 1;
-                for (size_t l = 2 * (size_t)u; l < 2 * (size_t)u + 2; ++l)
-                    for (const std::vector<UStrand>* list : {&nx[l], &pv[l]})
-                        for (UStrand t : *list) if (comp[us_index(t)] == NONE) { comp[us_index(t)] = c; stack.push_back(us_index(t)); }
-            }
-        }
-        std::vector<uint32_t> new_index(U, NONE);
-        uint32_t kept = 0;
-        for (uint32_t u = 0; u < U; ++u) if (comp_has_anchor[comp[u]] && depth[u] > 0.0) new_index[u] = kept++;
-        EditGraph out;
-        for (uint32_t u = 0; u < U; ++u) {
-            if (new_index[u] == NONE) continue;
-            out.number.push_back(number[u]); out.seq.push_back(std::move(seq[u])); out.depth.push_back(depth[u]); out.type.push_back(type[u]);
-            for (size_t r = 0; r < 2; ++r) {
-                std::vector<UStrand> a, b;
-                for (UStrand t : nx[2 * (size_t)u + r]) if (new_index[us_index(t)] != NONE) a.push_back(us_make(new_index[us_index(t)], us_reverse(t)));
-                for (UStrand t : pv[2 * (size_t)u + r]) if (new_index[us_index(t)] != NONE) b.push_back(us_make(new_index[us_index(t)], us_reverse(t)));
-                out.nx.push_back(std::move(a)); out.pv.push_back(std::move(b));
-            }
-        }
-        for (uint32_t i = 0; i < kept; ++i) { out.index[out.number[i]] = i; out.max_number = std::max(out.max_number, out.number[i]); }
-        *this = std::move(out);
-    }
-    void to(HostGraph& g) const { g.replace_unitigs(number, seq, depth, type, nx, pv); }
-};
-
 struct Bridge {
     int32_t start, end;
     std::vector<Path> all_paths;       // the trimmed paths, duplicates included
@@ -467,22 +381,11 @@ void combine_texts(const std::vector<std::string>& gfas, const std::vector<std::
         g.load_gfa(gfas[f].data(), gfas[f].size(), seqs);
         const uint32_t U = g.U;
         auto only = [&](UStrand s, uint32_t u, bool rev) { return g.next_size(s) == 1 && g.next_begin(s)[0] == us_make(u, rev); };
-        auto isolated_circular = [&](uint32_t u) {    // unitig.rs:275-281
-            const UStrand fw = us_make(u, false);
-            return g.next_size(fw) == 1 && g.prev_size(fw) == 1 && g.next_begin(fw)[0] == fw && g.prev_begin(fw)[0] == fw;
-        };
-        auto all_are = [&](const UStrand* b, uint32_t n, UStrand x) { for (uint32_t i = 0; i < n; ++i) if (b[i] != x) return false; return true; };
-        auto isolated_linear = [&](uint32_t u) {      // :283-292
-            const UStrand fw = us_make(u, false), rv = us_make(u, true);
-            if (g.next_size(fw) > 1 || g.prev_size(fw) > 1 || isolated_circular(u)) return false;
-            return all_are(g.next_begin(fw), g.next_size(fw), rv) && all_are(g.prev_begin(fw), g.prev_size(fw), rv) &&
-                   all_are(g.next_begin(rv), g.next_size(rv), fw) && all_are(g.prev_begin(rv), g.prev_size(rv), fw);
-        };
         std::string topology;                          // unitig_graph.rs:527-545
         if (U == 0) topology = "empty";
         else if (U > 1) topology = "fragmented";
         else if (g.n_links == 0) topology = "linear-open-open";
-        else if (isolated_circular(0)) topology = "circular";
+        else if (g.is_isolated_and_circular(0)) topology = "circular";
         else {
             const bool hs = only(us_make(0, true), 0, false), he = only(us_make(0, false), 0, true);
             const bool os = g.next_size(us_make(0, true)) == 0, oe = g.next_size(us_make(0, false)) == 0;
@@ -500,7 +403,8 @@ void combine_texts(const std::vector<std::string>& gfas, const std::vector<std::
             const char* colour = t == 1 ? "\tCL:Z:forestgreen" : t == 2 ? "\tCL:Z:pink" : t == 3 ? "\tCL:Z:steelblue" : "\tCL:Z:orangered";
             gfa += "S\t" + num + "\t" + seq + "\tDP:f:" + std::string(tmp, gfa_depth_text(tmp, g.depth_of(u))) + colour + "\n";
             fasta += ">" + num + " length=" + std::to_string(g.rec[u].len) +
-                     (isolated_circular(u) ? " circular=true topology=circular" : isolated_linear(u) ? " circular=false topology=linear" : "") + "\n" + seq + "\n";
+                     (g.is_isolated_and_circular(u) ? " circular=true topology=circular" : g.is_isolated_and_linear(u) ? " circular=false topology=linear" : "") +
+                     "\n" + seq + "\n";
         }
         for (uint32_t n = 0; n < U; ++n) {             // get_links_for_gfa(offset): forward_next, then reverse_next
             const uint32_t u = g.order[n];

@@ -19,6 +19,10 @@
  *   Bridge::new (best path of a bridge)     resolve.rs:430-462       -> ac_bridge_best_paths
  *   resolve.rs:41-67 on a loaded graph                               -> ac_resolve, ac_resolve_text, ac_resolve_stats
  *   resolve / combine (the whole subcommands)  resolve.rs:31-69, combine.rs:25-49 -> ac_resolve_dir, ac_combine_dir
+ *   clean (the whole subcommand)            clean.rs:23-149          -> ac_clean_gfa
+ *   clean.rs:26-45 on a GFA text            unitig_graph.rs:588-721  -> ac_clean_text
+ *   gfa2fasta (the whole subcommand)        gfa2fasta.rs:23-82       -> ac_gfa_to_fasta, ac_gfa_fasta_text
+ *   table (the whole subcommand)            table.rs:24-204, misc.rs:373-386 -> ac_table_text
  *   create_dotplot without the file         dotplot.rs:179-221       -> ac_dotplot_rgb
  *   dotplot (the whole subcommand)          dotplot.rs:44-52         -> ac_dotplot_dir, ac_png_write
  *
@@ -306,6 +310,29 @@ int ac_resolve_dir(const char* cluster_dir, int32_t verbose, int32_t device);
 /* `autocycler combine -a autocycler_dir -i gfa [gfa ...]` (main.rs:115-124, combine.rs:25-137): writes consensus_assembly.gfa, .fasta and
  * .yaml under autocycler_dir (created if needed) from the n_gfas GFAs in argument order.  Host only. */
 int ac_combine_dir(const char* autocycler_dir, const char* const* in_gfas, uint32_t n_gfas, int32_t verbose);
+
+/* `autocycler clean`, `autocycler gfa2fasta` and `autocycler table`: host only, no device and no handle.  The getters follow the
+ * two-call convention: `out` NULL asks for the length, then a buffer of that size takes the text (AC_ERANGE when `cap` is short).
+ * The reference's input errors are AC_EINPUT, with its messages; a tig both removed and duplicated, and a tig duplicated twice, which
+ * make the reference panic, are AC_EINPUT too.
+ *
+ * `autocycler clean -i in_gfa -o out_gfa [-r LIST] [-d LIST] [-m DEPTH]` (main.rs:69-90, clean.rs:23-149): remove and duplicate are the
+ * comma-separated tig lists (NULL for none), min_depth is NULL for none.  Removes, duplicates, drops low-depth tigs that leave no dead
+ * end, merges linear paths, renumbers and saves (Other unitigs CL:Z:orangered, no P lines). */
+int ac_clean_gfa(const char* in_gfa, const char* out_gfa, const char* remove, const char* duplicate, const double* min_depth, int32_t verbose);
+/* clean.rs:26-45 on a GFA text with the tig numbers already parsed (any order).  merge = 0 stops before merge_linear_paths and
+ * renumber_unitigs and saves the edited graph in its list order. */
+int ac_clean_text(const char* gfa_text, uint64_t length, const uint32_t* remove, uint64_t n_remove, const uint32_t* duplicate,
+                  uint64_t n_duplicate, const double* min_depth, int32_t merge, char* out, uint64_t cap, uint64_t* out_length);
+/* `autocycler gfa2fasta -i in_gfa -o out_fasta` (main.rs:183-192, gfa2fasta.rs:23-82): every non-empty unitig in the file's order,
+ * with circular=true / circular=false topology in the headers. */
+int ac_gfa_to_fasta(const char* in_gfa, const char* out_fasta, int32_t verbose);
+int ac_gfa_fasta_text(const char* gfa_text, uint64_t length, char* out, uint64_t cap, uint64_t* out_length);   /* save_graph_to_fasta's text */
+/* `autocycler table [-a dir] [-n name] [-f fields] [-s sigfigs]` (main.rs:276-299, table.rs:24-204): with autocycler_dir NULL the header
+ * line, else the name and each field's value from the directory's YAML files, tab-separated, newline included.  fields NULL takes the
+ * reference's default list.  verbose: the "not found" warnings on stderr.  Unlike the reference, nothing is printed before an error. */
+int ac_table_text(const char* autocycler_dir, const char* name, const char* fields, uint64_t sigfigs, int32_t verbose, char* out, uint64_t cap,
+                  uint64_t* length);
 
 /* `autocycler dotplot`.  The all-vs-all k-mer dots (dotplot.rs:202-211, 394-450) run on the GPU: every window of only ACGT gets its
  * canonical k-mer, the windows are grouped by it, and each ordered pair of windows in a group is one dot whose 64-bit key (pair of
