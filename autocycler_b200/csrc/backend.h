@@ -15,6 +15,9 @@
 #include <stdexcept>
 #include <string>
 
+// Kernels launched by this process (bench.py's "gpu_launches"); defined in pipeline.cu
+extern unsigned long long g_ac_kernel_launches;
+
 #ifdef AC_EMULATE
 // ------------------------------------------------------------------------------------------------
 #define AC_HD inline
@@ -45,6 +48,13 @@ inline void ac_copy_dd(void* dst, const void* src, size_t bytes, AcStream*) { me
 inline void ac_sync(AcStream*) {}
 inline void* ac_host_alloc(size_t bytes) { return malloc(bytes ? bytes : 1); }
 inline void ac_host_free(void* p) { free(p); }
+inline int ac_smem_optin() { return 227 * 1024; }         // what an H100 grants one CTA
+struct AcTimer { explicit AcTimer(AcStream*) {} void stop() {} float ms() const { return 0.f; } };
+struct DeviceContext {
+    int device; AcStream stream{};
+    DeviceContext(int device, void*) : device(device) {}
+    void make_current() const {}
+};
 
 template <class Body> inline void ac_launch(const char*, AcStream*, const Body& body, uint64_t n);
 template <int CTAS, class Body> inline void ac_launch_occ(const char* name, AcStream* st, const Body& body, uint64_t n) { ac_launch(name, st, body, n); }
@@ -124,12 +134,51 @@ inline uint64_t ac_sm_count() {
     if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
     return (uint64_t)sms;
 }
+// Opt-in shared memory one CTA may ask for (227 KiB on an H100), read once: every device a process drives is the same model
+inline int ac_smem_optin() {
+    static int optin = -1;
+    if (optin < 0) { int dev = 0; AC_CUDA_CHECK(cudaGetDevice(&dev)); AC_CUDA_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev)); }
+    return optin;
+}
+// Device time of what a stream runs between the constructor and stop() (two CUDA events); ms() once the stream has synced
+class AcTimer {
+    cudaEvent_t e0 = nullptr, e1 = nullptr; AcStream* st;
+public:
+    explicit AcTimer(AcStream* st) : st(st) { AC_CUDA_CHECK(cudaEventCreate(&e0)); AC_CUDA_CHECK(cudaEventCreate(&e1)); AC_CUDA_CHECK(cudaEventRecord(e0, st->s)); }
+    AcTimer(const AcTimer&) = delete; AcTimer& operator=(const AcTimer&) = delete;
+    ~AcTimer() { cudaEventDestroy(e0); cudaEventDestroy(e1); }
+    void stop() { AC_CUDA_CHECK(cudaEventRecord(e1, st->s)); }
+    float ms() const { float t = 0.f; AC_CUDA_CHECK(cudaEventElapsedTime(&t, e0, e1)); return t; }
+};
+// The device and stream a device object runs on: the caller's stream, or (null) a non-blocking stream of its own
+struct DeviceContext {
+    int device; AcStream stream; bool own_stream = false;
+    DeviceContext(int device, void* s) : device(device) {
+        int n = 0;
+        cudaError_t e = cudaGetDeviceCount(&n);
+        if (e != cudaSuccess || n == 0)
+            throw std::runtime_error(std::string("autocycler_gpu: no CUDA device available (") + cudaGetErrorString(e) + "); this library has no CPU path");
+        AC_CUDA_CHECK(cudaSetDevice(device));
+        if (s) stream.s = (cudaStream_t)s;
+        else { AC_CUDA_CHECK(cudaStreamCreateWithFlags(&stream.s, cudaStreamNonBlocking)); own_stream = true; }
+    }
+    DeviceContext(const DeviceContext&) = delete; DeviceContext& operator=(const DeviceContext&) = delete;
+    ~DeviceContext() { if (own_stream) { cudaSetDevice(device); cudaStreamDestroy(stream.s); } }
+    void make_current() const { AC_CUDA_CHECK(cudaSetDevice(device)); }
+};
 
 #ifdef __CUDACC__
 #include <cooperative_groups.h>
-// Every functor-body kernel is launched through this one grid-stride template; the launch counter
-// feeds bench.py's "gpu_launches".
-extern unsigned long long g_ac_kernel_launches;
+// Every kernel but the cooperative ones is launched here: a dynamic shared-memory size is opted into, a launch error names the kernel, the launch is counted
+// and AC_SYNC_LAUNCHES waits for it.
+template <class... P, class... A> inline void ac_launch_kernel(const char* name, AcStream* st, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, A... args) {
+    if (smem > 0) AC_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<grid, block, smem, st->s>>>(args...);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) throw std::runtime_error(std::string("launch ") + name + ": " + cudaGetErrorString(e));
+    ++g_ac_kernel_launches;
+    ac_debug_sync(name, st);
+}
 
 // The trip count is the same for every lane of a warp and the lanes meet again after each unit: bodies with data-dependent
 // latency (hash probes) otherwise let the lanes drift into different iterations and the warp issues every instruction for a
@@ -159,12 +208,7 @@ template <int CTAS, class Body> inline void ac_launch_occ(const char* name, AcSt
     if (n == 0) return;
     const int threads = 256;
     const uint64_t want = (n + threads - 1) / threads, max_blocks = ac_sm_count() * (uint64_t)CTAS * 2;   // two waves of resident CTAs, grid-stride beyond
-    const unsigned blocks = (unsigned)(want < max_blocks ? want : max_blocks);
-    ac_body_kernel_occ<Body, CTAS><<<blocks, threads, 0, st->s>>>(body, n);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) throw std::runtime_error(std::string("launch ") + name + ": " + cudaGetErrorString(e));
-    ++g_ac_kernel_launches;
-    ac_debug_sync(name, st);
+    ac_launch_kernel(name, st, ac_body_kernel_occ<Body, CTAS>, (unsigned)(want < max_blocks ? want : max_blocks), threads, 0, body, n);
 }
 
 // Cooperative launch (all CTAs co-resident): body(thread, n_threads, sync) walks its items with stride n_threads and may call
@@ -201,12 +245,82 @@ template <class Body> inline void ac_launch(const char* name, AcStream* st, cons
     const int threads = 256;
     uint64_t want = (n + threads - 1) / threads;
     const uint64_t max_blocks = ac_sm_count() * 16;   // every SM x 16 256-thread CTAs (two waves of the 8 an SM holds), grid-stride beyond that
-    unsigned blocks = (unsigned)(want < max_blocks ? want : max_blocks);
-    ac_body_kernel<Body><<<blocks, threads, 0, st->s>>>(body, n);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) throw std::runtime_error(std::string("launch ") + name + ": " + cudaGetErrorString(e));
-    ++g_ac_kernel_launches;
-    ac_debug_sync(name, st);
+    ac_launch_kernel(name, st, ac_body_kernel<Body>, (unsigned)(want < max_blocks ? want : max_blocks), threads, 0, body, n);
 }
 #endif   // __CUDACC__
 #endif
+
+struct DevBuf {
+    void* p = nullptr; size_t cap = 0;
+    void ensure(size_t bytes) {
+        if (bytes > cap) {
+            ac_dev_free(p); p = nullptr; cap = 0; p = ac_dev_alloc(bytes); cap = bytes;
+#ifdef AC_EMULATE
+            static const bool poison = getenv("AC_EMU_POISON") != nullptr;
+            if (poison) memset(p, 0xA5, cap);
+#endif
+        }
+    }
+    template <class T> T* as() { return (T*)p; }
+    ~DevBuf() { ac_dev_free(p); }
+};
+
+struct PinBuf {   // pinned host memory: D2H lands at DMA speed and the host graph works on it in place
+    void* p = nullptr; size_t cap = 0;
+    void ensure(size_t bytes) { if (bytes > cap) { ac_host_free(p); p = nullptr; cap = 0; p = ac_host_alloc(bytes); cap = bytes; } }
+    template <class T> T* as() { return (T*)p; }
+    ~PinBuf() { ac_host_free(p); }
+};
+
+// Exclusive scan from serial pieces, for small volumes: one thread sums each tile of TILE values, the tile sums are scanned the same way
+// one level up, then each thread writes its tile's prefixes.  out may alias in.  Returns the total when asked (one host round trip).
+template <class T, uint64_t TILE, int LEVELS> struct SerialScan {
+    DevBuf level[LEVELS];                    // the tile sums of every level
+    T run(AcStream* st, const T* in, T* out, uint64_t n, bool want_total, int l = 0);
+};
+#if defined(AC_EMULATE) || defined(__CUDACC__)
+template <class T, uint64_t TILE> struct ScanSumBody {
+    const T* in; uint64_t n; T* sums;
+    AC_D void operator()(uint64_t t) const {
+        const uint64_t lo = t * TILE, hi = lo + TILE < n ? lo + TILE : n;
+        T s = 0;
+        for (uint64_t x = lo; x < hi; ++x) s += in[x];
+        sums[t] = s;
+    }
+};
+template <class T, uint64_t TILE> struct ScanApplyBody {
+    const T* in; T* out; uint64_t n; const T* tile_off;
+    AC_D void operator()(uint64_t t) const {
+        const uint64_t lo = t * TILE, hi = lo + TILE < n ? lo + TILE : n;
+        T acc = tile_off ? tile_off[t] : 0;
+        for (uint64_t x = lo; x < hi; ++x) { const T v = in[x]; out[x] = acc; acc += v; }
+    }
+};
+template <class T, uint64_t TILE, int LEVELS> T SerialScan<T, TILE, LEVELS>::run(AcStream* st, const T* in, T* out, uint64_t n, bool want_total, int l) {
+    if (n == 0) return 0;
+    if (l >= LEVELS) throw std::runtime_error("scan too deep");
+    const uint64_t nb = (n + TILE - 1) / TILE;
+    if (nb == 1 && !want_total) { ac_launch("scan_apply", st, ScanApplyBody<T, TILE>{in, out, n, nullptr}, 1); return 0; }
+    level[l].ensure(nb * sizeof(T));
+    T* sums = level[l].template as<T>();
+    T total = 0;
+    ac_launch("scan_sum", st, ScanSumBody<T, TILE>{in, n, sums}, nb);
+    if (nb == 1) { ac_d2h(&total, sums, sizeof(T), st); ac_sync(st); }
+    else total = run(st, sums, sums, nb, want_total, l + 1);
+    ac_launch("scan_apply", st, ScanApplyBody<T, TILE>{in, out, n, nb == 1 ? nullptr : sums}, nb);
+    return total;
+}
+#endif
+
+// Exclusive scan of n u32 values in one launch (ac_scan_chained_kernel; serial tiles of 256 under emulation), with the state it keeps
+// from one scan to the next.  out may alias in.  Returns the total when asked: that costs one host round trip.
+struct DeviceScan {
+    uint32_t operator()(AcStream* st, const uint32_t* in, uint32_t* out, uint64_t n, bool want_total = true);
+    // in place; x[n-1] must be 0, so that the scanned x[n-1] is the total, which stays on the device (copied to total_dst)
+    void keep_total(AcStream* st, uint32_t* x, uint64_t n, uint32_t* total_dst) { (*this)(st, x, x, n, false); ac_copy_dd(total_dst, x + (n - 1), 4, st); }
+#ifndef AC_EMULATE
+    DevBuf state; unsigned long long epoch = 0, tickets = 0;
+#else
+    SerialScan<uint32_t, 256, 4> serial;
+#endif
+};

@@ -30,7 +30,7 @@
 #include <immintrin.h>
 #include <functional>
 #include <thread>
-#include "pipeline.h"
+#include "commands.h"
 
 namespace {
 thread_local std::string g_error;
@@ -64,6 +64,11 @@ struct ac_handle {
     LoadedInput loaded;                    // only when filled by ac_load_sequences (keeps the YAML details)
     std::unique_ptr<DevicePipeline> pipe;                   // the pipeline that finishes the graph (devices[0])
     std::vector<std::unique_ptr<DevicePipeline>> peers;     // ac_config.n_devices > 1: the pipelines of devices[1..]
+    // trim and resolve's alignments, cluster's distances and tree: on pipe's device and stream, made on first use
+    std::unique_ptr<DeviceAlign> aligner;
+    std::unique_ptr<DeviceCluster> clusterer;
+    DeviceAlign& align_device() { if (!aligner) aligner.reset(new DeviceAlign(pipe->context())); return *aligner; }
+    DeviceCluster& cluster_device() { if (!clusterer) clusterer.reset(new DeviceCluster(pipe->context())); return *clusterer; }
     const char* path_lines = nullptr; uint64_t path_lines_len = 0;     // ac_path_lines_render: this rank's P lines (pinned, owned by the pipeline)
     std::vector<int32_t> devices;
     PipelineResult res;
@@ -654,7 +659,7 @@ int ac_pairwise_distances(ac_handle* h, double* out, uint64_t cap) {
     std::vector<uint32_t> len(g.U);
     for (uint32_t u = 0; u < g.U; ++u) len[u] = g.rec[u].len;
     std::vector<uint64_t> shared(S * S);
-    h->pipe->pair_shared_lengths(g.path, g.path_off, (uint32_t)S, len.data(), g.U, shared.data());
+    h->cluster_device().pair_shared_lengths(g.path, g.path_off, (uint32_t)S, len.data(), g.U, shared.data());
     for (uint64_t a = 0; a < S; ++a) {
         const double a_len = (double)(uint32_t)shared[a * S + a];                    // the reference sums u32 lengths, then converts
         for (uint64_t b = 0; b < S; ++b) out[a * S + b] = 1.0 - ((double)shared[a * S + b] / a_len);
@@ -1020,7 +1025,7 @@ int ac_trim_paths(ac_handle* h, int32_t mode, const int32_t* paths, const uint64
     std::vector<uint32_t> w(weights, weights + n_weights);
     std::vector<uint8_t> ok_flags;
     TrimStats st;
-    trim_paths(*h->pipe, (TrimMode)mode, in, w, min_identity, max_unitigs, ok_flags, res, st);
+    trim_paths(h->align_device(), (TrimMode)mode, in, w, min_identity, max_unitigs, ok_flags, res, st);
     uint64_t at = 0;
     out_off[0] = 0;
     for (uint64_t x = 0; x < n_paths; ++x) {
@@ -1039,7 +1044,7 @@ int ac_trim(ac_handle* h, double min_identity, uint32_t max_unitigs, double mad)
     if (!h->built) return set_error(h, AC_EINVAL, "a graph must be built or loaded before ac_trim");
     ensure_graph(h);
     TrimStats st;
-    trim_graph(h->graph, h->seqs, *h->pipe, min_identity, max_unitigs, mad, false, st);
+    trim_graph(h->graph, h->seqs, h->align_device(), min_identity, max_unitigs, mad, false, st);
     h->infos.clear(); h->ascii.clear();      // the sequences are trimmed paths now: no bytes
     h->trim_yaml = trimmed_metrics_yaml(h->seqs); h->trimmed = true;
     h->t.trim_kernel = st.kernel_ms; h->trim_stats = st;
@@ -1078,7 +1083,7 @@ int ac_trim_dir(const char* cluster_dir, double min_identity, uint32_t max_uniti
     if ((rc = read_file(in_gfa, text)) != AC_OK || (rc = make_handle(device, h)) != AC_OK || (rc = load_input_gfa(h.get(), text)) != AC_OK) return rc;
     if (verbose && max_unitigs == 0) fprintf(stderr, "Since --max_unitigs was set to 0, trimming is disabled.\n\n");
     TrimStats ts;
-    trim_graph(h->graph, h->seqs, *h->pipe, min_identity, max_unitigs, mad, verbose != 0, ts);
+    trim_graph(h->graph, h->seqs, h->align_device(), min_identity, max_unitigs, mad, verbose != 0, ts);
     h->graph.gfa_text(h->seqs, h->gfa);
     if (!write_file(out_gfa, h->gfa)) return set_error(nullptr, AC_EIO, "cannot write " + out_gfa);
     if (!write_file(out_yaml, trimmed_metrics_yaml(h->seqs))) return set_error(nullptr, AC_EIO, "cannot write " + out_yaml);
@@ -1096,7 +1101,7 @@ int ac_upgma(ac_handle* h, const double* sym_dist, uint32_t n, const uint32_t* i
         for (uint64_t j = 0; j < n; ++j)
             if (i != j && sym_dist[i * n + j] != sym_dist[i * n + j]) return set_error(h, AC_EINPUT, "the distance matrix holds a NaN off its diagonal");
     std::vector<UpgmaMerge> m(n > 1 ? n - 1 : 0);
-    h->cluster_stats.upgma_ms = h->pipe->upgma(sym_dist, n, ids, m.data());
+    h->cluster_stats.upgma_ms = h->cluster_device().upgma(sym_dist, n, ids, m.data());
     for (size_t x = 0; x < m.size(); ++x) { node[x] = m[x].node; left[x] = m[x].left; right[x] = m[x].right; dist[x] = m[x].dist; }
     return ok(h);
     AC_GUARD_END(h)
@@ -1117,7 +1122,7 @@ int ac_cluster(ac_handle* h, double cutoff, int64_t min_assemblies, const uint16
     std::string text;
     h->graph.gfa_text(h->seqs, text);
     std::vector<HostSeq> seqs = h->seqs;
-    cluster_graph(text, h->graph, seqs, *h->pipe, cutoff, min_assemblies < 0 ? -1 : min_assemblies, man, 0xFFFFFFFFu, "clustering", false, h->cluster, h->cluster_stats);
+    cluster_graph(text, h->graph, seqs, h->cluster_device(), cutoff, min_assemblies < 0 ? -1 : min_assemblies, man, 0xFFFFFFFFu, "clustering", false, h->cluster, h->cluster_stats);
     h->clustered = true;
     return ok(h);
     AC_GUARD_END(h)
@@ -1181,7 +1186,7 @@ int ac_cluster_dir(const char* autocycler_dir, double cutoff, int64_t min_assemb
     if ((rc = read_file(gfa, text)) != AC_OK || (rc = make_handle(device, h)) != AC_OK || (rc = load_input_gfa(h.get(), text)) != AC_OK) return rc;
     const std::vector<uint16_t> man = manual ? parse_manual_clusters(manual) : std::vector<uint16_t>();
     if (verbose) fprintf(stderr, "Settings:\n  --autocycler_dir %s\n", dir.c_str());
-    cluster_graph(text, h->graph, h->seqs, *h->pipe, cutoff, min_assemblies < 0 ? -1 : min_assemblies, man, max_contigs, cdir, verbose != 0, h->cluster, h->cluster_stats);
+    cluster_graph(text, h->graph, h->seqs, h->cluster_device(), cutoff, min_assemblies < 0 ? -1 : min_assemblies, man, max_contigs, cdir, verbose != 0, h->cluster, h->cluster_stats);
     const ClusterResult& r = h->cluster;
     const std::string phylip = cdir + "/pairwise_distances.phylip", newick = cdir + "/clustering.newick", tsv = cdir + "/clustering.tsv";
     bool good = write_file(phylip, r.phylip) && write_file(newick, r.newick);
@@ -1221,7 +1226,7 @@ int ac_bridge_best_paths(ac_handle* h, const int32_t* paths, const uint64_t* pat
     std::vector<std::vector<uint32_t>> tot;
     std::vector<std::vector<int32_t>> bp;
     ResolveStats st;
-    bridge_best_paths(*h->pipe, groups, w, tot, bp, st);
+    bridge_best_paths(h->align_device(), groups, w, tot, bp, st);
     uint64_t at = 0;
     best_off[0] = 0;
     for (uint64_t g = 0; g < n_groups; ++g) {
@@ -1242,7 +1247,7 @@ int ac_resolve(ac_handle* h, int32_t verbose) {
     h->resolved = false;
     std::string text;                      // the graph as a 2_trimmed.gfa: resolve re-loads it for its second pass (resolve.rs:59)
     h->graph.gfa_text(h->seqs, text);
-    resolve_text(text, *h->pipe, verbose != 0, h->resolve, h->resolve_stats);
+    resolve_text(text, h->align_device(), verbose != 0, h->resolve, h->resolve_stats);
     h->resolved = true;
     return ok(h);
     AC_GUARD_END(h)
@@ -1278,7 +1283,7 @@ int ac_resolve_dir(const char* cluster_dir, int32_t verbose, int32_t device) {
     if (verbose) fprintf(stderr, "\nStarting autocycler resolve\n    This command resolves repeats in the unitig graph.\n\nSettings:\n  --cluster_dir %s\n\n", dir.c_str());
     if ((rc = load_input_gfa(h.get(), text)) != AC_OK) return rc;
     ResolveResult r; ResolveStats rs;
-    resolve_text(text, *h->pipe, verbose != 0, r, rs);     // the file's own text, as the reference re-reads it (resolve.rs:59)
+    resolve_text(text, h->align_device(), verbose != 0, r, rs);     // the file's own text, as the reference re-reads it (resolve.rs:59)
     const std::string bridged = dir + "/3_bridged.gfa", merged = dir + "/4_merged.gfa", final_gfa = dir + "/5_final.gfa";
     if (!write_file(bridged, r.bridged) || !write_file(merged, r.merged) || !write_file(final_gfa, r.final_gfa))
         return set_error(nullptr, AC_EIO, "cannot write the output files under " + dir);
@@ -1410,14 +1415,18 @@ int ac_table_text(const char* autocycler_dir, const char* name, const char* fiel
 
 // ---- `autocycler dotplot` (dotplot.rs) ------------------------------------------------------------------------------------------
 namespace {
-// One pipeline per device for the dotplot calls, kept for the process so that its device buffers are reused by the next call.  The
-// lock is held for the whole call: calls on one device run one at a time.
+// One dotplot device object per device, on a stream of its own, kept for the process so that its device buffers are reused by the next
+// call.  The lock is held for the whole call: calls on one device run one at a time.
 std::mutex g_dotplot_mu;
-DevicePipeline& dotplot_pipeline(int32_t device) {        // with g_dotplot_mu held
-    static std::vector<std::pair<int32_t, DevicePipeline*>> pipes;
-    for (auto& p : pipes) if (p.first == device) return *p.second;
-    pipes.emplace_back(device, new DevicePipeline(device, nullptr));
-    return *pipes.back().second;
+struct DotplotDevice {
+    DeviceContext ctx; DeviceDotplot plot;
+    explicit DotplotDevice(int32_t device) : ctx(device, nullptr), plot(ctx) {}
+};
+DeviceDotplot& dotplot_device(int32_t device) {           // with g_dotplot_mu held
+    static std::vector<std::pair<int32_t, DotplotDevice*>> devices;
+    for (auto& d : devices) if (d.first == device) return d.second->plot;
+    devices.emplace_back(device, new DotplotDevice(device));
+    return devices.back().second->plot;
 }
 void fill_info(const DotplotStats& st, ac_dotplot_info* info) {
     if (!info) return;
@@ -1455,7 +1464,7 @@ int ac_dotplot_rgb(const char* const* seqs, const uint64_t* lengths, const char*
     DotplotStats st;
     {
         std::lock_guard<std::mutex> lock(g_dotplot_mu);
-        dotplot_image(dotplot_pipeline(device), in, res, kmer, f.get(), img, st);
+        dotplot_image(dotplot_device(device), in, res, kmer, f.get(), img, st);
     }
     memcpy(rgb, img.data(), img.size());
     fill_info(st, info);
@@ -1475,7 +1484,7 @@ int ac_dotplot_dir(const char* input, const char* out_png, uint32_t res, uint32_
     DotplotStats st;
     {
         std::lock_guard<std::mutex> lock(g_dotplot_mu);
-        dotplot_image(dotplot_pipeline(device), seqs, res, kmer, f.get(), img, st);
+        dotplot_image(dotplot_device(device), seqs, res, kmer, f.get(), img, st);
     }
     if (!png_write(out_png, img.data(), res, res)) return set_error(nullptr, AC_EIO, std::string("cannot write ") + out_png);
     fill_info(st, info);

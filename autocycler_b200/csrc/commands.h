@@ -1,0 +1,100 @@
+// The device parts of `autocycler trim`, `resolve`, `cluster` and `dotplot`.  Each object owns its device buffers (allocated on first
+// use, kept for the next call) and runs on the device and stream of the DeviceContext it is given, which must outlive it.
+#pragma once
+#include <cstdint>
+#include <vector>
+
+#include "backend.h"
+#include "pipeline.h"
+
+// One overlap alignment of `autocycler trim` (trim.rs:366-479): path_a's first k entries against path_b's last k, k = min(max_unitigs, n).
+// Both paths are n signed unitig numbers in the caller's value array.  skip_diagonal: the start-end form (path_a == path_b, cells with
+// global_i == global_j stay -inf, :395).
+struct OverlapJob { uint64_t a_off, b_off; uint32_t n, k, skip_diagonal, pad; };
+// One column of the traceback (trim.rs:329-335): GAP = 0 as a unitig, NONE = -1 as an index.
+struct AlignPiece { int32_t a_unitig, a_index, b_unitig, b_index; };
+// One path distance of `autocycler resolve` (global_alignment_distance, resolve.rs:387-418): the n values at a_off (rows, the shorter
+// path) against the m values at b_off, signed unitig numbers in the caller's value array.
+struct BridgeJob { uint64_t a_off, b_off; uint32_t n, m; };
+// What one bridge_distances call ran: jobs whose three diagonals sat in shared memory, jobs whose diagonals sat in HBM scratch.
+struct BridgeRun { uint32_t shared_jobs = 0, hbm_jobs = 0; };
+
+// Trim's overlap alignments and resolve's bridge distances: one CTA per job sweeps the anti-diagonals, with the three live ones in
+// shared memory or, when they do not fit, in HBM scratch.
+class DeviceAlign {
+public:
+    explicit DeviceAlign(DeviceContext& ctx) : ctx(ctx) {}
+    ~DeviceAlign() { ctx.make_current(); }
+    // trim.rs overlap_alignment up to the traceback, for a batch of jobs: fill, right-edge maximum and traceback on the device.
+    // weights[|unitig|] = unitig length.  out[j] = the traceback's pieces in alignment order, empty when the best right-edge score is <= 0
+    // or the traceback ends on the left edge; the identity test is the caller's.  Returns the kernels' time in ms (0 under emulation).
+    float overlap_align(const int32_t* values, uint64_t n_values, const uint32_t* weights, uint64_t n_weights,
+                        const OverlapJob* jobs, uint32_t n_jobs, std::vector<std::vector<AlignPiece>>& out);
+    // resolve.rs:387-418 for a batch of path pairs: dist[x] = the u32 (wrapping) edit distance of job x, weights[|unitig|] = unitig
+    // length.  Returns the kernels' time in ms (0 under emulation).
+    float bridge_distances(const int32_t* values, uint64_t n_values, const uint32_t* weights, uint64_t n_weights,
+                           const BridgeJob* jobs, uint32_t n_jobs, uint32_t* dist, BridgeRun* run);
+private:
+    DeviceContext& ctx;
+    DevBuf trim_jobs, trim_vals, trim_w, trim_bits, trim_scratch, trim_out, trim_len;
+    DevBuf br_jobs, br_vals, br_w, br_scratch, br_dist;
+};
+
+// One merge of `autocycler cluster`'s UPGMA (cluster.rs:410-430): the new node's number, its left child (the cluster with the smaller
+// id), its right child, and the node's distance to the tips (half the merged pair's mean distance).
+struct UpgmaMerge { uint32_t node, left, right, pad; double dist; };
+
+class DeviceCluster {
+public:
+    explicit DeviceCluster(DeviceContext& ctx) : ctx(ctx) {}
+    ~DeviceCluster() { ctx.make_current(); }
+    // cluster.rs:132-151 pairwise_contig_distances, the integer part: shared[a * n_seqs + b] = total length of the unitigs that the
+    // paths of sequences a and b have in common (the diagonal is the length of a's own unitig set).  Host arrays in, host array out.
+    void pair_shared_lengths(const UStrand* path, const uint64_t* path_off, uint32_t n_seqs, const uint32_t* unitig_len, uint32_t n_unitigs, uint64_t* shared);
+    // cluster.rs:132-192: the same shared lengths turned into the asymmetric distance matrix on the device (copied back into
+    // asym[n_seqs * n_seqs]) and its symmetric max, which stays in HBM for upgma(nullptr, ...).  Returns the kernels' time in ms.
+    float cluster_distances(const UStrand* path, const uint64_t* path_off, uint32_t n_seqs, const uint32_t* unitig_len, uint32_t n_unitigs, double* asym);
+    // UPGMA (cluster.rs:395-480) in one persistent CTA: n - 1 merges of the n clusters ids[0..n) (strictly ascending), new nodes numbered
+    // from ids[n-1] + 1.  sym: a symmetric n x n host matrix, or null for the one cluster_distances left on the device (used up).
+    // Returns the kernel's time in ms (0 under emulation).
+    float upgma(const double* sym, uint32_t n, const uint32_t* ids, UpgmaMerge* merges);
+private:
+    void upload_paths(const UStrand* path, const uint64_t* path_off, uint32_t n, const uint32_t* unitig_len, uint32_t U);   // and clears the outputs
+    void share_lengths(uint64_t steps, uint32_t n, uint32_t U);
+    DeviceContext& ctx;
+    DevBuf d_path, d_path_off, d_len, member, d_shared, d_asym;      // the paths and lengths of the call, not the compress graph's
+    DevBuf upgma_m, upgma_alive, upgma_cnt, upgma_node, upgma_rd, upgma_rj, upgma_list, upgma_out, upgma_done;
+    uint32_t sym_n = 0;                                      // upgma_m holds cluster_distances' symmetric matrix of this many sequences (0: none)
+};
+
+// One sequence of `autocycler dotplot` (dotplot.rs:394-450): its bytes at off in the caller's byte array, its first window's global
+// index (ascending; a sequence shorter than k has no windows) and the pixel its box starts at.
+struct DotplotSeq { uint64_t off, window_base; uint32_t len, start_px; };
+// What one dotplot call ran: windows with only ACGT (the device's), their distinct canonical k-mers, dots (sum of the groups' squared
+// sizes) and the kernels' time in ms (CUDA events; 0 under emulation).
+struct DotplotRun { uint64_t windows = 0, groups = 0, dots = 0; float kernel_ms = 0.f; };
+
+// A dot's key (dotplot.rs:202-211 loop order, last writer wins): the pixel shows the dot with the largest (a * n + b, j, forward), so
+// the key packs the pair of sequences above bit 34, b's window j in bits 2-33, forward in bit 1, and bit 0 set (0 is "no dot").
+inline uint64_t dotplot_key(uint64_t pair, uint32_t j, bool forward) { return (pair << 34) | ((uint64_t)j << 2) | ((uint64_t)forward << 1) | 1u; }
+#define AC_DOTPLOT_MAX_SEQS 32768u    // n * n pairs fit the key's 30 pair bits
+#define AC_DOT_SCAN_TILE 32           // values per thread of the u64 scan
+
+class DeviceDotplot {
+public:
+    explicit DeviceDotplot(DeviceContext& ctx) : ctx(ctx) {}
+    ~DeviceDotplot() { ctx.make_current(); }
+    // dotplot.rs:202-211 for every ordered pair of sequences at once: each window of only ACGT is grouped with the windows that share its
+    // canonical k-mer, and each ordered pair of windows in a group is one dot at (pixel of the first, pixel of the second), pixel =
+    // start_px + round(position / bpp).  Every pixel keeps the largest dot key (dotplot_key); host_idx / host_key add the dots the host
+    // found for the windows that hold other bytes.  rgb (res x res x 3) holds the base image on entry and the image with the dots on
+    // return.  bytes: the sequences, uppercased, at seqs[s].off.
+    void dotplot(const uint8_t* bytes, uint64_t n_bytes, const DotplotSeq* seqs, uint32_t n_seqs, uint32_t k, double bpp, uint32_t res,
+                 const uint64_t* host_idx, const uint64_t* host_key, uint64_t n_host, uint8_t* rgb, DotplotRun* run);
+private:
+    template <int W> void windows(uint64_t N, uint32_t n_seqs, uint32_t k, double bpp, uint64_t mask);
+    DeviceContext& ctx;
+    DeviceScan scan;
+    SerialScan<uint64_t, AC_DOT_SCAN_TILE, 8> scan_u64;          // of the groups' dot counts
+    DevBuf d_bytes, d_seqs, d_keys, d_px, d_tag, d_rep, d_cnt, d_off, d_fill, d_gpx, d_gtag, d_table, d_gstart, d_gsize, d_gdots, d_pix, d_rgb, d_hidx, d_hkey;
+};

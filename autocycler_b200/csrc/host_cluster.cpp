@@ -1,5 +1,5 @@
-// `autocycler cluster` (cluster.rs:30-912) on the host, around the device's distance and UPGMA kernels (DevicePipeline::cluster_distances,
-// DevicePipeline::upgma).  The f64 operations are the reference's, in its order, except where the reference's own order is a HashMap's
+// `autocycler cluster` (cluster.rs:30-912) on the host, around the device's distance and UPGMA kernels (DeviceCluster::cluster_distances,
+// DeviceCluster::upgma).  The f64 operations are the reference's, in its order, except where the reference's own order is a HashMap's
 // (DESIGN.md §12): the balance score sums clusters in ascending number, and a cluster contained in several passed clusters names the
 // smallest of them.
 #include "host_cluster.h"
@@ -14,7 +14,7 @@
 
 #include "host_io.h"
 #include "host_trim.h"
-#include "pipeline.h"
+#include "commands.h"
 
 namespace {
 void fail(const std::string& m) { throw InputError{m}; }
@@ -348,7 +348,7 @@ std::string distance_matrix_text(const std::vector<HostSeq>& seqs, const double*
     return text;
 }
 
-void cluster_graph(const std::string& gfa, const HostGraph& g, std::vector<HostSeq>& seqs, DevicePipeline& pipe, double cutoff, int64_t min_assemblies_opt,
+void cluster_graph(const std::string& gfa, const HostGraph& g, std::vector<HostSeq>& seqs, DeviceCluster& device, double cutoff, int64_t min_assemblies_opt,
                    const std::vector<uint16_t>& manual, uint32_t max_contigs, const std::string& out_dir, bool verbose, ClusterResult& out, ClusterStats& st) {
     const size_t S = seqs.size();
     std::set<std::string> files;
@@ -377,7 +377,7 @@ void cluster_graph(const std::string& gfa, const HostGraph& g, std::vector<HostS
     for (uint32_t u = 0; u < g.U; ++u) len[u] = g.rec[u].len;
     std::vector<double> asym(S * S);
     st = ClusterStats(); st.n_seqs = (uint32_t)S;
-    st.distance_ms = pipe.cluster_distances(g.path, g.path_off, (uint32_t)S, len.data(), g.U, asym.data());
+    st.distance_ms = device.cluster_distances(g.path, g.path_off, (uint32_t)S, len.data(), g.U, asym.data());
     // two sequences whose unitig sets are both empty have no distance (0 / 0): the reference's UPGMA cannot finish on them either
     for (size_t a = 0; a < S; ++a)
         for (size_t b = a + 1; b < S; ++b)
@@ -397,12 +397,12 @@ void cluster_graph(const std::string& gfa, const HostGraph& g, std::vector<HostS
     bool ordered = true;
     for (size_t i = 0; i < S; ++i) { ids[i] = seqs[by_id[i]].id; ordered = ordered && by_id[i] == i; }
     std::vector<UpgmaMerge> merges(S ? S - 1 : 0);
-    if (ordered) st.upgma_ms = pipe.upgma(nullptr, (uint32_t)S, ids.data(), merges.data());
+    if (ordered) st.upgma_ms = device.upgma(nullptr, (uint32_t)S, ids.data(), merges.data());
     else {
         std::vector<double> sym(S * S);
         for (size_t x = 0; x < S; ++x)
             for (size_t y = 0; y < S; ++y) { const double ab = asym[by_id[x] * S + by_id[y]], ba = asym[by_id[y] * S + by_id[x]]; sym[x * S + y] = (ab != ab || ab < ba) ? ba : ab; }
-        st.upgma_ms = pipe.upgma(sym.data(), (uint32_t)S, ids.data(), merges.data());
+        st.upgma_ms = device.upgma(sym.data(), (uint32_t)S, ids.data(), merges.data());
     }
     Tree t;
     const uint32_t n_nodes = ids.back() + (uint32_t)S;

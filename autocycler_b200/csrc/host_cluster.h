@@ -7,7 +7,7 @@
 
 #include "host_graph.h"
 
-class DevicePipeline;
+class DeviceCluster;
 
 struct ClusterStats {
     float distance_ms = 0, upgma_ms = 0;     // distance and UPGMA kernels, CUDA events (0 under emulation)
@@ -28,7 +28,7 @@ struct ClusterResult {
 // whose paths have no length).  verbose: the reference's stderr report, without colours.
 // `gfa` must describe the same graph as `g` (the reference re-loads it per cluster).  seqs[].cluster is set to the clusters.
 // out_dir: the clustering directory the verbose report names.
-void cluster_graph(const std::string& gfa, const HostGraph& g, std::vector<HostSeq>& seqs, DevicePipeline& pipe, double cutoff, int64_t min_assemblies,
+void cluster_graph(const std::string& gfa, const HostGraph& g, std::vector<HostSeq>& seqs, DeviceCluster& device, double cutoff, int64_t min_assemblies,
                    const std::vector<uint16_t>& manual, uint32_t max_contigs, const std::string& out_dir, bool verbose, ClusterResult& out, ClusterStats& stats);
 
 // Sequence::consensus_weight (sequence.rs:104-109): the autocycler_consensus_weight= value of the header, 1 when absent or unparsable

@@ -543,7 +543,7 @@ static uint32_t px_of(uint32_t start, uint32_t pos, double bpp) {               
     return start + sat_u32(v);
 }
 
-void dotplot_image(DevicePipeline& pipe, const std::vector<DotplotInput>& seqs, uint32_t res, uint32_t kmer, const DotplotFont* font,
+void dotplot_image(DeviceDotplot& device, const std::vector<DotplotInput>& seqs, uint32_t res, uint32_t kmer, const DotplotFont* font,
                    std::vector<uint8_t>& rgb, DotplotStats& st) {
     st = DotplotStats();
     const uint32_t n = (uint32_t)seqs.size();
@@ -615,7 +615,7 @@ void dotplot_image(DevicePipeline& pipe, const std::vector<DotplotInput>& seqs, 
     hidx.reserve(host_pix.size()); hkey.reserve(host_pix.size());
     for (const auto& e : host_pix) { hidx.push_back(e.first); hkey.push_back(e.second); }
     DotplotRun run;
-    pipe.dotplot((const uint8_t*)bytes.data(), bytes.size(), ds.data(), n, kmer, p.bpp, res, hidx.data(), hkey.data(), hidx.size(), rgb.data(), &run);
+    device.dotplot((const uint8_t*)bytes.data(), bytes.size(), ds.data(), n, kmer, p.bpp, res, hidx.data(), hkey.data(), hidx.size(), rgb.data(), &run);
     st.groups = run.groups; st.dots = run.dots + host_dots; st.kernel_ms = run.kernel_ms;
     draw_boxes(rgb, res, p, false);                                            // the outlines once more, over the dots (:213-215)
 }

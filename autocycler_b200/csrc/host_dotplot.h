@@ -1,12 +1,12 @@
 // `autocycler dotplot` on the host (dotplot.rs): inputs, layout, boxes, the dots of the windows the device does not take, and the PNG.
-// The dots of every window of only ACGT run on the GPU (DevicePipeline::dotplot).  Citations are file:line in the reference's src/.
+// The dots of every window of only ACGT run on the GPU (DeviceDotplot::dotplot).  Citations are file:line in the reference's src/.
 #pragma once
 #include <cstdint>
 #include <memory>
 #include <string>
 #include <vector>
 
-#include "pipeline.h"
+#include "commands.h"
 
 struct DotplotInput { std::string filename, name, seq; };        // FileSeqName and the bytes, uppercased (dotplot.rs:106-110)
 
@@ -27,7 +27,7 @@ struct DotplotFont;
 std::shared_ptr<DotplotFont> dotplot_font_load(const std::string& path);
 std::shared_ptr<DotplotFont> dotplot_font_default(std::string* found_path);
 // create_dotplot (dotplot.rs:179-221) into rgb (res x res x 3): boxes, labels (none when font is null), dots (device), outlines again
-void dotplot_image(DevicePipeline& pipe, const std::vector<DotplotInput>& seqs, uint32_t res, uint32_t kmer, const DotplotFont* font,
+void dotplot_image(DeviceDotplot& device, const std::vector<DotplotInput>& seqs, uint32_t res, uint32_t kmer, const DotplotFont* font,
                    std::vector<uint8_t>& rgb, DotplotStats& st);
 // an RGB8 PNG (colour type 2, no interlace, zlib), written to path; false on an I/O error
 bool png_write(const std::string& path, const uint8_t* rgb, uint32_t width, uint32_t height);

@@ -1,6 +1,6 @@
 // `autocycler resolve` (resolve.rs:31-514): anchors, bridges, ambiguity and culling, and the graph edits that apply the bridges, on the
 // host; the one step whose cost grows quadratically — global_alignment_distance between every pair of a bridge's paths (:430-462) — runs
-// on the device (DevicePipeline::bridge_distances).  `autocycler combine` (combine.rs:90-137) works on loaded graphs alone.
+// on the device (DeviceAlign::bridge_distances).  `autocycler combine` (combine.rs:90-137) works on loaded graphs alone.
 //
 // The graph edits work on per-strand link lists (the reference's forward_next / reverse_next / forward_prev / reverse_prev vectors, in
 // their order), and the host graph's CSR is rebuilt once from them (HostGraph::replace_unitigs) for merge_linear_paths, renumber_unitigs
@@ -17,7 +17,7 @@
 
 #include "host_cluster.h"
 #include "host_edit.h"
-#include "pipeline.h"
+#include "commands.h"
 
 namespace {
 typedef std::vector<int32_t> Path;
@@ -34,7 +34,7 @@ inline char complement(char c) { return c == 'A' ? 'T' : c == 'C' ? 'G' : c == '
 // ------------------------------------------------------------------------------------------------
 // Bridge::new: the best path of every bridge
 // ------------------------------------------------------------------------------------------------
-void bridge_best_paths(DevicePipeline& pipe, const std::vector<std::vector<Path>>& groups, const std::vector<uint32_t>& weights,
+void bridge_best_paths(DeviceAlign& device, const std::vector<std::vector<Path>>& groups, const std::vector<uint32_t>& weights,
                        std::vector<std::vector<uint32_t>>& totals, std::vector<std::vector<int32_t>>& best, ResolveStats& stats) {
     const size_t G = groups.size();
     totals.assign(G, {}); best.assign(G, {});
@@ -76,7 +76,7 @@ void bridge_best_paths(DevicePipeline& pipe, const std::vector<std::vector<Path>
     std::vector<uint32_t> dist(jobs.size());
     if (jobs.size() > 0xFFFFFFFFull) throw std::runtime_error("too many distance jobs");
     BridgeRun run;
-    stats.kernel_ms += pipe.bridge_distances(values.data(), values.size(), weights.data(), weights.size(), jobs.data(), (uint32_t)jobs.size(), dist.data(), &run);
+    stats.kernel_ms += device.bridge_distances(values.data(), values.size(), weights.data(), weights.size(), jobs.data(), (uint32_t)jobs.size(), dist.data(), &run);
     stats.jobs += jobs.size(); stats.shared_jobs += run.shared_jobs; stats.hbm_jobs += run.hbm_jobs;
     // total(p) = sum over the other distinct paths q of mult(q) * D(p, q), mod 2^32 (copies of p itself add D(p, p) = 0)
     std::vector<std::vector<uint32_t>> dtotal(G);
@@ -252,7 +252,7 @@ void HostGraph::replace_unitigs(const std::vector<uint32_t>& numbers, const std:
     check_links();
 }
 
-void resolve_text(const std::string& trimmed_gfa, DevicePipeline& pipe, bool verbose, ResolveResult& out, ResolveStats& stats) {
+void resolve_text(const std::string& trimmed_gfa, DeviceAlign& device, bool verbose, ResolveResult& out, ResolveStats& stats) {
     stats = ResolveStats();
     HostGraph g;
     std::vector<HostSeq> seqs;
@@ -318,7 +318,7 @@ void resolve_text(const std::string& trimmed_gfa, DevicePipeline& pipe, bool ver
     }
     std::vector<std::vector<uint32_t>> totals;
     std::vector<Path> best;
-    bridge_best_paths(pipe, groups, weights, totals, best, stats);
+    bridge_best_paths(device, groups, weights, totals, best, stats);
     std::vector<Bridge> bridges(groups.size());
     for (size_t x = 0; x < groups.size(); ++x) {
         bridges[x].start = keys[x].first; bridges[x].end = keys[x].second;

@@ -1,5 +1,5 @@
 // `autocycler resolve` (resolve.rs:31-514) on the host graph, with the bridges' all-pairs path distances on the device
-// (DevicePipeline::bridge_distances), and `autocycler combine` (combine.rs:25-137), which needs no device.
+// (DeviceAlign::bridge_distances), and `autocycler combine` (combine.rs:25-137), which needs no device.
 #pragma once
 #include <cstdint>
 #include <string>
@@ -7,7 +7,7 @@
 
 #include "host_graph.h"
 
-class DevicePipeline;
+class DeviceAlign;
 
 struct ResolveStats {
     uint32_t anchors = 0;             // anchor unitigs (find_anchor_unitigs, :134-163)
@@ -25,13 +25,13 @@ struct ResolveStats {
 // order, duplicates included.  Identical paths are aligned once, and only pairs of distinct paths go to the device, all groups in one
 // round.  totals[g][x] = path x's u32 (wrapping) total of distances to the other paths; best[g] = the path the reference selects (empty
 // when every total is u32::MAX).  weights[|unitig|] = unitig length.
-void bridge_best_paths(DevicePipeline& pipe, const std::vector<std::vector<std::vector<int32_t>>>& groups, const std::vector<uint32_t>& weights,
+void bridge_best_paths(DeviceAlign& device, const std::vector<std::vector<std::vector<int32_t>>>& groups, const std::vector<uint32_t>& weights,
                        std::vector<std::vector<uint32_t>>& totals, std::vector<std::vector<int32_t>>& best, ResolveStats& stats);
 
 struct ResolveResult { std::string bridged, merged, final_gfa; };    // 3_bridged.gfa, 4_merged.gfa, 5_final.gfa
 
 // resolve.rs:41-67 minus the file I/O, on the text of a 2_trimmed.gfa.  verbose: a stderr report of the steps.
-void resolve_text(const std::string& trimmed_gfa, DevicePipeline& pipe, bool verbose, ResolveResult& out, ResolveStats& stats);
+void resolve_text(const std::string& trimmed_gfa, DeviceAlign& device, bool verbose, ResolveResult& out, ResolveStats& stats);
 
 // combine.rs:90-137 on the texts of the clusters' final GFAs, in order: consensus_assembly.gfa, .fasta and .yaml (CombineMetrics,
 // metrics.rs:229-242, as serde_yaml 0.9 writes it).  verbose: the per-cluster graph summary on stderr.

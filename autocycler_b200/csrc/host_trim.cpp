@@ -1,4 +1,4 @@
-// `autocycler trim` (trim.rs:36-326): the overlap alignments run on the device in batches (DevicePipeline::overlap_align: fill,
+// `autocycler trim` (trim.rs:36-326): the overlap alignments run on the device in batches (DeviceAlign::overlap_align: fill,
 // right-edge maximum and traceback); what is O(k) per alignment — the identity test (:468-475), find_midpoint (:482-507) and the
 // hairpin walk (:299-317) — and the graph edits run here, in f64 and u32 exactly as the reference writes them.
 #include "host_trim.h"
@@ -9,7 +9,7 @@
 #include <deque>
 #include <stdexcept>
 
-#include "pipeline.h"
+#include "commands.h"
 
 namespace {
 const int32_t GAP = 0;                 // trim.rs:32
@@ -30,7 +30,7 @@ uint32_t weight_of(const std::vector<uint32_t>& w, int32_t u) {
 struct Pair { const std::vector<int32_t>* a; const std::vector<int32_t>* b; bool skip; };
 
 // overlap_alignment (:366-479) for a batch: the device's traceback, then the identity test
-std::vector<Alignment> overlap_alignments(DevicePipeline& pipe, const std::vector<Pair>& pairs, const std::vector<uint32_t>& weights,
+std::vector<Alignment> overlap_alignments(DeviceAlign& device, const std::vector<Pair>& pairs, const std::vector<uint32_t>& weights,
                                           double min_identity, uint32_t max_unitigs, TrimStats& stats) {
     std::vector<int32_t> values;
     std::vector<OverlapJob> jobs(pairs.size());
@@ -48,7 +48,7 @@ std::vector<Alignment> overlap_alignments(DevicePipeline& pipe, const std::vecto
     }
     for (int32_t v : values) weight_of(weights, v);
     std::vector<std::vector<AlignPiece>> raw;
-    stats.kernel_ms += pipe.overlap_align(values.data(), values.size(), weights.data(), weights.size(), jobs.data(), (uint32_t)jobs.size(), raw);
+    stats.kernel_ms += device.overlap_align(values.data(), values.size(), weights.data(), weights.size(), jobs.data(), (uint32_t)jobs.size(), raw);
     stats.rounds += 1; stats.jobs += jobs.size();
     std::vector<Alignment> out(pairs.size());
     for (size_t x = 0; x < pairs.size(); ++x) {
@@ -142,7 +142,7 @@ uint64_t round_to_usize(double x) {   // (x).round() as usize: half away from ze
 }
 }  // namespace
 
-void trim_paths(DevicePipeline& pipe, TrimMode mode, const std::vector<std::vector<int32_t>>& paths, const std::vector<uint32_t>& weights,
+void trim_paths(DeviceAlign& device, TrimMode mode, const std::vector<std::vector<int32_t>>& paths, const std::vector<uint32_t>& weights,
                 double min_identity, uint32_t max_unitigs, std::vector<uint8_t>& trimmed, std::vector<std::vector<int32_t>>& out, TrimStats& stats) {
     const size_t N = paths.size();
     trimmed.assign(N, 0); out.assign(N, {});
@@ -157,7 +157,7 @@ void trim_paths(DevicePipeline& pipe, TrimMode mode, const std::vector<std::vect
             pairs[x] = mode == TRIM_HAIRPIN_END ? Pair{&rev[x], &paths[x], false} : Pair{&paths[x], &rev[x], false};
         }
     }
-    const std::vector<Alignment> al = overlap_alignments(pipe, pairs, weights, min_identity, max_unitigs, stats);
+    const std::vector<Alignment> al = overlap_alignments(device, pairs, weights, min_identity, max_unitigs, stats);
     for (size_t x = 0; x < N; ++x) {
         if (mode == TRIM_START_END) trimmed[x] = finish_start_end(paths[x], al[x], weights, out[x]);
         else if (mode == TRIM_HAIRPIN_END) trimmed[x] = finish_hairpin_end(paths[x], al[x], out[x]);
@@ -243,7 +243,7 @@ std::string seq_display(const HostSeq& s) {     // sequence.rs:112-135 without t
 void section(bool verbose, const char* title) { if (verbose) fprintf(stderr, "\n%s\n", title); }
 }  // namespace
 
-void trim_graph(HostGraph& g, std::vector<HostSeq>& seqs, DevicePipeline& pipe, double min_identity, uint32_t max_unitigs, double mad,
+void trim_graph(HostGraph& g, std::vector<HostSeq>& seqs, DeviceAlign& device, double min_identity, uint32_t max_unitigs, double mad,
                 bool verbose, TrimStats& stats) {
     const size_t S = seqs.size();
     if (g.n_seqs != S) throw std::runtime_error("trim: the graph's paths do not match its sequences");
@@ -267,7 +267,7 @@ void trim_graph(HostGraph& g, std::vector<HostSeq>& seqs, DevicePipeline& pipe, 
         std::vector<std::vector<int32_t>> rev(S);
         for (size_t q = 0; q < S; ++q) rev[q] = reverse_path(paths[q]);
         for (size_t q = 0; q < S; ++q) { pairs.push_back(Pair{&paths[q], &paths[q], true}); pairs.push_back(Pair{&paths[q], &rev[q], false}); }
-        const std::vector<Alignment> r1 = overlap_alignments(pipe, pairs, weights, min_identity, max_unitigs, stats);
+        const std::vector<Alignment> r1 = overlap_alignments(device, pairs, weights, min_identity, max_unitigs, stats);
         std::vector<uint8_t> start_ok(S, 0);
         std::vector<std::vector<int32_t>> path2(S);
         for (size_t q = 0; q < S; ++q) {
@@ -279,7 +279,7 @@ void trim_graph(HostGraph& g, std::vector<HostSeq>& seqs, DevicePipeline& pipe, 
         std::vector<std::vector<int32_t>> rev2(S);
         pairs.clear();
         for (size_t q = 0; q < S; ++q) { rev2[q] = reverse_path(path2[q]); pairs.push_back(Pair{&rev2[q], &path2[q], false}); }
-        const std::vector<Alignment> r2 = overlap_alignments(pipe, pairs, weights, min_identity, max_unitigs, stats);
+        const std::vector<Alignment> r2 = overlap_alignments(device, pairs, weights, min_identity, max_unitigs, stats);
         for (size_t q = 0; q < S; ++q) {
             std::vector<int32_t> t;
             const bool end_ok = finish_hairpin_end(path2[q], r2[q], t);

@@ -1,4 +1,4 @@
-// `autocycler trim` (trim.rs:36-326) on the host graph, with the overlap alignments on the device (DevicePipeline::overlap_align).
+// `autocycler trim` (trim.rs:36-326) on the host graph, with the overlap alignments on the device (DeviceAlign::overlap_align).
 #pragma once
 #include <cstdint>
 #include <string>
@@ -6,7 +6,7 @@
 
 #include "host_graph.h"
 
-class DevicePipeline;
+class DeviceAlign;
 
 enum TrimMode { TRIM_START_END = 0, TRIM_HAIRPIN_START = 1, TRIM_HAIRPIN_END = 2 };
 
@@ -21,13 +21,13 @@ struct TrimStats {
 
 // trim_path_start_end / trim_path_hairpin_start / trim_path_hairpin_end (trim.rs:288-326) for every path of a batch, one device round.
 // weights[|unitig|] = unitig length.  trimmed[x] = 0: path x is not trimmed (out[x] is empty).
-void trim_paths(DevicePipeline& pipe, TrimMode mode, const std::vector<std::vector<int32_t>>& paths, const std::vector<uint32_t>& weights,
+void trim_paths(DeviceAlign& device, TrimMode mode, const std::vector<std::vector<int32_t>>& paths, const std::vector<uint32_t>& weights,
                 double min_identity, uint32_t max_unitigs, std::vector<uint8_t>& trimmed, std::vector<std::vector<int32_t>>& out, TrimStats& stats);
 
 // trim.rs:43-51 minus the file I/O: trims the sequences' paths, drops length outliers, cleans up the graph (recalculate_depths,
 // remove_zero_depth_unitigs, merge_linear_paths, renumber_unitigs).  `seqs` becomes the kept sequences in their order.  verbose: the
 // reference's stderr report.
-void trim_graph(HostGraph& g, std::vector<HostSeq>& seqs, DevicePipeline& pipe, double min_identity, uint32_t max_unitigs, double mad,
+void trim_graph(HostGraph& g, std::vector<HostSeq>& seqs, DeviceAlign& device, double min_identity, uint32_t max_unitigs, double mad,
                 bool verbose, TrimStats& stats);
 
 // median_isize / mad_isize (misc.rs:399-423), which median_usize / mad_usize equal on lengths

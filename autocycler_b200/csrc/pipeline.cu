@@ -15,11 +15,7 @@
 #include <cmath>
 #include <vector>
 
-#ifndef AC_EMULATE
 unsigned long long g_ac_kernel_launches = 0;
-#else
-static unsigned long long g_ac_kernel_launches = 0;
-#endif
 
 #define AC_NONE32 0xFFFFFFFFu
 #define AC_CHUNK 32            // windows per thread in the insert kernel
@@ -951,11 +947,8 @@ template <class Less> static uint32_t* sort_indices(AcStream* stream, const Less
     const uint64_t tiles = ((uint64_t)n + AC_SORT_TILE - 1) / AC_SORT_TILE;
 #ifndef AC_EMULATE
     const size_t smem = AC_SORT_TILE * (sizeof(SortRec) + 2 * sizeof(uint16_t));
-    AC_CUDA_CHECK(cudaFuncSetAttribute(ac_tile_sort_kernel<Less>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));      // per device: cheap enough to repeat
-    ac_tile_sort_kernel<Less><<<(unsigned)tiles, 1024, smem, stream->s>>>(less, n, a, ra); ++g_ac_kernel_launches;      // 32 warps on the SM: the searches are chains of dependent shared-memory loads
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) throw std::runtime_error(std::string("launch tile sort: ") + cudaGetErrorString(e));
-    ac_debug_sync("tile_sort", stream);
+    // 32 warps on the SM: the searches are chains of dependent shared-memory loads.  The shared-memory opt-in is per device: cheap enough to repeat
+    ac_launch_kernel("tile_sort", stream, ac_tile_sort_kernel<Less>, (unsigned)tiles, 1024, smem, less, n, a, ra);
 #else
     ac_launch("tile_sort", stream, TileSortBody<Less>{less, n, a, ra}, tiles);
 #endif
@@ -1613,140 +1606,6 @@ struct PathWrapBody {       // one thread per (sequence, prefix or suffix)
     }
 };
 
-// ---- contig distances (cluster.rs:132-151): which sequences pass through each unitig, then every pair of them shares its length ----
-struct PathMemberBody {
-    const UStrand* path; const uint64_t* path_off; uint32_t n_seqs, words; uint32_t* member;
-    AC_D void operator()(uint64_t x) const {
-        uint32_t lo = 0, hi = n_seqs;                    // the sequence whose path holds step x
-        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (path_off[mid] <= x) lo = mid; else hi = mid; }
-        ac_atomic_or(&member[(size_t)(path[x] >> 1) * words + (lo >> 5)], 1u << (lo & 31));
-    }
-};
-struct PairShareBody {
-    const uint32_t* member; const uint32_t* unitig_len; uint32_t n_seqs, words; unsigned long long* shared;
-    AC_D void operator()(uint64_t u) const {
-        const uint32_t* m = member + (size_t)u * words;
-        const unsigned long long len = unitig_len[u];
-        for (uint32_t wa = 0; wa < words; ++wa)
-            for (uint32_t ba = m[wa]; ba; ba &= ba - 1) {
-                const uint32_t a = (wa << 5) + (uint32_t)ac_ctz(ba);
-                for (uint32_t wb = 0; wb < words; ++wb)
-                    for (uint32_t bb = m[wb]; bb; bb &= bb - 1)
-                        ac_atomic_add(&shared[(size_t)a * n_seqs + (wb << 5) + (uint32_t)ac_ctz(bb)], len);
-            }
-    }
-};
-// cluster.rs:145-149 and 177-192: the asymmetric distance 1 - shared / a_len (a_len: the u32 sum the reference converts) and its symmetric
-// max.  No multiply, so nothing contracts into an FMA, and f64 division is IEEE: the bits equal ac_pairwise_distances' host division.
-struct DistanceBody {
-    const unsigned long long* shared; uint32_t n; double* asym; double* sym;
-    AC_D void operator()(uint64_t x) const {
-        const uint64_t a = x / n, b = x % n;
-        const double d_ab = 1.0 - ((double)shared[x] / (double)(uint32_t)shared[a * n + a]);
-        const double d_ba = 1.0 - ((double)shared[b * n + a] / (double)(uint32_t)shared[b * n + b]);
-        asym[x] = d_ab;
-        sym[x] = (d_ab != d_ab || d_ab < d_ba) ? d_ba : d_ab;       // f64::max: a NaN loses
-    }
-};
-
-// ---- cluster: UPGMA (cluster.rs:395-480), see DESIGN.md §12 ----
-// Clusters are indexed by their smallest member in ascending id order, so a merge of a < b keeps index a (new_id = a.min(b)).  The n x n
-// working matrix M holds, above the diagonal, the mean distance D(i, j) of clusters i < j and, below it, their sum T(i, j) over all member
-// pairs; T(a u b, j) = T(a, j) + T(b, j) and D = T / (|a u b| |j|).  Every live row i keeps its least (D, j) over j > i.
-#define AC_UPGMA_NONE 0xFFFFFFFFu
-// get_closest_pair (:461-480) scans pairs (a, b) in ascending id order with a strict <: the least (distance, a, b) wins
-AC_HD bool upgma_less(double d1, uint32_t a1, uint32_t b1, double d2, uint32_t a2, uint32_t b2) {
-    return d1 < d2 || (d1 == d2 && (a1 < a2 || (a1 == a2 && b1 < b2)));
-}
-// least live (D(i, j), j) over j = from, from + step, ... < n, folded into (bd, bj)
-AC_HD void upgma_row_scan(const double* M, uint32_t n, const uint8_t* alive, uint32_t i, uint32_t from, uint32_t step, double& bd, uint32_t& bj) {
-    for (uint32_t j = from; j < n; j += step)
-        if (alive[j]) { const double d = M[(size_t)i * n + j]; if (upgma_less(d, i, j, bd, i, bj)) { bd = d; bj = j; } }
-}
-// cluster b has joined a (|a u b| = cnt_ab): the sum and the mean of (a u b, j)
-AC_HD void upgma_merge_entry(double* M, uint32_t n, uint32_t a, uint32_t b, uint32_t j, uint64_t cnt_ab, uint64_t cnt_j) {
-    double* t_a = j < a ? M + (size_t)a * n + j : M + (size_t)j * n + a;
-    const double t_b = j < b ? M[(size_t)b * n + j] : M[(size_t)j * n + b];
-    const double t = *t_a + t_b;
-    *t_a = t;
-    (j < a ? M[(size_t)j * n + a] : M[(size_t)a * n + j]) = t / (double)(cnt_ab * cnt_j);
-}
-// row i != a of a live cluster i < b after that merge: true when its minimum pointed at a or b and the row must be scanned again;
-// otherwise the minimum stands, unless the new D(i, a) undercuts it
-AC_HD bool upgma_row_after_merge(const double* M, uint32_t n, uint32_t a, uint32_t b, uint32_t i, double& rd, uint32_t& rj) {
-    if (rj == a || rj == b) return true;
-    if (i < a) { const double d = M[(size_t)i * n + a]; if (upgma_less(d, i, a, rd, i, rj)) { rd = d; rj = a; } }
-    return false;
-}
-
-#ifndef AC_EMULATE
-__device__ __forceinline__ void upgma_warp_min(double& d, uint32_t& a, uint32_t& b) {
-    for (int o = 16; o; o >>= 1) {
-        const double od = __shfl_down_sync(0xFFFFFFFFu, d, o);
-        const uint32_t oa = __shfl_down_sync(0xFFFFFFFFu, a, o), ob = __shfl_down_sync(0xFFFFFFFFu, b, o);
-        if (upgma_less(od, oa, ob, d, a, b)) { d = od; a = oa; b = ob; }
-    }
-}
-// One persistent CTA performs all n - 1 merges (no launch or grid barrier per merge).  Per merge: the least row minimum (block
-// reduction), the merged row (a thread per column), the rows whose minimum involved a or b (listed), then a warp per listed row scans it.
-__global__ void __launch_bounds__(1024) ac_upgma_kernel(double* M, uint32_t n, uint8_t* alive, uint32_t* cnt, uint32_t* node, double* rd, uint32_t* rj,
-                                                        uint32_t* list, UpgmaMerge* out, uint32_t first_node, uint32_t* done) {
-    __shared__ double s_d[32];
-    __shared__ uint32_t s_a[32], s_b[32], s_n, s_pair[2];
-    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-    for (uint32_t i = warp; i < n; i += 32) {
-        double bd = INFINITY; uint32_t bi = i, bj = AC_UPGMA_NONE;
-        upgma_row_scan(M, n, alive, i, i + 1 + lane, 32, bd, bj);
-        upgma_warp_min(bd, bi, bj);
-        if (lane == 0) { rd[i] = bd; rj[i] = bj; }
-    }
-    __syncthreads();
-    for (uint32_t step = 0; step + 1 < n; ++step) {
-        double bd = INFINITY; uint32_t ba = AC_UPGMA_NONE, bb = AC_UPGMA_NONE;
-        for (uint32_t i = tid; i < n; i += blockDim.x)
-            if (alive[i] && upgma_less(rd[i], i, rj[i], bd, ba, bb)) { bd = rd[i]; ba = i; bb = rj[i]; }
-        upgma_warp_min(bd, ba, bb);
-        if (lane == 0) { s_d[warp] = bd; s_a[warp] = ba; s_b[warp] = bb; }
-        __syncthreads();
-        if (warp == 0) {
-            bd = s_d[lane]; ba = s_a[lane]; bb = s_b[lane];
-            upgma_warp_min(bd, ba, bb);
-            if (lane == 0 && bb == AC_UPGMA_NONE) { s_pair[0] = AC_UPGMA_NONE; *done = step; }   // no comparable pair left (NaN distances)
-            else if (lane == 0) {
-                UpgmaMerge m; m.node = first_node + step; m.left = node[ba]; m.right = node[bb]; m.pad = 0; m.dist = bd / 2.0;
-                out[step] = m;
-                alive[bb] = 0; cnt[ba] += cnt[bb]; node[ba] = m.node;
-                s_pair[0] = ba; s_pair[1] = bb; s_n = 0;
-            }
-        }
-        __syncthreads();
-        const uint32_t a = s_pair[0], b = s_pair[1];
-        if (a == AC_UPGMA_NONE) return;                  // the same value for every thread
-        const uint64_t cab = cnt[a];
-        for (uint32_t j = tid; j < n; j += blockDim.x)
-            if (alive[j] && j != a) upgma_merge_entry(M, n, a, b, j, cab, cnt[j]);
-        __syncthreads();
-        for (uint32_t i = tid; i < b; i += blockDim.x) {
-            if (!alive[i]) continue;
-            double d = rd[i]; uint32_t j = rj[i];
-            if (i == a || upgma_row_after_merge(M, n, a, b, i, d, j)) list[atomicAdd(&s_n, 1u)] = i;
-            else if (j != rj[i]) { rd[i] = d; rj[i] = j; }
-        }
-        __syncthreads();
-        const uint32_t L = s_n;
-        for (uint32_t x = warp; x < L; x += 32) {
-            const uint32_t i = list[x];
-            double rbd = INFINITY; uint32_t ri = i, rbj = AC_UPGMA_NONE;
-            upgma_row_scan(M, n, alive, i, i + 1 + lane, 32, rbd, rbj);
-            upgma_warp_min(rbd, ri, rbj);
-            if (lane == 0) { rd[i] = rbd; rj[i] = rbj; }
-        }
-        __syncthreads();
-    }
-    if (tid == 0) *done = n - 1;
-}
-#endif
-
 struct PathOffBody {
     const SeqInfo* seqs; uint32_t n_seqs; const uint64_t* run_start; uint64_t n_runs; uint64_t* path_off;
     AC_D void operator()(uint64_t i) const {
@@ -1754,25 +1613,6 @@ struct PathOffBody {
         uint64_t lo = 0, hi = n_runs;               // first run with start >= seqs[i].start
         while (lo < hi) { const uint64_t mid = (lo + hi) >> 1; if (run_start[mid] < seqs[i].start) lo = mid + 1; else hi = mid; }
         path_off[i] = lo;
-    }
-};
-
-// 256-ary blocked exclusive scan built from serial per-thread pieces (volumes here are tiny: one
-// value per 64 coordinates or per unitig).  levels: sums[l+1][i] = sum of sums[l][256i .. 256i+255].
-struct ScanReduceBody {
-    const uint32_t* in; uint64_t n; uint32_t* sums;
-    AC_D void operator()(uint64_t i) const {
-        const uint64_t a = i * 256, b = (a + 256 < n) ? a + 256 : n;
-        uint32_t s = 0; for (uint64_t x = a; x < b; ++x) s += in[x];
-        sums[i] = s;
-    }
-};
-struct ScanApplyBody {
-    const uint32_t* in; uint64_t n; const uint32_t* block_off; uint32_t* out;
-    AC_D void operator()(uint64_t i) const {
-        const uint64_t a = i * 256, b = (a + 256 < n) ? a + 256 : n;
-        uint32_t s = block_off ? block_off[i] : 0;
-        for (uint64_t x = a; x < b; ++x) { const uint32_t v = in[x]; out[x] = s; s += v; }
     }
 };
 
@@ -1815,209 +1655,13 @@ template <int WH> struct LiteralScanBody {
 };
 
 // ------------------------------------------------------------------------------------------------
-// trim: overlap alignment of unitig paths (trim.rs:366-479), see DESIGN.md §9
+// DeviceScan (backend.h)
 // ------------------------------------------------------------------------------------------------
-// Every score is a sum of +w, -w and -(wi+wj)/2 with integral w < 2^32, so it is a multiple of 0.5 far below 2^52: f64 adds are exact
-// and the matrix is the same in any evaluation order (the CTA's anti-diagonal sweep, the emulation's row-major loop, the reference's).
-// The matrix itself is not kept: the traceback needs S[i-1][j] >= S[i][j-1] (:443) and path equality (:436), so the fill stores that
-// one comparison per cell, packed 32 cells to a word along anti-diagonals (d = i + j); each diagonal starts on a word boundary.
-#define AC_TRIM_GAP 0
-#define AC_TRIM_NONE (-1)
-AC_HD uint32_t trim_diag_lo(uint32_t d, uint32_t k) { return d > k ? d - k : 1u; }     // first row i of anti-diagonal d (2 <= d <= 2k)
-AC_HD uint32_t trim_diag_words(uint32_t d, uint32_t k) {                             // 32-bit words of diagonal d's bits (0 outside 2..2k)
-    if (d < 2 || d > 2 * k) return 0;
-    const uint32_t hi = d - 1 < k ? d - 1 : k;
-    return (hi - trim_diag_lo(d, k) + 1 + 31) / 32;
-}
-AC_HD uint64_t trim_bit_words(uint32_t k) { uint64_t w = 0; for (uint32_t d = 2; d <= 2 * k; ++d) w += trim_diag_words(d, k); return w; }
-// :396-405, one cell: the diagonal, up (i-1, j) and left (i, j-1) scores, the two unitigs and their weights
-AC_HD double trim_cell(double diag, double up, double left, int32_t a, int32_t b, double wa, double wb) {
-    const double match_score = diag + (a == b ? wa : -(wa + wb) / 2.0);
-    const double delete_score = up - wa, insert_score = left - wb;
-    const double m = match_score > delete_score ? match_score : delete_score;      // f64::max without NaNs
-    return m > insert_score ? m : insert_score;
-}
-// :413-419: the right edge S[i][k] is visited with i ascending and a strict > keeps the smallest i among ties
-AC_HD void trim_edge(double s, uint32_t i, double& best, uint32_t& best_i) { if (s > best) { best = s; best_i = i; } }
-// :431-461 from (max_i, k): writes the pieces in traceback order (last column first) and returns their count, or 0 when the walk ends
-// on the left edge (i > 0).  pa = path_a (its first k entries are rows 1..k), pb = path_b + n - k (columns 1..k), bits as above.
-AC_HD uint32_t trim_traceback(const int32_t* pa, const int32_t* pb, uint32_t n, uint32_t k, const uint32_t* bits, uint32_t max_i, AlignPiece* out) {
-    uint32_t i = max_i, j = k, cnt = 0;
-    uint64_t off = 0;
-    for (uint32_t d = 2; d < i + j; ++d) off += trim_diag_words(d, k);
-    while (i > 0 && j > 0) {
-        const uint32_t d = i + j;
-        const int32_t a = pa[i - 1], b = pb[j - 1];
-        const int32_t gi = (int32_t)(i - 1), gj = (int32_t)(n - k + j - 1);
-        if (a == b) {
-            out[cnt++] = AlignPiece{a, gi, b, gj};
-            --i; --j;
-            off -= trim_diag_words(d - 1, k) + trim_diag_words(d - 2, k);
-        } else {
-            const uint32_t t = i - trim_diag_lo(d, k);
-            if ((bits[off + t / 32] >> (t % 32)) & 1u) { out[cnt++] = AlignPiece{a, gi, AC_TRIM_GAP, AC_TRIM_NONE}; --i; }
-            else { out[cnt++] = AlignPiece{AC_TRIM_GAP, AC_TRIM_NONE, b, gj}; --j; }
-            off -= trim_diag_words(d - 1, k);
-        }
-    }
-    return i > 0 ? 0 : cnt;
-}
-// Per job: where its bit words, its traceback output (2k pieces), and, for windows beyond shared memory, its three diagonals (HBM) live.
-struct TrimLaunchJob { uint64_t a_off, b_off, bits_off, out_off, scratch_off; uint32_t n, k, skip, slot; };
-
 #ifndef AC_EMULATE
-// One CTA per job sweeps the 2k-1 anti-diagonals; the three live ones (d-2, d-1, d, indexed by row i) sit in shared memory, or in the
-// job's HBM scratch when 24 (k + 1) bytes exceed the CTA's shared memory (same code, another base pointer).  A thread owns a cell per
-// 1024 of its diagonal: the two path entries it reads are adjacent to its neighbours' (coalesced), and its warp packs the 32 traceback
-// bits with one ballot into one word.  Thread 0 then runs the O(k) traceback over those bits.
-__global__ void __launch_bounds__(1024) ac_overlap_align_kernel(const TrimLaunchJob* __restrict__ jobs, const int32_t* __restrict__ values,
-                                                                const uint32_t* __restrict__ weights, uint32_t* __restrict__ bits,
-                                                                double* scratch, AlignPiece* __restrict__ out, uint32_t* __restrict__ out_len, int use_shared) {
-    extern __shared__ double trim_smem[];
-    __shared__ double best;
-    __shared__ uint32_t best_i;
-    const TrimLaunchJob J = jobs[blockIdx.x];
-    const uint32_t k = J.k, tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-    double* D = use_shared ? trim_smem : scratch + J.scratch_off;
-    const int32_t* pa = values + J.a_off;
-    const int32_t* pb = values + J.b_off + (J.n - k);
-    uint32_t* B = bits + J.bits_off;
-    const uint32_t diag_shift = J.n - k;             // global_i == global_j  <=>  i - 1 == n - k + j - 1
-    if (tid == 0) { best = -INFINITY; best_i = 0; }
-    uint64_t off = 0;
-    for (uint32_t d = 2; d <= 2 * k; ++d) {
-        double* cur = D + (size_t)(d % 3) * (k + 1);
-        const double* prev = D + (size_t)((d - 1) % 3) * (k + 1);
-        const double* prev2 = D + (size_t)((d - 2) % 3) * (k + 1);
-        const uint32_t lo = trim_diag_lo(d, k), hi = d - 1 < k ? d - 1 : k, len = hi - lo + 1;
-        for (uint32_t base = 0; base < len; base += blockDim.x) {      // the same trip count for every thread: all lanes reach the ballot
-            const uint32_t t = base + tid;
-            bool up_wins = false;
-            if (t < len) {
-                const uint32_t i = lo + t, j = d - i;
-                const double up = i == 1 ? 0.0 : prev[i - 1];
-                const double left = j == 1 ? 0.0 : prev[i];
-                up_wins = up >= left;
-                double s = -INFINITY;
-                if (!(J.skip && i == j + diag_shift)) {
-                    const double diag = (i == 1 || j == 1) ? 0.0 : prev2[i - 1];
-                    const int32_t a = pa[i - 1], b = pb[j - 1];
-                    s = trim_cell(diag, up, left, a, b, (double)__ldg(weights + (a < 0 ? -a : a)), (double)__ldg(weights + (b < 0 ? -b : b)));
-                }
-                cur[i] = s;
-                if (j == k) trim_edge(s, i, best, best_i);         // one cell per diagonal, rows in ascending order
-            }
-            const uint32_t word = __ballot_sync(0xFFFFFFFFu, up_wins);
-            if (lane == 0 && base + warp * 32 < len) B[off + base / 32 + warp] = word;
-        }
-        off += (len + 31) / 32;
-        __syncthreads();
-    }
-    if (tid == 0) {
-        AlignPiece* o = out + J.out_off;
-        out_len[J.slot] = best > 0.0 ? trim_traceback(pa, pb, J.n, k, B, best_i, o) : 0;      // :422 max_score <= 0: no alignment
-    }
-}
-#endif
-
-// ------------------------------------------------------------------------------------------------
-// resolve: all-pairs path distances of a bridge (global_alignment_distance, resolve.rs:387-418), see DESIGN.md §13
-// ------------------------------------------------------------------------------------------------
-// D[i][j] over rows i (the shorter path a) and columns j (path b), in u32 with wraparound as the reference's release build computes it.
-// The sweep goes by anti-diagonals d = i + j; the three live ones (d-2, d-1, d) are indexed by row i, n + 1 words each.  Swapping the
-// two paths transposes the recurrence and applies the same adds and mins to the same operands, so D(a, b) == D(b, a) bit for bit.
-#define AC_BRIDGE_THREADS 256
-AC_HD uint32_t bridge_weight(const uint32_t* w, int32_t u) { return w[u < 0 ? (uint32_t)(-(int64_t)u) : (uint32_t)u]; }
-// One cell (i, j = d - i) of diagonal d from the two diagonals before it: the top edge (gaps in a), the left edge (gaps in b), or the
-// min of match/mismatch, delete and insert (:404-411).
-AC_HD void bridge_cell(uint32_t* cur, const uint32_t* prev, const uint32_t* prev2, uint32_t i, uint32_t j, const int32_t* pa, const int32_t* pb,
-                       const uint32_t* w) {
-    if (i == 0) { cur[0] = prev[0] + bridge_weight(w, pb[j - 1]); return; }
-    const int32_t a = pa[i - 1];
-    const uint32_t wa = bridge_weight(w, a);
-    if (j == 0) { cur[i] = prev[i - 1] + wa; return; }
-    const int32_t b = pb[j - 1];
-    const uint32_t wb = bridge_weight(w, b);
-    const uint32_t match_or_mismatch = prev2[i - 1] + (a == b ? 0u : (wa > wb ? wa : wb));
-    const uint32_t delete_cost = prev[i - 1] + wa, insert_cost = prev[i] + wb;
-    const uint32_t m = match_or_mismatch < delete_cost ? match_or_mismatch : delete_cost;
-    cur[i] = m < insert_cost ? m : insert_cost;
-}
-AC_HD uint32_t bridge_diag_lo(uint32_t d, uint32_t m) { return d > m ? d - m : 0u; }
-AC_HD uint32_t bridge_diag_hi(uint32_t d, uint32_t n) { return d < n ? d : n; }
-// Per job: its two paths, where its diagonals live when they exceed shared memory, and its output slot.
-struct BridgeLaunchJob { uint64_t a_off, b_off, scratch_off; uint32_t n, m, slot, pad; };
-
-#ifndef AC_EMULATE
-// One CTA per job.  The diagonals sit in dynamic shared memory, or in the job's HBM scratch when 12 (n + 1) bytes exceed the CTA's
-// shared memory (same code, another base pointer).  Thread t owns rows t, t + 256, ... of every diagonal: neighbouring threads read
-// neighbouring path entries and diagonal words.
-__global__ void __launch_bounds__(AC_BRIDGE_THREADS) ac_bridge_distance_kernel(const BridgeLaunchJob* __restrict__ jobs, const int32_t* __restrict__ values,
-                                                                               const uint32_t* __restrict__ weights, uint32_t* scratch,
-                                                                               uint32_t* __restrict__ dist, int use_shared) {
-    extern __shared__ uint32_t bridge_smem[];
-    const BridgeLaunchJob J = jobs[blockIdx.x];
-    const uint32_t n = J.n, m = J.m, stride = n + 1;
-    uint32_t* D = use_shared ? bridge_smem : scratch + J.scratch_off;
-    const int32_t* pa = values + J.a_off;
-    const int32_t* pb = values + J.b_off;
-    if (threadIdx.x == 0) D[0] = 0;                   // d = 0: D[0][0]
-    __syncthreads();
-    for (uint32_t d = 1; d <= n + m; ++d) {
-        uint32_t* cur = D + (size_t)(d % 3) * stride;
-        const uint32_t* prev = D + (size_t)((d - 1) % 3) * stride;
-        const uint32_t* prev2 = D + (size_t)((d + 1) % 3) * stride;     // d - 2 (mod 3); not read on d = 1
-        const uint32_t hi = bridge_diag_hi(d, n);
-        for (uint32_t i = bridge_diag_lo(d, m) + threadIdx.x; i <= hi; i += AC_BRIDGE_THREADS) bridge_cell(cur, prev, prev2, i, d - i, pa, pb, weights);
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) dist[J.slot] = D[(size_t)((n + m) % 3) * stride + n];
-}
-#endif
-
-#ifndef AC_EMULATE
-// Product scan: tiles of 4096 values, coalesced loads, warp-shuffle block scans (the functor bodies above are the
-// host-emulation form of the same two phases).
 #define AC_SCAN_TILE 4096
-__global__ void __launch_bounds__(256) ac_scan_reduce_kernel(const uint32_t* __restrict__ in, uint64_t n, uint32_t* __restrict__ sums) {
-    const uint64_t tile0 = (uint64_t)blockIdx.x * AC_SCAN_TILE;
-    uint32_t s = 0;
-#pragma unroll
-    for (int r = 0; r < AC_SCAN_TILE / 256; ++r) { const uint64_t i = tile0 + (uint64_t)r * 256 + threadIdx.x; if (i < n) s += in[i]; }
-    for (int o = 16; o; o >>= 1) s += __shfl_down_sync(0xFFFFFFFFu, s, o);
-    __shared__ uint32_t w[8];
-    if ((threadIdx.x & 31) == 0) w[threadIdx.x >> 5] = s;
-    __syncthreads();
-    if (threadIdx.x == 0) { uint32_t t = 0; for (int i = 0; i < 8; ++i) t += w[i]; sums[blockIdx.x] = t; }
-}
-__global__ void __launch_bounds__(256) ac_scan_apply_kernel(const uint32_t* in, uint64_t n, const uint32_t* __restrict__ block_off, uint32_t* out) {
-    __shared__ uint32_t warp_tot[8];
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t carry = block_off ? block_off[blockIdx.x] : 0;
-    const uint64_t tile0 = (uint64_t)blockIdx.x * AC_SCAN_TILE;
-#pragma unroll 1
-    for (int r = 0; r < AC_SCAN_TILE / 1024; ++r) {            // 1024 values per round, 4 consecutive values per thread
-        const uint64_t i = tile0 + (uint64_t)r * 1024 + threadIdx.x * 4;
-        uint32_t v[4];
-        if (i + 3 < n) { const uint4 q = *reinterpret_cast<const uint4*>(in + i); v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w; }
-        else { for (int j = 0; j < 4; ++j) v[j] = (i + j < n) ? in[i + j] : 0; }
-        const uint32_t t = v[0] + v[1] + v[2] + v[3];
-        uint32_t inc = t;
-        for (int o = 1; o < 32; o <<= 1) { const uint32_t u = __shfl_up_sync(0xFFFFFFFFu, inc, o); if (lane >= (uint32_t)o) inc += u; }
-        if (lane == 31) warp_tot[warp] = inc;
-        __syncthreads();
-        uint32_t wbase = 0, total = 0;
-        for (uint32_t w2 = 0; w2 < 8; ++w2) { const uint32_t x = warp_tot[w2]; if (w2 < warp) wbase += x; total += x; }
-        uint32_t e = carry + wbase + inc - t;
-        if (i + 3 < n) { uint4 q; q.x = e; q.y = e + v[0]; q.z = q.y + v[1]; q.w = q.z + v[2]; *reinterpret_cast<uint4*>(out + i) = q; }
-        else { for (int j = 0; j < 4; ++j) { if (i + j < n) out[i + j] = e; e += v[j]; } }
-        carry += total;
-        __syncthreads();
-    }
-}
-// The same scan in ONE launch ("chained scan with decoupled look-back"): a CTA takes the next tile by ticket, publishes the tile's sum,
-// finds its exclusive prefix by looking back over the tiles before it — their sums until one of them has its inclusive prefix out — and
-// scans its tile from registers (out may alias in).  A state word is [scan number:30 | status:2 | value:32], so words left by earlier
+// Tiles of 4096 values, coalesced loads, warp-shuffle block scans, in ONE launch ("chained scan with decoupled look-back"): a CTA takes
+// the next tile by ticket, publishes the tile's sum, finds its exclusive prefix by looking back over the tiles before it — their sums
+// until one of them has its inclusive prefix out — and scans its tile from registers (out may alias in).  A state word is [scan number:30 | status:2 | value:32], so words left by earlier
 // scans never match and nothing has to be cleared between scans; tickets count up for ever (the host passes where this scan's begin).
 #define AC_SCAN_STATE(epoch, status, value) (((unsigned long long)(epoch) << 34) | ((unsigned long long)(status) << 32) | (unsigned long long)(value))
 __global__ void __launch_bounds__(256) ac_scan_chained_kernel(const uint32_t* in, uint64_t n, uint32_t* out, unsigned long long* state, unsigned long long epoch,
@@ -2083,223 +1727,43 @@ __global__ void __launch_bounds__(256) ac_scan_chained_kernel(const uint32_t* in
         carry += total;
     }
 }
-#endif
-
-// ------------------------------------------------------------------------------------------------
-// dotplot: all-vs-all k-mer dots (dotplot.rs:394-450), see DESIGN.md §14
-// ------------------------------------------------------------------------------------------------
-// Window j of sequence b matches window p of sequence a forward when a[p..p+k] == b[j..j+k] and in reverse when revcomp(a[p..p+k]) ==
-// b[j..j+k] (get_all_kmer_positions, :433-450).  For windows of only ACGT both relations are "same canonical k-mer": forward when the
-// two windows have the same orientation, reverse otherwise.  So the dots are the ordered pairs of windows within each group of equal
-// canonical keys, and a pixel's colour is the one of its largest dotplot_key (pipeline.h), whatever order the dots arrive in.
-#define AC_DOT_SCAN_TILE 32    // values per thread of the u64 scan
-#define AC_DOT_CHUNK 64        // consecutive dots per thread
-AC_HD uint32_t dot_base(uint8_t c) { return c == 'A' ? 0u : c == 'C' ? 1u : c == 'G' ? 2u : c == 'T' ? 3u : 4u; }
-// (pos as f64 / bp_per_pixel).round() as u32 + start (:401, :405): round half away from zero, Rust's saturating cast (NaN to 0), a
-// wrapping u32 add.  The f64 division is IEEE round-to-nearest on the device as on the host, so both get the same pixel.
-AC_HD uint32_t dot_px(uint32_t start, uint32_t pos, double bpp) {
-    const double v = round((double)pos / bpp);
-    return start + (!(v > 0.0) ? 0u : v >= 4294967295.0 ? 0xFFFFFFFFu : (uint32_t)v);
+uint32_t DeviceScan::operator()(AcStream* st, const uint32_t* in, uint32_t* out, uint64_t n, bool want_total) {
+    if (n == 0) return 0;
+    const uint64_t nb = (n + AC_SCAN_TILE - 1) / AC_SCAN_TILE;
+    if (nb > 0x7FFFFFFFull) throw std::runtime_error("scan too large");
+    if ((nb + 4) * 8 > state.cap) {      // [0] ticket counter, [1] the total, [2..] one state word per tile; zeroed once: scan numbers start at 1
+        state.ensure((nb + 4) * 8 * 2);
+        ac_memset(state.p, 0, state.cap, st);
+        tickets = 0;
+    }
+    unsigned long long* s = state.as<unsigned long long>();
+    epoch = (epoch + 1) & 0x3FFFFFFFull; if (epoch == 0) epoch = 1;
+    ac_launch_kernel("scan", st, ac_scan_chained_kernel, (unsigned)nb, 256, 0, in, n, out, s + 2, epoch, s, tickets, (uint32_t)nb, (uint32_t*)(s + 1));
+    tickets += nb;
+    uint32_t total_sum = 0;
+    if (want_total) { ac_d2h(&total_sum, s + 1, sizeof(uint32_t), st); ac_sync(st); }
+    return total_sum;
 }
-
-// One thread per window: the window's 2-bit key on both strands (base b of a strand in word b / 32 at bit 2 (b % 32)), the smaller one
-// as the canonical key, the orientation, the pixel and the window's tag (dotplot_key with pair = the window's sequence).  A window with
-// another byte than ACGT gets rep = NONE: the host matches those (a reverse complement keeps such a byte, so they match nothing else).
-template <int W> struct DotWindowBody {
-    const uint8_t* bytes; const DotplotSeq* seqs; uint32_t n_seqs, k; double bpp;
-    uint64_t* keys; uint32_t* px; uint64_t* tag; uint32_t* rep;
-    AC_D void operator()(uint64_t i) const {
-        uint32_t lo = 0, hi = n_seqs;               // the last sequence whose first window is <= i (those without windows share the next base)
-        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (seqs[mid].window_base <= i) lo = mid; else hi = mid; }
-        const DotplotSeq s = seqs[lo];
-        const uint32_t j = (uint32_t)(i - s.window_base);
-        const uint8_t* w = bytes + s.off + j;
-        uint64_t f[W], r[W];
-        uint32_t bad = 0;
-#pragma unroll
-        for (int x = 0; x < W; ++x) {
-            uint64_t fw = 0, rw = 0;
-            const uint32_t b0 = 32u * (uint32_t)x, b1 = k < b0 + 32u ? k : b0 + 32u;
-            for (uint32_t b = b0; b < b1; ++b) {
-                const uint32_t c = dot_base(w[b]), d = dot_base(w[k - 1 - b]);
-                bad |= c >> 2;
-                fw |= (uint64_t)(c & 3u) << (2 * (b - b0));
-                rw |= (uint64_t)(3u - (d & 3u)) << (2 * (b - b0));
-            }
-            f[x] = fw; r[x] = rw;
-        }
-        int cmp = 0;
-#pragma unroll
-        for (int x = W - 1; x >= 0; --x) if (cmp == 0 && f[x] != r[x]) cmp = f[x] < r[x] ? -1 : 1;
-        const bool forward = cmp <= 0;              // a window that is its own reverse complement is forward: at one j the forward hit wins
-#pragma unroll
-        for (int x = 0; x < W; ++x) keys[i * W + x] = forward ? f[x] : r[x];
-        px[i] = dot_px(s.start_px, j, bpp);
-        tag[i] = ((uint64_t)lo << 34) | ((uint64_t)j << 2) | ((uint64_t)forward << 1) | 1u;
-        rep[i] = bad ? AC_NONE32 : (uint32_t)i;
-    }
-};
-
-// Open addressing over 8-byte slots: the key's hash in the high half, (window + 1) in the low half, 0 = empty.  A window that finds
-// its fingerprint compares the full key with the slot's window before it joins that window's group, so a hash collision never makes
-// a dot.  The table has at least twice as many slots as windows and cannot fill.
-template <int W> struct DotInsertBody {
-    const uint64_t* keys; uint64_t* table; uint64_t mask; uint32_t* rep;
-    AC_D void operator()(uint64_t i) const {
-        if (rep[i] == AC_NONE32) return;
-        uint64_t key[W];
-        uint64_t h = 0x243F6A8885A308D3ull;
-#pragma unroll
-        for (int x = 0; x < W; ++x) { key[x] = keys[i * W + x]; h ^= key[x]; h *= 0x9E3779B97F4A7C15ull; h ^= h >> 32; }
-        h ^= h >> 29; h *= 0xBF58476D1CE4E5B9ull; h ^= h >> 32;
-        const uint64_t mine = (h & 0xFFFFFFFF00000000ull) | (i + 1);
-        for (uint64_t s = h & mask;; s = (s + 1) & mask) {
-            uint64_t cur = ac_ld_volatile(table + s);
-            if (cur == 0) {
-                cur = ac_atomic_cas(table + s, (uint64_t)0, mine);
-                if (cur == 0) return;               // i leads its group (rep[i] == i already)
-            }
-            if ((cur >> 32) == (mine >> 32)) {
-                const uint64_t r = (cur & 0xFFFFFFFFull) - 1;
-                bool same = true;
-#pragma unroll
-                for (int x = 0; x < W; ++x) same &= keys[r * W + x] == key[x];
-                if (same) { rep[i] = (uint32_t)r; return; }
-            }
-        }
-    }
-};
-
-struct DotCountBody {                               // group sizes, at the group's leading window
-    const uint32_t* rep; uint32_t* cnt;
-    AC_D void operator()(uint64_t i) const { if (rep[i] != AC_NONE32) ac_atomic_add(cnt + rep[i], 1u); }
-};
-struct DotScatterBody {                             // counting sort by group: pixel and tag of every window, grouped
-    const uint32_t* rep; const uint32_t* off; uint32_t* fill; const uint32_t* px; const uint64_t* tag; uint32_t* gpx; uint64_t* gtag;
-    AC_D void operator()(uint64_t i) const {
-        const uint32_t r = rep[i];
-        if (r == AC_NONE32) return;
-        const uint32_t p = off[r] + ac_atomic_add(fill + r, 1u);
-        gpx[p] = px[i]; gtag[p] = tag[i];
-    }
-};
-struct DotLeadBody {                                // 1 at every group's leading window
-    const uint32_t* rep; uint32_t* flag;
-    AC_D void operator()(uint64_t i) const { flag[i] = rep[i] == (uint32_t)i ? 1u : 0u; }
-};
-struct DotGroupBody {                               // group g: where its windows start, how many, and its dots (size squared, u64)
-    const uint32_t* rep; const uint32_t* gid; const uint32_t* off; const uint32_t* cnt; uint32_t* gstart; uint32_t* gsize; uint64_t* gdots;
-    AC_D void operator()(uint64_t i) const {
-        if (rep[i] != (uint32_t)i) return;
-        const uint32_t g = gid[i];
-        gstart[g] = off[i]; gsize[g] = cnt[i]; gdots[g] = (uint64_t)cnt[i] * cnt[i];
-    }
-};
-// u64 exclusive scan: one thread per tile of AC_DOT_SCAN_TILE values sums its tile; the tile sums are scanned the same way; each
-// thread then writes its tile's prefix.  In place is allowed.
-struct DotScanSumBody {
-    const uint64_t* in; uint64_t n; uint64_t* sums;
-    AC_D void operator()(uint64_t t) const {
-        const uint64_t lo = t * AC_DOT_SCAN_TILE, hi = lo + AC_DOT_SCAN_TILE < n ? lo + AC_DOT_SCAN_TILE : n;
-        uint64_t s = 0;
-        for (uint64_t x = lo; x < hi; ++x) s += in[x];
-        sums[t] = s;
-    }
-};
-struct DotScanApplyBody {
-    const uint64_t* in; uint64_t* out; uint64_t n; const uint64_t* tile_off;
-    AC_D void operator()(uint64_t t) const {
-        const uint64_t lo = t * AC_DOT_SCAN_TILE, hi = lo + AC_DOT_SCAN_TILE < n ? lo + AC_DOT_SCAN_TILE : n;
-        uint64_t acc = tile_off ? tile_off[t] : 0;
-        for (uint64_t x = lo; x < hi; ++x) { const uint64_t v = in[x]; out[x] = acc; acc += v; }
-    }
-};
-// The dots, AC_DOT_CHUNK consecutive ones per thread over the scan of the groups' squared sizes, so that one large group (a
-// homopolymer) is spread over as many threads as its dots need.  Dot (u, v) of a group: u is the row window (sequence a, pixel x), v
-// the column window (sequence b, window j, pixel y).  The atomic is skipped when the pixel already holds a larger key: pixels on the
-// diagonals are hit many times when a pixel spans many bases.
-struct DotPairBody {
-    const uint64_t* goff; const uint32_t* gstart; const uint32_t* gsize; uint32_t G;
-    const uint32_t* gpx; const uint64_t* gtag; uint64_t n_dots; uint32_t n_seqs, res; uint64_t* pix;
-    AC_D void operator()(uint64_t t) const {
-        uint64_t d = t * AC_DOT_CHUNK;
-        const uint64_t end = d + AC_DOT_CHUNK < n_dots ? d + AC_DOT_CHUNK : n_dots;
-        uint32_t lo = 0, hi = G;                    // the group holding dot d: the last one that starts at or before it
-        while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (goff[mid] <= d) lo = mid; else hi = mid; }
-        uint32_t g = lo, base = gstart[g], s = gsize[g];
-        const uint64_t local = d - goff[g];
-        uint32_t uu = (uint32_t)(local / s), vv = (uint32_t)(local % s);
-        uint32_t xu = gpx[base + uu];
-        uint64_t tu = gtag[base + uu], pair_hi = ((tu >> 34) * n_seqs) << 34;
-        for (; d < end; ++d) {
-            const uint32_t y = gpx[base + vv];
-            if (xu < res && y < res) {
-                const uint64_t tv = gtag[base + vv];
-                const uint64_t key = ((tv & ~2ull) + pair_hi) | (~(tu ^ tv) & 2ull);
-                uint64_t* p = pix + (uint64_t)y * res + xu;
-                if (*p < key) ac_atomic_max(p, key);
-            }
-            if (++vv == s) {
-                vv = 0;
-                if (++uu == s) { uu = 0; if (++g >= G) break; base = gstart[g]; s = gsize[g]; }
-                xu = gpx[base + uu]; tu = gtag[base + uu]; pair_hi = ((tu >> 34) * n_seqs) << 34;
-            }
-        }
-    }
-};
-struct DotMergeBody {                               // the host's dots (windows with other bytes than ACGT) into the same maxima
-    const uint64_t* idx; const uint64_t* key; uint64_t* pix;
-    AC_D void operator()(uint64_t i) const { ac_atomic_max(pix + idx[i], key[i]); }
-};
-struct DotComposeBody {                             // a pixel with a dot: mediumblue (forward) or firebrick (reverse), :40-41
-    const uint64_t* pix; uint8_t* rgb;
-    AC_D void operator()(uint64_t p) const {
-        const uint64_t key = pix[p];
-        if (!key) return;
-        const bool fwd = (key & 2u) != 0;
-        rgb[3 * p] = fwd ? 0 : 178; rgb[3 * p + 1] = fwd ? 0 : 34; rgb[3 * p + 2] = fwd ? 205 : 34;
-    }
-};
+#else
+uint32_t DeviceScan::operator()(AcStream* st, const uint32_t* in, uint32_t* out, uint64_t n, bool want_total) { return serial.run(st, in, out, n, want_total); }
+#endif
 
 // ------------------------------------------------------------------------------------------------
 // host orchestration
 // ------------------------------------------------------------------------------------------------
-struct DevBuf {
-    void* p = nullptr; size_t cap = 0;
-    void ensure(size_t bytes) {
-        if (bytes > cap) {
-            ac_dev_free(p); p = nullptr; cap = 0; p = ac_dev_alloc(bytes); cap = bytes;
-#ifdef AC_EMULATE
-            static const bool poison = getenv("AC_EMU_POISON") != nullptr;
-            if (poison) memset(p, 0xA5, cap);
-#endif
-        }
-    }
-    template <class T> T* as() { return (T*)p; }
-    ~DevBuf() { ac_dev_free(p); }
-};
-
-struct PinBuf {   // pinned host memory: D2H lands at DMA speed and the host graph works on it in place
-    void* p = nullptr; size_t cap = 0;
-    void ensure(size_t bytes) { if (bytes > cap) { ac_host_free(p); p = nullptr; cap = 0; p = ac_host_alloc(bytes); cap = bytes; } }
-    template <class T> T* as() { return (T*)p; }
-    ~PinBuf() { ac_host_free(p); }
-};
-
-struct DevicePipeline::Impl {
-    int device = 0;
-    AcStream stream;
-    bool own_stream = false;
+struct DevicePipeline::Impl : DeviceContext {
+    Impl(int device, void* stream);
+    ~Impl();
     uint64_t total = 0; uint32_t n_seqs = 0, k = 0; int W = 0;
     DevBuf ascii, packed, seqs, slots, pos_slot, flags8, bmask, bcount, boff, counters, uid_rep, slot_unitig;
     DevBuf run_start, run_len, run_uk, run_dir, is_rep, rep_idx, run_unitig, unitigs, nchunks, chunk_off, partial, link_count, links;
-    DevBuf scan_tmp[4];
+    DeviceScan scan;
     DevBuf d_fixed, cand_flag, cand_index, d_cands, d_cand_at, d_deps, d_spec;
     DevBuf sort_a, sort_b, sort_ra, sort_rb, num_prefix, rank, d_len, d_depth, need, d_seq_off, d_arena, d_min_fpos, d_min_rpos;
     DevBuf strand_cnt, d_next_off, d_next, prev_cnt, d_prev_off, d_prev, d_path, d_path_off;
     DevBuf d_rec;
     PinBuf h_cands, h_deps, h_spec, h_fixed;
-    DevBuf dist_member, dist_shared, d_pred, d_level, d_flagmax, d_counters64, d_dirty, d_exhausted, d_arena2, d_arena3, d_pos, sort_c, sort_d, d_pos2, gfa_s_size, gfa_l_size, gfa_p_size, gfa_pieces, d_text, d_ptext, d_last, d_pbound, d_due;
+    DevBuf d_pred, d_level, d_flagmax, d_counters64, d_dirty, d_exhausted, d_arena2, d_arena3, d_pos, sort_c, sort_d, d_pos2, gfa_s_size, gfa_l_size, gfa_p_size, gfa_pieces, d_text, d_ptext, d_last, d_pbound, d_due;
     PinBuf h_order2, h_text, h_ptext, h_pbound;
     PinBuf h_rec, h_depth, h_order, h_arena, h_next_off, h_next, h_prev_off, h_prev, h_path, h_path_off, h_run_start, h_run_len;
 #ifndef AC_EMULATE
@@ -2331,51 +1795,6 @@ struct DevicePipeline::Impl {
 #endif
     }
 
-    // exclusive scan of n uint32 values; returns the total (when asked: it costs the one host round trip).  out may alias in.
-#ifndef AC_EMULATE
-    DevBuf scan_state; unsigned long long scan_epoch = 0, scan_tickets = 0;
-    uint32_t exclusive_scan(const uint32_t* in, uint32_t* out, uint64_t n, int = 0, bool want_total = true) {
-        if (n == 0) return 0;
-        const uint64_t nb = (n + AC_SCAN_TILE - 1) / AC_SCAN_TILE;
-        if (nb > 0x7FFFFFFFull) throw std::runtime_error("scan too large");
-        if ((nb + 4) * 8 > scan_state.cap) {      // [0] ticket counter, [1] the total, [2..] one state word per tile; zeroed once: scan numbers start at 1
-            scan_state.ensure((nb + 4) * 8 * 2);
-            ac_memset(scan_state.p, 0, scan_state.cap, &stream);
-            scan_tickets = 0;
-        }
-        unsigned long long* st = scan_state.as<unsigned long long>();
-        scan_epoch = (scan_epoch + 1) & 0x3FFFFFFFull; if (scan_epoch == 0) scan_epoch = 1;
-        ac_scan_chained_kernel<<<(unsigned)nb, 256, 0, stream.s>>>(in, n, out, st + 2, scan_epoch, st, scan_tickets, (uint32_t)nb, (uint32_t*)(st + 1)); ++g_ac_kernel_launches;
-        scan_tickets += nb;
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) throw std::runtime_error(std::string("launch scan: ") + cudaGetErrorString(e));
-        ac_debug_sync("scan", &stream);
-        uint32_t total_sum = 0;
-        if (want_total) { ac_d2h(&total_sum, st + 1, sizeof(uint32_t), &stream); ac_sync(&stream); }
-        return total_sum;
-    }
-#else
-    uint32_t exclusive_scan(const uint32_t* in, uint32_t* out, uint64_t n, int level = 0, bool want_total = true) {
-        if (n == 0) return 0;
-        if (level >= 4) throw std::runtime_error("scan too deep");
-        const uint64_t tile = 256;
-        const uint64_t nb = (n + tile - 1) / tile;
-        scan_tmp[level].ensure((nb + 4) * sizeof(uint32_t));
-        uint32_t* sums = scan_tmp[level].as<uint32_t>();
-        if (nb > 0x7FFFFFFFull) throw std::runtime_error("scan too large");
-        ac_launch("scan_reduce", &stream, ScanReduceBody{in, n, sums}, nb);
-        uint32_t total_sum = 0;
-        if (nb == 1) {
-            if (want_total) { ac_d2h(&total_sum, sums, sizeof(uint32_t), &stream); ac_sync(&stream); }
-            ac_launch("scan_apply", &stream, ScanApplyBody{in, n, nullptr, out}, nb);
-        } else {
-            total_sum = exclusive_scan(sums, sums, nb, level + 1, want_total);
-            ac_launch("scan_apply", &stream, ScanApplyBody{in, n, sums, out}, nb);
-        }
-        return total_sum;
-    }
-#endif
-
     // pipeline state shared by the stages
     std::vector<SeqInfo> host_seqs;
     uint64_t cap = 0, n_windows = 0, n_runs = 0, g_begin = 0, g_end = 0, n_slots_used = 0, n_dotted = 0, n_fwords = 0;
@@ -2384,11 +1803,6 @@ struct DevicePipeline::Impl {
     DevBuf run_hs, run_ts, claimed, claimed_cnt, occ_list, ext_filter, needles, hits, count_big, interior8;
     TableView table_view() { return TableView{slots.as<Slot>(), cap, packed.as<uint64_t>(), seqs.as<SeqInfo>(), n_seqs, big_counts ? count_big.as<uint32_t>() : nullptr, slot_gpos_bits(total), count_alarm()}; }
     static uint32_t count_alarm() { static const uint32_t a = getenv("AC_COUNT_ALARM") ? (uint32_t)atoi(getenv("AC_COUNT_ALARM")) : AC_SLOT_COUNT_ALARM; return a; }      // test hook: a lower threshold
-    void set_device() {
-#ifndef AC_EMULATE
-        AC_CUDA_CHECK(cudaSetDevice(device));
-#endif
-    }
     template <int W> void local_w(uint32_t seq_lo, uint32_t seq_hi, bool multi);
     template <int W> void insert_w();
     uint64_t safe_cap = 0;          // 1.5 slots per window of every sequence (all ranks'): holds any input, the union of the ranks' k-mers included
@@ -2409,10 +1823,6 @@ struct DevicePipeline::Impl {
     void pull_graph(PipelineResult& out, bool keep_positions);
     DevBuf d_small, d_totals, d_wrap_off, d_pre_len, d_suf_len, d_blob, d_blob_off;
     std::vector<char> path_blob; std::vector<uint32_t> path_pre, path_suf; uint64_t path_wrap_total = 0;
-    void scan_keep_total(uint32_t* x, uint64_t n, uint32_t* total_dst) {      // in place; x[n-1] must be 0, so the scanned x[n-1] is the total: kept on the device
-        exclusive_scan(x, x, n, 0, false);
-        ac_copy_dd(total_dst, x + (n - 1), 4, &stream);
-    }
     uint64_t uploaded_bytes = 0;
     uint64_t exp_n = 0, n_own_runs = 0; uint32_t own_seq_lo = 0, own_seq_hi = 0; bool exp_valid = false;      // exp_n: this rank's own distinct k-mers, counted before the merge
     void do_export_path_tokens(void* dst, uint64_t stride, const uint64_t* counts, uint32_t n_ranks);
@@ -2425,15 +1835,6 @@ struct DevicePipeline::Impl {
     void do_import_runs(const void* dev_ptr, uint64_t n);
     void do_import_runs_from(const void* const* ptrs, const uint64_t* counts, uint32_t n_ranks);
     DevBuf own_entries, own_runs;
-    DevBuf trim_jobs, trim_vals, trim_w, trim_bits, trim_scratch, trim_out, trim_len;      // overlap_align
-    DevBuf br_jobs, br_vals, br_w, br_scratch, br_dist;                                      // bridge_distances
-    DevBuf dp_bytes, dp_seqs, dp_keys, dp_px, dp_tag, dp_rep, dp_cnt, dp_off, dp_fill, dp_gpx, dp_gtag, dp_table, dp_gstart, dp_gsize, dp_gdots,
-           dp_pix, dp_rgb, dp_hidx, dp_hkey, dp_scan[8];                                      // dotplot
-    void scan_u64(uint64_t* x, uint64_t n, int level = 0);                                   // in place, exclusive
-    DevBuf dist_asym, upgma_m, upgma_alive, upgma_cnt, upgma_node, upgma_rd, upgma_rj, upgma_list, upgma_out, upgma_done;   // cluster_distances / upgma
-    uint32_t sym_n = 0;                                      // upgma_m holds cluster_distances' symmetric matrix of this many sequences (0: none)
-    void upload_paths(const UStrand* path, const uint64_t* path_off, uint32_t n, const uint32_t* unitig_len, uint32_t U);   // and clears the outputs
-    void share_lengths(uint64_t steps, uint32_t n, uint32_t U);
 #ifdef AC_EMULATE
     // AC_EMU_POISON=1 (CPU suite): before every table build, every device buffer a kernel writes is filled with a pattern, so a kernel that
     // reads what THIS build has not written (on the GPU: leftovers of the previous build, whose slot numbers differ from run to run, while
@@ -2442,7 +1843,7 @@ struct DevicePipeline::Impl {
         static const bool on = getenv("AC_EMU_POISON") != nullptr;
         if (!on) return;
         DevBuf* all[] = {&packed, &slots, &pos_slot, &flags8, &bmask, &bcount, &boff, &counters, &uid_rep, &slot_unitig, &run_start, &run_len, &run_uk, &run_dir, &is_rep, &rep_idx,
-                         &run_unitig, &unitigs, &nchunks, &chunk_off, &partial, &link_count, &links, &scan_tmp[0], &scan_tmp[1], &scan_tmp[2], &scan_tmp[3], &d_fixed, &cand_flag, &cand_index,
+                         &run_unitig, &unitigs, &nchunks, &chunk_off, &partial, &link_count, &links, &scan.serial.level[0], &scan.serial.level[1], &scan.serial.level[2], &scan.serial.level[3], &d_fixed, &cand_flag, &cand_index,
                          &d_cands, &d_cand_at, &d_deps, &d_spec, &sort_a, &sort_b, &sort_ra, &sort_rb, &num_prefix, &rank, &d_len, &d_depth, &need, &d_seq_off, &d_arena, &d_min_fpos, &d_min_rpos,
                          &strand_cnt, &d_next_off, &d_next, &prev_cnt, &d_prev_off, &d_prev, &d_path, &d_path_off, &d_rec, &d_pred, &d_level, &d_flagmax, &d_counters64, &d_dirty, &d_exhausted,
                          &d_arena2, &d_arena3, &d_pos, &sort_c, &sort_d, &d_pos2, &gfa_s_size, &gfa_l_size, &gfa_p_size, &gfa_pieces, &d_text, &d_ptext, &d_last, &run_hs, &run_ts, &claimed,
@@ -2461,45 +1862,26 @@ struct DevicePipeline::Impl {
 #endif
 };
 
-DevicePipeline::DevicePipeline(int device, void* stream) : impl(new Impl) {
-    impl->device = device; impl->before_results = &before_results;
+DevicePipeline::Impl::Impl(int device, void* stream) : DeviceContext(device, stream) {
 #ifndef AC_EMULATE
-    int n = 0;
-    cudaError_t e = cudaGetDeviceCount(&n);
-    if (e != cudaSuccess || n == 0)
-        throw std::runtime_error(std::string("autocycler_gpu: no CUDA device available (") + cudaGetErrorString(e) +
-                                 "); this library has no CPU path");
-    AC_CUDA_CHECK(cudaSetDevice(device));
-    if (stream) { impl->stream.s = (cudaStream_t)stream; }
-    else { AC_CUDA_CHECK(cudaStreamCreateWithFlags(&impl->stream.s, cudaStreamNonBlocking)); impl->own_stream = true; }
-    for (auto& ev : impl->ev) AC_CUDA_CHECK(cudaEventCreate(&ev));
-#else
-    (void)stream;
+    for (auto& e : ev) AC_CUDA_CHECK(cudaEventCreate(&e));
+#endif
+}
+DevicePipeline::Impl::~Impl() {        // the buffers go first (on this device), the stream last (DeviceContext)
+#ifndef AC_EMULATE
+    cudaSetDevice(device);
+    for (auto& e : ev) cudaEventDestroy(e);
 #endif
 }
 
-DevicePipeline::~DevicePipeline() {
-#ifndef AC_EMULATE
-    cudaSetDevice(impl->device);
-    for (auto& ev : impl->ev) cudaEventDestroy(ev);
-#endif
-    Impl* p = impl; impl = nullptr;
-#ifndef AC_EMULATE
-    cudaStream_t s = p->stream.s; bool own = p->own_stream;
-    delete p;
-    if (own) cudaStreamDestroy(s);
-#else
-    delete p;
-#endif
-}
+DevicePipeline::DevicePipeline(int device, void* stream) : impl(new Impl(device, stream)) { impl->before_results = &before_results; }
+DevicePipeline::~DevicePipeline() { delete impl; }
 
 unsigned long long DevicePipeline::kernel_launches() const { return g_ac_kernel_launches; }
+DeviceContext& DevicePipeline::context() { return *impl; }
 
 void DevicePipeline::upload(const uint8_t* ascii, uint64_t total, const SeqInfo* seqs, uint32_t n_seqs, uint32_t k, uint32_t seq_lo, uint32_t seq_hi) {
-    Impl& m = *impl;
-#ifndef AC_EMULATE
-    AC_CUDA_CHECK(cudaSetDevice(m.device));
-#endif
+    Impl& m = *impl; m.make_current();
     if (k < 3 || (k & 1) == 0) throw std::runtime_error("k must be odd and >= 3");
     const int W = (int)((2 * k + 63) / 64);
     if (W > AC_MAX_W) throw std::runtime_error("k-mer sizes above " + std::to_string(AC_MAX_K) + " are not supported by the GPU path (no CPU fallback exists)");
@@ -2538,321 +1920,9 @@ void DevicePipeline::set_path_line_texts(const char* blob, const uint32_t* prefi
     m.path_blob.assign(blob, blob + bytes);
 }
 
-void DevicePipeline::Impl::upload_paths(const UStrand* path, const uint64_t* path_off, uint32_t n, const uint32_t* unitig_len, uint32_t U) {
-    const uint64_t steps = path_off[n];
-    const uint32_t words = (n + 31) / 32;
-    d_path.ensure(steps * 4 + 4); d_path_off.ensure(((size_t)n + 1) * 8); d_len.ensure((size_t)U * 4 + 4);
-    dist_member.ensure((size_t)U * words * 4 + 4); dist_shared.ensure((size_t)n * n * 8);
-    if (steps) ac_h2d(d_path.p, path, steps * 4, &stream);
-    ac_h2d(d_path_off.p, path_off, ((size_t)n + 1) * 8, &stream);
-    if (U) ac_h2d(d_len.p, unitig_len, (size_t)U * 4, &stream);
-    ac_memset(dist_member.p, 0, (size_t)U * words * 4 + 4, &stream);
-    ac_memset(dist_shared.p, 0, (size_t)n * n * 8, &stream);
-}
-void DevicePipeline::Impl::share_lengths(uint64_t steps, uint32_t n, uint32_t U) {
-    const uint32_t words = (n + 31) / 32;
-    ac_launch("path_member", &stream, PathMemberBody{d_path.as<UStrand>(), d_path_off.as<uint64_t>(), n, words, dist_member.as<uint32_t>()}, steps);
-    ac_launch("pair_share", &stream, PairShareBody{dist_member.as<uint32_t>(), d_len.as<uint32_t>(), n, words, dist_shared.as<unsigned long long>()}, U);
-}
-
-void DevicePipeline::pair_shared_lengths(const UStrand* path, const uint64_t* path_off, uint32_t n, const uint32_t* unitig_len, uint32_t U, uint64_t* shared) {
-    Impl& m = *impl; m.set_device();
-    if (n == 0) return;
-    m.upload_paths(path, path_off, n, unitig_len, U);
-    m.share_lengths(path_off[n], n, U);
-    ac_d2h(shared, m.dist_shared.p, (size_t)n * n * 8, &m.stream);
-    ac_sync(&m.stream);
-}
-
-float DevicePipeline::cluster_distances(const UStrand* path, const uint64_t* path_off, uint32_t n, const uint32_t* unitig_len, uint32_t U, double* asym) {
-    Impl& m = *impl; m.set_device();
-    m.sym_n = 0;
-    if (n == 0) return 0.f;
-    const size_t nn = (size_t)n * n;
-    m.dist_asym.ensure(nn * 8); m.upgma_m.ensure(nn * 8);
-    float ms = 0.f;
-    m.upload_paths(path, path_off, n, unitig_len, U);
-#ifndef AC_EMULATE
-    cudaEvent_t e0, e1;                                       // the three kernels only: the uploads and memsets above are outside
-    AC_CUDA_CHECK(cudaEventCreate(&e0)); AC_CUDA_CHECK(cudaEventCreate(&e1));
-    AC_CUDA_CHECK(cudaEventRecord(e0, m.stream.s));
-#endif
-    m.share_lengths(path_off[n], n, U);
-    ac_launch("distance", &m.stream, DistanceBody{m.dist_shared.as<unsigned long long>(), n, m.dist_asym.as<double>(), m.upgma_m.as<double>()}, nn);
-#ifndef AC_EMULATE
-    AC_CUDA_CHECK(cudaEventRecord(e1, m.stream.s));
-#endif
-    ac_d2h(asym, m.dist_asym.p, nn * 8, &m.stream);
-    ac_sync(&m.stream);
-#ifndef AC_EMULATE
-    AC_CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-#endif
-    m.sym_n = n;
-    return ms;
-}
-
-float DevicePipeline::upgma(const double* sym, uint32_t n, const uint32_t* ids, UpgmaMerge* merges) {
-    Impl& m = *impl; m.set_device();
-    for (uint32_t i = 1; i < n; ++i) if (ids[i] <= ids[i - 1]) throw std::runtime_error("upgma: ids must be strictly ascending");
-    if (!sym && m.sym_n != n) throw std::runtime_error("upgma: no distance matrix of this size on the device");
-    m.sym_n = 0;                                              // the kernel works in place
-    if (n < 2) return 0.f;
-    const size_t nn = (size_t)n * n;
-    m.upgma_m.ensure(nn * 8); m.upgma_alive.ensure(n); m.upgma_cnt.ensure((size_t)n * 4); m.upgma_node.ensure((size_t)n * 4);
-    m.upgma_rd.ensure((size_t)n * 8); m.upgma_rj.ensure((size_t)n * 4); m.upgma_list.ensure((size_t)n * 4); m.upgma_out.ensure((size_t)n * sizeof(UpgmaMerge));
-    m.upgma_done.ensure(4);
-    if (sym) ac_h2d(m.upgma_m.p, sym, nn * 8, &m.stream);
-    const std::vector<uint32_t> ones(n, 1u);
-    ac_memset(m.upgma_alive.p, 1, n, &m.stream);
-    ac_h2d(m.upgma_cnt.p, ones.data(), (size_t)n * 4, &m.stream);
-    ac_h2d(m.upgma_node.p, ids, (size_t)n * 4, &m.stream);
-    double* M = m.upgma_m.as<double>(); uint8_t* alive = m.upgma_alive.as<uint8_t>(); uint32_t* cnt = m.upgma_cnt.as<uint32_t>(); uint32_t* node = m.upgma_node.as<uint32_t>();
-    double* rd = m.upgma_rd.as<double>(); uint32_t* rj = m.upgma_rj.as<uint32_t>(); UpgmaMerge* out = m.upgma_out.as<UpgmaMerge>();
-    const uint32_t first_node = ids[n - 1] + 1;
-    uint32_t done = 0;
-    float ms = 0.f;
-#ifndef AC_EMULATE
-    cudaEvent_t e0, e1;
-    AC_CUDA_CHECK(cudaEventCreate(&e0)); AC_CUDA_CHECK(cudaEventCreate(&e1));
-    AC_CUDA_CHECK(cudaEventRecord(e0, m.stream.s));
-    ac_upgma_kernel<<<1, 1024, 0, m.stream.s>>>(M, n, alive, cnt, node, rd, rj, m.upgma_list.as<uint32_t>(), out, first_node, m.upgma_done.as<uint32_t>());
-    AC_CUDA_CHECK(cudaGetLastError()); ++g_ac_kernel_launches; ac_debug_sync("upgma", &m.stream);
-    AC_CUDA_CHECK(cudaEventRecord(e1, m.stream.s));
-    ac_d2h(merges, out, (size_t)(n - 1) * sizeof(UpgmaMerge), &m.stream);
-    ac_d2h(&done, m.upgma_done.p, 4, &m.stream);
-    ac_sync(&m.stream);
-    AC_CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-#else
-    // the kernel's steps, serially: row minima, least pair, merged row, then the rows that must be scanned again
-    for (uint32_t i = 0; i < n; ++i) { rd[i] = INFINITY; rj[i] = AC_UPGMA_NONE; upgma_row_scan(M, n, alive, i, i + 1, 1, rd[i], rj[i]); }
-    done = n - 1;
-    for (uint32_t step = 0; step + 1 < n; ++step) {
-        double bd = INFINITY; uint32_t a = AC_UPGMA_NONE, b = AC_UPGMA_NONE;
-        for (uint32_t i = 0; i < n; ++i) if (alive[i] && upgma_less(rd[i], i, rj[i], bd, a, b)) { bd = rd[i]; a = i; b = rj[i]; }
-        if (b == AC_UPGMA_NONE) { done = step; break; }
-        UpgmaMerge mg; mg.node = first_node + step; mg.left = node[a]; mg.right = node[b]; mg.pad = 0; mg.dist = bd / 2.0;
-        out[step] = mg;
-        alive[b] = 0; cnt[a] += cnt[b]; node[a] = mg.node;
-        for (uint32_t j = 0; j < n; ++j) if (alive[j] && j != a) upgma_merge_entry(M, n, a, b, j, cnt[a], cnt[j]);
-        for (uint32_t i = 0; i < b; ++i)
-            if (alive[i] && (i == a || upgma_row_after_merge(M, n, a, b, i, rd[i], rj[i]))) {
-                rd[i] = INFINITY; rj[i] = AC_UPGMA_NONE; upgma_row_scan(M, n, alive, i, i + 1, 1, rd[i], rj[i]);
-            }
-    }
-    memcpy(merges, out, (size_t)(n - 1) * sizeof(UpgmaMerge));
-#endif
-    if (done != n - 1) throw std::runtime_error("upgma: no pair of clusters with a comparable (non-NaN) distance is left after " + std::to_string(done) + " merges");
-    return ms;
-}
-
-uint32_t DevicePipeline::overlap_shared_k_max() {
-#ifndef AC_EMULATE
-    impl->set_device();
-    static int optin = -1;                           // one device model per process
-    if (optin < 0) { int dev = 0; AC_CUDA_CHECK(cudaGetDevice(&dev)); AC_CUDA_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev)); }
-    const int budget = optin - 64;                   // the kernel's own static shared variables
-#else
-    const int budget = 227 * 1024 - 64;              // what an H100 grants one CTA
-#endif
-    return (uint32_t)(budget / 24) - 1;
-}
-
-float DevicePipeline::overlap_align(const int32_t* values, uint64_t n_values, const uint32_t* weights, uint64_t n_weights,
-                                    const OverlapJob* jobs, uint32_t n_jobs, std::vector<std::vector<AlignPiece>>& out) {
-    Impl& m = *impl; m.set_device();
-    out.assign(n_jobs, {});
-    const uint32_t shared_k = overlap_shared_k_max();
-    // windows of k = 0 have no cell; the others are launched largest first (a CTA per job, the long ones start before the short ones)
-    std::vector<uint32_t> run;
-    for (uint32_t x = 0; x < n_jobs; ++x) {
-        if (jobs[x].k > jobs[x].n) throw std::runtime_error("overlap_align: window larger than the path");
-        if (jobs[x].k > 0) run.push_back(x);
-    }
-    if (run.empty()) return 0.f;
-    std::stable_sort(run.begin(), run.end(), [&](uint32_t a, uint32_t b) { return jobs[a].k > jobs[b].k; });
-    std::vector<TrimLaunchJob> lj(run.size());
-    uint64_t bits_words = 0, out_pieces = 0, scratch = 0;
-    uint32_t n_shared = 0, k_shared = 0;
-    for (size_t r = 0; r < run.size(); ++r) {
-        const OverlapJob& J = jobs[run[r]];
-        if (J.a_off + J.n > n_values || J.b_off + J.n > n_values) throw std::runtime_error("overlap_align: path outside the value array");
-        TrimLaunchJob& L = lj[r];
-        L.a_off = J.a_off; L.b_off = J.b_off; L.n = J.n; L.k = J.k; L.skip = J.skip_diagonal ? 1 : 0; L.slot = (uint32_t)r;
-        L.bits_off = bits_words; bits_words += trim_bit_words(J.k);
-        L.out_off = out_pieces; out_pieces += 2ull * J.k;
-        L.scratch_off = 0;
-        if (J.k <= shared_k) { ++n_shared; k_shared = std::max(k_shared, J.k); }
-        else { L.scratch_off = scratch; scratch += 3ull * (J.k + 1); }
-    }
-    // jobs with shared-memory diagonals first (largest first), then the ones whose diagonals live in HBM
-    std::stable_partition(lj.begin(), lj.end(), [&](const TrimLaunchJob& L) { return L.k <= shared_k; });
-    m.trim_jobs.ensure(lj.size() * sizeof(TrimLaunchJob)); m.trim_vals.ensure(n_values * 4 + 4); m.trim_w.ensure(n_weights * 4 + 4);
-    m.trim_bits.ensure(bits_words * 4 + 4); m.trim_out.ensure(out_pieces * sizeof(AlignPiece) + 16); m.trim_len.ensure(run.size() * 4);
-    m.trim_scratch.ensure(scratch * 8 + 8);
-    ac_h2d(m.trim_jobs.p, lj.data(), lj.size() * sizeof(TrimLaunchJob), &m.stream);
-    if (n_values) ac_h2d(m.trim_vals.p, values, n_values * 4, &m.stream);
-    if (n_weights) ac_h2d(m.trim_w.p, weights, n_weights * 4, &m.stream);
-    for (uint64_t v = 0; v < n_values; ++v) { const int64_t a = values[v] < 0 ? -(int64_t)values[v] : values[v]; if ((uint64_t)a >= n_weights) throw std::runtime_error("overlap_align: unitig without a weight"); }
-    std::vector<uint32_t> len(run.size());
-    float ms = 0.f;
-#ifndef AC_EMULATE
-    cudaEvent_t e0, e1;
-    AC_CUDA_CHECK(cudaEventCreate(&e0)); AC_CUDA_CHECK(cudaEventCreate(&e1));
-    AC_CUDA_CHECK(cudaEventRecord(e0, m.stream.s));
-    const size_t smem = (size_t)24 * (k_shared + 1);
-    if (n_shared) {
-        AC_CUDA_CHECK(cudaFuncSetAttribute(ac_overlap_align_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        ac_overlap_align_kernel<<<n_shared, 1024, smem, m.stream.s>>>(m.trim_jobs.as<TrimLaunchJob>(), m.trim_vals.as<int32_t>(), m.trim_w.as<uint32_t>(),
-            m.trim_bits.as<uint32_t>(), m.trim_scratch.as<double>(), m.trim_out.as<AlignPiece>(), m.trim_len.as<uint32_t>(), 1);
-        AC_CUDA_CHECK(cudaGetLastError()); ++g_ac_kernel_launches; ac_debug_sync("overlap_align", &m.stream);
-    }
-    if (n_shared < lj.size()) {
-        ac_overlap_align_kernel<<<(unsigned)(lj.size() - n_shared), 1024, 0, m.stream.s>>>(m.trim_jobs.as<TrimLaunchJob>() + n_shared, m.trim_vals.as<int32_t>(),
-            m.trim_w.as<uint32_t>(), m.trim_bits.as<uint32_t>(), m.trim_scratch.as<double>(), m.trim_out.as<AlignPiece>(), m.trim_len.as<uint32_t>(), 0);
-        AC_CUDA_CHECK(cudaGetLastError()); ++g_ac_kernel_launches; ac_debug_sync("overlap_align_hbm", &m.stream);
-    }
-    AC_CUDA_CHECK(cudaEventRecord(e1, m.stream.s));
-    ac_d2h(len.data(), m.trim_len.p, run.size() * 4, &m.stream);
-    ac_sync(&m.stream);
-    AC_CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-#else
-    // the same per-cell recurrence, right-edge maximum and traceback, in row-major order (a topological order of the matrix)
-    (void)k_shared;
-    uint32_t* bits = m.trim_bits.as<uint32_t>();
-    memset(bits, 0, bits_words * 4);
-    for (const TrimLaunchJob& L : lj) {
-        const uint32_t k = L.k;
-        const int32_t* pa = m.trim_vals.as<int32_t>() + L.a_off;
-        const int32_t* pb = m.trim_vals.as<int32_t>() + L.b_off + (L.n - k);
-        const uint32_t* w = m.trim_w.as<uint32_t>();
-        std::vector<uint64_t> diag_off(2 * (size_t)k + 2, 0);
-        for (uint32_t d = 3; d <= 2 * k + 1; ++d) diag_off[d] = diag_off[d - 1] + trim_diag_words(d - 1, k);
-        std::vector<double> above(k + 1, 0.0), row(k + 1, 0.0);
-        double best = -INFINITY; uint32_t best_i = 0;
-        for (uint32_t i = 1; i <= k; ++i) {
-            row[0] = 0.0;
-            for (uint32_t j = 1; j <= k; ++j) {
-                const double up = above[j], left = row[j - 1];
-                const uint32_t d = i + j, t = i - trim_diag_lo(d, k);
-                if (up >= left) bits[L.bits_off + diag_off[d] + t / 32] |= 1u << (t % 32);
-                double s = -INFINITY;
-                if (!(L.skip && i == j + (L.n - k))) {
-                    const int32_t a = pa[i - 1], b = pb[j - 1];
-                    s = trim_cell(above[j - 1], up, left, a, b, (double)w[a < 0 ? -a : a], (double)w[b < 0 ? -b : b]);
-                }
-                row[j] = s;
-            }
-            trim_edge(row[k], i, best, best_i);
-            above.swap(row);
-        }
-        len[L.slot] = best > 0.0 ? trim_traceback(pa, pb, L.n, k, bits + L.bits_off, best_i, m.trim_out.as<AlignPiece>() + L.out_off) : 0;
-    }
-#endif
-    // the pieces of every job sit at the front of its 2k slots, last column first
-    for (const TrimLaunchJob& L : lj) {
-        if (!len[L.slot]) continue;
-        std::vector<AlignPiece>& o = out[run[L.slot]];
-        o.resize(len[L.slot]);
-        ac_d2h(o.data(), m.trim_out.as<AlignPiece>() + L.out_off, (size_t)len[L.slot] * sizeof(AlignPiece), &m.stream);
-    }
-    ac_sync(&m.stream);
-    for (auto& o : out) std::reverse(o.begin(), o.end());
-    return ms;
-}
-
-uint32_t DevicePipeline::bridge_shared_n_max() {
-#ifndef AC_EMULATE
-    impl->set_device();
-    static int optin = -1;                           // one device model per process
-    if (optin < 0) { int dev = 0; AC_CUDA_CHECK(cudaGetDevice(&dev)); AC_CUDA_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev)); }
-    const int budget = optin;                        // the kernel has no static shared variables
-#else
-    const int budget = 227 * 1024;                   // what an H100 grants one CTA
-#endif
-    return (uint32_t)(budget / 12) - 1;
-}
-
-float DevicePipeline::bridge_distances(const int32_t* values, uint64_t n_values, const uint32_t* weights, uint64_t n_weights,
-                                       const BridgeJob* jobs, uint32_t n_jobs, uint32_t* dist, BridgeRun* run_info) {
-    Impl& m = *impl; m.set_device();
-    if (run_info) *run_info = BridgeRun();
-    if (n_jobs == 0) return 0.f;
-    for (uint64_t v = 0; v < n_values; ++v) { const int64_t a = values[v] < 0 ? -(int64_t)values[v] : values[v]; if ((uint64_t)a >= n_weights) throw std::runtime_error("bridge_distances: unitig without a weight"); }
-    const uint32_t shared_n = bridge_shared_n_max();
-    // largest first (a CTA per job: the long ones start before the short ones); jobs with shared-memory diagonals, then the HBM ones
-    std::vector<BridgeLaunchJob> lj(n_jobs);
-    for (uint32_t x = 0; x < n_jobs; ++x) {
-        const BridgeJob& J = jobs[x];
-        if (J.n > J.m) throw std::runtime_error("bridge_distances: the rows must be the shorter path");
-        if (J.a_off + J.n > n_values || J.b_off + J.m > n_values) throw std::runtime_error("bridge_distances: path outside the value array");
-        lj[x] = BridgeLaunchJob{J.a_off, J.b_off, 0, J.n, J.m, x, 0};
-    }
-    std::stable_sort(lj.begin(), lj.end(), [](const BridgeLaunchJob& a, const BridgeLaunchJob& b) { return (uint64_t)a.n * a.m > (uint64_t)b.n * b.m; });
-    std::stable_partition(lj.begin(), lj.end(), [&](const BridgeLaunchJob& L) { return L.n <= shared_n; });
-    uint32_t n_shared = 0, n_max_shared = 0;
-    uint64_t scratch = 0;
-    for (BridgeLaunchJob& L : lj) {
-        if (L.n <= shared_n) { ++n_shared; n_max_shared = std::max(n_max_shared, L.n); }
-        else { L.scratch_off = scratch; scratch += 3ull * (L.n + 1); }
-    }
-    if (run_info) { run_info->shared_jobs = n_shared; run_info->hbm_jobs = n_jobs - n_shared; }
-    m.br_jobs.ensure(lj.size() * sizeof(BridgeLaunchJob)); m.br_vals.ensure(n_values * 4 + 4); m.br_w.ensure(n_weights * 4 + 4);
-    m.br_scratch.ensure(scratch * 4 + 4); m.br_dist.ensure((size_t)n_jobs * 4);
-    ac_h2d(m.br_jobs.p, lj.data(), lj.size() * sizeof(BridgeLaunchJob), &m.stream);
-    if (n_values) ac_h2d(m.br_vals.p, values, n_values * 4, &m.stream);
-    if (n_weights) ac_h2d(m.br_w.p, weights, n_weights * 4, &m.stream);
-    float ms = 0.f;
-#ifndef AC_EMULATE
-    cudaEvent_t e0, e1;
-    AC_CUDA_CHECK(cudaEventCreate(&e0)); AC_CUDA_CHECK(cudaEventCreate(&e1));
-    AC_CUDA_CHECK(cudaEventRecord(e0, m.stream.s));
-    if (n_shared) {
-        const size_t smem = (size_t)12 * (n_max_shared + 1);
-        AC_CUDA_CHECK(cudaFuncSetAttribute(ac_bridge_distance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        ac_bridge_distance_kernel<<<n_shared, AC_BRIDGE_THREADS, smem, m.stream.s>>>(m.br_jobs.as<BridgeLaunchJob>(), m.br_vals.as<int32_t>(), m.br_w.as<uint32_t>(),
-            m.br_scratch.as<uint32_t>(), m.br_dist.as<uint32_t>(), 1);
-        AC_CUDA_CHECK(cudaGetLastError()); ++g_ac_kernel_launches; ac_debug_sync("bridge_distance", &m.stream);
-    }
-    if (n_shared < n_jobs) {
-        ac_bridge_distance_kernel<<<n_jobs - n_shared, AC_BRIDGE_THREADS, 0, m.stream.s>>>(m.br_jobs.as<BridgeLaunchJob>() + n_shared, m.br_vals.as<int32_t>(),
-            m.br_w.as<uint32_t>(), m.br_scratch.as<uint32_t>(), m.br_dist.as<uint32_t>(), 0);
-        AC_CUDA_CHECK(cudaGetLastError()); ++g_ac_kernel_launches; ac_debug_sync("bridge_distance_hbm", &m.stream);
-    }
-    AC_CUDA_CHECK(cudaEventRecord(e1, m.stream.s));
-    ac_d2h(dist, m.br_dist.p, (size_t)n_jobs * 4, &m.stream);
-    ac_sync(&m.stream);
-    AC_CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-#else
-    // the same diagonals and per-cell body, one job and one cell at a time
-    const int32_t* vals = m.br_vals.as<int32_t>();
-    const uint32_t* w = m.br_w.as<uint32_t>();
-    std::vector<uint32_t> own;
-    for (const BridgeLaunchJob& L : lj) {
-        const uint32_t stride = L.n + 1;
-        uint32_t* D;
-        if (L.n <= shared_n) { own.assign(3 * (size_t)stride, 0xA5A5A5A5u); D = own.data(); }
-        else D = m.br_scratch.as<uint32_t>() + L.scratch_off;
-        D[0] = 0;
-        for (uint32_t d = 1; d <= L.n + L.m; ++d) {
-            uint32_t* cur = D + (size_t)(d % 3) * stride;
-            const uint32_t* prev = D + (size_t)((d - 1) % 3) * stride;
-            const uint32_t* prev2 = D + (size_t)((d + 1) % 3) * stride;
-            for (uint32_t i = bridge_diag_lo(d, L.m); i <= bridge_diag_hi(d, L.n); ++i) bridge_cell(cur, prev, prev2, i, d - i, vals + L.a_off, vals + L.b_off, w);
-        }
-        m.br_dist.as<uint32_t>()[L.slot] = D[(size_t)((L.n + L.m) % 3) * stride + L.n];
-    }
-    ac_d2h(dist, m.br_dist.p, (size_t)n_jobs * 4, &m.stream);
-#endif
-    return ms;
-}
-
 void DevicePipeline::find_literals(const uint8_t* ascii_host, uint64_t total_bytes, const SeqInfo* host_seq, uint32_t n, uint32_t h,
                                    const uint64_t* needle_words, uint32_t n_needles, std::vector<LiteralHit>& out) {
-    Impl& m = *impl; m.set_device();
+    Impl& m = *impl; m.make_current();
     const int WH = (int)((2 * h + 63) / 64);
     if (WH > 2) throw std::runtime_error("end repair literals longer than 64 bases are not supported by the GPU path");
     const KParams p = make_kparams(h, WH);
@@ -2988,7 +2058,7 @@ template <int W> uint64_t DevicePipeline::Impl::list_claimed(bool with_filter) {
     const uint64_t n_words = (total + 31) / 32;
     claimed_cnt.ensure((n_words + 1) * 4);
     ac_launch("claimed_count", &stream, ClaimedCountBody{claimed.as<uint32_t>(), n_words, claimed_cnt.as<uint32_t>()}, n_words + 1);
-    const uint64_t n = exclusive_scan(claimed_cnt.as<uint32_t>(), claimed_cnt.as<uint32_t>(), n_words + 1);
+    const uint64_t n = scan(&stream, claimed_cnt.as<uint32_t>(), claimed_cnt.as<uint32_t>(), n_words + 1);
     occ_list.ensure((n + 1) * 4);
     if (with_filter) {
         // two entries per distinct k-mer, 3 bits each: about 4 entries per word, one test in 200 passes by chance (26 MB for BASELINE
@@ -3061,7 +2131,7 @@ template <int W> void DevicePipeline::Impl::runs_local_w() {
     bmask.ensure(n_bwords * sizeof(uint32_t)); bcount.ensure(n_bwords * sizeof(uint32_t)); boff.ensure(n_bwords * sizeof(uint32_t));
     ac_launch("boundaries", &stream, BoundaryBody{packed.as<uint64_t>(), seqs.as<SeqInfo>(), n_seqs, p.h, g_begin, g_end, pos_slot.as<uint32_t>(),
                                                   flags8.as<uint8_t>(), interior8.as<uint8_t>(), bmask.as<uint32_t>(), bcount.as<uint32_t>()}, n_bwords * 32);
-    n_runs = exclusive_scan(bcount.as<uint32_t>(), boff.as<uint32_t>(), n_bwords);
+    n_runs = scan(&stream, bcount.as<uint32_t>(), boff.as<uint32_t>(), n_bwords);
     mark(6);
     run_start.ensure(n_runs * sizeof(uint64_t)); run_len.ensure(n_runs * 4); run_hs.ensure(n_runs * 4); run_ts.ensure(n_runs * 4);
     ac_launch("run_scatter", &stream, RunScatterBody{bmask.as<uint32_t>(), boff.as<uint32_t>(), run_start.as<uint64_t>()}, n_bwords);
@@ -3116,7 +2186,7 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
     ac_launch("run_key", &stream, RunKeyBody{packed.as<uint64_t>(), p.h, run_start.as<uint64_t>(), run_hs.as<uint32_t>(), run_ts.as<uint32_t>(),
                                              run_uk.as<uint32_t>(), run_dir.as<uint8_t>(), uid_rep.as<uint32_t>()}, n_runs);
     ac_launch("rep_flag", &stream, RepFlagBody{run_uk.as<uint32_t>(), uid_rep.as<uint32_t>(), is_rep.as<uint32_t>()}, n_runs);
-    const uint32_t n_unitigs = exclusive_scan(is_rep.as<uint32_t>(), rep_idx.as<uint32_t>(), n_runs);
+    const uint32_t n_unitigs = scan(&stream, is_rep.as<uint32_t>(), rep_idx.as<uint32_t>(), n_runs);
     unitigs.ensure((size_t)n_unitigs * sizeof(DeviceUnitig));
     ac_launch("run_assign", &stream, RunAssignBody{run_start.as<uint64_t>(), run_len.as<uint32_t>(), run_uk.as<uint32_t>(), run_dir.as<uint8_t>(),
                                                    uid_rep.as<uint32_t>(), rep_idx.as<uint32_t>(), run_hs.as<uint32_t>(), run_ts.as<uint32_t>(), tv,
@@ -3127,7 +2197,7 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
     nchunks.ensure(((size_t)n_unitigs + 1) * 4); chunk_off.ensure(((size_t)n_unitigs + 1) * 4);
     ac_launch("chunk_count", &stream, ChunkCountBody{unitigs.as<DeviceUnitig>(), nchunks.as<uint32_t>()}, n_unitigs);
     ac_memset(nchunks.as<uint32_t>() + n_unitigs, 0, 4, &stream);
-    const uint32_t n_chunks = exclusive_scan(nchunks.as<uint32_t>(), chunk_off.as<uint32_t>(), (uint64_t)n_unitigs + 1);
+    const uint32_t n_chunks = scan(&stream, nchunks.as<uint32_t>(), chunk_off.as<uint32_t>(), (uint64_t)n_unitigs + 1);
     partial.ensure((size_t)n_chunks * sizeof(MinPartial<W>));
     ac_launch("chunk_min", &stream, ChunkMinBody<W>{packed.as<uint64_t>(), seqs.as<SeqInfo>(), n_seqs, p, unitigs.as<DeviceUnitig>(), n_unitigs,
                                                     chunk_off.as<uint32_t>(), partial.as<MinPartial<W>>()}, n_chunks);
@@ -3155,7 +2225,7 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
     {   // the arena must stay below 4 GB for the 32-bit scan; sum(len) <= windows
         if (n_windows + (uint64_t)U * 2 * AC_SEQ_SLACK >= 0xFFFFFFF0ull) throw std::runtime_error("unitig sequence arena would exceed 4 GB");
     }
-    const uint64_t arena_bytes = exclusive_scan(need.as<uint32_t>(), need.as<uint32_t>(), (uint64_t)U + 1);
+    const uint64_t arena_bytes = scan(&stream, need.as<uint32_t>(), need.as<uint32_t>(), (uint64_t)U + 1);
     ac_launch("seq_off", &stream, SeqOffBody{need.as<uint32_t>(), d_seq_off.as<uint64_t>()}, U);
     d_arena.ensure(arena_bytes);
     ac_launch("emit_seq", &stream, EmitSeqBody{packed.as<uint64_t>(), p.h, unitigs.as<DeviceUnitig>(), U, chunk_off.as<uint32_t>(), rank.as<uint32_t>(),
@@ -3166,13 +2236,13 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
     prev_cnt.ensure(((size_t)n_strands + 1) * 4); d_prev_off.ensure(((size_t)n_strands + 1) * 4);
     ac_launch("link_count", &stream, LinkCountBody{link_count.as<uint32_t>(), rank.as<uint32_t>(), unitigs.as<DeviceUnitig>(), n_strands, strand_cnt.as<uint32_t>()},
               (uint64_t)n_strands + 1);
-    const uint64_t n_links = exclusive_scan(strand_cnt.as<uint32_t>(), d_next_off.as<uint32_t>(), (uint64_t)n_strands + 1);
+    const uint64_t n_links = scan(&stream, strand_cnt.as<uint32_t>(), d_next_off.as<uint32_t>(), (uint64_t)n_strands + 1);
     d_next.ensure(n_links * 4); d_prev.ensure(n_links * 4);
     ac_memset(prev_cnt.p, 0, ((size_t)n_strands + 1) * 4, &stream);
     d_small.ensure(64); ac_memset(d_small.p, 0, 64, &stream);           // [0] hairpin links
     ac_launch("link_order", &stream, LinkOrderBody{link_count.as<uint32_t>(), links.as<uint32_t>(), rank.as<uint32_t>(), unitigs.as<DeviceUnitig>(),
                                                    d_next_off.as<uint32_t>(), d_next.as<UStrand>(), prev_cnt.as<uint32_t>(), d_small.as<uint32_t>()}, n_strands);
-    exclusive_scan(prev_cnt.as<uint32_t>(), d_prev_off.as<uint32_t>(), (uint64_t)n_strands + 1, 0, false);      // the total is n_links again: no read-back, the stream carries on
+    scan(&stream, prev_cnt.as<uint32_t>(), d_prev_off.as<uint32_t>(), (uint64_t)n_strands + 1, false);      // the total is n_links again: no read-back, the stream carries on
     ac_memset(prev_cnt.p, 0, ((size_t)n_strands + 1) * 4, &stream);    // reused as the fill cursor
     ac_launch("prev_fill", &stream, PrevFillBody{d_next_off.as<uint32_t>(), d_next.as<UStrand>(), d_prev_off.as<uint32_t>(), prev_cnt.as<uint32_t>(), d_prev.as<UStrand>()}, n_strands);
     ac_launch("prev_sort", &stream, PrevSortBody{d_prev_off.as<uint32_t>(), d_prev.as<UStrand>()}, n_strands);
@@ -3198,7 +2268,7 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
     const CandidateView cview{ord_in, d_next_off.as<uint32_t>(), d_next.as<UStrand>(), d_prev_off.as<uint32_t>(), d_prev.as<UStrand>(), fix_start, fix_end};
     cand_flag.ensure((2 * (size_t)U + 1) * 4); cand_index.ensure((2 * (size_t)U + 1) * 4);
     ac_launch("candidate_flag", &stream, CandidateFlagBody{cview, U, cand_flag.as<uint32_t>()}, 2ull * U + 1);
-    const uint64_t n_cands = exclusive_scan(cand_flag.as<uint32_t>(), cand_index.as<uint32_t>(), 2ull * U + 1);
+    const uint64_t n_cands = scan(&stream, cand_flag.as<uint32_t>(), cand_index.as<uint32_t>(), 2ull * U + 1);
     d_cands.ensure((n_cands + 1) * sizeof(ExpandCandidate)); d_cand_at.ensure(2 * (size_t)U * 4 + 4); d_deps.ensure((size_t)U * sizeof(ExpandDeps) + 4); d_spec.ensure((n_cands + 1) * 4);
     ac_launch("candidate_fill", &stream, CandidateFillBody{cview, cand_flag.as<uint32_t>(), cand_index.as<uint32_t>(), d_cands.as<ExpandCandidate>(), d_cand_at.as<int32_t>()}, 2ull * U);
     ac_launch("dependents", &stream, DependentsBody{d_next_off.as<uint32_t>(), d_next.as<UStrand>(), d_prev_off.as<uint32_t>(), d_prev.as<UStrand>(), d_cand_at.as<int32_t>(),
@@ -3284,11 +2354,11 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
                 ac_memset(d_last.p, 0, steps + 8, &stream);
                 ac_launch("path_last", &stream, PathLastBody{d_path_off.as<uint64_t>(), d_last.as<uint8_t>()}, n_seqs);
                 ac_launch("path_size", &stream, PathSizeBody{d_path.as<UStrand>(), d_pos2.as<uint32_t>(), d_last.as<uint8_t>(), steps, gfa_p_size.as<uint32_t>()}, steps + 1);
-                scan_keep_total(gfa_p_size.as<uint32_t>(), steps + 1, d_totals.as<uint32_t>() + 3);
+                scan.keep_total(&stream, gfa_p_size.as<uint32_t>(), steps + 1, d_totals.as<uint32_t>() + 3);
             }
-            scan_keep_total(gfa_s_size.as<uint32_t>(), (uint64_t)U + 1, d_totals.as<uint32_t>() + 0);
-            scan_keep_total(gfa_l_size.as<uint32_t>(), (uint64_t)U + 1, d_totals.as<uint32_t>() + 1);
-            scan_keep_total(gfa_pieces.as<uint32_t>(), (uint64_t)U + 1, d_totals.as<uint32_t>() + 2);
+            scan.keep_total(&stream, gfa_s_size.as<uint32_t>(), (uint64_t)U + 1, d_totals.as<uint32_t>() + 0);
+            scan.keep_total(&stream, gfa_l_size.as<uint32_t>(), (uint64_t)U + 1, d_totals.as<uint32_t>() + 1);
+            scan.keep_total(&stream, gfa_pieces.as<uint32_t>(), (uint64_t)U + 1, d_totals.as<uint32_t>() + 2);
             uint32_t tot[4];
             ac_d2h(tot, d_totals.p, 16, &stream); ac_sync(&stream);
             const uint64_t s_bytes = tot[0], l_bytes = tot[1], n_pieces = tot[2], p_list_bytes = tot[3];
@@ -3421,7 +2491,7 @@ void DevicePipeline::Impl::do_render_path_lines(const void* tokens, uint64_t n_t
         ac_memset(d_own_last.p, 0, steps + 8, &stream);
         ac_launch("path_last", &stream, PathLastBody{d_own_off.as<uint64_t>(), d_own_last.as<uint8_t>()}, n_own);
         ac_launch("path_size", &stream, PathSizeBody{(const UStrand*)tokens, nullptr, d_own_last.as<uint8_t>(), steps, d_own_size.as<uint32_t>()}, steps + 1);
-        const uint64_t list_bytes = exclusive_scan(d_own_size.as<uint32_t>(), d_own_size.as<uint32_t>(), steps + 1);
+        const uint64_t list_bytes = scan(&stream, d_own_size.as<uint32_t>(), d_own_size.as<uint32_t>(), steps + 1);
         total_bytes = list_bytes + (wrap_hi - wrap_lo);
         d_ptext.ensure(total_bytes + 64);
         const PathLineView pv{d_own_off.as<uint64_t>(), n_own, d_own_size.as<uint32_t>(), d_wrap_off.as<uint64_t>() + own_seq_lo, d_pre_len.as<uint32_t>() + own_seq_lo,
@@ -3444,36 +2514,36 @@ void DevicePipeline::Impl::do_render_path_lines(const void* tokens, uint64_t n_t
     default: throw std::runtime_error("upload() must precede build()"); }
 
 void DevicePipeline::build_local(uint32_t seq_lo, uint32_t seq_hi, bool multi) {
-    Impl& m = *impl; m.set_device(); const int W = m.W;
+    Impl& m = *impl; m.make_current(); const int W = m.W;
     AC_DISPATCH_W(m.local_w, seq_lo, seq_hi, multi)
 }
 uint64_t DevicePipeline::count_entries() {
-    Impl& m = *impl; m.set_device(); const int W = m.W;
+    Impl& m = *impl; m.make_current(); const int W = m.W;
     uint64_t count = 0;
     AC_DISPATCH_W(count = m.do_count_entries)
     return count;
 }
-void DevicePipeline::export_entries(void* dst, uint64_t cap_records) { impl->set_device(); impl->do_export_entries(dst, cap_records); }
+void DevicePipeline::export_entries(void* dst, uint64_t cap_records) { impl->make_current(); impl->do_export_entries(dst, cap_records); }
 void DevicePipeline::merge_entries(const void* dev_ptr, uint64_t n) {
-    Impl& m = *impl; m.set_device(); const int W = m.W;
+    Impl& m = *impl; m.make_current(); const int W = m.W;
     AC_DISPATCH_W(m.merge_w, dev_ptr, n)
 }
 void DevicePipeline::runs_local() {
-    Impl& m = *impl; m.set_device(); const int W = m.W;
+    Impl& m = *impl; m.make_current(); const int W = m.W;
     AC_DISPATCH_W(m.runs_local_w)
 }
 uint64_t DevicePipeline::local_runs() const { return impl->n_runs; }
-void DevicePipeline::export_runs(void* dst, uint64_t cap_records) { impl->set_device(); impl->do_export_runs(dst, cap_records); }
-void DevicePipeline::import_runs(const void* dev_ptr, uint64_t n) { impl->set_device(); impl->do_import_runs(dev_ptr, n); }
+void DevicePipeline::export_runs(void* dst, uint64_t cap_records) { impl->make_current(); impl->do_export_runs(dst, cap_records); }
+void DevicePipeline::import_runs(const void* dev_ptr, uint64_t n) { impl->make_current(); impl->do_import_runs(dev_ptr, n); }
 void DevicePipeline::import_runs_padded(const void* dev_ptr, uint64_t stride, const uint64_t* counts, uint32_t n_ranks) {
     if (n_ranks == 0 || n_ranks > AC_MAX_RANKS) throw std::runtime_error("import_runs_padded: bad rank count");
     const void* ptrs[AC_MAX_RANKS];
     for (uint32_t q = 0; q < n_ranks; ++q) { if (counts[q] > stride) throw std::runtime_error("import_runs_padded: a rank holds more records than the stride"); ptrs[q] = (const char*)dev_ptr + (size_t)q * stride * sizeof(RunRec); }
     import_runs_from(ptrs, counts, n_ranks);
 }
-void DevicePipeline::import_runs_from(const void* const* ptrs, const uint64_t* counts, uint32_t n_ranks) { impl->set_device(); impl->do_import_runs_from(ptrs, counts, n_ranks); }
+void DevicePipeline::import_runs_from(const void* const* ptrs, const uint64_t* counts, uint32_t n_ranks) { impl->make_current(); impl->do_import_runs_from(ptrs, counts, n_ranks); }
 const void* DevicePipeline::export_entries_own(uint64_t* n) {
-    Impl& m = *impl; m.set_device(); const int W = m.W;
+    Impl& m = *impl; m.make_current(); const int W = m.W;
     uint64_t count = 0;
     AC_DISPATCH_W(count = m.do_count_entries)
     m.own_entries.ensure((count + 1) * sizeof(SlotRec));
@@ -3482,7 +2552,7 @@ const void* DevicePipeline::export_entries_own(uint64_t* n) {
     return m.own_entries.p;
 }
 const void* DevicePipeline::export_runs_own(uint64_t* n) {
-    Impl& m = *impl; m.set_device();
+    Impl& m = *impl; m.make_current();
     m.own_runs.ensure((m.n_runs + 1) * sizeof(RunRec));
     m.do_export_runs(m.own_runs.p, m.n_runs);
     *n = m.n_runs;
@@ -3506,7 +2576,7 @@ void DevicePipeline::enable_peer_access(const int* devices, int n) {
 #endif
 }
 void DevicePipeline::finish(PipelineResult& out, bool keep_positions, bool fused, bool split_paths) {
-    Impl& m = *impl; m.set_device(); const int W = m.W;
+    Impl& m = *impl; m.make_current(); const int W = m.W;
     if (split_paths && !fused) throw std::runtime_error("split path lines need the fused finish");
     AC_DISPATCH_W(m.finish_w, out, keep_positions, fused, split_paths)
 }
@@ -3518,119 +2588,19 @@ void* DevicePipeline::strand_block(uint32_t seq_lo, uint32_t seq_hi, uint64_t* n
     *n_bytes = b1 - b0;
     return m.ascii.as<uint8_t>() + b0;
 }
-void DevicePipeline::export_path_tokens(void* dst, uint64_t stride, const uint64_t* counts, uint32_t n_ranks) { impl->set_device(); impl->do_export_path_tokens(dst, stride, counts, n_ranks); }
-void DevicePipeline::render_path_lines(const void* tokens, uint64_t n_tokens, const char** text, uint64_t* bytes) { impl->set_device(); impl->do_render_path_lines(tokens, n_tokens, text, bytes); }
+void DevicePipeline::export_path_tokens(void* dst, uint64_t stride, const uint64_t* counts, uint32_t n_ranks) { impl->make_current(); impl->do_export_path_tokens(dst, stride, counts, n_ranks); }
+void DevicePipeline::render_path_lines(const void* tokens, uint64_t n_tokens, const char** text, uint64_t* bytes) { impl->make_current(); impl->do_render_path_lines(tokens, n_tokens, text, bytes); }
 void DevicePipeline::fetch_graph(PipelineResult& out, bool keep_positions) {
-    Impl& m = *impl; m.set_device();
+    Impl& m = *impl; m.make_current();
     if (m.stage < 2 || !out.fused) throw std::runtime_error("fetch_graph follows a fused build");
     if (out.graph_fetched) return;
     m.pull_graph(out, keep_positions);
 }
 
-void DevicePipeline::complete(PipelineResult& out) { impl->set_device(); impl->do_complete(out); }
+void DevicePipeline::complete(PipelineResult& out) { impl->make_current(); impl->do_complete(out); }
 
 void DevicePipeline::build(PipelineResult& out, bool keep_positions, bool fused) {   // single GPU: every sequence is local, nothing to exchange
     build_local(0, impl->n_seqs, false);
     runs_local();
     finish(out, keep_positions, fused);
-}
-
-void DevicePipeline::Impl::scan_u64(uint64_t* x, uint64_t n, int level) {
-    if (n == 0) return;
-    if (level >= 8) throw std::runtime_error("dotplot: scan too deep");
-    const uint64_t nb = (n + AC_DOT_SCAN_TILE - 1) / AC_DOT_SCAN_TILE;
-    if (nb == 1) { ac_launch("dot_scan_apply", &stream, DotScanApplyBody{x, x, n, nullptr}, 1); return; }
-    dp_scan[level].ensure(nb * 8);
-    uint64_t* sums = dp_scan[level].as<uint64_t>();
-    ac_launch("dot_scan_sum", &stream, DotScanSumBody{x, n, sums}, nb);
-    scan_u64(sums, nb, level + 1);
-    ac_launch("dot_scan_apply", &stream, DotScanApplyBody{x, x, n, sums}, nb);
-}
-
-template <int W> static void dot_windows(DevicePipeline::Impl& m, uint64_t N, uint32_t n_seqs, uint32_t k, double bpp, uint64_t mask) {
-    ac_launch("dot_windows", &m.stream, DotWindowBody<W>{m.dp_bytes.as<uint8_t>(), m.dp_seqs.as<DotplotSeq>(), n_seqs, k, bpp, m.dp_keys.as<uint64_t>(),
-                                                         m.dp_px.as<uint32_t>(), m.dp_tag.as<uint64_t>(), m.dp_rep.as<uint32_t>()}, N);
-    ac_launch("dot_insert", &m.stream, DotInsertBody<W>{m.dp_keys.as<uint64_t>(), m.dp_table.as<uint64_t>(), mask, m.dp_rep.as<uint32_t>()}, N);
-}
-
-void DevicePipeline::dotplot(const uint8_t* bytes, uint64_t n_bytes, const DotplotSeq* seqs, uint32_t n_seqs, uint32_t k, double bpp, uint32_t res,
-                             const uint64_t* host_idx, const uint64_t* host_key, uint64_t n_host, uint8_t* rgb, DotplotRun* run) {
-    Impl& m = *impl; m.set_device();
-    if (k < 1 || k > 128) throw std::runtime_error("dotplot: k must be 1..128");
-    if (n_seqs == 0 || n_seqs > AC_DOTPLOT_MAX_SEQS) throw std::runtime_error("dotplot: 1 to 32768 sequences");
-    uint64_t N = 0;
-    for (uint32_t s = 0; s < n_seqs; ++s) {
-        const uint64_t nw = seqs[s].len >= k ? seqs[s].len - k + 1 : 0;
-        if (seqs[s].window_base != N || seqs[s].off + seqs[s].len > n_bytes) throw std::runtime_error("dotplot: bad sequence layout");
-        N += nw;
-    }
-    if (N >= 0xFFFFFFFFull) throw std::runtime_error("dotplot: too many windows");
-    const int W = (int)((2 * k + 63) / 64);
-    const uint64_t P = (uint64_t)res * res;
-    DotplotRun r; r.windows = N;
-    m.dp_bytes.ensure(n_bytes + 8); m.dp_seqs.ensure((size_t)n_seqs * sizeof(DotplotSeq));
-    m.dp_pix.ensure(P * 8); m.dp_rgb.ensure(P * 3);
-    if (n_bytes) ac_h2d(m.dp_bytes.p, bytes, n_bytes, &m.stream);
-    ac_h2d(m.dp_seqs.p, seqs, (size_t)n_seqs * sizeof(DotplotSeq), &m.stream);
-    ac_h2d(m.dp_rgb.p, rgb, P * 3, &m.stream);
-    ac_memset(m.dp_pix.p, 0, P * 8, &m.stream);
-    if (n_host) {
-        m.dp_hidx.ensure(n_host * 8); m.dp_hkey.ensure(n_host * 8);
-        ac_h2d(m.dp_hidx.p, host_idx, n_host * 8, &m.stream); ac_h2d(m.dp_hkey.p, host_key, n_host * 8, &m.stream);
-    }
-#ifndef AC_EMULATE
-    cudaEvent_t e0, e1;
-    AC_CUDA_CHECK(cudaEventCreate(&e0)); AC_CUDA_CHECK(cudaEventCreate(&e1));
-    AC_CUDA_CHECK(cudaEventRecord(e0, m.stream.s));
-#endif
-    if (N) {
-        uint64_t cap = 64;
-        while (cap < 2 * N) cap <<= 1;
-        m.dp_keys.ensure(N * W * 8); m.dp_px.ensure(N * 4); m.dp_tag.ensure(N * 8); m.dp_rep.ensure(N * 4); m.dp_cnt.ensure(N * 4 + 4);
-        m.dp_off.ensure(N * 4 + 4); m.dp_fill.ensure(N * 4 + 4); m.dp_gpx.ensure(N * 4); m.dp_gtag.ensure(N * 8); m.dp_table.ensure(cap * 8);
-        ac_memset(m.dp_table.p, 0, cap * 8, &m.stream);
-        ac_memset(m.dp_cnt.p, 0, N * 4, &m.stream); ac_memset(m.dp_fill.p, 0, N * 4, &m.stream);
-        switch (W) {
-            case 1: dot_windows<1>(m, N, n_seqs, k, bpp, cap - 1); break;
-            case 2: dot_windows<2>(m, N, n_seqs, k, bpp, cap - 1); break;
-            case 3: dot_windows<3>(m, N, n_seqs, k, bpp, cap - 1); break;
-            default: dot_windows<4>(m, N, n_seqs, k, bpp, cap - 1); break;
-        }
-        uint32_t* rep = m.dp_rep.as<uint32_t>();
-        uint32_t* cnt = m.dp_cnt.as<uint32_t>();
-        uint32_t* off = m.dp_off.as<uint32_t>();
-        ac_launch("dot_count", &m.stream, DotCountBody{rep, cnt}, N);
-        m.exclusive_scan(cnt, off, N, 0, false);
-        ac_launch("dot_scatter", &m.stream, DotScatterBody{rep, off, m.dp_fill.as<uint32_t>(), m.dp_px.as<uint32_t>(), m.dp_tag.as<uint64_t>(),
-                                                           m.dp_gpx.as<uint32_t>(), m.dp_gtag.as<uint64_t>()}, N);
-        uint32_t* flag = m.dp_fill.as<uint32_t>();          // the fill counts are spent: the leading-window flags, then their ranks
-        ac_launch("dot_lead", &m.stream, DotLeadBody{rep, flag}, N);
-        const uint32_t G = m.exclusive_scan(flag, flag, N);
-        r.groups = G;
-        if (G) {
-            m.dp_gstart.ensure((size_t)G * 4); m.dp_gsize.ensure((size_t)G * 4); m.dp_gdots.ensure(((size_t)G + 1) * 8);
-            uint64_t* gdots = m.dp_gdots.as<uint64_t>();
-            ac_memset(gdots + G, 0, 8, &m.stream);
-            ac_launch("dot_group", &m.stream, DotGroupBody{rep, flag, off, cnt, m.dp_gstart.as<uint32_t>(), m.dp_gsize.as<uint32_t>(), gdots}, N);
-            m.scan_u64(gdots, (uint64_t)G + 1);
-            uint64_t D = 0;
-            ac_d2h(&D, gdots + G, 8, &m.stream); ac_sync(&m.stream);
-            r.dots = D;
-            ac_launch("dot_pairs", &m.stream, DotPairBody{gdots, m.dp_gstart.as<uint32_t>(), m.dp_gsize.as<uint32_t>(), G, m.dp_gpx.as<uint32_t>(),
-                                                          m.dp_gtag.as<uint64_t>(), D, n_seqs, res, m.dp_pix.as<uint64_t>()},
-                      (D + AC_DOT_CHUNK - 1) / AC_DOT_CHUNK);
-        }
-    }
-    if (n_host) ac_launch("dot_merge", &m.stream, DotMergeBody{m.dp_hidx.as<uint64_t>(), m.dp_hkey.as<uint64_t>(), m.dp_pix.as<uint64_t>()}, n_host);
-    ac_launch("dot_compose", &m.stream, DotComposeBody{m.dp_pix.as<uint64_t>(), m.dp_rgb.as<uint8_t>()}, P);
-#ifndef AC_EMULATE
-    AC_CUDA_CHECK(cudaEventRecord(e1, m.stream.s));
-#endif
-    ac_d2h(rgb, m.dp_rgb.p, P * 3, &m.stream);
-    ac_sync(&m.stream);
-#ifndef AC_EMULATE
-    AC_CUDA_CHECK(cudaEventElapsedTime(&r.kernel_ms, e0, e1));
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-#endif
-    if (run) *run = r;
 }

@@ -68,7 +68,7 @@ def run_trim(args):
     ms = sorted(times)[len(times) // 2] * 1e3
     kms = sorted(kernel_ms)[len(kernel_ms) // 2]
     card = gpu_identity(torch.cuda.current_device())
-    # DevicePipeline::overlap_shared_k_max: three f64 diagonals of k + 1 entries per CTA, beside 64 bytes of static shared memory
+    # overlap_shared_k_max (align.cu): three f64 diagonals of k + 1 entries per CTA, beside 64 bytes of static shared memory
     shared_k = (torch.cuda.get_device_properties(torch.cuda.current_device()).shared_memory_per_block_optin - 64) // 24 - 1
     line = {
         "impl": "b200", "command": "trim", "metric": TRIM_METRIC, "value": round(stats["dp_cells"] / (ms / 1e3), 1), "unit": "cells/s",

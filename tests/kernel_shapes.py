@@ -31,11 +31,11 @@ def device_shared_optin():
     return v.value
 
 
-def overlap_shared_k_max(optin):         # pipeline.cu overlap_shared_k_max: three f64 diagonals of k + 1 cells, 64 B of static shared
+def overlap_shared_k_max(optin):         # align.cu overlap_shared_k_max: three f64 diagonals of k + 1 cells, 64 B of static shared
     return (optin - 64) // 24 - 1
 
 
-def bridge_shared_n_max(optin):          # pipeline.cu bridge_shared_n_max: three u32 diagonals of n + 1 cells
+def bridge_shared_n_max(optin):          # align.cu bridge_shared_n_max: three u32 diagonals of n + 1 cells
     return optin // 12 - 1
 
 
