@@ -79,6 +79,15 @@ class AcDotplotInfo(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class AcSubsampleInfo(C.Structure):
+    _fields_ = [("genome_size", C.c_uint64), ("reads_per_subset", C.c_uint64), ("input_count", C.c_uint64), ("input_bases", C.c_uint64),
+                ("input_n50", C.c_uint64), ("windows", C.c_uint64), ("bytes_scanned", C.c_uint64), ("kernel_ms", C.c_float),
+                ("read_ms", C.c_double), ("shuffle_ms", C.c_double), ("write_ms", C.c_double), ("copy_ms", C.c_double)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_sequence", "ac_clear_sequences", "ac_upload",
            "ac_build", "ac_compress", "ac_simplify", "ac_merge_linear_paths", "ac_renumber_unitigs", "ac_load_gfa", "ac_bind_host_to_device", "ac_decompress_gfa", "ac_pairwise_distances", "ac_distance_matrix_text", "ac_sequence_reconstruct", "ac_counts_get", "ac_unitigs_copy", "ac_path_copy", "ac_gfa_size", "ac_gfa_copy",
            "ac_timings_get", "ac_compress_dir", "ac_compress_dir_devices", "ac_load_sequences", "ac_sequence_get",
@@ -89,7 +98,8 @@ EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_seq
            "ac_cluster", "ac_cluster_text", "ac_cluster_assignments", "ac_cluster_stats", "ac_upgma", "ac_cluster_dir",
            "ac_bridge_best_paths", "ac_resolve", "ac_resolve_text", "ac_resolve_stats", "ac_resolve_dir", "ac_combine_dir",
            "ac_dotplot_rgb", "ac_dotplot_dir", "ac_png_write",
-           "ac_clean_gfa", "ac_clean_text", "ac_gfa_to_fasta", "ac_gfa_fasta_text", "ac_table_text"]
+           "ac_clean_gfa", "ac_clean_text", "ac_gfa_to_fasta", "ac_gfa_fasta_text", "ac_table_text",
+           "ac_subsample_dir", "ac_genome_size", "ac_subsample_words", "ac_subsample_shuffle"]
 
 _libs = {}
 
@@ -194,6 +204,11 @@ def load_library(path=None):
                                   C.POINTER(C.c_double), C.c_int32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     lib.ac_gfa_to_fasta.argtypes = [C.c_char_p, C.c_char_p, C.c_int32]
     lib.ac_gfa_fasta_text.argtypes = [C.c_char_p, C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
+    lib.ac_subsample_dir.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint64, C.c_double, C.c_uint64, C.c_int32, C.c_int32,
+                                     C.POINTER(AcSubsampleInfo)]
+    lib.ac_genome_size.argtypes = [C.c_char_p, C.POINTER(C.c_uint64)]
+    lib.ac_subsample_words.argtypes = [C.c_uint64, C.c_uint32, C.POINTER(C.c_uint32), C.c_uint64]
+    lib.ac_subsample_shuffle.argtypes = [C.c_uint64, C.c_uint64, C.POINTER(C.c_uint32)]
     lib.ac_table_text.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint64, C.c_int32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     _libs[path] = lib
     return lib
@@ -692,3 +707,35 @@ def table(autocycler_dir=None, name="", fields=None, sigfigs=3, verbose=False, l
     lib = lib or load_library()
     return _host_text(lib, lib.ac_table_text, None if autocycler_dir is None else os.fsencode(autocycler_dir), name.encode(),
                       None if fields is None else fields.encode(), sigfigs, 1 if verbose else 0)
+
+
+def subsample(reads, out_dir, genome_size, count=4, min_read_depth=25.0, seed=0, device=0, verbose=False, lib=None):
+    """`autocycler subsample` (subsample.rs:29-43): sample_01.fastq .. and subsample.yaml under out_dir; returns the info dict."""
+    lib = lib or load_library()
+    info = AcSubsampleInfo()
+    _raise_unless_ok(lib, lib.ac_subsample_dir(os.fsencode(reads), os.fsencode(out_dir), str(genome_size).encode(), count, float(min_read_depth),
+                                               seed, device, 1 if verbose else 0, C.byref(info)))
+    return info.as_dict()
+
+
+def genome_size(text, lib=None):   # subsample.rs:83-101
+    lib = lib or load_library()
+    out = C.c_uint64()
+    _raise_unless_ok(lib, lib.ac_genome_size(text.encode(), C.byref(out)))
+    return out.value
+
+
+def subsample_words(seed, n, rounds=12, lib=None):
+    """The first n u32 words of StdRng::seed_from_u64(seed) (ChaCha12), or of its 20-round form."""
+    lib = lib or load_library()
+    out = (C.c_uint32 * max(1, n))()
+    _raise_unless_ok(lib, lib.ac_subsample_words(seed, rounds, out, n))
+    return list(out)[:n]
+
+
+def subsample_shuffle(n, seed, lib=None):
+    """(0..n).shuffle(&mut StdRng::seed_from_u64(seed)) as a list."""
+    lib = lib or load_library()
+    out = (C.c_uint32 * max(1, n))()
+    _raise_unless_ok(lib, lib.ac_subsample_shuffle(n, seed, out))
+    return list(out)[:n]

@@ -26,6 +26,7 @@
 #include "host_resolve.h"
 #include "host_clean.h"
 #include "host_dotplot.h"
+#include "host_subsample.h"
 #include <mutex>
 #include <immintrin.h>
 #include <functional>
@@ -1505,5 +1506,82 @@ int ac_png_write(const char* path, const uint8_t* rgb, uint32_t width, uint32_t 
     AC_GUARD_END(nullptr)
 }
 
-}  // extern "C"
+// ---- `autocycler subsample` (subsample.rs) --------------------------------------------------------------------------------------
+namespace {
+// One subsample device object per device, as for dotplot: its buffers (and pinned windows) are kept for the next call on that device.
+std::mutex g_subsample_mu;
+struct SubsampleDevice {
+    DeviceContext ctx; DeviceSubsample sub;
+    explicit SubsampleDevice(int32_t device) : ctx(device, nullptr), sub(ctx) {}
+};
+DeviceSubsample& subsample_device(int32_t device) {        // with g_subsample_mu held
+    static std::vector<std::pair<int32_t, SubsampleDevice*>> devices;
+    for (auto& d : devices) if (d.first == device) return d.second->sub;
+    devices.emplace_back(device, new SubsampleDevice(device));
+    return devices.back().second->sub;
+}
+}  // namespace
 
+int ac_subsample_dir(const char* reads, const char* out_dir, const char* genome_size, uint64_t count, double min_read_depth, uint64_t seed,
+                     int32_t device, int32_t verbose, ac_subsample_info* info) {
+    if (!reads || !out_dir || !genome_size) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    const std::string in = reads, dir = out_dir;
+    const uint64_t gsize = parse_genome_size(genome_size);                    // subsample.rs:31-33, then check_settings (:47-55)
+    int rc;
+    if ((rc = check_file(in)) != AC_OK) return rc;
+    struct stat st;
+    if (stat(dir.c_str(), &st) == 0 && !S_ISDIR(st.st_mode)) return set_error(nullptr, AC_EINPUT, dir + " exists but is not a directory");
+    if (gsize < 1) return set_error(nullptr, AC_EINPUT, "--genome_size must be at least 1");
+    if (count < 2) return set_error(nullptr, AC_EINPUT, "--count must be at least 2");
+    if (min_read_depth <= 0.0) return set_error(nullptr, AC_EINPUT, "--min_read_depth must be greater than 0");
+    if (!make_dirs(dir)) return set_error(nullptr, AC_EINPUT, "failed to create directory " + dir + "\n" + strerror(errno));
+    if (verbose) fprintf(stderr, "\nStarting autocycler subsample\n    This command subsamples a long-read set into subsets that are maximally independent "
+                                 "from each other.\n\nSettings:\n  --reads %s\n  --out_dir %s\n  --genome_size %llu\n  --count %llu\n  --min_read_depth %s\n"
+                                 "  --seed %llu\n\n", in.c_str(), dir.c_str(), (unsigned long long)gsize, (unsigned long long)count,
+                         format_float(min_read_depth).c_str(), (unsigned long long)seed);
+    SubsampleRun run;
+    try {
+        std::lock_guard<std::mutex> lock(g_subsample_mu);
+        subsample_run(subsample_device(device), in, dir, gsize, count, min_read_depth, seed, subsample_window_size(), verbose != 0, run);
+    } catch (const AcIoError& e) { return set_error(nullptr, AC_EIO, e.msg); }
+    catch (const std::length_error& e) { return set_error(nullptr, AC_ERANGE, e.what()); }
+    if (info) {
+        info->genome_size = run.genome_size; info->reads_per_subset = run.reads_per_subset;
+        info->input_count = run.input.count; info->input_bases = run.input.bases; info->input_n50 = run.input.n50;
+        info->windows = run.windows; info->bytes_scanned = run.bytes_scanned; info->kernel_ms = run.kernel_ms;
+        info->read_ms = run.read_ms; info->shuffle_ms = run.shuffle_ms; info->write_ms = run.write_ms; info->copy_ms = run.copy_ms;
+    }
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
+int ac_subsample_words(uint64_t seed, uint32_t rounds, uint32_t* out, uint64_t n) {
+    if (!out && n) return set_error(nullptr, AC_EINVAL, "null argument");
+    if (rounds != 12 && rounds != 20) return set_error(nullptr, AC_EINVAL, "rounds must be 12 or 20");
+    AC_GUARD_BEGIN
+    const std::vector<uint32_t> w = subsample_rng_words(seed, n, (int)rounds);
+    if (n) memcpy(out, w.data(), n * 4);
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
+int ac_subsample_shuffle(uint64_t n, uint64_t seed, uint32_t* order) {
+    if (!order && n) return set_error(nullptr, AC_EINVAL, "null argument");
+    if (n >= 0xFFFFFFFFull) return set_error(nullptr, AC_ERANGE, "2^32 - 1 reads or more");
+    AC_GUARD_BEGIN
+    const std::vector<uint32_t> o = subsample_shuffle(n, seed);
+    if (n) memcpy(order, o.data(), n * 4);
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
+int ac_genome_size(const char* text, uint64_t* size) {
+    if (!text || !size) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    *size = parse_genome_size(text);
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
+}  // extern "C"

@@ -1,5 +1,5 @@
 // `autocycler compress`, `autocycler decompress`, `autocycler cluster`, `autocycler trim`, `autocycler resolve`, `autocycler combine`, `autocycler dotplot`,
-// `autocycler clean`, `autocycler gfa2fasta` and `autocycler table` with the reference's flags (main.rs:126-162), messages and exit codes
+// `autocycler clean`, `autocycler gfa2fasta`, `autocycler table` and `autocycler subsample` with the reference's flags (main.rs:126-162), messages and exit codes
 // (misc.rs:130-136: "Error: <text>" on stderr, exit 1), running the H100 path through the C ABI.
 #include <cstdio>
 #include <cstdlib>
@@ -38,6 +38,17 @@ struct Args {
         const double x = integral ? (double)strtoul(v, &end, 10) : strtod(v, &end);
         const bool bad = u32 ? (*v == '-' || x > 0xFFFFFFFFul) : (integral && (*v == '-' || *v == '+'));
         if (!*v || *end || bad) { fprintf(stderr, "error: invalid value '%s' for '%s'\n%s", v, flag.c_str(), u32 ? "" : usage); exit(2); }
+        return x;
+    }
+    // The value as an exact u64 (digits only, at most 2^64 - 1): a seed must not go through a double, which rounds above 2^53.
+    uint64_t u64() {
+        const char* v = value();
+        uint64_t x = 0; bool bad = !*v;
+        for (const char* q = v; *q && !bad; ++q) {
+            if (*q < '0' || *q > '9' || x > (UINT64_MAX - (uint64_t)(*q - '0')) / 10) bad = true;
+            else x = x * 10 + (uint64_t)(*q - '0');
+        }
+        if (bad) { fprintf(stderr, "error: invalid value '%s' for '%s'\n%s", v, flag.c_str(), usage); exit(2); }
         return x;
     }
     int help() const { fprintf(stderr, "%s", usage); return 0; }
@@ -244,6 +255,25 @@ static int table_main(int argc, char** argv) {
     return finish(rc);
 }
 
+// `autocycler subsample` (main.rs:249-274, subsample.rs:29-43)
+static int subsample_main(int argc, char** argv) {
+    Args a{argc, argv, "Usage: autocycler subsample --reads <READS> --out_dir <OUT_DIR> --genome_size <GENOME_SIZE> [--count 4] [--min_read_depth 25.0] [--seed 0] [--device N]\n"};
+    std::string reads, out, gsize; bool has_gsize = false; uint64_t count = 4, seed = 0; double depth = 25.0; int device = 0;
+    while (a.next()) {
+        if (a.is("-r", "--reads")) reads = a.value();
+        else if (a.is("-o", "--out_dir")) out = a.value();
+        else if (a.is("-g", "--genome_size")) { gsize = a.value(); has_gsize = true; }
+        else if (a.is("-c", "--count")) count = a.u64();
+        else if (a.is("-d", "--min_read_depth")) depth = a.number(false);
+        else if (a.is("-s", "--seed")) seed = a.u64();
+        else if (a.is("--device")) device = atoi(a.value());
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
+    }
+    if (reads.empty() || out.empty() || !has_gsize) return a.missing();
+    return finish(ac_subsample_dir(reads.c_str(), out.c_str(), gsize.c_str(), count, depth, seed, device, 1, nullptr));
+}
+
 int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "dotplot") == 0) return dotplot_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "resolve") == 0) return resolve_main(argc, argv);
@@ -255,6 +285,7 @@ int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "clean") == 0) return clean_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "gfa2fasta") == 0) return gfa2fasta_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "table") == 0) return table_main(argc, argv);
+    if (argc >= 2 && strcmp(argv[1], "subsample") == 0) return subsample_main(argc, argv);
     fprintf(stderr, "%s", compress_usage);
     return 2;
 }

@@ -1,4 +1,4 @@
-// The device parts of `autocycler trim`, `resolve`, `cluster` and `dotplot`.  Each object owns its device buffers (allocated on first
+// The device parts of `autocycler trim`, `resolve`, `cluster`, `dotplot` and `subsample`.  Each object owns its device buffers (allocated on first
 // use, kept for the next call) and runs on the device and stream of the DeviceContext it is given, which must outlive it.
 #pragma once
 #include <cstdint>
@@ -97,4 +97,47 @@ private:
     DeviceScan scan;
     SerialScan<uint64_t, AC_DOT_SCAN_TILE, 8> scan_u64;          // of the groups' dot counts
     DevBuf d_bytes, d_seqs, d_keys, d_px, d_tag, d_rep, d_cnt, d_off, d_fill, d_gpx, d_gtag, d_table, d_gstart, d_gsize, d_gdots, d_pix, d_rgb, d_hidx, d_hkey;
+};
+
+// One FASTQ record of `autocycler subsample` in its window: where its header, sequence and quality start (the '@', the line ends and
+// a trailing '\r' left out) and their lengths; the quality has seq_len bytes.
+struct SubRecord { uint64_t head, seq, qual; uint32_t head_len, seq_len; };
+// Why a record is refused, in the order the record body checks.  A window's first refused record is kept as (record << 3) | reason.
+enum SubReason : uint32_t { SUB_NO_AT = 1, SUB_NO_PLUS = 2, SUB_TRUNCATED = 3, SUB_UNEQUAL = 4, SUB_TOO_LONG = 5 };
+#define AC_SUB_NONE64 0xFFFFFFFFFFFFFFFFull
+// What one window scan found: complete records (every record when the window ends the file), the bytes they span (the next window
+// starts there) and the first refused record (AC_SUB_NONE64: none).
+struct SubScan { uint64_t records = 0, cut = 0, bad = AC_SUB_NONE64; };
+// One subset's rows of the statistics: count, bases, and the ascending n50 (metrics.rs:44-62).
+struct SubStats { uint64_t count = 0, bases = 0, n50 = 0; };
+#define AC_SUB_SCAN_TILE 32          // values per thread of the u64 scans (histogram rows, output offsets)
+
+class DeviceSubsample {
+public:
+    explicit DeviceSubsample(DeviceContext& ctx) : ctx(ctx) {}
+    ~DeviceSubsample() { ctx.make_current(); }
+    // Pass 1 over one window of n bytes of FASTQ text (host memory; eof: the window ends the file).  Finds its complete records (at eof,
+    // every record, the last one possibly without its newline), checks them and appends their sequence lengths to the file-wide length
+    // array at `first` when keep_lengths.  The records stay on the device for gather() until the next scan.
+    SubScan scan_window(const uint8_t* bytes, uint64_t n, bool eof, uint64_t first, bool keep_lengths);
+    // The input's statistics over the first n lengths.
+    SubStats input_stats(uint64_t n);
+    // rank[order[p]] = p for the shuffled read order (n reads).
+    void set_order(const uint32_t* order, uint64_t n);
+    // Every subset's statistics at once: read r is in subset i when (rank[r] - starts[i]) mod n < rps.
+    void subset_stats(uint64_t n, const uint64_t* starts, uint32_t count, uint64_t rps, SubStats* out);
+    // Pass 2 for the window last scanned (its first record `first`): subset (start, rps)'s records, each as `@head\nseq\n+\nqual\n`, in
+    // input order, into host_out (window bytes + 1 fit).  Returns the bytes written.
+    uint64_t gather(uint64_t first, uint64_t n, uint64_t start, uint64_t rps, uint8_t* host_out);
+    // Pinned host memory for the windows and the gathered output, kept with the device buffers.
+    PinBuf h_win, h_out;
+    float kernel_ms = 0.f;           // the kernels of every call so far (CUDA events; 0 under emulation)
+    double copy_ms = 0.0;            // host wall time of the window uploads and the gathered output's copies back
+private:
+    void rows(uint64_t n, const uint64_t* starts, uint32_t count, uint64_t rps, SubStats* out);
+    DeviceContext& ctx;
+    DeviceScan scan;
+    SerialScan<uint64_t, AC_SUB_SCAN_TILE, 8> scan_u64;
+    uint64_t win_records = 0, win_bytes = 0;
+    DevBuf d_bytes, d_mask, d_cnt, d_line, d_rec, d_bad, d_len, d_len_tmp, d_rank, d_starts, d_h1, d_s1, d_h2, d_s2, d_row, d_size, d_out;
 };

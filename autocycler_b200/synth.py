@@ -152,3 +152,50 @@ def write_assemblies(assemblies, directory, width=0):
 
 def total_bases(assemblies):
     return sum(len(s) for _, recs in assemblies for _, s in recs)
+
+
+def make_reads(genome, depth=None, n_reads=None, n50=15_000, sigma=0.5, seed=1, length=None, min_length=0, max_length=None):
+    """Seeded long reads cut from a circular genome (make_genome): log-normal lengths whose length-weighted median (the usual N50) is
+    about n50, or all of one `length`; either strand; random qualities '!'..'J'.  Stops at `n_reads` reads or at depth x the genome's
+    length in bases.  Yields (name, sequence bytes, quality bytes)."""
+    rng = SplitMix64(seed)
+    glen = len(genome)
+    mu = np.log(n50) - sigma * sigma
+    target = None if depth is None else int(depth * glen)
+    made, bases = 0, 0
+    while (n_reads is None or made < n_reads) and (target is None or bases < target):
+        if length is not None:
+            L = length
+        else:
+            u1, u2 = rng.uniform(2)
+            z = np.sqrt(-2.0 * np.log(max(u1, 1e-300))) * np.cos(2.0 * np.pi * u2)
+            L = max(min_length, int(np.exp(mu + sigma * z)))
+            if max_length is not None:
+                L = min(L, max_length)
+        start = rng.below(glen)
+        idx = (np.arange(start, start + L) % glen) if start + L > glen else slice(start, start + L)
+        seq = genome[idx]
+        if rng.below(2):
+            seq = revcomp(seq)
+        qual = (rng.u64((L + 7) // 8).view(np.uint8)[:L] % np.uint8(42)) + np.uint8(33)
+        made += 1
+        bases += L
+        yield (f"read_{made} length={L}", seq.tobytes(), qual.tobytes())
+
+
+def write_reads(reads, path, gz=False, crlf=False, plus_header=False, final_newline=True):
+    """reads as FASTQ at path (gzipped when gz): CRLF line ends, '+' lines that repeat the header and a last record without its
+    newline on request."""
+    import gzip
+    eol = b"\r\n" if crlf else b"\n"
+    out = gzip.open(path, "wb", compresslevel=1) if gz else open(path, "wb")
+    with out as f:
+        pending = None
+        for name, seq, qual in reads:
+            if pending is not None:
+                f.write(pending + eol)
+            head = name.encode() if isinstance(name, str) else name
+            f.write(b"@" + head + eol + seq + eol + b"+" + (head if plus_header else b"") + eol)
+            pending = qual
+        if pending is not None:
+            f.write(pending + (eol if final_newline else b""))

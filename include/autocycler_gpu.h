@@ -25,6 +25,9 @@
  *   table (the whole subcommand)            table.rs:24-204, misc.rs:373-386 -> ac_table_text
  *   create_dotplot without the file         dotplot.rs:179-221       -> ac_dotplot_rgb
  *   dotplot (the whole subcommand)          dotplot.rs:44-52         -> ac_dotplot_dir, ac_png_write
+ *   subsample (the whole subcommand)        subsample.rs:29-43       -> ac_subsample_dir
+ *   parse_genome_size                       subsample.rs:83-101      -> ac_genome_size
+ *   StdRng::seed_from_u64 + shuffle         subsample.rs:151-153     -> ac_subsample_words, ac_subsample_shuffle
  *
  * Conventions: every function returns 0 on success and a negative AC_E* code on failure; the message
  * is available from ac_last_error(handle) (or ac_last_error(NULL) when no handle exists).  No C++
@@ -367,6 +370,37 @@ int ac_dotplot_dir(const char* input, const char* out_png, uint32_t res, uint32_
                    ac_dotplot_info* info);
 /* rgb (width * height * 3 bytes, row-major) as an 8-bit RGB PNG at path.  Host only. */
 int ac_png_write(const char* path, const uint8_t* rgb, uint32_t width, uint32_t height);
+
+/* `autocycler subsample -r reads -o out_dir -g genome_size [-c count] [-d min_read_depth] [-s seed]` (main.rs:249-274,
+ * subsample.rs:29-43).  The FASTQ file (gzipped or not; every gzip member is read) streams through windows of host and device memory;
+ * the record scan, the read statistics (count, bases, the reference's ascending n50) and the split into subsets run on the GPU, the
+ * seeded shuffle (rand 0.9's StdRng, ChaCha12) on the host.  Writes sample_01.fastq .. sample_NN.fastq and subsample.yaml as the
+ * reference does (DESIGN.md section 16).  The reference's settings checks and messages in its order (AC_EINPUT); a malformed record is
+ * AC_EINPUT "Error reading FASTQ file: record N: <reason>" before any sample file exists; 2^32 - 1 reads or more, or a read of 2^32
+ * bases or more, is AC_ERANGE.  The window is 1 GiB unless AC_SUBSAMPLE_WINDOW gives another size in bytes; it grows for a record
+ * longer than it.  When the file fits one window the second pass reuses the device copy, else the file is read again.
+ * Calls on one device run one at a time.  info may be NULL. */
+typedef struct {
+    uint64_t genome_size;              /* parse_genome_size */
+    uint64_t reads_per_subset;         /* calculate_subsets */
+    uint64_t input_count, input_bases, input_n50;
+    uint64_t windows;                  /* windows of the first pass */
+    uint64_t bytes_scanned;            /* FASTQ bytes of the first pass (after gunzip) */
+    float kernel_ms;                   /* CUDA events around each call's kernels, summed (0 under emulation); the spans include the host's
+                                          reads of a count or an offset */
+    double read_ms;                    /* host: reading and gunzipping the file, both passes */
+    double shuffle_ms;                 /* host: the seeded shuffle */
+    double write_ms;                   /* host: writing the sample files and subsample.yaml */
+    double copy_ms;                    /* host wall time of the window uploads and the sample bytes' copies back */
+} ac_subsample_info;
+int ac_subsample_dir(const char* reads, const char* out_dir, const char* genome_size, uint64_t count, double min_read_depth, uint64_t seed,
+                     int32_t device, int32_t verbose, ac_subsample_info* info);
+/* parse_genome_size (subsample.rs:83-101): AC_EINPUT "cannot interpret genome size".  Host only. */
+int ac_genome_size(const char* text, uint64_t* size);
+/* The first n u32 words of StdRng::seed_from_u64(seed) (rounds 12), or of the same generator with 20 rounds (ChaCha20).  Host only. */
+int ac_subsample_words(uint64_t seed, uint32_t rounds, uint32_t* out, uint64_t n);
+/* (0..n).shuffle(&mut StdRng::seed_from_u64(seed)) (subsample.rs:151-153): order[p] = the read at shuffled position p.  Host only. */
+int ac_subsample_shuffle(uint64_t n, uint64_t seed, uint32_t* order);
 
 #ifdef __cplusplus
 }
