@@ -11,6 +11,7 @@ Names and argument meaning follow the reference (rrwick/Autocycler v0.6.1):
     trim_path_start_end / _hairpin_start / _hairpin_end         trim.rs:288-326 (batch forms over lists of paths)
     unitig_graph.trim(min_identity, max_unitigs, mad)          trim.rs:43-51 (trim minus the file I/O)
     trim(cluster_dir, min_identity, max_unitigs, mad, ...)     trim.rs:36-53
+    trim_dirs([cluster_dir, ...]) / resolve_dirs([...])        the same for several clusters, one device call per round
     bridge_best_paths(groups, weights)                         resolve.rs:430-462 (Bridge::new for a batch of bridges)
     unitig_graph.resolve() / resolve_text() / resolve_stats()   resolve.rs:41-67 (resolve minus the file I/O)
     resolve(cluster_dir), combine(autocycler_dir, in_gfas)      resolve.rs:31-69, combine.rs:25-49
@@ -71,6 +72,14 @@ class AcResolveInfo(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class AcBatchInfo(C.Structure):
+    _fields_ = [("clusters", C.c_uint32), ("launches", C.c_uint32), ("jobs", C.c_uint64), ("cells", C.c_uint64), ("buffer_bytes", C.c_uint64),
+                ("kernel_ms", C.c_float)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 class AcDotplotInfo(C.Structure):
     _fields_ = [("windows", C.c_uint64), ("groups", C.c_uint64), ("dots", C.c_uint64), ("host_windows", C.c_uint64),
                 ("bp_per_pixel", C.c_double), ("text_height", C.c_float), ("kernel_ms", C.c_float)]
@@ -94,9 +103,9 @@ EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_seq
            "ac_build_local", "ac_entries_count", "ac_entries_export", "ac_entries_merge", "ac_runs_local", "ac_runs_export",
            "ac_runs_import", "ac_runs_import_padded", "ac_build_finish", "ac_compress_finish", "ac_gfa_data",
            "ac_compress_finish_split", "ac_path_tokens_export", "ac_path_lines_render", "ac_path_lines_data", "ac_upload_shard", "ac_strand_block",
-           "ac_trim_paths", "ac_trim", "ac_trim_yaml", "ac_trim_stats", "ac_trim_dir",
+           "ac_trim_paths", "ac_trim", "ac_trim_yaml", "ac_trim_stats", "ac_trim_dir", "ac_trim_dirs",
            "ac_cluster", "ac_cluster_text", "ac_cluster_assignments", "ac_cluster_stats", "ac_upgma", "ac_cluster_dir",
-           "ac_bridge_best_paths", "ac_resolve", "ac_resolve_text", "ac_resolve_stats", "ac_resolve_dir", "ac_combine_dir",
+           "ac_bridge_best_paths", "ac_resolve", "ac_resolve_text", "ac_resolve_stats", "ac_resolve_dir", "ac_resolve_dirs", "ac_combine_dir",
            "ac_dotplot_rgb", "ac_dotplot_dir", "ac_png_write",
            "ac_clean_gfa", "ac_clean_text", "ac_gfa_to_fasta", "ac_gfa_fasta_text", "ac_table_text",
            "ac_subsample_dir", "ac_genome_size", "ac_subsample_words", "ac_subsample_shuffle"]
@@ -180,6 +189,8 @@ def load_library(path=None):
     lib.ac_trim_yaml.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     lib.ac_trim_stats.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)]
     lib.ac_trim_dir.argtypes = [C.c_char_p, C.c_double, C.c_uint32, C.c_double, C.c_uint32, C.c_int32, C.c_int32]
+    lib.ac_trim_dirs.argtypes = [C.POINTER(C.c_char_p), C.c_uint32, C.c_double, C.c_uint32, C.c_double, C.c_uint32, C.c_int32, C.c_int32,
+                                 C.POINTER(AcBatchInfo)]
     lib.ac_cluster.argtypes = [C.c_void_p, C.c_double, C.c_int64, C.POINTER(C.c_uint16), C.c_uint64]
     lib.ac_cluster_text.argtypes = [C.c_void_p, C.c_int32, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     lib.ac_cluster_assignments.argtypes = [C.c_void_p, C.POINTER(C.c_uint16), C.POINTER(C.c_uint8), C.c_uint64]
@@ -194,6 +205,7 @@ def load_library(path=None):
     lib.ac_resolve_text.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     lib.ac_resolve_stats.argtypes = [C.c_void_p, C.POINTER(AcResolveInfo)]
     lib.ac_resolve_dir.argtypes = [C.c_char_p, C.c_int32, C.c_int32]
+    lib.ac_resolve_dirs.argtypes = [C.POINTER(C.c_char_p), C.c_uint32, C.c_int32, C.c_int32, C.POINTER(AcBatchInfo)]
     lib.ac_combine_dir.argtypes = [C.c_char_p, C.POINTER(C.c_char_p), C.c_uint32, C.c_int32]
     lib.ac_dotplot_rgb.argtypes = [C.POINTER(C.c_char_p), C.POINTER(C.c_uint64), C.POINTER(C.c_char_p), C.POINTER(C.c_char_p), C.c_uint32,
                                    C.c_uint32, C.c_uint32, C.c_char_p, C.c_int32, C.c_void_p, C.POINTER(AcDotplotInfo)]
@@ -564,6 +576,25 @@ def trim(cluster_dir, min_identity=0.75, max_unitigs=5000, mad=5.0, threads=8, d
     _raise_unless_ok(lib, lib.ac_trim_dir(os.fsencode(cluster_dir), float(min_identity), max_unitigs, float(mad), threads, device, 1 if verbose else 0))
 
 
+VERBOSE_REPORT, VERBOSE_BANNER = 1, 2
+
+
+def _dir_array(cluster_dirs):
+    names = [os.fsencode(d) for d in cluster_dirs]
+    return (C.c_char_p * max(1, len(names)))(*names), len(names)
+
+
+def trim_dirs(cluster_dirs, min_identity=0.75, max_unitigs=5000, mad=5.0, threads=8, device=0, verbose=False, lib=None):
+    """trim() for several cluster directories in one call, every round's alignments of all clusters in one device call.  verbose: True
+    for the reports, or VERBOSE_REPORT | VERBOSE_BANNER.  -> the batch info dict: clusters, launches, jobs, cells, buffer_bytes,
+    kernel_ms."""
+    lib = lib or load_library()
+    dirs, n = _dir_array(cluster_dirs)
+    info = AcBatchInfo()
+    _raise_unless_ok(lib, lib.ac_trim_dirs(dirs, n, float(min_identity), max_unitigs, float(mad), threads, device, int(verbose), C.byref(info)))
+    return info.as_dict()
+
+
 def upgma(matrix, ids, lib=None, device=0, handle=None):
     """UPGMA (cluster.rs:395-480) on the GPU: matrix is a symmetric n x n distance matrix (nested lists or an array) of the clusters `ids`
     (strictly ascending).  -> ([(node, left, right, node distance)] in merge order, kernel milliseconds)."""
@@ -615,6 +646,16 @@ def resolve(cluster_dir, verbose=False, device=0, lib=None):
     """resolve.rs:31-69: reads <cluster_dir>/2_trimmed.gfa, writes 3_bridged.gfa, 4_merged.gfa and 5_final.gfa."""
     lib = lib or load_library()
     _raise_unless_ok(lib, lib.ac_resolve_dir(os.fsencode(cluster_dir), 1 if verbose else 0, device))
+
+
+def resolve_dirs(cluster_dirs, verbose=False, device=0, lib=None):
+    """resolve() for several cluster directories in one call, all their bridges' distances in one device call.  verbose as for
+    trim_dirs.  -> the batch info dict."""
+    lib = lib or load_library()
+    dirs, n = _dir_array(cluster_dirs)
+    info = AcBatchInfo()
+    _raise_unless_ok(lib, lib.ac_resolve_dirs(dirs, n, int(verbose), device, C.byref(info)))
+    return info.as_dict()
 
 
 def combine(autocycler_dir, in_gfas, verbose=False, lib=None):

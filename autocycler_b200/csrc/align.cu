@@ -209,10 +209,11 @@ static void check_weights(const int32_t* values, uint64_t n_values, uint64_t n_w
 }
 
 float DeviceAlign::overlap_align(const int32_t* values, uint64_t n_values, const uint32_t* weights, uint64_t n_weights,
-                                 const OverlapJob* jobs, uint32_t n_jobs, std::vector<std::vector<AlignPiece>>& out) {
+                                 const OverlapJob* jobs, uint32_t n_jobs, std::vector<std::vector<AlignPiece>>& out, AlignRun* run_info) {
     ctx.make_current();
     AcStream* st = &ctx.stream;
     out.assign(n_jobs, {});
+    if (run_info) *run_info = AlignRun();
     const uint32_t shared_k = overlap_shared_k_max();
     std::vector<uint32_t> run;                       // windows of k = 0 have no cell
     for (uint32_t x = 0; x < n_jobs; ++x) {
@@ -234,6 +235,11 @@ float DeviceAlign::overlap_align(const int32_t* values, uint64_t n_values, const
     uint32_t k_shared = 0; uint64_t scratch = 0;
     const auto rows = [](const TrimLaunchJob& L) { return L.k; };
     const uint32_t n_shared = plan_jobs(lj, shared_k, rows, rows, k_shared, scratch);
+    if (run_info) {
+        run_info->shared_jobs = n_shared; run_info->hbm_jobs = (uint32_t)lj.size() - n_shared;
+        run_info->buffer_bytes = lj.size() * sizeof(TrimLaunchJob) + n_values * 4 + n_weights * 4 + bits_words * 4 + out_pieces * sizeof(AlignPiece) +
+                                 run.size() * 4 + scratch * 8;
+    }
     trim_jobs.ensure(lj.size() * sizeof(TrimLaunchJob)); trim_vals.ensure(n_values * 4 + 4); trim_w.ensure(n_weights * 4 + 4);
     trim_bits.ensure(bits_words * 4 + 4); trim_out.ensure(out_pieces * sizeof(AlignPiece) + 16); trim_len.ensure(run.size() * 4);
     trim_scratch.ensure(scratch * 8 + 8);
@@ -296,10 +302,10 @@ float DeviceAlign::overlap_align(const int32_t* values, uint64_t n_values, const
 }
 
 float DeviceAlign::bridge_distances(const int32_t* values, uint64_t n_values, const uint32_t* weights, uint64_t n_weights,
-                                    const BridgeJob* jobs, uint32_t n_jobs, uint32_t* dist, BridgeRun* run_info) {
+                                    const BridgeJob* jobs, uint32_t n_jobs, uint32_t* dist, AlignRun* run_info) {
     ctx.make_current();
     AcStream* st = &ctx.stream;
-    if (run_info) *run_info = BridgeRun();
+    if (run_info) *run_info = AlignRun();
     if (n_jobs == 0) return 0.f;
     check_weights(values, n_values, n_weights, "bridge_distances");
     const uint32_t shared_n = bridge_shared_n_max();
@@ -313,7 +319,10 @@ float DeviceAlign::bridge_distances(const int32_t* values, uint64_t n_values, co
     uint32_t n_max_shared = 0; uint64_t scratch = 0;
     const uint32_t n_shared = plan_jobs(lj, shared_n, [](const BridgeLaunchJob& L) { return L.n; },
                                         [](const BridgeLaunchJob& L) { return (uint64_t)L.n * L.m; }, n_max_shared, scratch);
-    if (run_info) { run_info->shared_jobs = n_shared; run_info->hbm_jobs = n_jobs - n_shared; }
+    if (run_info) {
+        run_info->shared_jobs = n_shared; run_info->hbm_jobs = n_jobs - n_shared;
+        run_info->buffer_bytes = lj.size() * sizeof(BridgeLaunchJob) + n_values * 4 + n_weights * 4 + scratch * 4 + (uint64_t)n_jobs * 4;
+    }
     br_jobs.ensure(lj.size() * sizeof(BridgeLaunchJob)); br_vals.ensure(n_values * 4 + 4); br_w.ensure(n_weights * 4 + 4);
     br_scratch.ensure(scratch * 4 + 4); br_dist.ensure((size_t)n_jobs * 4);
     ac_h2d(br_jobs.p, lj.data(), lj.size() * sizeof(BridgeLaunchJob), st);

@@ -188,6 +188,7 @@ int check_path(const ac_handle* h, const int32_t* paths, const uint64_t* path_of
 
 #define AC_GUARD_BEGIN try {
 #define AC_GUARD_END(h) } catch (const InputError& e) { return set_error(h, AC_EINPUT, e.msg); } \
+    catch (const RangeError& e) { return set_error(h, AC_ERANGE, e.msg); } \
     catch (const NoDevice& e) { return set_error(h, AC_ENODEVICE, e.msg); } \
     catch (const std::bad_alloc&) { return set_error(h, AC_ERANGE, "out of host memory"); } \
     catch (const std::exception& e) { std::string m = e.what(); \
@@ -1010,6 +1011,155 @@ int ac_decompress_gfa(const char* in_gfa, const char* out_dir, const char* out_f
     AC_GUARD_END(nullptr)
 }
 
+// ---- what ac_trim_dirs and ac_resolve_dirs share ----
+namespace {
+// Every directory's report, kept in memory while the clusters go through the phases together and printed to stderr in argument order
+// when the call returns, whether it succeeded or not.
+struct DirReports {
+    struct Report { char* buf = nullptr; size_t len = 0; FILE* f = nullptr; };
+    std::vector<Report> r;
+    explicit DirReports(uint32_t n) : r(n) {
+        for (Report& x : r) if (!(x.f = open_memstream(&x.buf, &x.len))) throw std::bad_alloc();
+    }
+    FILE* operator[](size_t i) const { return r[i].f; }
+    ~DirReports() {
+        for (Report& x : r) { fclose(x.f); fwrite(x.buf, 1, x.len, stderr); free(x.buf); }
+        fflush(stderr);
+    }
+};
+
+// The cluster directories of a batch: none null, and none given twice (the two runs would write the same files).  Called per directory,
+// after its existence check, so the error order is the single call's.
+struct DirSet {
+    std::set<std::string> seen;
+    int add(const std::string& dir) {
+        char* r = realpath(dir.c_str(), nullptr);
+        const std::string key = r ? r : dir;
+        free(r);
+        if (!seen.insert(key).second) return set_error(nullptr, AC_EINPUT, "cluster directory given twice: " + dir);
+        return AC_OK;
+    }
+};
+
+// load_input_gfa's codes and messages, into a graph of the caller's
+int load_graph(const std::string& text, HostGraph& g, std::vector<HostSeq>& seqs) {
+    const int rc = [&]() -> int {
+        AC_GUARD_BEGIN
+        g.load_gfa(text.data(), text.size(), seqs);
+        return AC_OK;
+        AC_GUARD_END(nullptr)
+    }();
+    return rc == AC_EINVAL ? AC_EINPUT : rc;
+}
+
+void fill_batch_info(const AlignBatch& b, ac_batch_info* info) {
+    if (!info) return;
+    info->clusters = b.clusters; info->launches = b.launches; info->jobs = b.jobs; info->cells = b.cells; info->buffer_bytes = b.buffer_bytes;
+    info->kernel_ms = b.kernel_ms;
+}
+
+// trim.rs:36-67 for n directories; ac_trim_dir is n = 1
+int trim_dirs(const char* const* cluster_dirs, uint32_t n, double min_identity, uint32_t max_unitigs, double mad, uint32_t threads, int32_t device,
+              int32_t verbose, ac_batch_info* info) {
+    if (!cluster_dirs || n == 0) return set_error(nullptr, AC_EINVAL, n == 0 ? "no cluster directory" : "null argument");
+    for (uint32_t i = 0; i < n; ++i) if (!cluster_dirs[i]) return set_error(nullptr, AC_EINVAL, "null argument");
+    if (info) *info = ac_batch_info{};
+    AC_GUARD_BEGIN
+    DirReports reports(n);
+    DirSet dirs;
+    std::vector<HostGraph> graphs(n);
+    std::vector<std::vector<HostSeq>> seqs(n);
+    Handle h;
+    for (uint32_t i = 0; i < n; ++i) {
+        FILE* log = reports[i];
+        const std::string dir = cluster_dirs[i], in_gfa = dir + "/1_untrimmed.gfa";
+        if (verbose & AC_VERBOSE_BANNER)
+            fprintf(log, "\nStarting autocycler trim (%s)\n\nSettings:\n  --cluster_dir %s\n  --min_identity %g\n  --max_unitigs %u\n  --mad %g\n  --threads %u\n\n",
+                    ac_version(), dir.c_str(), min_identity, max_unitigs, mad, threads);
+        // check_settings, trim.rs:56-67 (misc.rs:98-119)
+        int rc;
+        if ((rc = check_dir(dir)) != AC_OK || (rc = dirs.add(dir)) != AC_OK || (rc = check_file(in_gfa)) != AC_OK) return rc;
+        if (!(min_identity >= 0.0 && min_identity <= 1.0)) return set_error(nullptr, AC_EINPUT, "--min_identity must be between 0.0 and 1 (inclusive)");
+        if (threads < 1) return set_error(nullptr, AC_EINPUT, "--threads cannot be less than 1");
+        if (threads > 100) return set_error(nullptr, AC_EINPUT, "--threads cannot be greater than 100");
+        if (mad < 0.0) return set_error(nullptr, AC_EINPUT, "--mad cannot be less than 0");
+        std::string text;
+        if ((rc = read_file(in_gfa, text)) != AC_OK || (!h && (rc = make_handle(device, h)) != AC_OK) || (rc = load_graph(text, graphs[i], seqs[i])) != AC_OK) return rc;
+        if ((verbose & AC_VERBOSE_REPORT) && max_unitigs == 0) fprintf(log, "Since --max_unitigs was set to 0, trimming is disabled.\n\n");
+    }
+    std::vector<TrimCluster> clusters;
+    for (uint32_t i = 0; i < n; ++i) clusters.push_back(TrimCluster{&graphs[i], &seqs[i], (verbose & AC_VERBOSE_REPORT) ? reports[i] : nullptr, TrimStats()});
+    AlignBatch batch;
+    trim_graphs(h->align_device(), clusters, min_identity, max_unitigs, mad, batch);
+    std::vector<std::string> gfa(n), yaml(n);
+    for (uint32_t i = 0; i < n; ++i) { graphs[i].gfa_text(seqs[i], gfa[i]); yaml[i] = trimmed_metrics_yaml(seqs[i]); }
+    for (uint32_t i = 0; i < n; ++i) {
+        const std::string dir = cluster_dirs[i], out_gfa = dir + "/2_trimmed.gfa", out_yaml = dir + "/2_trimmed.yaml";
+        if (!write_file(out_gfa, gfa[i])) return set_error(nullptr, AC_EIO, "cannot write " + out_gfa);
+        if (!write_file(out_yaml, yaml[i])) return set_error(nullptr, AC_EIO, "cannot write " + out_yaml);
+        const TrimStats& ts = clusters[i].stats;
+        if (!(verbose & AC_VERBOSE_REPORT)) continue;
+        if (n == 1) fprintf(reports[i], "\nFinished!\nUnitig graph of trimmed sequences: %s\n(%llu alignments, %llu DP cells, alignment kernels %.2f ms)\n\n", out_gfa.c_str(),
+                            (unsigned long long)ts.jobs, (unsigned long long)ts.cells, (double)ts.kernel_ms);
+        else fprintf(reports[i], "\nFinished!\nUnitig graph of trimmed sequences: %s\n(%llu alignments, %llu DP cells)\n\n", out_gfa.c_str(),
+                     (unsigned long long)ts.jobs, (unsigned long long)ts.cells);
+    }
+    if (verbose && n > 1)
+        fprintf(reports[n - 1], "Trimmed %u clusters: %u kernel launches, %llu alignments, %llu DP cells, alignment kernels %.2f ms\n", batch.clusters, batch.launches,
+                (unsigned long long)batch.jobs, (unsigned long long)batch.cells, (double)batch.kernel_ms);
+    fill_batch_info(batch, info);
+    return ok(h.get());
+    AC_GUARD_END(nullptr)
+}
+
+// resolve.rs:31-75 for n directories; ac_resolve_dir is n = 1
+int resolve_dirs(const char* const* cluster_dirs, uint32_t n, int32_t verbose, int32_t device, ac_batch_info* info) {
+    if (!cluster_dirs || n == 0) return set_error(nullptr, AC_EINVAL, n == 0 ? "no cluster directory" : "null argument");
+    for (uint32_t i = 0; i < n; ++i) if (!cluster_dirs[i]) return set_error(nullptr, AC_EINVAL, "null argument");
+    if (info) *info = ac_batch_info{};
+    AC_GUARD_BEGIN
+    DirReports reports(n);
+    DirSet dirs;
+    std::vector<std::string> texts(n);
+    Handle h;
+    for (uint32_t i = 0; i < n; ++i) {
+        FILE* log = reports[i];
+        const std::string dir = cluster_dirs[i], trimmed = dir + "/2_trimmed.gfa";
+        if (verbose & AC_VERBOSE_BANNER) fprintf(log, "\nStarting autocycler resolve (%s)\n\n", ac_version());
+        // check_settings, resolve.rs:72-75 (misc.rs:98-119)
+        int rc;
+        if ((rc = check_dir(dir)) != AC_OK || (rc = dirs.add(dir)) != AC_OK || (rc = check_file(trimmed)) != AC_OK) return rc;
+        if ((rc = read_file(trimmed, texts[i])) != AC_OK || (!h && (rc = make_handle(device, h)) != AC_OK)) return rc;
+        if (verbose & AC_VERBOSE_REPORT)
+            fprintf(log, "\nStarting autocycler resolve\n    This command resolves repeats in the unitig graph.\n\nSettings:\n  --cluster_dir %s\n\n", dir.c_str());
+        HostGraph g; std::vector<HostSeq> seqs;
+        if ((rc = load_graph(texts[i], g, seqs)) != AC_OK) return rc;
+    }
+    std::vector<ResolveCluster> clusters;      // the files' own texts, as the reference re-reads them (resolve.rs:59)
+    for (uint32_t i = 0; i < n; ++i) clusters.push_back(ResolveCluster{&texts[i], (verbose & AC_VERBOSE_REPORT) ? reports[i] : nullptr, {}, {}});
+    AlignBatch batch;
+    resolve_texts(h->align_device(), clusters, batch);
+    for (uint32_t i = 0; i < n; ++i) {
+        const std::string dir = cluster_dirs[i], bridged = dir + "/3_bridged.gfa", merged = dir + "/4_merged.gfa", final_gfa = dir + "/5_final.gfa";
+        const ResolveResult& r = clusters[i].out;
+        if (!write_file(bridged, r.bridged) || !write_file(merged, r.merged) || !write_file(final_gfa, r.final_gfa))
+            return set_error(nullptr, AC_EIO, "cannot write the output files under " + dir);
+        const ResolveStats& rs = clusters[i].stats;
+        if (!(verbose & AC_VERBOSE_REPORT)) continue;
+        if (n == 1) fprintf(reports[i], "\nFinished!\nFinal consensus graph: %s\n(%llu distance jobs, %llu DP cells, distance kernels %.2f ms)\n\n", final_gfa.c_str(),
+                            (unsigned long long)rs.jobs, (unsigned long long)rs.cells, (double)rs.kernel_ms);
+        else fprintf(reports[i], "\nFinished!\nFinal consensus graph: %s\n(%llu distance jobs, %llu DP cells)\n\n", final_gfa.c_str(),
+                     (unsigned long long)rs.jobs, (unsigned long long)rs.cells);
+    }
+    if (verbose && n > 1)
+        fprintf(reports[n - 1], "Resolved %u clusters: %u kernel launches, %llu distance jobs, %llu DP cells, distance kernels %.2f ms\n", batch.clusters, batch.launches,
+                (unsigned long long)batch.jobs, (unsigned long long)batch.cells, (double)batch.kernel_ms);
+    fill_batch_info(batch, info);
+    return ok(h.get());
+    AC_GUARD_END(nullptr)
+}
+}  // namespace
+
 // trim.rs:288-326 for a batch of caller paths, one device round of overlap alignments
 int ac_trim_paths(ac_handle* h, int32_t mode, const int32_t* paths, const uint64_t* path_off, uint64_t n_paths,
                   const uint32_t* weights, uint64_t n_weights, double min_identity, uint32_t max_unitigs,
@@ -1071,27 +1221,12 @@ int ac_trim_stats(const ac_handle* h, uint64_t* jobs, uint64_t* cells, uint32_t*
 
 int ac_trim_dir(const char* cluster_dir, double min_identity, uint32_t max_unitigs, double mad, uint32_t threads, int32_t device, int32_t verbose) {
     if (!cluster_dir) return set_error(nullptr, AC_EINVAL, "null argument");
-    AC_GUARD_BEGIN
-    // check_settings, trim.rs:56-67 (misc.rs:98-119)
-    const std::string dir = cluster_dir, in_gfa = dir + "/1_untrimmed.gfa", out_gfa = dir + "/2_trimmed.gfa", out_yaml = dir + "/2_trimmed.yaml";
-    int rc;
-    if ((rc = check_dir(dir)) != AC_OK || (rc = check_file(in_gfa)) != AC_OK) return rc;
-    if (!(min_identity >= 0.0 && min_identity <= 1.0)) return set_error(nullptr, AC_EINPUT, "--min_identity must be between 0.0 and 1 (inclusive)");
-    if (threads < 1) return set_error(nullptr, AC_EINPUT, "--threads cannot be less than 1");
-    if (threads > 100) return set_error(nullptr, AC_EINPUT, "--threads cannot be greater than 100");
-    if (mad < 0.0) return set_error(nullptr, AC_EINPUT, "--mad cannot be less than 0");
-    std::string text; Handle h;
-    if ((rc = read_file(in_gfa, text)) != AC_OK || (rc = make_handle(device, h)) != AC_OK || (rc = load_input_gfa(h.get(), text)) != AC_OK) return rc;
-    if (verbose && max_unitigs == 0) fprintf(stderr, "Since --max_unitigs was set to 0, trimming is disabled.\n\n");
-    TrimStats ts;
-    trim_graph(h->graph, h->seqs, h->align_device(), min_identity, max_unitigs, mad, verbose != 0, ts);
-    h->graph.gfa_text(h->seqs, h->gfa);
-    if (!write_file(out_gfa, h->gfa)) return set_error(nullptr, AC_EIO, "cannot write " + out_gfa);
-    if (!write_file(out_yaml, trimmed_metrics_yaml(h->seqs))) return set_error(nullptr, AC_EIO, "cannot write " + out_yaml);
-    if (verbose) fprintf(stderr, "\nFinished!\nUnitig graph of trimmed sequences: %s\n(%llu alignments, %llu DP cells, alignment kernels %.2f ms)\n\n", out_gfa.c_str(),
-                         (unsigned long long)ts.jobs, (unsigned long long)ts.cells, (double)ts.kernel_ms);
-    return ok(h.get());
-    AC_GUARD_END(nullptr)
+    return trim_dirs(&cluster_dir, 1, min_identity, max_unitigs, mad, threads, device, verbose ? AC_VERBOSE_REPORT : 0, nullptr);
+}
+
+int ac_trim_dirs(const char* const* cluster_dirs, uint32_t n, double min_identity, uint32_t max_unitigs, double mad, uint32_t threads,
+                 int32_t device, int32_t verbose, ac_batch_info* info) {
+    return trim_dirs(cluster_dirs, n, min_identity, max_unitigs, mad, threads, device, verbose, info);
 }
 
 // UPGMA (cluster.rs:395-480) on a caller's symmetric matrix: the kernel that ac_cluster runs on the distances it leaves on the device
@@ -1274,24 +1409,11 @@ int ac_resolve_stats(const ac_handle* h, ac_resolve_info* out) {
 
 int ac_resolve_dir(const char* cluster_dir, int32_t verbose, int32_t device) {
     if (!cluster_dir) return set_error(nullptr, AC_EINVAL, "null argument");
-    AC_GUARD_BEGIN
-    // check_settings, resolve.rs:72-75 (misc.rs:98-119)
-    const std::string dir = cluster_dir, trimmed = dir + "/2_trimmed.gfa";
-    int rc;
-    if ((rc = check_dir(dir)) != AC_OK || (rc = check_file(trimmed)) != AC_OK) return rc;
-    std::string text; Handle h;
-    if ((rc = read_file(trimmed, text)) != AC_OK || (rc = make_handle(device, h)) != AC_OK) return rc;
-    if (verbose) fprintf(stderr, "\nStarting autocycler resolve\n    This command resolves repeats in the unitig graph.\n\nSettings:\n  --cluster_dir %s\n\n", dir.c_str());
-    if ((rc = load_input_gfa(h.get(), text)) != AC_OK) return rc;
-    ResolveResult r; ResolveStats rs;
-    resolve_text(text, h->align_device(), verbose != 0, r, rs);     // the file's own text, as the reference re-reads it (resolve.rs:59)
-    const std::string bridged = dir + "/3_bridged.gfa", merged = dir + "/4_merged.gfa", final_gfa = dir + "/5_final.gfa";
-    if (!write_file(bridged, r.bridged) || !write_file(merged, r.merged) || !write_file(final_gfa, r.final_gfa))
-        return set_error(nullptr, AC_EIO, "cannot write the output files under " + dir);
-    if (verbose) fprintf(stderr, "\nFinished!\nFinal consensus graph: %s\n(%llu distance jobs, %llu DP cells, distance kernels %.2f ms)\n\n", final_gfa.c_str(),
-                         (unsigned long long)rs.jobs, (unsigned long long)rs.cells, (double)rs.kernel_ms);
-    return ok(h.get());
-    AC_GUARD_END(nullptr)
+    return resolve_dirs(&cluster_dir, 1, verbose ? AC_VERBOSE_REPORT : 0, device, nullptr);
+}
+
+int ac_resolve_dirs(const char* const* cluster_dirs, uint32_t n, int32_t verbose, int32_t device, ac_batch_info* info) {
+    return resolve_dirs(cluster_dirs, n, verbose, device, info);
 }
 
 int ac_combine_dir(const char* autocycler_dir, const char* const* in_gfas, uint32_t n_gfas, int32_t verbose) {

@@ -51,10 +51,22 @@ struct Args {
         if (bad) { fprintf(stderr, "error: invalid value '%s' for '%s'\n%s", v, flag.c_str(), usage); exit(2); }
         return x;
     }
+    // One or more values: the flag's value and every argument after it up to the next flag
+    std::vector<std::string> values() {
+        std::vector<std::string> v{value()};
+        while (i + 1 < argc && argv[i + 1][0] != '-') v.push_back(argv[++i]);
+        return v;
+    }
     int help() const { fprintf(stderr, "%s", usage); return 0; }
     int missing() const { fprintf(stderr, "%s", usage); return 2; }
     int unexpected() const { fprintf(stderr, "error: unexpected argument '%s'\n%s", flag.c_str(), usage); return 2; }
 };
+
+static std::vector<const char*> c_strings(const std::vector<std::string>& v) {
+    std::vector<const char*> p;
+    for (const std::string& s : v) p.push_back(s.c_str());
+    return p;
+}
 
 static int finish(int rc) {
     if (rc == AC_OK) return 0;
@@ -106,12 +118,13 @@ static int decompress_main(int argc, char** argv) {
     return finish(ac_decompress_gfa(in.c_str(), out_dir.empty() ? nullptr : out_dir.c_str(), out_file.empty() ? nullptr : out_file.c_str(), device, 1));
 }
 
-// `autocycler trim` (main.rs:301-322, trim.rs:36-101)
+// `autocycler trim` (main.rs:301-322, trim.rs:36-101): -c takes one or more cluster directories, up to the next flag, trimmed together
+// (ac_trim_dirs); the library prints each directory's Starting block and report, in argument order
 static int trim_main(int argc, char** argv) {
-    Args a{argc, argv, "Usage: autocycler trim --cluster_dir <CLUSTER_DIR> [--min_identity 0.75] [--max_unitigs 5000] [--mad 5.0] [--threads 8] [--device N]\n"};
-    std::string dir; double min_identity = 0.75, mad = 5.0; unsigned long max_unitigs = 5000, threads = 8; int device = 0;
+    Args a{argc, argv, "Usage: autocycler trim --cluster_dir <CLUSTER_DIR>... [--min_identity 0.75] [--max_unitigs 5000] [--mad 5.0] [--threads 8] [--device N]\n"};
+    std::vector<std::string> dirs; double min_identity = 0.75, mad = 5.0; unsigned long max_unitigs = 5000, threads = 8; int device = 0;
     while (a.next()) {
-        if (a.is("-c", "--cluster_dir")) dir = a.value();
+        if (a.is("-c", "--cluster_dir")) dirs = a.values();
         else if (a.is("--min_identity")) min_identity = a.number(false);
         else if (a.is("--max_unitigs")) max_unitigs = (unsigned long)a.number(true);
         else if (a.is("--mad")) mad = a.number(false);
@@ -120,12 +133,12 @@ static int trim_main(int argc, char** argv) {
         else if (a.is("-h", "--help")) return a.help();
         else return a.unexpected();
     }
-    if (dir.empty()) return a.missing();
+    if (dirs.empty() || dirs[0].empty()) return a.missing();
     if (max_unitigs > 0xFFFFFFFFul) max_unitigs = 0xFFFFFFFFul;
     if (threads > 0xFFFFFFFFul) threads = 0xFFFFFFFFul;
-    fprintf(stderr, "\nStarting autocycler trim (%s)\n\nSettings:\n  --cluster_dir %s\n  --min_identity %g\n  --max_unitigs %lu\n  --mad %g\n  --threads %lu\n\n",
-            ac_version(), dir.c_str(), min_identity, max_unitigs, mad, threads);
-    return finish(ac_trim_dir(dir.c_str(), min_identity, (uint32_t)max_unitigs, mad, (uint32_t)threads, device, 1));
+    const std::vector<const char*> ptrs = c_strings(dirs);
+    return finish(ac_trim_dirs(ptrs.data(), (uint32_t)ptrs.size(), min_identity, (uint32_t)max_unitigs, mad, (uint32_t)threads, device,
+                               AC_VERBOSE_REPORT | AC_VERBOSE_BANNER, nullptr));
 }
 
 // `autocycler cluster` (main.rs:92-113, cluster.rs:30-114)
@@ -148,20 +161,20 @@ static int cluster_main(int argc, char** argv) {
     return finish(ac_cluster_dir(dir.c_str(), cutoff, min_assemblies, (uint32_t)max_contigs, has_manual ? manual.c_str() : nullptr, device, 1));
 }
 
-// `autocycler resolve` (main.rs:238-247, resolve.rs:31-111)
+// `autocycler resolve` (main.rs:238-247, resolve.rs:31-111): -c takes one or more cluster directories, as for trim (ac_resolve_dirs)
 static int resolve_main(int argc, char** argv) {
-    Args a{argc, argv, "Usage: autocycler resolve --cluster_dir <CLUSTER_DIR> [--verbose] [--device N]\n"};
-    std::string dir; bool verbose = false; int device = 0;
+    Args a{argc, argv, "Usage: autocycler resolve --cluster_dir <CLUSTER_DIR>... [--verbose] [--device N]\n"};
+    std::vector<std::string> dirs; bool verbose = false; int device = 0;
     while (a.next()) {
-        if (a.is("-c", "--cluster_dir")) dir = a.value();
+        if (a.is("-c", "--cluster_dir")) dirs = a.values();
         else if (a.is("--verbose")) verbose = true;
         else if (a.is("--device")) device = atoi(a.value());
         else if (a.is("-h", "--help")) return a.help();
         else return a.unexpected();
     }
-    if (dir.empty()) return a.missing();
-    fprintf(stderr, "\nStarting autocycler resolve (%s)\n\n", ac_version());
-    return finish(ac_resolve_dir(dir.c_str(), verbose ? 1 : 0, device));
+    if (dirs.empty() || dirs[0].empty()) return a.missing();
+    const std::vector<const char*> ptrs = c_strings(dirs);
+    return finish(ac_resolve_dirs(ptrs.data(), (uint32_t)ptrs.size(), (verbose ? AC_VERBOSE_REPORT : 0) | AC_VERBOSE_BANNER, device, nullptr));
 }
 
 // `autocycler combine` (main.rs:115-124, combine.rs:25-87): -i takes one or more GFAs, up to the next flag
@@ -170,13 +183,12 @@ static int combine_main(int argc, char** argv) {
     std::string dir; std::vector<std::string> gfas;
     while (a.next()) {
         if (a.is("-a", "--autocycler_dir")) dir = a.value();
-        else if (a.is("-i", "--in_gfas")) { gfas.push_back(a.value()); while (a.i + 1 < argc && argv[a.i + 1][0] != '-') gfas.push_back(argv[++a.i]); }
+        else if (a.is("-i", "--in_gfas")) { const std::vector<std::string> v = a.values(); gfas.insert(gfas.end(), v.begin(), v.end()); }
         else if (a.is("-h", "--help")) return a.help();
         else return a.unexpected();
     }
     if (dir.empty() || gfas.empty()) return a.missing();
-    std::vector<const char*> ptrs;
-    for (const std::string& g : gfas) ptrs.push_back(g.c_str());
+    const std::vector<const char*> ptrs = c_strings(gfas);
     fprintf(stderr, "\nStarting autocycler combine (%s)\n\n", ac_version());
     return finish(ac_combine_dir(dir.c_str(), ptrs.data(), (uint32_t)ptrs.size(), 1));
 }

@@ -16,8 +16,22 @@ struct AlignPiece { int32_t a_unitig, a_index, b_unitig, b_index; };
 // One path distance of `autocycler resolve` (global_alignment_distance, resolve.rs:387-418): the n values at a_off (rows, the shorter
 // path) against the m values at b_off, signed unitig numbers in the caller's value array.
 struct BridgeJob { uint64_t a_off, b_off; uint32_t n, m; };
-// What one bridge_distances call ran: jobs whose three diagonals sat in shared memory, jobs whose diagonals sat in HBM scratch.
-struct BridgeRun { uint32_t shared_jobs = 0, hbm_jobs = 0; };
+// What one overlap_align or bridge_distances call ran: jobs whose live diagonals sat in shared memory, jobs whose diagonals sat in HBM
+// scratch (one launch for each form that has jobs), and the device buffer bytes the call planned for its jobs, paths, weights, scratch
+// and outputs.
+struct AlignRun {
+    uint32_t shared_jobs = 0, hbm_jobs = 0;
+    uint64_t buffer_bytes = 0;
+    uint32_t launches() const { return (shared_jobs > 0) + (hbm_jobs > 0); }
+};
+
+// What a batch of trim or resolve clusters ran on the device, over all its overlap_align or bridge_distances calls: clusters, kernel
+// launches, jobs, DP cells, the largest call's planned buffer bytes and the kernels' time (CUDA events; 0 under emulation).
+struct AlignBatch {
+    uint32_t clusters = 0, launches = 0;
+    uint64_t jobs = 0, cells = 0, buffer_bytes = 0;
+    float kernel_ms = 0.f;
+};
 
 // Trim's overlap alignments and resolve's bridge distances: one CTA per job sweeps the anti-diagonals, with the three live ones in
 // shared memory or, when they do not fit, in HBM scratch.
@@ -29,11 +43,11 @@ public:
     // weights[|unitig|] = unitig length.  out[j] = the traceback's pieces in alignment order, empty when the best right-edge score is <= 0
     // or the traceback ends on the left edge; the identity test is the caller's.  Returns the kernels' time in ms (0 under emulation).
     float overlap_align(const int32_t* values, uint64_t n_values, const uint32_t* weights, uint64_t n_weights,
-                        const OverlapJob* jobs, uint32_t n_jobs, std::vector<std::vector<AlignPiece>>& out);
+                        const OverlapJob* jobs, uint32_t n_jobs, std::vector<std::vector<AlignPiece>>& out, AlignRun* run = nullptr);
     // resolve.rs:387-418 for a batch of path pairs: dist[x] = the u32 (wrapping) edit distance of job x, weights[|unitig|] = unitig
     // length.  Returns the kernels' time in ms (0 under emulation).
     float bridge_distances(const int32_t* values, uint64_t n_values, const uint32_t* weights, uint64_t n_weights,
-                           const BridgeJob* jobs, uint32_t n_jobs, uint32_t* dist, BridgeRun* run);
+                           const BridgeJob* jobs, uint32_t n_jobs, uint32_t* dist, AlignRun* run);
 private:
     DeviceContext& ctx;
     DevBuf trim_jobs, trim_vals, trim_w, trim_bits, trim_scratch, trim_out, trim_len;

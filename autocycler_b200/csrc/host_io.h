@@ -8,6 +8,7 @@
 #include "host_graph.h"
 
 struct InputError { std::string msg; };        // the reference's quit_with_error (misc.rs:130-136)
+struct RangeError { std::string msg; };        // an input beyond what the device code can index (AC_ERANGE)
 
 struct ContigDetails { std::string name, description; uint64_t length; };
 struct AssemblyDetails { std::string filename; std::vector<ContigDetails> contigs; };

@@ -18,6 +18,7 @@
 #include "host_cluster.h"
 #include "host_edit.h"
 #include "commands.h"
+#include "host_io.h"
 
 namespace {
 typedef std::vector<int32_t> Path;
@@ -34,72 +35,111 @@ inline char complement(char c) { return c == 'A' ? 'T' : c == 'C' ? 'G' : c == '
 // ------------------------------------------------------------------------------------------------
 // Bridge::new: the best path of every bridge
 // ------------------------------------------------------------------------------------------------
-void bridge_best_paths(DeviceAlign& device, const std::vector<std::vector<Path>>& groups, const std::vector<uint32_t>& weights,
-                       std::vector<std::vector<uint32_t>>& totals, std::vector<std::vector<int32_t>>& best, ResolveStats& stats) {
-    const size_t G = groups.size();
-    totals.assign(G, {}); best.assign(G, {});
-    // distinct paths per group (first appearance order) and their multiplicities
-    std::vector<std::vector<uint32_t>> which(G);          // group entry -> distinct index
-    std::vector<std::vector<const Path*>> distinct(G);
-    std::vector<std::vector<uint32_t>> mult(G);
+void bridge_best_paths(DeviceAlign& device, std::vector<BridgeSet>& sets, AlignBatch& batch) {
+    // distinct paths per group (first appearance order) and their multiplicities; every set's unitigs rebased onto its part of the
+    // concatenated weight table, sign * (|u| + base): a job only compares the paths of one set
+    struct JobRef { uint32_t s, g, p, q; };
+    struct SetWork {
+        std::vector<std::vector<uint32_t>> which;          // group entry -> distinct index
+        std::vector<std::vector<const Path*>> distinct;
+        std::vector<std::vector<uint32_t>> mult;
+    };
+    std::vector<SetWork> work(sets.size());
     std::vector<int32_t> values;
-    std::vector<std::vector<uint64_t>> offset(G);
+    std::vector<uint32_t> weights;
     std::vector<BridgeJob> jobs;
-    struct JobRef { uint32_t g, p, q; };
     std::vector<JobRef> refs;
-    for (size_t g = 0; g < G; ++g) {
-        std::map<Path, uint32_t> seen;
-        for (const Path& p : groups[g]) {
-            for (int32_t u : p) if (u == 0 || abs_u32(u) >= weights.size()) throw std::runtime_error("unitig " + std::to_string(u) + " has no weight");
-            stats.longest_path = std::max<uint64_t>(stats.longest_path, p.size());
-            auto it = seen.find(p);
-            if (it == seen.end()) {
-                it = seen.emplace(p, (uint32_t)distinct[g].size()).first;
-                distinct[g].push_back(&p); mult[g].push_back(0);
-                offset[g].push_back(values.size()); values.insert(values.end(), p.begin(), p.end());
+    for (size_t s = 0; s < sets.size(); ++s) {
+        const std::vector<std::vector<Path>>& groups = *sets[s].groups;
+        const std::vector<uint32_t>& w = *sets[s].weights;
+        ResolveStats& stats = *sets[s].stats;
+        SetWork& W = work[s];
+        const uint64_t base = weights.size();
+        weights.insert(weights.end(), w.begin(), w.end());
+        const size_t G = groups.size();
+        W.which.assign(G, {}); W.distinct.assign(G, {}); W.mult.assign(G, {});
+        std::vector<std::vector<uint64_t>> offset(G);
+        for (size_t g = 0; g < G; ++g) {
+            std::map<Path, uint32_t> seen;
+            for (const Path& p : groups[g]) {
+                for (int32_t u : p) if (u == 0 || abs_u32(u) >= w.size()) throw std::runtime_error("unitig " + std::to_string(u) + " has no weight");
+                stats.longest_path = std::max<uint64_t>(stats.longest_path, p.size());
+                auto it = seen.find(p);
+                if (it == seen.end()) {
+                    it = seen.emplace(p, (uint32_t)W.distinct[g].size()).first;
+                    W.distinct[g].push_back(&p); W.mult[g].push_back(0);
+                    offset[g].push_back(values.size());
+                    for (int32_t u : p) {
+                        const uint64_t a = abs_u32(u) + base;
+                        if (a >= 0x80000000ull) throw RangeError{"unitig " + std::to_string(a) + " of the batch's weight table does not fit 31 bits"};
+                        values.push_back(u < 0 ? -(int32_t)a : (int32_t)a);
+                    }
+                }
+                W.which[g].push_back(it->second); W.mult[g][it->second] += 1;
             }
-            which[g].push_back(it->second); mult[g][it->second] += 1;
+            const uint32_t K = (uint32_t)W.distinct[g].size();
+            for (uint32_t p = 0; p < K; ++p)
+                for (uint32_t q = p + 1; q < K; ++q) {
+                    // the shorter path on the rows (D is symmetric bit for bit, DESIGN.md §13)
+                    const bool swap = W.distinct[g][q]->size() < W.distinct[g][p]->size();
+                    const uint32_t r = swap ? q : p, c = swap ? p : q;
+                    const uint64_t n = W.distinct[g][r]->size(), m = W.distinct[g][c]->size();
+                    if (m > 0x7FFFFFFFull) throw std::runtime_error("paths longer than 2^31 unitigs are not supported");
+                    jobs.push_back(BridgeJob{offset[g][r], offset[g][c], (uint32_t)n, (uint32_t)m});
+                    refs.push_back(JobRef{(uint32_t)s, (uint32_t)g, p, q});
+                    stats.cells += n * m; stats.jobs += 1;
+                    batch.cells += n * m;
+                }
         }
-        const uint32_t K = (uint32_t)distinct[g].size();
-        for (uint32_t p = 0; p < K; ++p)
-            for (uint32_t q = p + 1; q < K; ++q) {
-                // the shorter path on the rows (D is symmetric bit for bit, DESIGN.md §13)
-                const bool swap = distinct[g][q]->size() < distinct[g][p]->size();
-                const uint32_t r = swap ? q : p, c = swap ? p : q;
-                const uint64_t n = distinct[g][r]->size(), m = distinct[g][c]->size();
-                if (m > 0x7FFFFFFFull) throw std::runtime_error("paths longer than 2^31 unitigs are not supported");
-                jobs.push_back(BridgeJob{offset[g][r], offset[g][c], (uint32_t)n, (uint32_t)m});
-                refs.push_back(JobRef{(uint32_t)g, p, q});
-                stats.cells += n * m;
-            }
     }
     std::vector<uint32_t> dist(jobs.size());
     if (jobs.size() > 0xFFFFFFFFull) throw std::runtime_error("too many distance jobs");
-    BridgeRun run;
-    stats.kernel_ms += device.bridge_distances(values.data(), values.size(), weights.data(), weights.size(), jobs.data(), (uint32_t)jobs.size(), dist.data(), &run);
-    stats.jobs += jobs.size(); stats.shared_jobs += run.shared_jobs; stats.hbm_jobs += run.hbm_jobs;
+    AlignRun run;
+    batch.kernel_ms += device.bridge_distances(values.data(), values.size(), weights.data(), weights.size(), jobs.data(), (uint32_t)jobs.size(), dist.data(), &run);
+    batch.launches += run.launches(); batch.jobs += jobs.size(); batch.buffer_bytes = std::max(batch.buffer_bytes, run.buffer_bytes);
+    if (sets.size() == 1) {               // a shared launch's split and time belong to no one set
+        ResolveStats& stats = *sets[0].stats;
+        stats.shared_jobs += run.shared_jobs; stats.hbm_jobs += run.hbm_jobs; stats.kernel_ms += batch.kernel_ms;
+    }
     // total(p) = sum over the other distinct paths q of mult(q) * D(p, q), mod 2^32 (copies of p itself add D(p, p) = 0)
-    std::vector<std::vector<uint32_t>> dtotal(G);
-    for (size_t g = 0; g < G; ++g) dtotal[g].assign(distinct[g].size(), 0u);
+    std::vector<std::vector<std::vector<uint32_t>>> dtotal(sets.size());
+    for (size_t s = 0; s < sets.size(); ++s) {
+        dtotal[s].resize(work[s].distinct.size());
+        for (size_t g = 0; g < work[s].distinct.size(); ++g) dtotal[s][g].assign(work[s].distinct[g].size(), 0u);
+    }
     for (size_t x = 0; x < refs.size(); ++x) {
         const JobRef& r = refs[x];
-        dtotal[r.g][r.p] += mult[r.g][r.q] * dist[x];
-        dtotal[r.g][r.q] += mult[r.g][r.p] * dist[x];
+        const std::vector<std::vector<uint32_t>>& mult = work[r.s].mult;
+        dtotal[r.s][r.g][r.p] += mult[r.g][r.q] * dist[x];
+        dtotal[r.s][r.g][r.q] += mult[r.g][r.p] * dist[x];
     }
     // the reference's selection loop over the original order (:440-453): a copy of a path has the same total and never replaces an
     // equal best, so the selected path is the one the all-pairs loop selects
-    for (size_t g = 0; g < G; ++g) {
-        uint32_t best_total = 0xFFFFFFFFu;
-        const Path* b = nullptr;
-        static const Path empty;
-        for (size_t x = 0; x < groups[g].size(); ++x) {
-            const uint32_t total = dtotal[g][which[g][x]];
-            totals[g].push_back(total);
-            const Path& cur = groups[g][x];
-            if (total < best_total || (total == best_total && cur < (b ? *b : empty))) { best_total = total; b = &cur; }
+    for (size_t s = 0; s < sets.size(); ++s) {
+        const std::vector<std::vector<Path>>& groups = *sets[s].groups;
+        const size_t G = groups.size();
+        sets[s].totals.assign(G, {}); sets[s].best.assign(G, {});
+        for (size_t g = 0; g < G; ++g) {
+            uint32_t best_total = 0xFFFFFFFFu;
+            const Path* b = nullptr;
+            static const Path empty;
+            for (size_t x = 0; x < groups[g].size(); ++x) {
+                const uint32_t total = dtotal[s][g][work[s].which[g][x]];
+                sets[s].totals[g].push_back(total);
+                const Path& cur = groups[g][x];
+                if (total < best_total || (total == best_total && cur < (b ? *b : empty))) { best_total = total; b = &cur; }
+            }
+            if (b) sets[s].best[g] = *b;
         }
-        if (b) best[g] = *b;
     }
+}
+
+void bridge_best_paths(DeviceAlign& device, const std::vector<std::vector<Path>>& groups, const std::vector<uint32_t>& weights,
+                       std::vector<std::vector<uint32_t>>& totals, std::vector<std::vector<int32_t>>& best, ResolveStats& stats) {
+    std::vector<BridgeSet> one{BridgeSet{&groups, &weights, &stats, {}, {}}};
+    AlignBatch batch;
+    bridge_best_paths(device, one, batch);
+    totals = std::move(one[0].totals); best = std::move(one[0].best);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -141,7 +181,7 @@ size_t determine_ambiguity(std::vector<Bridge>& bridges) {
 // keys; a flag can only clear when one of its keys' counts falls to 1 or 0.  So the conflicting set is kept ordered, and only the
 // bridges of a key whose count has just dropped below 2 are looked at again (each key at most once): the same bridges go in the same
 // order, without the quadratic recomputation.
-size_t cull_ambiguity(std::vector<Bridge>& bridges, bool verbose) {
+size_t cull_ambiguity(std::vector<Bridge>& bridges, FILE* log) {
     const size_t B = bridges.size();
     std::unordered_map<int32_t, uint32_t> sc, ec;
     std::unordered_map<int32_t, std::vector<uint32_t>> s_members, e_members;
@@ -161,13 +201,13 @@ size_t cull_ambiguity(std::vector<Bridge>& bridges, bool verbose) {
     for (uint32_t x = 0; x < B; ++x) if (bridges[x].conflicting) ambi.insert(x);
     size_t culled = 0;
     if (ambi.empty()) return 0;
-    if (verbose) fprintf(stderr, "\nCulling conflicting bridges\nCulled bridges:\n");
+    if (log) fprintf(log, "\nCulling conflicting bridges\nCulled bridges:\n");
     while (!ambi.empty()) {
         const uint32_t c = *ambi.begin();
         ambi.erase(ambi.begin());
         alive[c] = 0; ++culled;
         const Bridge& b = bridges[c];
-        if (verbose) fprintf(stderr, "  %d -> %d (%zux)\n", b.start, b.end, b.depth());
+        if (log) fprintf(log, "  %d -> %d (%zux)\n", b.start, b.end, b.depth());
         std::vector<const std::vector<uint32_t>*> recheck;
         auto drop = [&](std::unordered_map<int32_t, uint32_t>& counts, std::unordered_map<int32_t, std::vector<uint32_t>>& members, int32_t key) {
             const uint32_t before = counts[key]--;
@@ -181,7 +221,7 @@ size_t cull_ambiguity(std::vector<Bridge>& bridges, bool verbose) {
     std::vector<Bridge> kept;
     for (uint32_t x = 0; x < B; ++x) if (alive[x]) kept.push_back(std::move(bridges[x]));
     bridges.swap(kept);
-    if (verbose) fprintf(stderr, "\n%zu conflicting bridge%s culled\n\n", culled, culled == 1 ? "" : "s");
+    if (log) fprintf(log, "\n%zu conflicting bridge%s culled\n\n", culled, culled == 1 ? "" : "s");
     return culled;
 }
 
@@ -210,9 +250,9 @@ void apply_bridges(EditGraph& G, const std::vector<Bridge>& bridges, double brid
     G.prune();
 }
 
-void section(bool verbose, const char* title) { if (verbose) fprintf(stderr, "\n%s\n", title); }
-void graph_info(bool verbose, const HostGraph& g) {
-    if (verbose) fprintf(stderr, "%u unitig%s, %llu link%s\ntotal length: %llu bp\n\n", g.U, g.U == 1 ? "" : "s", (unsigned long long)g.link_count_single(),
+void section(FILE* log, const char* title) { if (log) fprintf(log, "\n%s\n", title); }
+void graph_info(FILE* log, const HostGraph& g) {
+    if (log) fprintf(log, "%u unitig%s, %llu link%s\ntotal length: %llu bp\n\n", g.U, g.U == 1 ? "" : "s", (unsigned long long)g.link_count_single(),
                          g.link_count_single() == 1 ? "" : "s", (unsigned long long)g.total_length());
 }
 }  // namespace
@@ -252,14 +292,29 @@ void HostGraph::replace_unitigs(const std::vector<uint32_t>& numbers, const std:
     check_links();
 }
 
-void resolve_text(const std::string& trimmed_gfa, DeviceAlign& device, bool verbose, ResolveResult& out, ResolveStats& stats) {
-    stats = ResolveStats();
+namespace {
+// One cluster between the phases of resolve_texts
+struct ResolveWork {
+    ResolveCluster* c;
     HostGraph g;
     std::vector<HostSeq> seqs;
-    g.load_gfa(trimmed_gfa.data(), trimmed_gfa.size(), seqs);
-    section(verbose, "Loading graph");
-    graph_info(verbose, g);
     EditGraph loaded;
+    std::vector<uint32_t> weights;                        // by unitig number: its length
+    std::vector<std::pair<int32_t, int32_t>> keys;        // per bridge: its (start, end)
+    std::vector<std::vector<Path>> groups;                // per bridge: its trimmed paths
+};
+
+// loading, anchors and the bridges' paths
+void resolve_prepare(ResolveWork& w) {
+    FILE* log = w.c->log;
+    ResolveStats& stats = w.c->stats;
+    stats = ResolveStats();
+    HostGraph& g = w.g;
+    std::vector<HostSeq>& seqs = w.seqs;
+    g.load_gfa(w.c->text->data(), w.c->text->size(), seqs);
+    section(log, "Loading graph");
+    graph_info(log, g);
+    EditGraph& loaded = w.loaded;
     loaded.from(g);
     const size_t S = seqs.size();
     std::vector<Path> seq_path(S);
@@ -282,20 +337,18 @@ void resolve_text(const std::string& trimmed_gfa, DeviceAlign& device, bool verb
         if (occ[i] == all_ids) { loaded.type[i] = 1; anchors.push_back(loaded.number[i]); is_anchor_num[loaded.number[i]] = 1; }
     }
     stats.anchors = (uint32_t)anchors.size();
-    section(verbose, "Finding anchor unitigs");
-    if (verbose) fprintf(stderr, "%zu anchor unitig%s found\n\n", anchors.size(), anchors.size() == 1 ? "" : "s");
+    section(log, "Finding anchor unitigs");
+    if (log) fprintf(log, "%zu anchor unitig%s found\n\n", anchors.size(), anchors.size() == 1 ? "" : "s");
 
     // create_bridges (:166-190): every sequence path consensus_weight times, anchor-to-anchor segments (no wrap-around) in the greater of
     // their two orientations, grouped by (first, last) in order of appearance
-    std::vector<uint32_t> weights((size_t)loaded.max_number + 1, 0);
-    for (uint32_t i = 0; i < g.U; ++i) weights[loaded.number[i]] = (uint32_t)loaded.seq[i].size();
+    w.weights.assign((size_t)loaded.max_number + 1, 0);
+    for (uint32_t i = 0; i < g.U; ++i) w.weights[loaded.number[i]] = (uint32_t)loaded.seq[i].size();
     std::map<std::pair<int32_t, int32_t>, uint32_t> group_of;
-    std::vector<std::pair<int32_t, int32_t>> keys;
-    std::vector<std::vector<Path>> groups;
     for (size_t q = 0; q < S; ++q) {
-        const uint64_t w = sequence_consensus_weight(seqs[q]);
-        if (verbose) fprintf(stderr, "%s %s (%llu bp) consensus weight = %llu\n", seqs[q].filename.c_str(), seqs[q].contig_header.substr(0, seqs[q].contig_header.find(' ')).c_str(),
-                             (unsigned long long)seqs[q].length, (unsigned long long)w);
+        const uint64_t wt = sequence_consensus_weight(seqs[q]);
+        if (log) fprintf(log, "%s %s (%llu bp) consensus weight = %llu\n", seqs[q].filename.c_str(), seqs[q].contig_header.substr(0, seqs[q].contig_header.find(' ')).c_str(),
+                         (unsigned long long)seqs[q].length, (unsigned long long)wt);
         const Path& p = seq_path[q];
         std::vector<Path> segs;
         size_t last = 0; bool have_last = false;
@@ -308,62 +361,91 @@ void resolve_text(const std::string& trimmed_gfa, DeviceAlign& device, bool verb
             }
             last = i; have_last = true;
         }
-        for (uint64_t c = 0; c < w; ++c)
+        for (uint64_t c = 0; c < wt; ++c)
             for (const Path& sgm : segs) {
                 const std::pair<int32_t, int32_t> key(sgm.front(), sgm.back());
                 auto it = group_of.find(key);
-                if (it == group_of.end()) { it = group_of.emplace(key, (uint32_t)groups.size()).first; groups.emplace_back(); keys.push_back(key); }
-                groups[it->second].emplace_back(sgm.begin() + 1, sgm.end() - 1);     // Bridge::new drops the start and the end (:432-437)
+                if (it == group_of.end()) { it = group_of.emplace(key, (uint32_t)w.groups.size()).first; w.groups.emplace_back(); w.keys.push_back(key); }
+                w.groups[it->second].emplace_back(sgm.begin() + 1, sgm.end() - 1);     // Bridge::new drops the start and the end (:432-437)
             }
     }
-    std::vector<std::vector<uint32_t>> totals;
-    std::vector<Path> best;
-    bridge_best_paths(device, groups, weights, totals, best, stats);
-    std::vector<Bridge> bridges(groups.size());
-    for (size_t x = 0; x < groups.size(); ++x) {
-        bridges[x].start = keys[x].first; bridges[x].end = keys[x].second;
-        bridges[x].all_paths = std::move(groups[x]); bridges[x].best_path = std::move(best[x]);
+}
+
+// the bridges with their best paths, ambiguity, both passes and the three texts.  shared: the distances ran in a launch with other
+// clusters, so the report leaves the kernel time out.
+void resolve_finish(ResolveWork& w, std::vector<Path>& best, bool shared) {
+    FILE* log = w.c->log;
+    ResolveStats& stats = w.c->stats;
+    ResolveResult& out = w.c->out;
+    const EditGraph& loaded = w.loaded;
+    std::vector<Bridge> bridges(w.groups.size());
+    for (size_t x = 0; x < w.groups.size(); ++x) {
+        bridges[x].start = w.keys[x].first; bridges[x].end = w.keys[x].second;
+        bridges[x].all_paths = std::move(w.groups[x]); bridges[x].best_path = std::move(best[x]);
     }
     std::sort(bridges.begin(), bridges.end(), bridge_less);
-    const double bridge_depth = (double)S;           // sequences.len(), not the weighted count
+    const double bridge_depth = (double)w.seqs.size();   // sequences.len(), not the weighted count
     stats.conflicting_bridges = (uint32_t)determine_ambiguity(bridges);
     stats.unique_bridges = (uint32_t)(bridges.size() - stats.conflicting_bridges);
-    section(verbose, "Building bridges");
-    if (verbose) fprintf(stderr, "     Unique bridges: %u\nConflicting bridges: %u\n(%llu distance jobs, %llu DP cells, distance kernels %.2f ms)\n\n", stats.unique_bridges,
-                         stats.conflicting_bridges, (unsigned long long)stats.jobs, (unsigned long long)stats.cells, (double)stats.kernel_ms);
+    section(log, "Building bridges");
+    if (log && shared) fprintf(log, "     Unique bridges: %u\nConflicting bridges: %u\n(%llu distance jobs, %llu DP cells)\n\n", stats.unique_bridges,
+                               stats.conflicting_bridges, (unsigned long long)stats.jobs, (unsigned long long)stats.cells);
+    else if (log) fprintf(log, "     Unique bridges: %u\nConflicting bridges: %u\n(%llu distance jobs, %llu DP cells, distance kernels %.2f ms)\n\n", stats.unique_bridges,
+                          stats.conflicting_bridges, (unsigned long long)stats.jobs, (unsigned long long)stats.cells, (double)stats.kernel_ms);
 
     // first pass: the unique bridges, 3_bridged.gfa, merge, 4_merged.gfa
-    section(verbose, "Applying unique bridges");
+    section(log, "Applying unique bridges");
     const std::vector<HostSeq> none;
     EditGraph G = loaded;
     apply_bridges(G, bridges, bridge_depth);
     HostGraph h;
-    h.k = g.k;
+    h.k = w.g.k;
     G.to(h);
     h.gfa_text(none, out.bridged);
     h.merge_linear_paths(false);
-    graph_info(verbose, h);
+    graph_info(log, h);
     h.renumber();
     h.gfa_text(none, out.merged);
 
     // culling, and the second pass on the graph as loaded (the same anchors marked) when anything was culled
-    const size_t culled = cull_ambiguity(bridges, verbose);
+    const size_t culled = cull_ambiguity(bridges, log);
     stats.culled_bridges = (uint32_t)culled;
     if (culled > 0) {
-        section(verbose, "Applying final bridges");
+        section(log, "Applying final bridges");
         EditGraph G2 = loaded;
         apply_bridges(G2, bridges, bridge_depth);
         HostGraph h2;
-        h2.k = g.k;
+        h2.k = w.g.k;
         G2.to(h2);
         h2.merge_linear_paths(false);
-        graph_info(verbose, h2);
+        graph_info(log, h2);
         h2.renumber();
         h2.gfa_text(none, out.final_gfa, true);
     } else {
-        if (verbose && !bridges.empty()) fprintf(stderr, "All bridges were unique, no culling necessary.\n\n");
+        if (log && !bridges.empty()) fprintf(log, "All bridges were unique, no culling necessary.\n\n");
         h.gfa_text(none, out.final_gfa, true);
     }
+}
+}  // namespace
+
+void resolve_texts(DeviceAlign& device, std::vector<ResolveCluster>& clusters, AlignBatch& batch) {
+    std::vector<ResolveWork> work(clusters.size());
+    std::vector<BridgeSet> sets;
+    for (size_t c = 0; c < clusters.size(); ++c) {
+        work[c].c = &clusters[c];
+        resolve_prepare(work[c]);
+        sets.push_back(BridgeSet{&work[c].groups, &work[c].weights, &clusters[c].stats, {}, {}});
+    }
+    batch.clusters += (uint32_t)clusters.size();
+    bridge_best_paths(device, sets, batch);
+    for (size_t c = 0; c < clusters.size(); ++c) resolve_finish(work[c], sets[c].best, clusters.size() > 1);
+}
+
+void resolve_text(const std::string& trimmed_gfa, DeviceAlign& device, bool verbose, ResolveResult& out, ResolveStats& stats) {
+    std::vector<ResolveCluster> one{ResolveCluster{&trimmed_gfa, verbose ? stderr : nullptr, {}, {}}};
+    AlignBatch batch;
+    resolve_texts(device, one, batch);
+    out = std::move(one[0].out); stats = one[0].stats;
 }
 
 // ------------------------------------------------------------------------------------------------

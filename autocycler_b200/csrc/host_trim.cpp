@@ -10,6 +10,7 @@
 #include <stdexcept>
 
 #include "commands.h"
+#include "host_io.h"
 
 namespace {
 const int32_t GAP = 0;                 // trim.rs:32
@@ -29,43 +30,76 @@ uint32_t weight_of(const std::vector<uint32_t>& w, int32_t u) {
 
 struct Pair { const std::vector<int32_t>* a; const std::vector<int32_t>* b; bool skip; };
 
-// overlap_alignment (:366-479) for a batch: the device's traceback, then the identity test
-std::vector<Alignment> overlap_alignments(DeviceAlign& device, const std::vector<Pair>& pairs, const std::vector<uint32_t>& weights,
-                                          double min_identity, uint32_t max_unitigs, TrimStats& stats) {
+// One cluster's part of a device round: its pairs, its weight table (by its own unitig numbers) and, after the round, its alignments
+struct PairSet {
+    std::vector<Pair> pairs;
+    const std::vector<uint32_t>* weights;
+    TrimStats* stats;
+    std::vector<Alignment> out;
+};
+
+// sign * (|u| + base): a cluster's unitig number in the batch's concatenated weight table
+int32_t rebase(int32_t u, uint64_t base) {
+    const uint64_t a = (u < 0 ? (uint64_t)(-(int64_t)u) : (uint64_t)u) + base;
+    if (a >= 0x80000000ull) throw RangeError{"unitig " + std::to_string(a) + " of the batch's weight table does not fit 31 bits"};
+    return u < 0 ? -(int32_t)a : (int32_t)a;
+}
+int32_t unbase(int32_t v, uint64_t base) { return v == GAP ? GAP : v < 0 ? v + (int32_t)base : v - (int32_t)base; }
+
+// overlap_alignment (:366-479) for every pair of every set in one device round: the device's traceback, then the identity test.  The
+// sets' weight tables are concatenated and each set's unitigs rebased onto its part of it; path equality only compares unitigs of one
+// set, so the rebased alignments are the sets' own.
+void overlap_alignments(DeviceAlign& device, const std::vector<PairSet*>& sets, double min_identity, uint32_t max_unitigs, AlignBatch& batch) {
     std::vector<int32_t> values;
-    std::vector<OverlapJob> jobs(pairs.size());
-    for (size_t x = 0; x < pairs.size(); ++x) {
-        const Pair& p = pairs[x];
-        if (p.a->size() != p.b->size()) throw std::runtime_error("overlap_alignment: paths of different lengths");   // :379
-        const uint64_t n = p.a->size();
-        if (n > 0x7FFFFFFFull) throw std::runtime_error("paths longer than 2^31 unitigs are not supported");
-        OverlapJob& J = jobs[x];
-        J.n = (uint32_t)n; J.k = (uint32_t)std::min<uint64_t>(max_unitigs, n); J.skip_diagonal = p.skip ? 1 : 0; J.pad = 0;
-        J.a_off = values.size(); values.insert(values.end(), p.a->begin(), p.a->end());
-        if (p.b == p.a) J.b_off = J.a_off;
-        else { J.b_off = values.size(); values.insert(values.end(), p.b->begin(), p.b->end()); }
-        stats.cells += (uint64_t)J.k * J.k; stats.max_window = std::max(stats.max_window, J.k); stats.max_path = std::max<uint64_t>(stats.max_path, n);
-    }
-    for (int32_t v : values) weight_of(weights, v);
-    std::vector<std::vector<AlignPiece>> raw;
-    stats.kernel_ms += device.overlap_align(values.data(), values.size(), weights.data(), weights.size(), jobs.data(), (uint32_t)jobs.size(), raw);
-    stats.rounds += 1; stats.jobs += jobs.size();
-    std::vector<Alignment> out(pairs.size());
-    for (size_t x = 0; x < pairs.size(); ++x) {
-        const std::vector<AlignPiece>& al = raw[x];
-        if (al.empty()) continue;
-        uint32_t a_len = 0, b_len = 0, matches = 0;                       // u32 sums (:468-471)
-        for (const AlignPiece& p : al) {
-            if (p.a_unitig != GAP) a_len += weight_of(weights, p.a_unitig);
-            if (p.b_unitig != GAP) b_len += weight_of(weights, p.b_unitig);
-            if (p.a_unitig == p.b_unitig) matches += weight_of(weights, p.a_unitig);
+    std::vector<uint32_t> weights;
+    std::vector<OverlapJob> jobs;
+    std::vector<uint64_t> base(sets.size());
+    for (size_t s = 0; s < sets.size(); ++s) {
+        const PairSet& S = *sets[s];
+        base[s] = weights.size();
+        weights.insert(weights.end(), S.weights->begin(), S.weights->end());
+        const size_t first = values.size();
+        for (const Pair& p : S.pairs) {
+            if (p.a->size() != p.b->size()) throw std::runtime_error("overlap_alignment: paths of different lengths");   // :379
+            const uint64_t n = p.a->size();
+            if (n > 0x7FFFFFFFull) throw std::runtime_error("paths longer than 2^31 unitigs are not supported");
+            OverlapJob J;
+            J.n = (uint32_t)n; J.k = (uint32_t)std::min<uint64_t>(max_unitigs, n); J.skip_diagonal = p.skip ? 1 : 0; J.pad = 0;
+            J.a_off = values.size(); values.insert(values.end(), p.a->begin(), p.a->end());
+            if (p.b == p.a) J.b_off = J.a_off;
+            else { J.b_off = values.size(); values.insert(values.end(), p.b->begin(), p.b->end()); }
+            jobs.push_back(J);
+            S.stats->cells += (uint64_t)J.k * J.k; S.stats->max_window = std::max(S.stats->max_window, J.k); S.stats->max_path = std::max<uint64_t>(S.stats->max_path, n);
+            batch.cells += (uint64_t)J.k * J.k;
         }
-        const double mean_length = ((double)a_len + (double)b_len) / 2.0;
-        const double identity = (double)matches / mean_length;
-        if (identity < min_identity) continue;
-        out[x].assign(al.begin(), al.end());
+        for (size_t v = first; v < values.size(); ++v) { weight_of(*S.weights, values[v]); values[v] = rebase(values[v], base[s]); }
+        S.stats->rounds += 1; S.stats->jobs += S.pairs.size();
     }
-    return out;
+    std::vector<std::vector<AlignPiece>> raw;
+    AlignRun run;
+    batch.kernel_ms += device.overlap_align(values.data(), values.size(), weights.data(), weights.size(), jobs.data(), (uint32_t)jobs.size(), raw, &run);
+    batch.launches += run.launches(); batch.jobs += jobs.size(); batch.buffer_bytes = std::max(batch.buffer_bytes, run.buffer_bytes);
+    size_t x = 0;
+    for (size_t s = 0; s < sets.size(); ++s) {
+        PairSet& S = *sets[s];
+        const std::vector<uint32_t>& w = *S.weights;
+        S.out.assign(S.pairs.size(), {});
+        for (size_t q = 0; q < S.pairs.size(); ++q, ++x) {
+            std::vector<AlignPiece>& al = raw[x];
+            if (al.empty()) continue;
+            for (AlignPiece& p : al) { p.a_unitig = unbase(p.a_unitig, base[s]); p.b_unitig = unbase(p.b_unitig, base[s]); }
+            uint32_t a_len = 0, b_len = 0, matches = 0;                       // u32 sums (:468-471)
+            for (const AlignPiece& p : al) {
+                if (p.a_unitig != GAP) a_len += weight_of(w, p.a_unitig);
+                if (p.b_unitig != GAP) b_len += weight_of(w, p.b_unitig);
+                if (p.a_unitig == p.b_unitig) matches += weight_of(w, p.a_unitig);
+            }
+            const double mean_length = ((double)a_len + (double)b_len) / 2.0;
+            const double identity = (double)matches / mean_length;
+            if (identity < min_identity) continue;
+            S.out[q].assign(al.begin(), al.end());
+        }
+    }
 }
 
 size_t find_midpoint(const Alignment& al, const std::vector<uint32_t>& w) {     // :482-507
@@ -157,7 +191,11 @@ void trim_paths(DeviceAlign& device, TrimMode mode, const std::vector<std::vecto
             pairs[x] = mode == TRIM_HAIRPIN_END ? Pair{&rev[x], &paths[x], false} : Pair{&paths[x], &rev[x], false};
         }
     }
-    const std::vector<Alignment> al = overlap_alignments(device, pairs, weights, min_identity, max_unitigs, stats);
+    PairSet set{std::move(pairs), &weights, &stats, {}};
+    AlignBatch batch;
+    overlap_alignments(device, {&set}, min_identity, max_unitigs, batch);
+    stats.kernel_ms += batch.kernel_ms;
+    const std::vector<Alignment>& al = set.out;
     for (size_t x = 0; x < N; ++x) {
         if (mode == TRIM_START_END) trimmed[x] = finish_start_end(paths[x], al[x], weights, out[x]);
         else if (mode == TRIM_HAIRPIN_END) trimmed[x] = finish_hairpin_end(paths[x], al[x], out[x]);
@@ -240,74 +278,99 @@ namespace {
 std::string seq_display(const HostSeq& s) {     // sequence.rs:112-135 without the bracketed extras
     return s.filename + " " + s.contig_header.substr(0, s.contig_header.find(' ')) + " (" + std::to_string(s.length) + " bp)";
 }
-void section(bool verbose, const char* title) { if (verbose) fprintf(stderr, "\n%s\n", title); }
+void section(FILE* log, const char* title) { if (log) fprintf(log, "\n%s\n", title); }
 }  // namespace
 
-void trim_graph(HostGraph& g, std::vector<HostSeq>& seqs, DeviceAlign& device, double min_identity, uint32_t max_unitigs, double mad,
-                bool verbose, TrimStats& stats) {
-    const size_t S = seqs.size();
-    if (g.n_seqs != S) throw std::runtime_error("trim: the graph's paths do not match its sequences");
-    // unitig lengths before any edit (:44), by unitig number
+namespace {
+// One cluster between the phases of trim_graphs
+struct TrimWork {
+    TrimCluster* c;
+    size_t S = 0;
     uint32_t max_number = 0;
-    for (uint32_t u = 0; u < g.U; ++u) max_number = std::max(max_number, g.number[u]);
-    std::vector<uint32_t> weights((size_t)max_number + 1, 0);
-    std::vector<uint32_t> index_of((size_t)max_number + 1, 0xFFFFFFFFu);
-    for (uint32_t u = 0; u < g.U; ++u) { weights[g.number[u]] = g.rec[u].len; index_of[g.number[u]] = u; }
-    std::vector<std::vector<int32_t>> paths(S);
+    std::vector<uint32_t> weights, index_of;                   // by unitig number: length before any edit (:44), index in the graph
+    std::vector<std::vector<int32_t>> paths, rev, path2, rev2, se_path, hp_path;
+    std::vector<uint8_t> se_ok, hp_ok, start_ok;
+    PairSet set;
+    uint32_t path_length(const std::vector<int32_t>& p) const { uint32_t t = 0; for (int32_t u : p) t += weight_of(weights, u); return t; }
+};
+
+// the weights and the paths by unitig number, and round 1: start-end and hairpin start (trim_start_end_overlap, :113-136, and
+// trim_harpin_overlap, :139-186)
+void trim_prepare(TrimWork& w, uint32_t max_unitigs) {
+    HostGraph& g = *w.c->g;
+    const size_t S = w.S = w.c->seqs->size();
+    if (g.n_seqs != S) throw std::runtime_error("trim: the graph's paths do not match its sequences");
+    for (uint32_t u = 0; u < g.U; ++u) w.max_number = std::max(w.max_number, g.number[u]);
+    w.weights.assign((size_t)w.max_number + 1, 0);
+    w.index_of.assign((size_t)w.max_number + 1, 0xFFFFFFFFu);
+    for (uint32_t u = 0; u < g.U; ++u) { w.weights[g.number[u]] = g.rec[u].len; w.index_of[g.number[u]] = u; }
+    w.paths.assign(S, {});
     for (size_t q = 0; q < S; ++q)
-        for (uint64_t x = g.path_off[q]; x < g.path_off[q + 1]; ++x) { const int32_t num = (int32_t)g.number[us_index(g.path[x])]; paths[q].push_back(us_reverse(g.path[x]) ? -num : num); }
-    auto path_length = [&](const std::vector<int32_t>& p) { uint32_t t = 0; for (int32_t u : p) t += weight_of(weights, u); return t; };
+        for (uint64_t x = g.path_off[q]; x < g.path_off[q + 1]; ++x) { const int32_t num = (int32_t)g.number[us_index(g.path[x])]; w.paths[q].push_back(us_reverse(g.path[x]) ? -num : num); }
+    w.se_ok.assign(S, 0); w.hp_ok.assign(S, 0); w.se_path.assign(S, {}); w.hp_path.assign(S, {});
+    w.set.weights = &w.weights; w.set.stats = &w.c->stats;
+    if (max_unitigs == 0) return;
+    w.rev.assign(S, {});
+    for (size_t q = 0; q < S; ++q) w.rev[q] = reverse_path(w.paths[q]);
+    for (size_t q = 0; q < S; ++q) { w.set.pairs.push_back(Pair{&w.paths[q], &w.paths[q], true}); w.set.pairs.push_back(Pair{&w.paths[q], &w.rev[q], false}); }
+}
 
-    // trim_start_end_overlap (:113-136) and trim_harpin_overlap (:139-186): start-end and hairpin start in one device round, hairpin
-    // end on the hairpin-start results in a second
-    std::vector<uint8_t> se_ok(S, 0), hp_ok(S, 0);
-    std::vector<std::vector<int32_t>> se_path(S), hp_path(S);
-    if (max_unitigs > 0) {
-        std::vector<Pair> pairs;
-        std::vector<std::vector<int32_t>> rev(S);
-        for (size_t q = 0; q < S; ++q) rev[q] = reverse_path(paths[q]);
-        for (size_t q = 0; q < S; ++q) { pairs.push_back(Pair{&paths[q], &paths[q], true}); pairs.push_back(Pair{&paths[q], &rev[q], false}); }
-        const std::vector<Alignment> r1 = overlap_alignments(device, pairs, weights, min_identity, max_unitigs, stats);
-        std::vector<uint8_t> start_ok(S, 0);
-        std::vector<std::vector<int32_t>> path2(S);
-        for (size_t q = 0; q < S; ++q) {
-            se_ok[q] = finish_start_end(paths[q], r1[2 * q], weights, se_path[q]);
-            std::vector<int32_t> t;
-            start_ok[q] = finish_hairpin_end(rev[q], r1[2 * q + 1], t);
-            path2[q] = start_ok[q] ? reverse_path(t) : paths[q];
-        }
-        std::vector<std::vector<int32_t>> rev2(S);
-        pairs.clear();
-        for (size_t q = 0; q < S; ++q) { rev2[q] = reverse_path(path2[q]); pairs.push_back(Pair{&rev2[q], &path2[q], false}); }
-        const std::vector<Alignment> r2 = overlap_alignments(device, pairs, weights, min_identity, max_unitigs, stats);
-        for (size_t q = 0; q < S; ++q) {
-            std::vector<int32_t> t;
-            const bool end_ok = finish_hairpin_end(path2[q], r2[q], t);
-            hp_ok[q] = start_ok[q] || end_ok;
-            if (hp_ok[q]) hp_path[q] = end_ok ? t : path2[q];
-        }
-        if (verbose) {
-            section(verbose, "Trim start-end overlaps");
-            for (size_t q = 0; q < S; ++q)
-                if (se_ok[q]) fprintf(stderr, "%s: trimmed to %u bp\n", seq_display(seqs[q]).c_str(), path_length(se_path[q]));
-                else fprintf(stderr, "%s: not trimmed\n", seq_display(seqs[q]).c_str());
-            section(verbose, "Trim hairpin overlaps");
-            for (size_t q = 0; q < S; ++q)
-                if (hp_ok[q]) fprintf(stderr, "%s: trimmed to %u bp\n", seq_display(seqs[q]).c_str(), path_length(hp_path[q]));
-                else fprintf(stderr, "%s: not trimmed\n", seq_display(seqs[q]).c_str());
-        }
+// round 1's results, and round 2: hairpin end on the hairpin-start results
+void trim_round2(TrimWork& w) {
+    const size_t S = w.S;
+    const std::vector<Alignment> r1 = std::move(w.set.out);
+    w.start_ok.assign(S, 0); w.path2.assign(S, {});
+    for (size_t q = 0; q < S; ++q) {
+        w.se_ok[q] = finish_start_end(w.paths[q], r1[2 * q], w.weights, w.se_path[q]);
+        std::vector<int32_t> t;
+        w.start_ok[q] = finish_hairpin_end(w.rev[q], r1[2 * q + 1], t);
+        w.path2[q] = w.start_ok[q] ? reverse_path(t) : w.paths[q];
     }
+    w.rev2.assign(S, {});
+    w.set.pairs.clear();
+    for (size_t q = 0; q < S; ++q) { w.rev2[q] = reverse_path(w.path2[q]); w.set.pairs.push_back(Pair{&w.rev2[q], &w.path2[q], false}); }
+}
 
+// round 2's results and their report
+void trim_apply_round2(TrimWork& w) {
+    const size_t S = w.S;
+    FILE* log = w.c->log;
+    const std::vector<HostSeq>& seqs = *w.c->seqs;
+    for (size_t q = 0; q < S; ++q) {
+        std::vector<int32_t> t;
+        const bool end_ok = finish_hairpin_end(w.path2[q], w.set.out[q], t);
+        w.hp_ok[q] = w.start_ok[q] || end_ok;
+        if (w.hp_ok[q]) w.hp_path[q] = end_ok ? t : w.path2[q];
+    }
+    if (log) {
+        section(log, "Trim start-end overlaps");
+        for (size_t q = 0; q < S; ++q)
+            if (w.se_ok[q]) fprintf(log, "%s: trimmed to %u bp\n", seq_display(seqs[q]).c_str(), w.path_length(w.se_path[q]));
+            else fprintf(log, "%s: not trimmed\n", seq_display(seqs[q]).c_str());
+        section(log, "Trim hairpin overlaps");
+        for (size_t q = 0; q < S; ++q)
+            if (w.hp_ok[q]) fprintf(log, "%s: trimmed to %u bp\n", seq_display(seqs[q]).c_str(), w.path_length(w.hp_path[q]));
+            else fprintf(log, "%s: not trimmed\n", seq_display(seqs[q]).c_str());
+    }
+}
+
+// choose_trim_type, the length outliers and the clean-up
+void trim_finish(TrimWork& w, double mad) {
+    const size_t S = w.S;
+    FILE* log = w.c->log;
+    HostGraph& g = *w.c->g;
+    std::vector<HostSeq>& seqs = *w.c->seqs;
+    std::vector<std::vector<int32_t>>& paths = w.paths;
     // choose_trim_type (:189-226): on a tie, start-end
-    const size_t se_count = std::count(se_ok.begin(), se_ok.end(), 1), hp_count = std::count(hp_ok.begin(), hp_ok.end(), 1);
+    const size_t se_count = std::count(w.se_ok.begin(), w.se_ok.end(), 1), hp_count = std::count(w.hp_ok.begin(), w.hp_ok.end(), 1);
     if (se_count > 0 || hp_count > 0) {
         const bool use_se = se_count >= hp_count;
-        if (verbose && use_se && hp_count > 0) fprintf(stderr, "\nStart-end trimming was more successful than hairpin trimming. Discarding hairpin trimming.\n");
-        if (verbose && !use_se && se_count > 0) fprintf(stderr, "\nHairpin trimming was more successful than start-end trimming. Discarding start-end trimming.\n");
+        if (log && use_se && hp_count > 0) fprintf(log, "\nStart-end trimming was more successful than hairpin trimming. Discarding hairpin trimming.\n");
+        if (log && !use_se && se_count > 0) fprintf(log, "\nHairpin trimming was more successful than start-end trimming. Discarding start-end trimming.\n");
         for (size_t q = 0; q < S; ++q) {
-            if (!(use_se ? se_ok[q] : hp_ok[q])) continue;
-            paths[q] = use_se ? se_path[q] : hp_path[q];
-            seqs[q].length = path_length(paths[q]);
+            if (!(use_se ? w.se_ok[q] : w.hp_ok[q])) continue;
+            paths[q] = use_se ? w.se_path[q] : w.hp_path[q];
+            seqs[q].length = w.path_length(paths[q]);
         }
     }
 
@@ -318,12 +381,12 @@ void trim_graph(HostGraph& g, std::vector<HostSeq>& seqs, DeviceAlign& device, d
         for (size_t q = 0; q < S; ++q) lengths[q] = (int64_t)seqs[q].length;
         const int64_t median = median_i64(lengths), dev = mad_i64(lengths);
         const uint64_t lo = round_to_usize((double)median - ((double)dev * mad)), hi = round_to_usize((double)median + ((double)dev * mad));
-        section(verbose, "Exclude outliers");
-        if (verbose) fprintf(stderr, "Median sequence length:    %lld bp\nMedian absolute deviation: %lld bp\nAllowed length range:      %llu-%llu bp\n\n",
-                             (long long)median, (long long)dev, (unsigned long long)lo, (unsigned long long)hi);
+        section(log, "Exclude outliers");
+        if (log) fprintf(log, "Median sequence length:    %lld bp\nMedian absolute deviation: %lld bp\nAllowed length range:      %llu-%llu bp\n\n",
+                         (long long)median, (long long)dev, (unsigned long long)lo, (unsigned long long)hi);
         for (size_t q = 0; q < S; ++q) {
             keep[q] = lo <= seqs[q].length && seqs[q].length <= hi;
-            if (verbose) fprintf(stderr, "%s: %s\n", seq_display(seqs[q]).c_str(), keep[q] ? "kept" : "excluded");
+            if (log) fprintf(log, "%s: %s\n", seq_display(seqs[q]).c_str(), keep[q] ? "kept" : "excluded");
         }
     }
 
@@ -336,8 +399,8 @@ void trim_graph(HostGraph& g, std::vector<HostSeq>& seqs, DeviceAlign& device, d
         for (size_t x = 0; x < p.size(); ++x) {
             const int32_t s = paths[q][x];
             const uint32_t num = (uint32_t)(s < 0 ? -s : s);
-            if (num > max_number || index_of[num] == 0xFFFFFFFFu) throw std::runtime_error("unitig " + std::to_string(num) + " not found in unitig index");
-            p[x] = us_make(index_of[num], s < 0);
+            if (num > w.max_number || w.index_of[num] == 0xFFFFFFFFu) throw std::runtime_error("unitig " + std::to_string(num) + " not found in unitig index");
+            p[x] = us_make(w.index_of[num], s < 0);
         }
         new_paths.push_back(std::move(p));
         kept.push_back(seqs[q]);
@@ -350,9 +413,33 @@ void trim_graph(HostGraph& g, std::vector<HostSeq>& seqs, DeviceAlign& device, d
     g.remove_zero_depth_unitigs();
     g.merge_linear_paths(true);
     g.renumber();
-    section(verbose, "Clean graph");
-    if (verbose) fprintf(stderr, "%u unitig%s, %llu link%s\ntotal length: %llu bp\n\n", g.U, g.U == 1 ? "" : "s", (unsigned long long)g.link_count_single(),
-                         g.link_count_single() == 1 ? "" : "s", (unsigned long long)g.total_length());
+    section(log, "Clean graph");
+    if (log) fprintf(log, "%u unitig%s, %llu link%s\ntotal length: %llu bp\n\n", g.U, g.U == 1 ? "" : "s", (unsigned long long)g.link_count_single(),
+                     g.link_count_single() == 1 ? "" : "s", (unsigned long long)g.total_length());
+}
+}  // namespace
+
+void trim_graphs(DeviceAlign& device, std::vector<TrimCluster>& clusters, double min_identity, uint32_t max_unitigs, double mad, AlignBatch& batch) {
+    std::vector<TrimWork> work(clusters.size());
+    std::vector<PairSet*> sets;
+    for (size_t c = 0; c < clusters.size(); ++c) { work[c].c = &clusters[c]; trim_prepare(work[c], max_unitigs); sets.push_back(&work[c].set); }
+    batch.clusters += (uint32_t)clusters.size();
+    if (max_unitigs > 0) {
+        overlap_alignments(device, sets, min_identity, max_unitigs, batch);
+        for (TrimWork& w : work) trim_round2(w);
+        overlap_alignments(device, sets, min_identity, max_unitigs, batch);
+        for (TrimWork& w : work) trim_apply_round2(w);
+    }
+    for (TrimWork& w : work) trim_finish(w, mad);
+    if (clusters.size() == 1) clusters[0].stats.kernel_ms = batch.kernel_ms;     // a shared launch's time belongs to no one cluster
+}
+
+void trim_graph(HostGraph& g, std::vector<HostSeq>& seqs, DeviceAlign& device, double min_identity, uint32_t max_unitigs, double mad,
+                bool verbose, TrimStats& stats) {
+    std::vector<TrimCluster> one{TrimCluster{&g, &seqs, verbose ? stderr : nullptr, TrimStats()}};
+    AlignBatch batch;
+    trim_graphs(device, one, min_identity, max_unitigs, mad, batch);
+    stats = one[0].stats;
 }
 
 std::string trimmed_metrics_yaml(const std::vector<HostSeq>& seqs) {

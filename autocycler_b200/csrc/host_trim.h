@@ -1,12 +1,14 @@
 // `autocycler trim` (trim.rs:36-326) on the host graph, with the overlap alignments on the device (DeviceAlign::overlap_align).
 #pragma once
 #include <cstdint>
+#include <cstdio>
 #include <string>
 #include <vector>
 
 #include "host_graph.h"
 
 class DeviceAlign;
+struct AlignBatch;
 
 enum TrimMode { TRIM_START_END = 0, TRIM_HAIRPIN_START = 1, TRIM_HAIRPIN_END = 2 };
 
@@ -24,9 +26,23 @@ struct TrimStats {
 void trim_paths(DeviceAlign& device, TrimMode mode, const std::vector<std::vector<int32_t>>& paths, const std::vector<uint32_t>& weights,
                 double min_identity, uint32_t max_unitigs, std::vector<uint8_t>& trimmed, std::vector<std::vector<int32_t>>& out, TrimStats& stats);
 
+// One cluster of trim_graphs: its graph and sequences (trimmed in place), where its report goes (null: no report) and what its
+// alignments were.  stats.kernel_ms is set only when the batch holds this one cluster: a shared launch's time is the batch's.
+struct TrimCluster {
+    HostGraph* g;
+    std::vector<HostSeq>* seqs;
+    FILE* log;
+    TrimStats stats;
+};
+
+// trim_graph for several clusters, phase by phase: every cluster prepares its round-1 pairs, one device round aligns them all, every
+// cluster applies its results and prepares round 2, a second device round, then every cluster finishes on its own.  So the device work
+// is two overlap_align calls (at most four launches) whatever the number of clusters.
+void trim_graphs(DeviceAlign& device, std::vector<TrimCluster>& clusters, double min_identity, uint32_t max_unitigs, double mad, AlignBatch& batch);
+
 // trim.rs:43-51 minus the file I/O: trims the sequences' paths, drops length outliers, cleans up the graph (recalculate_depths,
 // remove_zero_depth_unitigs, merge_linear_paths, renumber_unitigs).  `seqs` becomes the kept sequences in their order.  verbose: the
-// reference's stderr report.
+// reference's stderr report.  trim_graphs with one cluster.
 void trim_graph(HostGraph& g, std::vector<HostSeq>& seqs, DeviceAlign& device, double min_identity, uint32_t max_unitigs, double mad,
                 bool verbose, TrimStats& stats);
 

@@ -15,10 +15,10 @@
  *   compress (the whole subcommand)         compress.rs:32-50        -> ac_compress_dir
  *   trim_path_start_end / _hairpin_start / _hairpin_end   trim.rs:288-326 -> ac_trim_paths
  *   trim.rs:43-51 on a loaded graph (trim minus the file I/O)     -> ac_trim
- *   trim (the whole subcommand)             trim.rs:36-53            -> ac_trim_dir
+ *   trim (the whole subcommand)             trim.rs:36-53            -> ac_trim_dir, ac_trim_dirs (several clusters)
  *   Bridge::new (best path of a bridge)     resolve.rs:430-462       -> ac_bridge_best_paths
  *   resolve.rs:41-67 on a loaded graph                               -> ac_resolve, ac_resolve_text, ac_resolve_stats
- *   resolve / combine (the whole subcommands)  resolve.rs:31-69, combine.rs:25-49 -> ac_resolve_dir, ac_combine_dir
+ *   resolve / combine (the whole subcommands)  resolve.rs:31-69, combine.rs:25-49 -> ac_resolve_dir, ac_resolve_dirs, ac_combine_dir
  *   clean (the whole subcommand)            clean.rs:23-149          -> ac_clean_gfa
  *   clean.rs:26-45 on a GFA text            unitig_graph.rs:588-721  -> ac_clean_text
  *   gfa2fasta (the whole subcommand)        gfa2fasta.rs:23-82       -> ac_gfa_to_fasta, ac_gfa_fasta_text
@@ -244,6 +244,29 @@ int ac_trim_stats(const ac_handle* h, uint64_t* jobs, uint64_t* cells, uint32_t*
  * The reference's setting checks and messages (AC_EINPUT). */
 int ac_trim_dir(const char* cluster_dir, double min_identity, uint32_t max_unitigs, double mad, uint32_t threads, int32_t device, int32_t verbose);
 
+/* Several clusters in one call (ac_trim_dirs, ac_resolve_dirs): every cluster goes through each phase, and each device step is one
+ * call over all of them, so a trim makes at most four kernel launches and a resolve at most two, whatever the number of clusters.
+ * Every directory's outputs are byte for byte those of the single-directory call.  Every directory is checked, read and loaded before
+ * any device work, and files are written only after every cluster has finished: an error writes nothing, and it is the error the
+ * single-directory call gives for the first failing directory in argument order.  A directory given twice (after realpath) is
+ * AC_EINPUT "cluster directory given twice: <dir>"; a rebased unitig number at or above 2^31 is AC_ERANGE.
+ * verbose: AC_VERBOSE_REPORT for the single call's report and AC_VERBOSE_BANNER for the `Starting autocycler <command> (<version>)`
+ * block the command-line tool prints, per directory, in argument order, after the last cluster finishes.  With more than one directory
+ * the reports leave out the kernel time, which a shared launch cannot split by cluster, and one closing line gives the batch's totals. */
+#define AC_VERBOSE_REPORT 1
+#define AC_VERBOSE_BANNER 2
+typedef struct {
+    uint32_t clusters;                 /* directories */
+    uint32_t launches;                 /* kernel launches made */
+    uint64_t jobs;                     /* alignments (trim) or distance jobs (resolve) */
+    uint64_t cells;                    /* DP cells: sum of k^2 (trim) or n * m (resolve) */
+    uint64_t buffer_bytes;             /* the largest device call's planned buffers: jobs, paths, weights, scratch and outputs */
+    float kernel_ms;                   /* CUDA events around the launches; 0 under emulation */
+} ac_batch_info;
+/* `autocycler trim -c dir [dir ...]`: ac_trim_dir for n cluster directories with the same settings.  info may be NULL. */
+int ac_trim_dirs(const char* const* cluster_dirs, uint32_t n, double min_identity, uint32_t max_unitigs, double mad, uint32_t threads,
+                 int32_t device, int32_t verbose, ac_batch_info* info);
+
 /* `autocycler cluster`.  The contig distances (cluster.rs:132-192) and UPGMA (:395-480) run on the GPU: the symmetric matrix stays in
  * HBM and one persistent CTA performs all n - 1 merges; the tree, clustering, QC and the output files are built on the host.  Averages
  * are kept as sums over member pairs (T(A u B, C) = T(A, C) + T(B, C)), see DESIGN.md section 12. */
@@ -310,6 +333,8 @@ int ac_resolve_stats(const ac_handle* h, ac_resolve_info* out);
 /* `autocycler resolve -c cluster_dir` (main.rs:238-247, resolve.rs:31-75): reads 2_trimmed.gfa, writes 3_bridged.gfa, 4_merged.gfa and
  * 5_final.gfa.  The reference's checks (AC_EINPUT). */
 int ac_resolve_dir(const char* cluster_dir, int32_t verbose, int32_t device);
+/* `autocycler resolve -c dir [dir ...]`: ac_resolve_dir for n cluster directories, as ac_trim_dirs does for trim.  info may be NULL. */
+int ac_resolve_dirs(const char* const* cluster_dirs, uint32_t n, int32_t verbose, int32_t device, ac_batch_info* info);
 /* `autocycler combine -a autocycler_dir -i gfa [gfa ...]` (main.rs:115-124, combine.rs:25-137): writes consensus_assembly.gfa, .fasta and
  * .yaml under autocycler_dir (created if needed) from the n_gfas GFAs in argument order.  Host only. */
 int ac_combine_dir(const char* autocycler_dir, const char* const* in_gfas, uint32_t n_gfas, int32_t verbose);
