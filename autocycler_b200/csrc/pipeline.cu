@@ -1751,56 +1751,70 @@ uint32_t DeviceScan::operator()(AcStream* st, const uint32_t* in, uint32_t* out,
 // ------------------------------------------------------------------------------------------------
 // host orchestration
 // ------------------------------------------------------------------------------------------------
-struct DevicePipeline::Impl : DeviceContext {
-    Impl(int device, void* stream);
-    ~Impl();
-    uint64_t total = 0; uint32_t n_seqs = 0, k = 0; int W = 0;
-    DevBuf ascii, packed, seqs, slots, pos_slot, flags8, bmask, bcount, boff, counters, uid_rep, slot_unitig;
-    DevBuf run_start, run_len, run_uk, run_dir, is_rep, rep_idx, run_unitig, unitigs, nchunks, chunk_off, partial, link_count, links;
-    DeviceScan scan;
-    DevBuf d_fixed, cand_flag, cand_index, d_cands, d_cand_at, d_deps, d_spec;
-    DevBuf sort_a, sort_b, sort_ra, sort_rb, num_prefix, rank, d_len, d_depth, need, d_seq_off, d_arena, d_min_fpos, d_min_rpos;
-    DevBuf strand_cnt, d_next_off, d_next, prev_cnt, d_prev_off, d_prev, d_path, d_path_off;
-    DevBuf d_rec;
-    PinBuf h_cands, h_deps, h_spec, h_fixed;
-    DevBuf d_pred, d_level, d_flagmax, d_counters64, d_dirty, d_exhausted, d_arena2, d_arena3, d_pos, sort_c, sort_d, d_pos2, gfa_s_size, gfa_l_size, gfa_p_size, gfa_pieces, d_text, d_ptext, d_last, d_pbound, d_due;
-    PinBuf h_order2, h_text, h_ptext, h_pbound;
-    PinBuf h_rec, h_depth, h_order, h_arena, h_next_off, h_next, h_prev_off, h_prev, h_path, h_path_off, h_run_start, h_run_len;
-#ifndef AC_EMULATE
-    cudaEvent_t ev[24];
+// Under emulation a buffer kernels write joins its owner's set when it is constructed, so poisoning reaches each one; the product keeps nothing.
+#ifdef AC_EMULATE
+struct ScratchSet { std::vector<DevBuf*> bufs; };
+struct ScratchBuf : DevBuf { explicit ScratchBuf(ScratchSet& set) { set.bufs.push_back(this); } };
+#else
+struct ScratchSet {};
+struct ScratchBuf : DevBuf { explicit ScratchBuf(ScratchSet&) {} };
 #endif
 
-    void mark(int i) {
+// The stage boundaries a build records on the pipeline's stream, in that order; complete() turns pairs of them into PipelineTimings.
+enum Mark {
+    UPLOAD_BEGIN, UPLOAD_END,                                                          // upload()
+    PACK_BEGIN, PACK_END, SAMPLE_END, INSERT_BEGIN, INSERT_END, TABLE_END,             // build_local(); INSERT_* around the last attempt's insert kernel
+    RUNS_BEGIN, ADJACENCY_END, BOUNDARIES_END,                                         // runs_local()
+    FINISH_BEGIN, UNITIGS_END, SEEDS_END, LINKS_END, SEED_SORT_END, WORK_LIST_END, SIMPLIFY_END, GFA_END,   // finish()
+    ALL_BUT_ARENA, RESULTS_END, N_MARKS                                                // the copies to the host: all but the arena, then the arena
+};
+// The last stage a call completed: upload() or find_literals(), build_local(), runs_local()
+enum class Stage { UPLOADED, TABLE, RUNS };
+
+struct DevicePipeline::Impl : DeviceContext {
+    uint64_t total = 0; uint32_t n_seqs = 0, k = 0, U = 0, n_chunks = 0; int W = 0;      // U, n_chunks: unitigs and their 64-base chunks (finish)
+    // inputs: what upload(), set_path_line_texts() and find_literals() copy from the host
+    DevBuf ascii, seqs, d_wrap_off, d_pre_len, d_suf_len, d_blob, d_blob_off, needles;
+    // scratch: everything the kernels write, by the stage that sizes it
+    ScratchSet scratch;
+    ScratchBuf packed{scratch}, interior8{scratch}, slots{scratch}, pos_slot{scratch}, counters{scratch}, count_big{scratch}, claimed{scratch}, claimed_cnt{scratch}, occ_list{scratch},   // table
+        ext_filter{scratch}, hits{scratch};
+    ScratchBuf flags8{scratch}, bmask{scratch}, bcount{scratch}, boff{scratch}, run_start{scratch}, run_len{scratch}, run_hs{scratch}, run_ts{scratch};   // runs
+    ScratchBuf run_uk{scratch}, run_dir{scratch}, is_rep{scratch}, rep_idx{scratch}, run_unitig{scratch}, uid_rep{scratch}, slot_unitig{scratch}, unitigs{scratch}, nchunks{scratch},   // graph
+        chunk_off{scratch}, partial{scratch}, link_count{scratch}, links{scratch}, sort_a{scratch}, sort_b{scratch}, sort_ra{scratch}, sort_rb{scratch}, rank{scratch}, d_len{scratch},
+        d_depth{scratch}, need{scratch}, d_seq_off{scratch}, d_min_fpos{scratch}, d_min_rpos{scratch}, d_arena{scratch}, strand_cnt{scratch}, d_next_off{scratch}, d_next{scratch},
+        prev_cnt{scratch}, d_prev_off{scratch}, d_prev{scratch}, d_small{scratch}, d_path{scratch}, d_path_off{scratch}, d_rec{scratch}, num_prefix{scratch}, d_fixed{scratch}, cand_flag{scratch},
+        cand_index{scratch}, d_cands{scratch}, d_cand_at{scratch}, d_deps{scratch}, d_spec{scratch};
+    ScratchBuf d_pred{scratch}, d_level{scratch}, d_flagmax{scratch}, d_counters64{scratch}, d_dirty{scratch}, d_exhausted{scratch}, d_due{scratch}, d_arena2{scratch}, d_arena3{scratch},   // simplify
+        d_pos{scratch}, sort_c{scratch}, sort_d{scratch};
+    ScratchBuf d_pos2{scratch}, gfa_s_size{scratch}, gfa_l_size{scratch}, gfa_p_size{scratch}, gfa_pieces{scratch}, d_last{scratch}, d_totals{scratch}, d_text{scratch}, d_own_off{scratch},   // GFA, path lines
+        d_own_last{scratch}, d_own_size{scratch}, d_ptext{scratch};
+    ScratchBuf own_entries{scratch}, own_runs{scratch};   // exchange
+    DeviceScan scan;
+    PinBuf h_rec, h_depth, h_order, h_order2, h_arena, h_next_off, h_next, h_prev_off, h_prev, h_path, h_path_off, h_run_start, h_run_len;
+    PinBuf h_cands, h_deps, h_spec, h_fixed, h_text, h_ptext;
 #ifndef AC_EMULATE
-        AC_CUDA_CHECK(cudaEventRecord(ev[i], stream.s));
+    cudaEvent_t ev[N_MARKS];
+    Impl(int device, void* stream) : DeviceContext(device, stream) { for (auto& e : ev) AC_CUDA_CHECK(cudaEventCreate(&e)); }
+    ~Impl() { cudaSetDevice(device); for (auto& e : ev) cudaEventDestroy(e); }      // the buffers go first (on this device), the stream last (DeviceContext)
+    void mark(Mark m) { AC_CUDA_CHECK(cudaEventRecord(ev[m], stream.s)); }
+    void wait_mark(Mark m) { AC_CUDA_CHECK(cudaEventSynchronize(ev[m])); }
+    float between(Mark a, Mark b) { float ms = 0; AC_CUDA_CHECK(cudaEventElapsedTime(&ms, ev[a], ev[b])); return ms; }
 #else
-        (void)i;
+    Impl(int device, void* stream) : DeviceContext(device, stream) {}
+    void mark(Mark) {}
+    void wait_mark(Mark) {}
+    float between(Mark, Mark) { return 0.f; }
 #endif
-    }
-    void wait_mark(int i) {
-#ifndef AC_EMULATE
-        AC_CUDA_CHECK(cudaEventSynchronize(ev[i]));
-#else
-        (void)i;
-#endif
-    }
     bool arena_pending = false;
     const std::function<void()>* before_results = nullptr;   // -> DevicePipeline::before_results
-    void do_complete(PipelineResult& out);
-    float between(int a, int b) {
-#ifndef AC_EMULATE
-        float ms = 0; AC_CUDA_CHECK(cudaEventElapsedTime(&ms, ev[a], ev[b])); return ms;
-#else
-        (void)a; (void)b; return 0.f;
-#endif
-    }
 
     // pipeline state shared by the stages
     std::vector<SeqInfo> host_seqs;
     uint64_t cap = 0, n_windows = 0, n_runs = 0, g_begin = 0, g_end = 0, n_slots_used = 0, n_dotted = 0, n_fwords = 0;
     bool any_dotted = false, is_multi = false, big_counts = false;      // big_counts: depths live in count_big (a 20-bit slot count neared its end)
-    int stage = 0;
-    DevBuf run_hs, run_ts, claimed, claimed_cnt, occ_list, ext_filter, needles, hits, count_big, interior8;
+    Stage stage = Stage::UPLOADED;
+    void require(Stage s, const char* message) const { if (stage < s) throw std::runtime_error(message); }
     TableView table_view() { return TableView{slots.as<Slot>(), cap, packed.as<uint64_t>(), seqs.as<SeqInfo>(), n_seqs, big_counts ? count_big.as<uint32_t>() : nullptr, slot_gpos_bits(total), count_alarm()}; }
     static uint32_t count_alarm() { static const uint32_t a = getenv("AC_COUNT_ALARM") ? (uint32_t)atoi(getenv("AC_COUNT_ALARM")) : AC_SLOT_COUNT_ALARM; return a; }      // test hook: a lower threshold
     template <int W> void local_w(uint32_t seq_lo, uint32_t seq_hi, bool multi);
@@ -1810,69 +1824,37 @@ struct DevicePipeline::Impl : DeviceContext {
     std::vector<std::pair<const void*, uint64_t>> merged;      // the (records, count) of every merge_entries since build_local
     template <int W> void merge_w(const void* dev_ptr, uint64_t n);
     template <int W> void runs_local_w();
-    template <int W> void finish_w(PipelineResult& out, bool keep_positions, bool fused, bool split_paths);
+    // the stages of finish(), in their order; R carries what each leaves to the next
+    template <int W> void unitigs_w(PipelineResult& out);
+    void host_arrays(), paths(), work_list(), simplify(), renumber(), gfa(bool split_paths);
+    void results(PipelineResult& out, bool keep_positions, bool fused);
     // what a finished build leaves in HBM for pull_graph() (at once in a plain build, on request after a fused one)
     struct Pending {
-        uint32_t U = 0, n_strands = 0; uint64_t n_links = 0, n_cands = 0;
+        uint64_t n_links = 0, n_cands = 0;
         uint32_t* order_built = nullptr; uint32_t* final_order = nullptr; uint8_t* fix_start = nullptr;
         DevBuf* arena_src = nullptr; uint64_t arena_final = 0;
-        bool any_moved = false, gfa_on_device = false, hairpins_ready = false, paths_split = false;
+        bool any_moved = false, gfa_on_device = false, paths_split = false;
         uint64_t bases_removed = 0, gfa_bytes = 0;
     } R;
-    bool pending_keep_positions = false;
     void pull_graph(PipelineResult& out, bool keep_positions);
-    DevBuf d_small, d_totals, d_wrap_off, d_pre_len, d_suf_len, d_blob, d_blob_off;
     std::vector<char> path_blob; std::vector<uint32_t> path_pre, path_suf; uint64_t path_wrap_total = 0;
     uint64_t uploaded_bytes = 0;
     uint64_t exp_n = 0, n_own_runs = 0; uint32_t own_seq_lo = 0, own_seq_hi = 0; bool exp_valid = false;      // exp_n: this rank's own distinct k-mers, counted before the merge
-    void do_export_path_tokens(void* dst, uint64_t stride, const uint64_t* counts, uint32_t n_ranks);
-    void do_render_path_lines(const void* tokens, uint64_t n_tokens, const char** text, uint64_t* bytes);
-    DevBuf d_own_off, d_own_last, d_own_size; uint64_t path_lines_d2h = 0;
     template <int W> uint64_t list_claimed(bool with_filter);
-    template <int W> uint64_t do_count_entries();
-    void do_export_entries(void* dst, uint64_t cap_records);
-    void do_export_runs(void* dst, uint64_t cap_records);
-    void do_import_runs(const void* dev_ptr, uint64_t n);
-    void do_import_runs_from(const void* const* ptrs, const uint64_t* counts, uint32_t n_ranks);
-    DevBuf own_entries, own_runs;
+    template <int W> uint64_t count_entries_w();
 #ifdef AC_EMULATE
-    // AC_EMU_POISON=1 (CPU suite): before every table build, every device buffer a kernel writes is filled with a pattern, so a kernel that
-    // reads what THIS build has not written (on the GPU: leftovers of the previous build, whose slot numbers differ from run to run, while
-    // the emulation reproduces them exactly) shows up on the CPU as well.
-    void poison() {
-        static const bool on = getenv("AC_EMU_POISON") != nullptr;
-        if (!on) return;
-        DevBuf* all[] = {&packed, &slots, &pos_slot, &flags8, &bmask, &bcount, &boff, &counters, &uid_rep, &slot_unitig, &run_start, &run_len, &run_uk, &run_dir, &is_rep, &rep_idx,
-                         &run_unitig, &unitigs, &nchunks, &chunk_off, &partial, &link_count, &links, &scan.serial.level[0], &scan.serial.level[1], &scan.serial.level[2], &scan.serial.level[3], &d_fixed, &cand_flag, &cand_index,
-                         &d_cands, &d_cand_at, &d_deps, &d_spec, &sort_a, &sort_b, &sort_ra, &sort_rb, &num_prefix, &rank, &d_len, &d_depth, &need, &d_seq_off, &d_arena, &d_min_fpos, &d_min_rpos,
-                         &strand_cnt, &d_next_off, &d_next, &prev_cnt, &d_prev_off, &d_prev, &d_path, &d_path_off, &d_rec, &d_pred, &d_level, &d_flagmax, &d_counters64, &d_dirty, &d_exhausted,
-                         &d_arena2, &d_arena3, &d_pos, &sort_c, &sort_d, &d_pos2, &gfa_s_size, &gfa_l_size, &gfa_p_size, &gfa_pieces, &d_text, &d_ptext, &d_last, &run_hs, &run_ts, &claimed,
-                         &claimed_cnt, &occ_list, &ext_filter, &count_big, &interior8, &d_small, &d_totals, &d_own_off, &d_own_last, &d_own_size, &own_entries, &own_runs, &d_due};
-        for (DevBuf* b : all) if (b->p) memset(b->p, 0xA5, b->cap);
-    }
-    void poison_table() {          // and before every attempt at the table: a retry must not read what the failed attempt left
-        static const bool on = getenv("AC_EMU_POISON") != nullptr;
-        if (!on) return;
-        DevBuf* all[] = {&slots, &pos_slot, &claimed, &claimed_cnt, &occ_list, &count_big, &counters};
-        for (DevBuf* b : all) if (b->p) memset(b->p, 0xA5, b->cap);
-    }
+    // AC_EMU_POISON=1 (CPU suite): before every table build, every scratch buffer is filled with a pattern, so a kernel that reads what
+    // THIS build has not written (on the GPU: leftovers of the previous build, whose slot numbers differ from run to run, while the
+    // emulation reproduces them exactly) shows up on the CPU as well.
+    static void fill(DevBuf* b) { static const bool on = getenv("AC_EMU_POISON") != nullptr; if (on && b->p) memset(b->p, 0xA5, b->cap); }
+    void poison() { for (DevBuf* b : scratch.bufs) fill(b); for (DevBuf& b : scan.serial.level) fill(&b); }
+    // and before every attempt at the table: a retry must not read what the failed attempt left
+    void poison_table() { for (DevBuf* b : {&slots, &pos_slot, &claimed, &claimed_cnt, &occ_list, &count_big, &counters}) fill(b); }
 #else
     void poison() {}
     void poison_table() {}
 #endif
 };
-
-DevicePipeline::Impl::Impl(int device, void* stream) : DeviceContext(device, stream) {
-#ifndef AC_EMULATE
-    for (auto& e : ev) AC_CUDA_CHECK(cudaEventCreate(&e));
-#endif
-}
-DevicePipeline::Impl::~Impl() {        // the buffers go first (on this device), the stream last (DeviceContext)
-#ifndef AC_EMULATE
-    cudaSetDevice(device);
-    for (auto& e : ev) cudaEventDestroy(e);
-#endif
-}
 
 DevicePipeline::DevicePipeline(int device, void* stream) : impl(new Impl(device, stream)) { impl->before_results = &before_results; }
 DevicePipeline::~DevicePipeline() { delete impl; }
@@ -1887,9 +1869,9 @@ void DevicePipeline::upload(const uint8_t* ascii, uint64_t total, const SeqInfo*
     if (W > AC_MAX_W) throw std::runtime_error("k-mer sizes above " + std::to_string(AC_MAX_K) + " are not supported by the GPU path (no CPU fallback exists)");
     if (total >= 0xFFFFFFF0ull) throw std::runtime_error("more than 2^32 padded input bytes are not supported");
     if (n_seqs == 0 || total == 0) throw std::runtime_error("no sequences");
-    m.total = total; m.n_seqs = n_seqs; m.k = k; m.W = W; m.stage = 0;
+    m.total = total; m.n_seqs = n_seqs; m.k = k; m.W = W; m.stage = Stage::UPLOADED;
     m.host_seqs.assign(seqs, seqs + n_seqs);
-    m.mark(0);
+    m.mark(UPLOAD_BEGIN);
     m.ascii.ensure(total);
     if (seq_lo == 0 && seq_hi >= n_seqs) { ac_h2d(m.ascii.p, ascii, total, &m.stream); m.uploaded_bytes = total; }
     else {              // a shard: only the strands of sequences [seq_lo, seq_hi); the caller's collective brings the other ranks' blocks (strand_block)
@@ -1910,7 +1892,7 @@ void DevicePipeline::upload(const uint8_t* ascii, uint64_t total, const SeqInfo*
         if (!m.path_blob.empty()) ac_h2d(m.d_blob.p, m.path_blob.data(), m.path_blob.size(), &m.stream);
         ac_sync(&m.stream);                  // the staging vectors above are locals
     } else m.path_wrap_total = 0;
-    m.mark(1);
+    m.mark(UPLOAD_END);
 }
 
 void DevicePipeline::set_path_line_texts(const char* blob, const uint32_t* prefix_len, const uint32_t* suffix_len, uint32_t n) {
@@ -1934,8 +1916,7 @@ void DevicePipeline::find_literals(const uint8_t* ascii_host, uint64_t total_byt
     ac_launch("pack", &m.stream, PackBody{m.ascii.as<uint8_t>(), total_bytes, m.packed.as<uint64_t>(), nullptr, 0, nullptr}, n_words);
     // needle table (host-built, tiny)
     uint64_t cap = 64; while (cap < 4ull * n_needles) cap <<= 1;
-    std::vector<NeedleSlot> table(cap);
-    for (auto& t : table) { t.w[0] = t.w[1] = 0; t.id = 0; t.used = 0; }
+    std::vector<NeedleSlot> table(cap);          // all zero: no slot used
     for (uint32_t i = 0; i < n_needles; ++i) {
         Key<2> k2; k2.w[0] = needle_words[2 * i]; k2.w[1] = needle_words[2 * i + 1]; k2.d = 0;
         uint64_t hsh;
@@ -1960,8 +1941,15 @@ void DevicePipeline::find_literals(const uint8_t* ascii_host, uint64_t total_byt
         if (found <= hit_cap) { out.resize(found); if (found) { ac_d2h(out.data(), m.hits.p, found * sizeof(LiteralHit), &m.stream); ac_sync(&m.stream); } break; }
         hit_cap = found + 1024;        // short literals match often: run again with room for all of them
     }
-    m.stage = 0;
+    m.stage = Stage::UPLOADED;
 }
+
+// One instantiation of every k-mer kernel per key width: W = ceil(2k / 64) words, k up to 511.
+#define AC_W_CASE(fn, n, ...) case n: fn<n>(__VA_ARGS__); break;
+#define AC_DISPATCH_W(fn, ...) switch (W) { AC_W_CASE(fn, 1, __VA_ARGS__) AC_W_CASE(fn, 2, __VA_ARGS__) AC_W_CASE(fn, 3, __VA_ARGS__) AC_W_CASE(fn, 4, __VA_ARGS__) \
+    AC_W_CASE(fn, 5, __VA_ARGS__) AC_W_CASE(fn, 6, __VA_ARGS__) AC_W_CASE(fn, 7, __VA_ARGS__) AC_W_CASE(fn, 8, __VA_ARGS__) AC_W_CASE(fn, 9, __VA_ARGS__) AC_W_CASE(fn, 10, __VA_ARGS__) \
+    AC_W_CASE(fn, 11, __VA_ARGS__) AC_W_CASE(fn, 12, __VA_ARGS__) AC_W_CASE(fn, 13, __VA_ARGS__) AC_W_CASE(fn, 14, __VA_ARGS__) AC_W_CASE(fn, 15, __VA_ARGS__) AC_W_CASE(fn, 16, __VA_ARGS__) \
+    default: throw std::runtime_error("upload() must precede build()"); }
 
 // ---- stage 1: pack + k-mer table over this rank's sequences ----
 #define AC_N_COUNTERS 4          // InsertBody::counters
@@ -1979,13 +1967,13 @@ template <int W> void DevicePipeline::Impl::local_w(uint32_t seq_lo, uint32_t se
     cap = (n_windows + n_windows / 2 + 64 + 3) & ~3ull;      // a multiple of 4: the table is probed in groups of four slots
     if (cap >= 0xFFFFFFF0ull) throw std::runtime_error("input too large for 32-bit slot indices");
 
-    mark(2);
+    mark(PACK_BEGIN);
     const uint64_t n_words = (total + 31) / 32;
     packed.ensure((n_words + W + 2) * sizeof(uint64_t));
     ac_memset(packed.as<uint64_t>() + n_words, 0, (W + 2) * sizeof(uint64_t), &stream);
     interior8.ensure(n_words + 8);
     ac_launch("pack", &stream, PackBody{ascii.as<uint8_t>(), total, packed.as<uint64_t>(), seqs.as<SeqInfo>(), n_seqs, interior8.as<uint8_t>()}, n_words);
-    mark(3);
+    mark(PACK_END);
 
     // ---- size the table: distinct canonical k-mers estimated from the 1/64 of them whose hash ends in six zero bits ----
     // (sampling by hash value keeps or drops a k-mer with ALL its occurrences, so 64 x the sample's distinct count is an
@@ -2009,13 +1997,13 @@ template <int W> void DevicePipeline::Impl::local_w(uint32_t seq_lo, uint32_t se
             cap = std::min<uint64_t>(safe_cap, ((uint64_t)((double)est / load) + 4096 + 3) & ~3ull);
         }
     }
-    mark(15);
+    mark(SAMPLE_END);
     this->safe_cap = safe_cap;
     table_attempt = 0;
     merged.clear();
     insert_w<W>();
-    mark(4);
-    stage = 1;
+    mark(TABLE_END);
+    stage = Stage::TABLE;
 }
 
 // The table over this rank's windows at `cap`, started again at the safe size if the probe limit trips and with the counts in the side
@@ -2039,9 +2027,9 @@ template <int W> void DevicePipeline::Impl::insert_w() {
         const InsertBody<W> ins{tv, p, interior8.as<uint8_t>(), (uint32_t)g_first, (uint32_t)g_begin, (uint32_t)g_end, is_multi, pos_slot.as<uint32_t>(), counters.as<unsigned long long>(), false, claimed.as<uint32_t>()};
         // (a software-pipelined form of the one-window loop — the next unit's keys built and its home group in flight while the current one is
         // probed — needed 75 registers and was slower; it is not kept)
-        mark(20);
+        mark(INSERT_BEGIN);
         ac_launch_occ<AC_INSERT_CTAS>("insert", &stream, ins, (g_end - g_first + 63) / 64 * 32);     // one warp per 64 windows
-        mark(21);
+        mark(INSERT_END);
         ac_d2h(hc, counters.p, sizeof hc, &stream); ac_sync(&stream);
         if (hc[2] && cap != safe_cap) { cap = safe_cap; continue; }         // the estimate was off (it is an estimate): start again with the safe size
         if (hc[2]) throw std::runtime_error("k-mer table overflow");
@@ -2072,20 +2060,21 @@ template <int W> uint64_t DevicePipeline::Impl::list_claimed(bool with_filter) {
                                                           table_view(), make_kparams(k, W), interior8.as<uint8_t>(), with_filter ? ext_filter.as<uint64_t>() : nullptr, n_fwords}, n_words * 32);
     return n;
 }
-template <int W> uint64_t DevicePipeline::Impl::do_count_entries() {
-    if (stage < 1) throw std::runtime_error("build_local must precede the entry export");
+template <int W> uint64_t DevicePipeline::Impl::count_entries_w() {
+    require(Stage::TABLE, "build_local must precede the entry export");
     exp_n = list_claimed<W>(false);        // before any merge: the local table
     exp_valid = true;
     return exp_n;
 }
-void DevicePipeline::Impl::do_export_entries(void* dst, uint64_t cap_records) {
-    if (cap_records < exp_n) throw std::runtime_error("entry buffer too small");
-    ac_launch("export_scatter", &stream, ExportScatterBody{table_view(), occ_list.as<uint32_t>(), (SlotRec*)dst}, exp_n);
-    ac_sync(&stream);
+void DevicePipeline::export_entries(void* dst, uint64_t cap_records) {
+    Impl& m = *impl; m.make_current();
+    if (cap_records < m.exp_n) throw std::runtime_error("entry buffer too small");
+    ac_launch("export_scatter", &m.stream, ExportScatterBody{m.table_view(), m.occ_list.as<uint32_t>(), (SlotRec*)dst}, m.exp_n);
+    ac_sync(&m.stream);
 }
 
 template <int W> void DevicePipeline::Impl::merge_w(const void* dev_ptr, uint64_t n) {
-    if (stage < 1) throw std::runtime_error("build_local must precede merge_entries");
+    require(Stage::TABLE, "build_local must precede merge_entries");
     const KParams p = make_kparams(k, W);
     ac_launch("merge", &stream, MergeBody<W>{table_view(), p, (const SlotRec*)dev_ptr, pos_slot.as<uint32_t>(), counters.as<unsigned long long>(), claimed.as<uint32_t>()}, n);
     merged.emplace_back(dev_ptr, n);      // folded in again if the union overflows the table (runs_local_w)
@@ -2093,9 +2082,9 @@ template <int W> void DevicePipeline::Impl::merge_w(const void* dev_ptr, uint64_
 
 // ---- stage 2: adjacency over the (now global) table, unitig occurrences along this rank's sequences ----
 template <int W> void DevicePipeline::Impl::runs_local_w() {
-    if (stage < 1) throw std::runtime_error("build_local must precede runs_local");
+    require(Stage::TABLE, "build_local must precede runs_local");
     const KParams p = make_kparams(k, W);
-    mark(13);
+    mark(RUNS_BEGIN);
     if (is_multi) {      // the merges may have tripped the limits too
         unsigned long long hc[AC_N_COUNTERS];
         ac_d2h(hc, counters.p, sizeof hc, &stream); ac_sync(&stream);
@@ -2125,60 +2114,80 @@ template <int W> void DevicePipeline::Impl::runs_local_w() {
         if (getenv("AC_HOST_PROFILE")) fprintf(stderr, "[device] adjacency flags for this rank's own k-mers: at most %llu of %llu\n", (unsigned long long)n_adj, (unsigned long long)n_slots_used);
         ac_launch("adjacency", &stream, AdjacencyOwnBody<W>{adj, claimed_cnt.as<uint32_t>(), g_begin >> 5, std::min<uint64_t>((g_end + 31) >> 5, n_cw)}, n_adj);
     } else ac_launch("adjacency", &stream, adj, n_slots_used);
-    mark(5);
+    mark(ADJACENCY_END);
 
     const uint64_t n_bwords = (total + 31) / 32;
     bmask.ensure(n_bwords * sizeof(uint32_t)); bcount.ensure(n_bwords * sizeof(uint32_t)); boff.ensure(n_bwords * sizeof(uint32_t));
     ac_launch("boundaries", &stream, BoundaryBody{packed.as<uint64_t>(), seqs.as<SeqInfo>(), n_seqs, p.h, g_begin, g_end, pos_slot.as<uint32_t>(),
                                                   flags8.as<uint8_t>(), interior8.as<uint8_t>(), bmask.as<uint32_t>(), bcount.as<uint32_t>()}, n_bwords * 32);
     n_runs = scan(&stream, bcount.as<uint32_t>(), boff.as<uint32_t>(), n_bwords);
-    mark(6);
+    mark(BOUNDARIES_END);
     run_start.ensure(n_runs * sizeof(uint64_t)); run_len.ensure(n_runs * 4); run_hs.ensure(n_runs * 4); run_ts.ensure(n_runs * 4);
     ac_launch("run_scatter", &stream, RunScatterBody{bmask.as<uint32_t>(), boff.as<uint32_t>(), run_start.as<uint64_t>()}, n_bwords);
     ac_launch("run_ends", &stream, RunEndsLocalBody{seqs.as<SeqInfo>(), n_seqs, run_start.as<uint64_t>(), n_runs, pos_slot.as<uint32_t>(),
                                                     run_len.as<uint32_t>(), run_hs.as<uint32_t>(), run_ts.as<uint32_t>()}, n_runs);
     n_own_runs = n_runs;
-    stage = 2;
+    stage = Stage::RUNS;
 }
 
-void DevicePipeline::Impl::do_export_runs(void* dst, uint64_t cap_records) {
-    if (stage < 2) throw std::runtime_error("runs_local must precede export_runs");
-    if (cap_records < n_runs) throw std::runtime_error("run buffer too small");
-    ac_launch("run_export", &stream, RunExportBody{run_start.as<uint64_t>(), run_len.as<uint32_t>(), run_hs.as<uint32_t>(), run_ts.as<uint32_t>(),
-                                                   slots.as<Slot>(), slot_gpos_bits(total), (RunRec*)dst}, n_runs);
-    ac_sync(&stream);
+void DevicePipeline::export_runs(void* dst, uint64_t cap_records) {
+    Impl& m = *impl; m.make_current();
+    m.require(Stage::RUNS, "runs_local must precede export_runs");
+    if (cap_records < m.n_runs) throw std::runtime_error("run buffer too small");
+    ac_launch("run_export", &m.stream, RunExportBody{m.run_start.as<uint64_t>(), m.run_len.as<uint32_t>(), m.run_hs.as<uint32_t>(), m.run_ts.as<uint32_t>(),
+                                                     m.slots.as<Slot>(), slot_gpos_bits(m.total), (RunRec*)dst}, m.n_runs);
+    ac_sync(&m.stream);
 }
 
-void DevicePipeline::Impl::do_import_runs(const void* dev_ptr, uint64_t n) {
-    if (stage < 2) throw std::runtime_error("runs_local must precede import_runs");
-    n_runs = n;
-    run_start.ensure(n_runs * sizeof(uint64_t)); run_len.ensure(n_runs * 4); run_hs.ensure(n_runs * 4); run_ts.ensure(n_runs * 4);
-    RunImportBody body{(const RunRec*)dev_ptr, pos_slot.as<uint32_t>(), run_start.as<uint64_t>(), run_len.as<uint32_t>(), run_hs.as<uint32_t>(), run_ts.as<uint32_t>(), 0, {0}, {nullptr}};
-    ac_launch("run_import", &stream, body, n_runs);
+void DevicePipeline::import_runs(const void* dev_ptr, uint64_t n) {
+    Impl& m = *impl; m.make_current();
+    m.require(Stage::RUNS, "runs_local must precede import_runs");
+    m.n_runs = n;
+    m.run_start.ensure(n * sizeof(uint64_t)); m.run_len.ensure(n * 4); m.run_hs.ensure(n * 4); m.run_ts.ensure(n * 4);
+    RunImportBody body{(const RunRec*)dev_ptr, m.pos_slot.as<uint32_t>(), m.run_start.as<uint64_t>(), m.run_len.as<uint32_t>(), m.run_hs.as<uint32_t>(), m.run_ts.as<uint32_t>(), 0, {0}, {nullptr}};
+    ac_launch("run_import", &m.stream, body, n);
 }
 
-void DevicePipeline::Impl::do_import_runs_from(const void* const* ptrs, const uint64_t* counts, uint32_t n_ranks) {
-    if (stage < 2) throw std::runtime_error("runs_local must precede import_runs");
+void DevicePipeline::import_runs_from(const void* const* ptrs, const uint64_t* counts, uint32_t n_ranks) {
+    Impl& m = *impl; m.make_current();
+    m.require(Stage::RUNS, "runs_local must precede import_runs");
     if (n_ranks == 0 || n_ranks > AC_MAX_RANKS) throw std::runtime_error("import_runs: bad rank count");
-    RunImportBody body{nullptr, pos_slot.as<uint32_t>(), nullptr, nullptr, nullptr, nullptr, n_ranks, {0}, {nullptr}};
+    RunImportBody body{nullptr, m.pos_slot.as<uint32_t>(), nullptr, nullptr, nullptr, nullptr, n_ranks, {0}, {nullptr}};
     for (uint32_t q = 0; q < n_ranks; ++q) { body.first[q + 1] = body.first[q] + counts[q]; body.src[q] = (const RunRec*)ptrs[q]; }
-    n_runs = body.first[n_ranks];
-    run_start.ensure(n_runs * sizeof(uint64_t)); run_len.ensure(n_runs * 4); run_hs.ensure(n_runs * 4); run_ts.ensure(n_runs * 4);
-    body.run_start = run_start.as<uint64_t>(); body.run_len = run_len.as<uint32_t>(); body.run_hs = run_hs.as<uint32_t>(); body.run_ts = run_ts.as<uint32_t>();
-    ac_launch("run_import", &stream, body, n_runs);
+    const uint64_t n = m.n_runs = body.first[n_ranks];
+    m.run_start.ensure(n * sizeof(uint64_t)); m.run_len.ensure(n * 4); m.run_hs.ensure(n * 4); m.run_ts.ensure(n * 4);
+    body.run_start = m.run_start.as<uint64_t>(); body.run_len = m.run_len.as<uint32_t>(); body.run_hs = m.run_hs.as<uint32_t>(); body.run_ts = m.run_ts.as<uint32_t>();
+    ac_launch("run_import", &m.stream, body, n);
 }
 
 // ---- stage 3: unitigs, seeds, links, seed order and the host-ready arrays (over every occurrence handed to it) ----
-template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool keep_positions, bool fused, bool split_paths) {
-    if (stage < 2) throw std::runtime_error("runs_local must precede finish");
+void DevicePipeline::finish(PipelineResult& out, bool keep_positions, bool fused, bool split_paths) {
+    Impl& m = *impl; m.make_current(); const int W = m.W;
+    if (split_paths && !fused) throw std::runtime_error("split path lines need the fused finish");
+    AC_DISPATCH_W(m.unitigs_w, out)
+    m.host_arrays();
+    m.paths();
+    m.work_list();
+    // simplify_structure and save_gfa on the device: fused builds only (a plain build hands the host the graph as built)
+    if (fused && m.R.n_cands > 0) m.simplify();
+    m.mark(SIMPLIFY_END);
+    if (fused) {
+        m.renumber();
+        if (m.U < 100000000u) m.gfa(split_paths);
+    }
+    m.mark(GFA_END);
+    m.results(out, keep_positions, fused);
+}
+
+// The part that depends on the key width: run keys, unitigs, their seed k-mers and the links
+template <int W> void DevicePipeline::Impl::unitigs_w(PipelineResult& out) {
+    require(Stage::RUNS, "runs_local must precede finish");
     const KParams p = make_kparams(k, W);
     const TableView tv = table_view();
     out = PipelineResult();
     out.W = W; out.capacity = cap; out.n_slots_used = n_slots_used; out.n_dotted = n_dotted;
-    const uint64_t n_runs = this->n_runs;
-    const bool any_dotted = this->any_dotted;
-    const uint64_t n_windows = this->n_windows;
-    mark(14);
+    R = Pending();
+    mark(FINISH_BEGIN);
     run_uk.ensure(n_runs * 4); run_dir.ensure(n_runs);
     is_rep.ensure(n_runs * 4); rep_idx.ensure(n_runs * 4); run_unitig.ensure(n_runs * 4);
     uid_rep.ensure(cap * 4); slot_unitig.ensure(cap * 4);
@@ -2186,57 +2195,58 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
     ac_launch("run_key", &stream, RunKeyBody{packed.as<uint64_t>(), p.h, run_start.as<uint64_t>(), run_hs.as<uint32_t>(), run_ts.as<uint32_t>(),
                                              run_uk.as<uint32_t>(), run_dir.as<uint8_t>(), uid_rep.as<uint32_t>()}, n_runs);
     ac_launch("rep_flag", &stream, RepFlagBody{run_uk.as<uint32_t>(), uid_rep.as<uint32_t>(), is_rep.as<uint32_t>()}, n_runs);
-    const uint32_t n_unitigs = scan(&stream, is_rep.as<uint32_t>(), rep_idx.as<uint32_t>(), n_runs);
-    unitigs.ensure((size_t)n_unitigs * sizeof(DeviceUnitig));
+    U = scan(&stream, is_rep.as<uint32_t>(), rep_idx.as<uint32_t>(), n_runs);
+    unitigs.ensure((size_t)U * sizeof(DeviceUnitig));
     ac_launch("run_assign", &stream, RunAssignBody{run_start.as<uint64_t>(), run_len.as<uint32_t>(), run_uk.as<uint32_t>(), run_dir.as<uint8_t>(),
                                                    uid_rep.as<uint32_t>(), rep_idx.as<uint32_t>(), run_hs.as<uint32_t>(), run_ts.as<uint32_t>(), tv,
                                                    run_unitig.as<uint32_t>(), unitigs.as<DeviceUnitig>(), slot_unitig.as<uint32_t>()}, n_runs);
-    mark(7);
+    mark(UNITIGS_END);
 
     // ---- seed k-mer / orientation per unitig ----
-    nchunks.ensure(((size_t)n_unitigs + 1) * 4); chunk_off.ensure(((size_t)n_unitigs + 1) * 4);
-    ac_launch("chunk_count", &stream, ChunkCountBody{unitigs.as<DeviceUnitig>(), nchunks.as<uint32_t>()}, n_unitigs);
-    ac_memset(nchunks.as<uint32_t>() + n_unitigs, 0, 4, &stream);
-    const uint32_t n_chunks = scan(&stream, nchunks.as<uint32_t>(), chunk_off.as<uint32_t>(), (uint64_t)n_unitigs + 1);
+    nchunks.ensure(((size_t)U + 1) * 4); chunk_off.ensure(((size_t)U + 1) * 4);
+    ac_launch("chunk_count", &stream, ChunkCountBody{unitigs.as<DeviceUnitig>(), nchunks.as<uint32_t>()}, U);
+    ac_memset(nchunks.as<uint32_t>() + U, 0, 4, &stream);
+    n_chunks = scan(&stream, nchunks.as<uint32_t>(), chunk_off.as<uint32_t>(), (uint64_t)U + 1);
     partial.ensure((size_t)n_chunks * sizeof(MinPartial<W>));
-    ac_launch("chunk_min", &stream, ChunkMinBody<W>{packed.as<uint64_t>(), seqs.as<SeqInfo>(), n_seqs, p, unitigs.as<DeviceUnitig>(), n_unitigs,
+    ac_launch("chunk_min", &stream, ChunkMinBody<W>{packed.as<uint64_t>(), seqs.as<SeqInfo>(), n_seqs, p, unitigs.as<DeviceUnitig>(), U,
                                                     chunk_off.as<uint32_t>(), partial.as<MinPartial<W>>()}, n_chunks);
-    ac_launch("unitig_min", &stream, UnitigMinBody<W>{chunk_off.as<uint32_t>(), partial.as<MinPartial<W>>(), unitigs.as<DeviceUnitig>()}, n_unitigs);
-    mark(8);
+    ac_launch("unitig_min", &stream, UnitigMinBody<W>{chunk_off.as<uint32_t>(), partial.as<MinPartial<W>>(), unitigs.as<DeviceUnitig>()}, U);
+    mark(SEEDS_END);
 
     // ---- links ----
-    link_count.ensure((size_t)n_unitigs * 2 * 4); links.ensure((size_t)n_unitigs * 2 * AC_MAX_LINKS * 4);
+    link_count.ensure((size_t)U * 2 * 4); links.ensure((size_t)U * 2 * AC_MAX_LINKS * 4);
     ac_launch("links", &stream, LinkBody<W>{tv, p, any_dotted, unitigs.as<DeviceUnitig>(), pos_slot.as<uint32_t>(), slot_unitig.as<uint32_t>(),
-                                            link_count.as<uint32_t>(), links.as<uint32_t>()}, (uint64_t)n_unitigs * 2);
-    mark(9);
+                                            link_count.as<uint32_t>(), links.as<uint32_t>()}, (uint64_t)U * 2);
+    mark(LINKS_END);
+}
 
+// Seed order, the host-ready arrays in it, the unitigs' sequences in one arena, and the links as CSR
+void DevicePipeline::Impl::host_arrays() {
     // ---- seed order: stable LSD radix sort of the unitigs by their seed k-mer ----
-    const uint32_t U = n_unitigs;
     sort_a.ensure((size_t)U * 4); sort_b.ensure((size_t)U * 4); sort_ra.ensure((size_t)U * sizeof(SortRec)); sort_rb.ensure((size_t)U * sizeof(SortRec));
     const SeedLess seed_less{unitigs.as<DeviceUnitig>(), W};
     const uint32_t* perm = sort_indices(&stream, seed_less, U, sort_a.as<uint32_t>(), sort_b.as<uint32_t>(), sort_ra.as<SortRec>(), sort_rb.as<SortRec>());
-    mark(10);
-
+    mark(SEED_SORT_END);
     // ---- host-ready arrays in seed order ----
     rank.ensure((size_t)U * 4); d_len.ensure((size_t)U * 4); d_depth.ensure((size_t)U * 4); need.ensure(((size_t)U + 1) * 4);
     d_seq_off.ensure((size_t)U * 8); d_min_fpos.ensure((size_t)U * 4); d_min_rpos.ensure((size_t)U * 4);
     ac_launch("seed_gather", &stream, SeedGatherBody{perm, unitigs.as<DeviceUnitig>(), U, rank.as<uint32_t>(), d_len.as<uint32_t>(), d_depth.as<uint32_t>(),
                                                      need.as<uint32_t>(), d_min_fpos.as<uint32_t>(), d_min_rpos.as<uint32_t>()}, (uint64_t)U + 1);
-    {   // the arena must stay below 4 GB for the 32-bit scan; sum(len) <= windows
-        if (n_windows + (uint64_t)U * 2 * AC_SEQ_SLACK >= 0xFFFFFFF0ull) throw std::runtime_error("unitig sequence arena would exceed 4 GB");
-    }
+    // the arena must stay below 4 GB for the 32-bit scan; sum(len) <= windows
+    if (n_windows + (uint64_t)U * 2 * AC_SEQ_SLACK >= 0xFFFFFFF0ull) throw std::runtime_error("unitig sequence arena would exceed 4 GB");
     const uint64_t arena_bytes = scan(&stream, need.as<uint32_t>(), need.as<uint32_t>(), (uint64_t)U + 1);
     ac_launch("seq_off", &stream, SeqOffBody{need.as<uint32_t>(), d_seq_off.as<uint64_t>()}, U);
     d_arena.ensure(arena_bytes);
-    ac_launch("emit_seq", &stream, EmitSeqBody{packed.as<uint64_t>(), p.h, unitigs.as<DeviceUnitig>(), U, chunk_off.as<uint32_t>(), rank.as<uint32_t>(),
+    ac_launch("emit_seq", &stream, EmitSeqBody{packed.as<uint64_t>(), make_kparams(k, W).h, unitigs.as<DeviceUnitig>(), U, chunk_off.as<uint32_t>(), rank.as<uint32_t>(),
                                                d_seq_off.as<uint64_t>(), d_arena.as<char>()}, n_chunks);
+    R.arena_final = arena_bytes; R.arena_src = &d_arena;
     // links -> CSR in seed-strand order
     const uint32_t n_strands = 2 * U;
     strand_cnt.ensure(((size_t)n_strands + 1) * 4); d_next_off.ensure(((size_t)n_strands + 1) * 4);
     prev_cnt.ensure(((size_t)n_strands + 1) * 4); d_prev_off.ensure(((size_t)n_strands + 1) * 4);
     ac_launch("link_count", &stream, LinkCountBody{link_count.as<uint32_t>(), rank.as<uint32_t>(), unitigs.as<DeviceUnitig>(), n_strands, strand_cnt.as<uint32_t>()},
               (uint64_t)n_strands + 1);
-    const uint64_t n_links = scan(&stream, strand_cnt.as<uint32_t>(), d_next_off.as<uint32_t>(), (uint64_t)n_strands + 1);
+    const uint64_t n_links = R.n_links = scan(&stream, strand_cnt.as<uint32_t>(), d_next_off.as<uint32_t>(), (uint64_t)n_strands + 1);
     d_next.ensure(n_links * 4); d_prev.ensure(n_links * 4);
     ac_memset(prev_cnt.p, 0, ((size_t)n_strands + 1) * 4, &stream);
     d_small.ensure(64); ac_memset(d_small.p, 0, 64, &stream);           // [0] hairpin links
@@ -2246,7 +2256,10 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
     ac_memset(prev_cnt.p, 0, ((size_t)n_strands + 1) * 4, &stream);    // reused as the fill cursor
     ac_launch("prev_fill", &stream, PrevFillBody{d_next_off.as<uint32_t>(), d_next.as<UStrand>(), d_prev_off.as<uint32_t>(), prev_cnt.as<uint32_t>(), d_prev.as<UStrand>()}, n_strands);
     ac_launch("prev_sort", &stream, PrevSortBody{d_prev_off.as<uint32_t>(), d_prev.as<UStrand>()}, n_strands);
-    // paths
+}
+
+// The path of every sequence, the unitig records the host works on, and their numbering
+void DevicePipeline::Impl::paths() {
     d_path.ensure(n_runs * 4); d_path_off.ensure(((size_t)n_seqs + 1) * 8);
     ac_launch("path", &stream, PathBody{seqs.as<SeqInfo>(), n_seqs, run_start.as<uint64_t>(), run_len.as<uint32_t>(), run_unitig.as<uint32_t>(), rank.as<uint32_t>(),
                                         unitigs.as<DeviceUnitig>(), d_path.as<UStrand>(), d_min_fpos.as<uint32_t>(), d_min_rpos.as<uint32_t>()}, n_runs);
@@ -2257,136 +2270,140 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
     num_prefix.ensure((size_t)U * 8);
     ac_launch("number_key", &stream, NumberKeyBody{d_rec.as<UnitigRec>(), d_arena.as<char>(), num_prefix.as<uint64_t>()}, U);
     const NumberLess number_less{d_rec.as<UnitigRec>(), d_depth.as<uint32_t>(), d_arena.as<char>(), num_prefix.as<uint64_t>(), nullptr};
-    uint32_t* ord_in = sort_indices(&stream, number_less, U, sort_a.as<uint32_t>(), sort_b.as<uint32_t>(), sort_ra.as<SortRec>(), sort_rb.as<SortRec>());
-    // the work list of expand_repeats, in the numbering order just found
+    R.order_built = sort_indices(&stream, number_less, U, sort_a.as<uint32_t>(), sort_b.as<uint32_t>(), sort_ra.as<SortRec>(), sort_rb.as<SortRec>());
+}
+
+// The work list of expand_repeats, in the numbering order just found
+void DevicePipeline::Impl::work_list() {
     d_fixed.ensure((size_t)U * 4); ac_memset(d_fixed.p, 0, (size_t)U * 4, &stream);
-    uint8_t* seed_start = d_fixed.as<uint8_t>(); uint8_t* seed_end = seed_start + U; uint8_t* fix_start = seed_end + U; uint8_t* fix_end = fix_start + U;
+    uint8_t* seed_start = d_fixed.as<uint8_t>(); uint8_t* seed_end = seed_start + U; uint8_t* fix_start = R.fix_start = seed_end + U; uint8_t* fix_end = fix_start + U;
     ac_launch("fixed_seed", &stream, FixedSeedBody{d_path_off.as<uint64_t>(), d_path.as<UStrand>(), seed_start, seed_end}, n_seqs);
     ac_copy_dd(fix_start, seed_start, (size_t)U * 2, &stream);
     ac_launch("fixed_spread", &stream, FixedSpreadBody{seed_start, seed_end, d_next_off.as<uint32_t>(), d_next.as<UStrand>(), d_prev_off.as<uint32_t>(), d_prev.as<UStrand>(),
                                                        fix_start, fix_end}, U);
-    const CandidateView cview{ord_in, d_next_off.as<uint32_t>(), d_next.as<UStrand>(), d_prev_off.as<uint32_t>(), d_prev.as<UStrand>(), fix_start, fix_end};
+    const CandidateView cview{R.order_built, d_next_off.as<uint32_t>(), d_next.as<UStrand>(), d_prev_off.as<uint32_t>(), d_prev.as<UStrand>(), fix_start, fix_end};
     cand_flag.ensure((2 * (size_t)U + 1) * 4); cand_index.ensure((2 * (size_t)U + 1) * 4);
     ac_launch("candidate_flag", &stream, CandidateFlagBody{cview, U, cand_flag.as<uint32_t>()}, 2ull * U + 1);
-    const uint64_t n_cands = scan(&stream, cand_flag.as<uint32_t>(), cand_index.as<uint32_t>(), 2ull * U + 1);
+    const uint64_t n_cands = R.n_cands = scan(&stream, cand_flag.as<uint32_t>(), cand_index.as<uint32_t>(), 2ull * U + 1);
     d_cands.ensure((n_cands + 1) * sizeof(ExpandCandidate)); d_cand_at.ensure(2 * (size_t)U * 4 + 4); d_deps.ensure((size_t)U * sizeof(ExpandDeps) + 4); d_spec.ensure((n_cands + 1) * 4);
     ac_launch("candidate_fill", &stream, CandidateFillBody{cview, cand_flag.as<uint32_t>(), cand_index.as<uint32_t>(), d_cands.as<ExpandCandidate>(), d_cand_at.as<int32_t>()}, 2ull * U);
     ac_launch("dependents", &stream, DependentsBody{d_next_off.as<uint32_t>(), d_next.as<UStrand>(), d_prev_off.as<uint32_t>(), d_prev.as<UStrand>(), d_cand_at.as<int32_t>(),
                                                     d_deps.as<ExpandDeps>()}, U);
     ac_launch("common_length", &stream, CommonLengthBody{d_cands.as<ExpandCandidate>(), d_rec.as<UnitigRec>(), d_arena.as<char>(), d_spec.as<uint32_t>()}, n_cands);
-    // ---- simplify_structure and save_gfa on the device: fused builds only (a plain build hands the host the graph as built) ----
-    R = Pending();
-    R.U = U; R.n_links = n_links; R.n_cands = n_cands; R.n_strands = n_strands; R.order_built = ord_in; R.fix_start = fix_start;
-    R.arena_final = arena_bytes; R.arena_src = &d_arena;
-    mark(11);
-    if (fused && n_cands > 0) {
-        d_pred.ensure(n_cands * 7 * 4); d_level.ensure(n_cands * 4); d_flagmax.ensure(32); d_counters64.ensure((AC_PASS_WORDS + 8) * 8);
-        d_dirty.ensure(((n_cands + 63) / 64) * 8 + 8); d_exhausted.ensure(n_cands + 8);
-        unsigned long long* c64 = d_counters64.as<unsigned long long>();         // SimplifyCoopBody's counters, then its eight result words
-        unsigned long long* res = c64 + AC_PASS_WORDS;
-        ac_launch("level_pred", &stream, LevelPredBody{d_cands.as<ExpandCandidate>(), d_deps.as<ExpandDeps>(), d_pred.as<int32_t>()}, n_cands);
-        ac_memset(d_level.p, 0, n_cands * 4, &stream); ac_memset(d_flagmax.p, 0, 32, &stream);
-        ac_launch_coop("levels", &stream, LevelsCoopBody{d_pred.as<int32_t>(), d_level.as<uint32_t>(), d_flagmax.as<uint32_t>(), n_cands}, n_cands, 4096);
-        ac_memset(d_counters64.p, 0, (AC_PASS_WORDS + 8) * 8, &stream);
-        const RelocBoundBody bound_body{d_cands.as<ExpandCandidate>(), d_rec.as<UnitigRec>(), d_cand_at.as<int32_t>(), c64 + AC_PASS_SET(1) + 1};     // the first pass's bound: into the set it does not use
-        ac_launch("reloc_bound", &stream, bound_body, n_cands);
-        uint32_t fm[8]; unsigned long long h64[AC_PASS_WORDS + 8];
-        ac_d2h(fm, d_flagmax.p, 32, &stream); ac_d2h(h64, c64, sizeof h64, &stream); ac_sync(&stream);
-        if (fm[4]) throw std::runtime_error("candidate levels did not settle");
-        unsigned long long bound = 0; for (int x = 0; x < AC_BOUND_STRIPES; ++x) bound += h64[AC_PASS_SET(1) + 1 + x];
-        if (arena_bytes + bound >= 0xFFFFFFF0ull) throw std::runtime_error("unitig sequence arena would exceed 4 GB");
-        // room for the first pass and, usually, for all that follow (each later pass can ask for less than the one before it asked for at most)
-        d_arena2.ensure(arena_bytes + 2 * bound + 64);
-        ac_copy_dd(d_arena2.p, d_arena.p, arena_bytes, &stream);
-        const unsigned long long start = arena_bytes;
-        ac_h2d(c64, &start, 8, &stream);
-        ac_memset(c64 + AC_PASS_SET(1), 0, AC_PASS_SET_WORDS * 8, &stream);
-        ac_memset(d_dirty.p, 0, ((n_cands + 63) / 64) * 8 + 8, &stream); ac_memset(d_exhausted.p, 0, n_cands + 8, &stream);
-        // `while expand_repeats() > 0 {}`: one launch for as many passes as the arena has room for
-        static const bool always_grow = getenv("AC_DEVICE_TIGHT_ARENA") != nullptr;   // test hook: one pass per launch, the growth path before every pass
-        uint32_t next_set = 0, next_due = 0; uint64_t passes = 0;
-        const uint32_t due_stride = fm[3] + 2;
-        d_due.ensure((size_t)3 * due_stride * 4); ac_memset(d_due.p, 0, (size_t)3 * due_stride * 4, &stream);
-        for (bool first = true;; first = false) {
-            const ApplyLevelBody apply{d_cands.as<ExpandCandidate>(), d_deps.as<ExpandDeps>(), d_level.as<uint32_t>(), 0, d_spec.as<uint32_t>(),
-                                       d_rec.as<UnitigRec>(), d_arena2.as<char>(), c64, c64, d_dirty.as<uint64_t>(), d_exhausted.as<uint8_t>(), first, c64 + AC_PASS_REMOVED};
-            const uint64_t room = always_grow ? 0 : d_arena2.cap;
-            ac_launch_coop("simplify", &stream, SimplifyCoopBody{apply, bound_body, n_cands, d_flagmax.as<uint32_t>() + 3, c64, res, room, next_set, first,
-                                                                 d_due.as<uint32_t>(), due_stride, next_due}, n_cands, 64);
-            ac_d2h(h64, c64, sizeof h64, &stream); ac_sync(&stream);
-            const unsigned long long* r = h64 + AC_PASS_WORDS;
-            R.arena_final = h64[0]; R.bases_removed = h64[AC_PASS_REMOVED]; R.any_moved = r[1] != 0;
-            passes += r[2]; next_set = (uint32_t)r[5]; next_due = (uint32_t)r[7];
-            if (getenv("AC_HOST_PROFILE")) fprintf(stderr, "[device] expand_repeats launch: %llu passes (%llu so far), %u levels, %llu candidates, %llu left on the work list, last pass moved %llu bases\n",
-                                                   r[2], (unsigned long long)passes, fm[3], (unsigned long long)n_cands, r[4], r[0]);
-            if (r[0] == 0) break;                                                          // the last expand_repeats() call moved nothing
-            if (passes > 1000000) throw std::runtime_error("repeat expansion did not settle");
-            bound = r[3];                                                                  // the launch stopped for want of room: make it
-            if (R.arena_final + bound >= 0xFFFFFFF0ull) throw std::runtime_error("unitig sequence arena would exceed 4 GB");
-            d_arena3.ensure(std::max<size_t>((R.arena_final + bound) * 2 + 64, d_arena3.cap + (always_grow ? 64 : 0)));
-            ac_copy_dd(d_arena3.p, d_arena2.p, R.arena_final, &stream); ac_sync(&stream);
-            std::swap(d_arena2.p, d_arena3.p); std::swap(d_arena2.cap, d_arena3.cap);
-        }
-        R.arena_src = &d_arena2;
-    }
-    mark(17);
-    if (fused) {      // simplify_structure ends with renumber_unitigs (:38): stable with respect to the numbering the passes ran in
-        if (R.any_moved) {
-            d_pos.ensure((size_t)U * 4); sort_c.ensure((size_t)U * 4); sort_d.ensure((size_t)U * 4);
-            ac_launch("inverse_perm", &stream, InversePermBody{ord_in, d_pos.as<uint32_t>()}, U);
-            ac_launch("number_key", &stream, NumberKeyBody{d_rec.as<UnitigRec>(), R.arena_src->as<char>(), num_prefix.as<uint64_t>()}, U);
-            const NumberLess final_less{d_rec.as<UnitigRec>(), d_depth.as<uint32_t>(), R.arena_src->as<char>(), num_prefix.as<uint64_t>(), d_pos.as<uint32_t>()};
-            R.final_order = sort_indices(&stream, final_less, U, sort_c.as<uint32_t>(), sort_d.as<uint32_t>(), sort_ra.as<SortRec>(), sort_rb.as<SortRec>());
-        } else R.final_order = ord_in;     // nothing moved: the stable sort would change nothing
-        if (U < 100000000u) {          // save_gfa (unitig_graph.rs:317-360): H, S, L and P lines rendered here
-            uint32_t* fin = R.final_order;
-            d_pos2.ensure((size_t)U * 4);
-            ac_launch("inverse_perm", &stream, InversePermBody{fin, d_pos2.as<uint32_t>()}, U);
-            const GfaView gv{fin, d_pos2.as<uint32_t>(), d_rec.as<UnitigRec>(), R.arena_src->as<char>(), d_depth.as<uint32_t>(), d_next_off.as<uint32_t>(), d_next.as<UStrand>()};
-            gfa_s_size.ensure(((size_t)U + 1) * 4); gfa_l_size.ensure(((size_t)U + 1) * 4); gfa_pieces.ensure(((size_t)U + 1) * 4);
-            const uint64_t steps = split_paths ? 0 : n_runs;     // split_paths: the P lines are printed by the ranks that own the sequences (render_path_lines)
-            d_last.ensure(steps + 8); gfa_p_size.ensure((steps + 1) * 4);
-            ac_launch("gfa_size", &stream, GfaSizeBody{gv, U, gfa_s_size.as<uint32_t>(), gfa_l_size.as<uint32_t>()}, (uint64_t)U + 1);
-            ac_launch("gfa_chunk_count", &stream, GfaChunkCountBody{gv, U, gfa_pieces.as<uint32_t>()}, (uint64_t)U + 1);
-            // the scans, their totals read back together (one round trip)
-            d_totals.ensure(64); ac_memset(d_totals.p, 0, 64, &stream);
-            if (!split_paths) {
-                ac_memset(d_last.p, 0, steps + 8, &stream);
-                ac_launch("path_last", &stream, PathLastBody{d_path_off.as<uint64_t>(), d_last.as<uint8_t>()}, n_seqs);
-                ac_launch("path_size", &stream, PathSizeBody{d_path.as<UStrand>(), d_pos2.as<uint32_t>(), d_last.as<uint8_t>(), steps, gfa_p_size.as<uint32_t>()}, steps + 1);
-                scan.keep_total(&stream, gfa_p_size.as<uint32_t>(), steps + 1, d_totals.as<uint32_t>() + 3);
-            }
-            scan.keep_total(&stream, gfa_s_size.as<uint32_t>(), (uint64_t)U + 1, d_totals.as<uint32_t>() + 0);
-            scan.keep_total(&stream, gfa_l_size.as<uint32_t>(), (uint64_t)U + 1, d_totals.as<uint32_t>() + 1);
-            scan.keep_total(&stream, gfa_pieces.as<uint32_t>(), (uint64_t)U + 1, d_totals.as<uint32_t>() + 2);
-            uint32_t tot[4];
-            ac_d2h(tot, d_totals.p, 16, &stream); ac_sync(&stream);
-            const uint64_t s_bytes = tot[0], l_bytes = tot[1], n_pieces = tot[2], p_list_bytes = tot[3];
-            char head[64]; const uint64_t head_bytes = (uint64_t)snprintf(head, sizeof head, "H\tVN:Z:1.0\tKM:i:%u\n", k);
-            if (path_wrap_total == 0 && n_seqs) throw std::runtime_error("set_path_line_texts() must precede a build that renders the GFA");
-            const uint64_t p_bytes = split_paths ? 0 : p_list_bytes + path_wrap_total;
-            R.gfa_bytes = head_bytes + s_bytes + l_bytes + p_bytes;
-            d_text.ensure(R.gfa_bytes + 64);
-            char* text = d_text.as<char>();
-            ac_h2d(text, head, head_bytes, &stream);       // `head` is on the stack: synchronised below before it goes out of scope (h2d from pageable memory is staged by the driver at call time)
-            ac_launch("gfa_segment", &stream, GfaSegmentBody{gv, gfa_s_size.as<uint32_t>(), text + head_bytes}, U);
-            ac_launch("gfa_sequence", &stream, GfaSequenceBody{gv, U, gfa_pieces.as<uint32_t>(), gfa_s_size.as<uint32_t>(), text + head_bytes}, n_pieces);
-            ac_launch("gfa_link", &stream, GfaLinkBody{gv, gfa_l_size.as<uint32_t>(), text + head_bytes + s_bytes}, U);
-            const PathLineView pv{d_path_off.as<uint64_t>(), n_seqs, gfa_p_size.as<uint32_t>(), d_wrap_off.as<uint64_t>(), d_pre_len.as<uint32_t>(), d_suf_len.as<uint32_t>(),
-                                  d_blob.as<char>(), d_blob_off.as<uint64_t>(), 0};
-            char* p_text = text + head_bytes + s_bytes + l_bytes;
-            if (!split_paths) {
-                ac_launch("path_text", &stream, PathTextFullBody{d_path.as<UStrand>(), d_pos2.as<uint32_t>(), d_last.as<uint8_t>(), pv, p_text}, steps);
-                ac_launch("path_wrap", &stream, PathWrapBody{pv, p_text}, 2ull * n_seqs);
-            }
-            R.paths_split = split_paths;
-            R.gfa_on_device = true;
-        }
-    }
-    mark(18);
-    R.hairpins_ready = true;
+    mark(WORK_LIST_END);
+}
 
-    // ---- results to the host (pinned) ----
+// simplify_structure's repeat expansion: `while expand_repeats() > 0 {}`
+void DevicePipeline::Impl::simplify() {
+    const uint64_t n_cands = R.n_cands, arena_bytes = R.arena_final;
+    d_pred.ensure(n_cands * 7 * 4); d_level.ensure(n_cands * 4); d_flagmax.ensure(32); d_counters64.ensure((AC_PASS_WORDS + 8) * 8);
+    d_dirty.ensure(((n_cands + 63) / 64) * 8 + 8); d_exhausted.ensure(n_cands + 8);
+    unsigned long long* c64 = d_counters64.as<unsigned long long>();         // SimplifyCoopBody's counters, then its eight result words
+    unsigned long long* res = c64 + AC_PASS_WORDS;
+    ac_launch("level_pred", &stream, LevelPredBody{d_cands.as<ExpandCandidate>(), d_deps.as<ExpandDeps>(), d_pred.as<int32_t>()}, n_cands);
+    ac_memset(d_level.p, 0, n_cands * 4, &stream); ac_memset(d_flagmax.p, 0, 32, &stream);
+    ac_launch_coop("levels", &stream, LevelsCoopBody{d_pred.as<int32_t>(), d_level.as<uint32_t>(), d_flagmax.as<uint32_t>(), n_cands}, n_cands, 4096);
+    ac_memset(d_counters64.p, 0, (AC_PASS_WORDS + 8) * 8, &stream);
+    const RelocBoundBody bound_body{d_cands.as<ExpandCandidate>(), d_rec.as<UnitigRec>(), d_cand_at.as<int32_t>(), c64 + AC_PASS_SET(1) + 1};     // the first pass's bound: into the set it does not use
+    ac_launch("reloc_bound", &stream, bound_body, n_cands);
+    uint32_t fm[8]; unsigned long long h64[AC_PASS_WORDS + 8];
+    ac_d2h(fm, d_flagmax.p, 32, &stream); ac_d2h(h64, c64, sizeof h64, &stream); ac_sync(&stream);
+    if (fm[4]) throw std::runtime_error("candidate levels did not settle");
+    unsigned long long bound = 0; for (int x = 0; x < AC_BOUND_STRIPES; ++x) bound += h64[AC_PASS_SET(1) + 1 + x];
+    if (arena_bytes + bound >= 0xFFFFFFF0ull) throw std::runtime_error("unitig sequence arena would exceed 4 GB");
+    // room for the first pass and, usually, for all that follow (each later pass can ask for less than the one before it asked for at most)
+    d_arena2.ensure(arena_bytes + 2 * bound + 64);
+    ac_copy_dd(d_arena2.p, d_arena.p, arena_bytes, &stream);
+    const unsigned long long start = arena_bytes;
+    ac_h2d(c64, &start, 8, &stream);
+    ac_memset(c64 + AC_PASS_SET(1), 0, AC_PASS_SET_WORDS * 8, &stream);
+    ac_memset(d_dirty.p, 0, ((n_cands + 63) / 64) * 8 + 8, &stream); ac_memset(d_exhausted.p, 0, n_cands + 8, &stream);
+    // one launch for as many passes as the arena has room for
+    static const bool always_grow = getenv("AC_DEVICE_TIGHT_ARENA") != nullptr;   // test hook: one pass per launch, the growth path before every pass
+    uint32_t next_set = 0, next_due = 0; uint64_t passes = 0;
+    const uint32_t due_stride = fm[3] + 2;
+    d_due.ensure((size_t)3 * due_stride * 4); ac_memset(d_due.p, 0, (size_t)3 * due_stride * 4, &stream);
+    for (bool first = true;; first = false) {
+        const ApplyLevelBody apply{d_cands.as<ExpandCandidate>(), d_deps.as<ExpandDeps>(), d_level.as<uint32_t>(), 0, d_spec.as<uint32_t>(),
+                                   d_rec.as<UnitigRec>(), d_arena2.as<char>(), c64, c64, d_dirty.as<uint64_t>(), d_exhausted.as<uint8_t>(), first, c64 + AC_PASS_REMOVED};
+        const uint64_t room = always_grow ? 0 : d_arena2.cap;
+        ac_launch_coop("simplify", &stream, SimplifyCoopBody{apply, bound_body, n_cands, d_flagmax.as<uint32_t>() + 3, c64, res, room, next_set, first,
+                                                             d_due.as<uint32_t>(), due_stride, next_due}, n_cands, 64);
+        ac_d2h(h64, c64, sizeof h64, &stream); ac_sync(&stream);
+        const unsigned long long* r = h64 + AC_PASS_WORDS;
+        R.arena_final = h64[0]; R.bases_removed = h64[AC_PASS_REMOVED]; R.any_moved = r[1] != 0;
+        passes += r[2]; next_set = (uint32_t)r[5]; next_due = (uint32_t)r[7];
+        if (getenv("AC_HOST_PROFILE")) fprintf(stderr, "[device] expand_repeats launch: %llu passes (%llu so far), %u levels, %llu candidates, %llu left on the work list, last pass moved %llu bases\n",
+                                               r[2], (unsigned long long)passes, fm[3], (unsigned long long)n_cands, r[4], r[0]);
+        if (r[0] == 0) break;                                                          // the last expand_repeats() call moved nothing
+        if (passes > 1000000) throw std::runtime_error("repeat expansion did not settle");
+        bound = r[3];                                                                  // the launch stopped for want of room: make it
+        if (R.arena_final + bound >= 0xFFFFFFF0ull) throw std::runtime_error("unitig sequence arena would exceed 4 GB");
+        d_arena3.ensure(std::max<size_t>((R.arena_final + bound) * 2 + 64, d_arena3.cap + (always_grow ? 64 : 0)));
+        ac_copy_dd(d_arena3.p, d_arena2.p, R.arena_final, &stream); ac_sync(&stream);
+        std::swap(d_arena2.p, d_arena3.p); std::swap(d_arena2.cap, d_arena3.cap);
+    }
+    R.arena_src = &d_arena2;
+}
+
+// simplify_structure ends with renumber_unitigs (:38): stable with respect to the numbering the passes ran in
+void DevicePipeline::Impl::renumber() {
+    if (!R.any_moved) { R.final_order = R.order_built; return; }     // nothing moved: the stable sort would change nothing
+    d_pos.ensure((size_t)U * 4); sort_c.ensure((size_t)U * 4); sort_d.ensure((size_t)U * 4);
+    ac_launch("inverse_perm", &stream, InversePermBody{R.order_built, d_pos.as<uint32_t>()}, U);
+    ac_launch("number_key", &stream, NumberKeyBody{d_rec.as<UnitigRec>(), R.arena_src->as<char>(), num_prefix.as<uint64_t>()}, U);
+    const NumberLess final_less{d_rec.as<UnitigRec>(), d_depth.as<uint32_t>(), R.arena_src->as<char>(), num_prefix.as<uint64_t>(), d_pos.as<uint32_t>()};
+    R.final_order = sort_indices(&stream, final_less, U, sort_c.as<uint32_t>(), sort_d.as<uint32_t>(), sort_ra.as<SortRec>(), sort_rb.as<SortRec>());
+}
+
+// save_gfa (unitig_graph.rs:317-360): H, S, L and P lines rendered here.  split_paths: the P lines are printed by the ranks that own the
+// sequences (render_path_lines).
+void DevicePipeline::Impl::gfa(bool split_paths) {
+    d_pos2.ensure((size_t)U * 4);
+    ac_launch("inverse_perm", &stream, InversePermBody{R.final_order, d_pos2.as<uint32_t>()}, U);
+    const GfaView gv{R.final_order, d_pos2.as<uint32_t>(), d_rec.as<UnitigRec>(), R.arena_src->as<char>(), d_depth.as<uint32_t>(), d_next_off.as<uint32_t>(), d_next.as<UStrand>()};
+    gfa_s_size.ensure(((size_t)U + 1) * 4); gfa_l_size.ensure(((size_t)U + 1) * 4); gfa_pieces.ensure(((size_t)U + 1) * 4);
+    const uint64_t steps = split_paths ? 0 : n_runs;
+    d_last.ensure(steps + 8); gfa_p_size.ensure((steps + 1) * 4);
+    ac_launch("gfa_size", &stream, GfaSizeBody{gv, U, gfa_s_size.as<uint32_t>(), gfa_l_size.as<uint32_t>()}, (uint64_t)U + 1);
+    ac_launch("gfa_chunk_count", &stream, GfaChunkCountBody{gv, U, gfa_pieces.as<uint32_t>()}, (uint64_t)U + 1);
+    // the scans, their totals read back together (one round trip)
+    d_totals.ensure(64); ac_memset(d_totals.p, 0, 64, &stream);
+    if (!split_paths) {
+        ac_memset(d_last.p, 0, steps + 8, &stream);
+        ac_launch("path_last", &stream, PathLastBody{d_path_off.as<uint64_t>(), d_last.as<uint8_t>()}, n_seqs);
+        ac_launch("path_size", &stream, PathSizeBody{d_path.as<UStrand>(), d_pos2.as<uint32_t>(), d_last.as<uint8_t>(), steps, gfa_p_size.as<uint32_t>()}, steps + 1);
+        scan.keep_total(&stream, gfa_p_size.as<uint32_t>(), steps + 1, d_totals.as<uint32_t>() + 3);
+    }
+    scan.keep_total(&stream, gfa_s_size.as<uint32_t>(), (uint64_t)U + 1, d_totals.as<uint32_t>() + 0);
+    scan.keep_total(&stream, gfa_l_size.as<uint32_t>(), (uint64_t)U + 1, d_totals.as<uint32_t>() + 1);
+    scan.keep_total(&stream, gfa_pieces.as<uint32_t>(), (uint64_t)U + 1, d_totals.as<uint32_t>() + 2);
+    uint32_t tot[4];
+    ac_d2h(tot, d_totals.p, 16, &stream); ac_sync(&stream);
+    const uint64_t s_bytes = tot[0], l_bytes = tot[1], n_pieces = tot[2], p_list_bytes = tot[3];
+    char head[64]; const uint64_t head_bytes = (uint64_t)snprintf(head, sizeof head, "H\tVN:Z:1.0\tKM:i:%u\n", k);
+    if (path_wrap_total == 0 && n_seqs) throw std::runtime_error("set_path_line_texts() must precede a build that renders the GFA");
+    const uint64_t p_bytes = split_paths ? 0 : p_list_bytes + path_wrap_total;
+    R.gfa_bytes = head_bytes + s_bytes + l_bytes + p_bytes;
+    d_text.ensure(R.gfa_bytes + 64);
+    char* text = d_text.as<char>();
+    ac_h2d(text, head, head_bytes, &stream);       // `head` is on the stack: synchronised below before it goes out of scope (h2d from pageable memory is staged by the driver at call time)
+    ac_launch("gfa_segment", &stream, GfaSegmentBody{gv, gfa_s_size.as<uint32_t>(), text + head_bytes}, U);
+    ac_launch("gfa_sequence", &stream, GfaSequenceBody{gv, U, gfa_pieces.as<uint32_t>(), gfa_s_size.as<uint32_t>(), text + head_bytes}, n_pieces);
+    ac_launch("gfa_link", &stream, GfaLinkBody{gv, gfa_l_size.as<uint32_t>(), text + head_bytes + s_bytes}, U);
+    const PathLineView pv{d_path_off.as<uint64_t>(), n_seqs, gfa_p_size.as<uint32_t>(), d_wrap_off.as<uint64_t>(), d_pre_len.as<uint32_t>(), d_suf_len.as<uint32_t>(),
+                          d_blob.as<char>(), d_blob_off.as<uint64_t>(), 0};
+    char* p_text = text + head_bytes + s_bytes + l_bytes;
+    if (!split_paths) {
+        ac_launch("path_text", &stream, PathTextFullBody{d_path.as<UStrand>(), d_pos2.as<uint32_t>(), d_last.as<uint8_t>(), pv, p_text}, steps);
+        ac_launch("path_wrap", &stream, PathWrapBody{pv, p_text}, 2ull * n_seqs);
+    }
+    R.paths_split = split_paths;
+    R.gfa_on_device = true;
+}
+
+// ---- results to the host (pinned) ----
+void DevicePipeline::Impl::results(PipelineResult& out, bool keep_positions, bool fused) {
     if (before_results && *before_results) (*before_results)();
     out.fused = fused; out.graph_fetched = false;
     if (fused && !R.gfa_on_device) throw std::runtime_error("fused build: the device GFA writer did not run");
@@ -2397,22 +2414,21 @@ template <int W> void DevicePipeline::Impl::finish_w(PipelineResult& out, bool k
     }
     uint32_t small[16];
     ac_d2h(small, d_small.p, 64, &stream); ac_sync(&stream); d2h += 64;
-    out.links_single = (n_links - small[0]) / 2 + small[0];
+    out.links_single = (R.n_links - small[0]) / 2 + small[0];
     out.length_before = n_slots_used;                      // every canonical k-mer lies in exactly one unitig and a trimmed unitig is as long as its chain
     out.length_after = n_slots_used - R.bases_removed;
     out.gfa_text = R.gfa_on_device ? h_text.as<char>() : nullptr; out.gfa_bytes = R.gfa_on_device ? R.gfa_bytes : 0;
-    out.n_unitigs = U; out.n_runs = n_runs; out.n_seqs = n_seqs; out.n_links = n_links;
+    out.n_unitigs = U; out.n_runs = n_runs; out.n_seqs = n_seqs; out.n_links = R.n_links;
     out.h2d_bytes = uploaded_bytes + (uint64_t)n_seqs * sizeof(SeqInfo);
     out.d2h_bytes = d2h;
-    pending_keep_positions = keep_positions;
     if (!fused) pull_graph(out, keep_positions);
-    else { mark(16); mark(12); arena_pending = true; }
+    else { mark(ALL_BUT_ARENA); mark(RESULTS_END); arena_pending = true; }
 }
 
 // The graph arrays (unitig records, sequences, links, paths, and the numbering and expand_repeats work list of the graph as built, or
 // the final numbering after a fused build) into pinned host memory: at once in a plain build, on request after a fused one.
 void DevicePipeline::Impl::pull_graph(PipelineResult& out, bool keep_positions) {
-    const uint32_t U = R.U; const uint64_t n_links = R.n_links, n_cands = R.n_cands; const uint32_t n_strands = R.n_strands;
+    const uint64_t n_links = R.n_links, n_cands = R.n_cands; const uint32_t n_strands = 2 * U;
     const uint64_t arena_cap = R.arena_final + R.arena_final / 4 + (1u << 20);     // head room for relocations during repeat expansion
     h_rec.ensure((size_t)U * sizeof(UnitigRec)); h_depth.ensure((size_t)U * 4);
     h_arena.ensure(arena_cap); h_next_off.ensure(((size_t)n_strands + 1) * 4); h_prev_off.ensure(((size_t)n_strands + 1) * 4);
@@ -2435,11 +2451,11 @@ void DevicePipeline::Impl::pull_graph(PipelineResult& out, bool keep_positions) 
     } else { h_order2.ensure((size_t)U * 4 + 4); if (U) { ac_d2h(h_order2.p, R.final_order, (size_t)U * 4, &stream); d2h += (size_t)U * 4; } }
     // The sequences (most of the bytes) go last: the caller gets the graph structure as soon as everything else has
     // landed and lists the repeat-expansion candidates while the arena is still on its way (complete() waits for it).
-    mark(16);
+    mark(ALL_BUT_ARENA);
     pull(h_arena, *R.arena_src, R.arena_final);
     out.d2h_bytes += d2h;
-    mark(12);
-    wait_mark(16);
+    mark(RESULTS_END);
+    wait_mark(ALL_BUT_ARENA);
     out.graph_fetched = true;
     out.rec = h_rec.as<UnitigRec>(); out.depth = h_depth.as<uint32_t>();
     out.order = plain ? h_order.as<uint32_t>() : nullptr; out.final_order = plain ? nullptr : h_order2.as<uint32_t>();
@@ -2453,65 +2469,62 @@ void DevicePipeline::Impl::pull_graph(PipelineResult& out, bool keep_positions) 
     arena_pending = true;
 }
 
-void DevicePipeline::Impl::do_complete(PipelineResult& out) {
-    if (!arena_pending) return;
-    ac_sync(&stream);
-    arena_pending = false;
-    out.t.h2d = between(0, 1); out.t.pack = between(2, 3); out.t.insert = between(15, 4); out.t.insert_kernel = between(20, 21); out.t.sample = between(3, 15); out.t.adjacency = between(13, 5);
-    out.t.boundaries = between(5, 6); out.t.runs = between(14, 7); out.t.unitigs = between(7, 8); out.t.links = between(8, 9);
-    out.t.seed_sort = between(9, 10); out.t.emit = between(10, 11); out.t.simplify = between(11, 17); out.t.gfa = between(17, 18);
-    out.t.d2h = between(18, 12); out.t.total = between(2, 4) + between(13, 6) + between(14, 12);
+void DevicePipeline::complete(PipelineResult& out) {
+    Impl& m = *impl; m.make_current();
+    if (!m.arena_pending) return;
+    ac_sync(&m.stream);
+    m.arena_pending = false;
+    PipelineTimings& t = out.t;
+    const struct { float* field; Mark from, to; } spans[] = {
+        {&t.h2d, UPLOAD_BEGIN, UPLOAD_END}, {&t.pack, PACK_BEGIN, PACK_END}, {&t.sample, PACK_END, SAMPLE_END}, {&t.insert, SAMPLE_END, TABLE_END},
+        {&t.insert_kernel, INSERT_BEGIN, INSERT_END}, {&t.adjacency, RUNS_BEGIN, ADJACENCY_END}, {&t.boundaries, ADJACENCY_END, BOUNDARIES_END},
+        {&t.runs, FINISH_BEGIN, UNITIGS_END}, {&t.unitigs, UNITIGS_END, SEEDS_END}, {&t.links, SEEDS_END, LINKS_END}, {&t.seed_sort, LINKS_END, SEED_SORT_END},
+        {&t.emit, SEED_SORT_END, WORK_LIST_END}, {&t.simplify, WORK_LIST_END, SIMPLIFY_END}, {&t.gfa, SIMPLIFY_END, GFA_END}, {&t.d2h, GFA_END, RESULTS_END}};
+    for (const auto& s : spans) *s.field = m.between(s.from, s.to);
+    t.total = m.between(PACK_BEGIN, TABLE_END) + m.between(RUNS_BEGIN, BOUNDARIES_END) + m.between(FINISH_BEGIN, RESULTS_END);
 }
 
 // ---- multi-GPU, path lines by owner (DESIGN.md §7): the rank that finished the graph hands every occurrence's final "<number><sign>" to
 // the rank that owns the sequence; every rank prints the P lines of its own sequences and copies them out through its own PCIe link ----
-void DevicePipeline::Impl::do_export_path_tokens(void* dst, uint64_t stride, const uint64_t* counts, uint32_t n_ranks) {
-    if (stage < 2 || !R.gfa_on_device || !R.paths_split) throw std::runtime_error("export_path_tokens follows a finish with split path lines");
+void DevicePipeline::export_path_tokens(void* dst, uint64_t stride, const uint64_t* counts, uint32_t n_ranks) {
+    Impl& m = *impl; m.make_current();
+    if (m.stage < Stage::RUNS || !m.R.gfa_on_device || !m.R.paths_split) throw std::runtime_error("export_path_tokens follows a finish with split path lines");
     if (n_ranks == 0 || n_ranks > AC_MAX_RANKS) throw std::runtime_error("export_path_tokens: bad rank count");
-    PathTokenBody body{d_path.as<UStrand>(), d_pos2.as<uint32_t>(), (uint32_t*)dst, stride, n_ranks, {0}};
+    PathTokenBody body{m.d_path.as<UStrand>(), m.d_pos2.as<uint32_t>(), (uint32_t*)dst, stride, n_ranks, {0}};
     for (uint32_t q = 0; q < n_ranks; ++q) { if (counts[q] > stride) throw std::runtime_error("export_path_tokens: a rank holds more occurrences than the stride"); body.first[q + 1] = body.first[q] + counts[q]; }
-    if (body.first[n_ranks] != n_runs) throw std::runtime_error("export_path_tokens: the counts do not add up to the occurrences imported");
-    ac_launch("path_tokens", &stream, body, n_runs);
+    if (body.first[n_ranks] != m.n_runs) throw std::runtime_error("export_path_tokens: the counts do not add up to the occurrences imported");
+    ac_launch("path_tokens", &m.stream, body, m.n_runs);
 }
-void DevicePipeline::Impl::do_render_path_lines(const void* tokens, uint64_t n_tokens, const char** text, uint64_t* bytes) {
-    if (stage < 2) throw std::runtime_error("runs_local must precede render_path_lines");
-    if (n_tokens != n_own_runs) throw std::runtime_error("render_path_lines: one token per occurrence of this rank's sequences is expected");
-    if (path_pre.size() != n_seqs) throw std::runtime_error("set_path_line_texts() must precede render_path_lines");
-    const uint32_t n_own = own_seq_hi - own_seq_lo;
+void DevicePipeline::render_path_lines(const void* tokens, uint64_t n_tokens, const char** text, uint64_t* bytes) {
+    Impl& m = *impl; m.make_current();
+    m.require(Stage::RUNS, "runs_local must precede render_path_lines");
+    if (n_tokens != m.n_own_runs) throw std::runtime_error("render_path_lines: one token per occurrence of this rank's sequences is expected");
+    if (m.path_pre.size() != m.n_seqs) throw std::runtime_error("set_path_line_texts() must precede render_path_lines");
+    const uint32_t lo = m.own_seq_lo, hi = m.own_seq_hi, n_own = hi - lo;
     uint64_t wrap_lo = 0, wrap_hi = 0;
-    for (uint32_t i = 0; i < own_seq_hi; ++i) { if (i == own_seq_lo) wrap_lo = wrap_hi; wrap_hi += (uint64_t)path_pre[i] + path_suf[i]; }
-    if (own_seq_lo == own_seq_hi) wrap_lo = wrap_hi;
-    mark(19);
+    for (uint32_t i = 0; i < hi; ++i) { const uint64_t b = (uint64_t)m.path_pre[i] + m.path_suf[i]; wrap_hi += b; if (i < lo) wrap_lo += b; }
     uint64_t total_bytes = 0;
     if (n_own) {
         const uint64_t steps = n_tokens;
-        d_own_off.ensure(((size_t)n_own + 1) * 8); d_own_last.ensure(steps + 8); d_own_size.ensure((steps + 1) * 4);
+        m.d_own_off.ensure(((size_t)n_own + 1) * 8); m.d_own_last.ensure(steps + 8); m.d_own_size.ensure((steps + 1) * 4);
         // this rank's occurrences are the first n_own_runs entries of run_start (the finishing rank imported its own block first)
-        ac_launch("path_off", &stream, PathOffBody{seqs.as<SeqInfo>() + own_seq_lo, n_own, run_start.as<uint64_t>(), steps, d_own_off.as<uint64_t>()}, (uint64_t)n_own + 1);
-        ac_memset(d_own_last.p, 0, steps + 8, &stream);
-        ac_launch("path_last", &stream, PathLastBody{d_own_off.as<uint64_t>(), d_own_last.as<uint8_t>()}, n_own);
-        ac_launch("path_size", &stream, PathSizeBody{(const UStrand*)tokens, nullptr, d_own_last.as<uint8_t>(), steps, d_own_size.as<uint32_t>()}, steps + 1);
-        const uint64_t list_bytes = scan(&stream, d_own_size.as<uint32_t>(), d_own_size.as<uint32_t>(), steps + 1);
+        ac_launch("path_off", &m.stream, PathOffBody{m.seqs.as<SeqInfo>() + lo, n_own, m.run_start.as<uint64_t>(), steps, m.d_own_off.as<uint64_t>()}, (uint64_t)n_own + 1);
+        ac_memset(m.d_own_last.p, 0, steps + 8, &m.stream);
+        ac_launch("path_last", &m.stream, PathLastBody{m.d_own_off.as<uint64_t>(), m.d_own_last.as<uint8_t>()}, n_own);
+        ac_launch("path_size", &m.stream, PathSizeBody{(const UStrand*)tokens, nullptr, m.d_own_last.as<uint8_t>(), steps, m.d_own_size.as<uint32_t>()}, steps + 1);
+        const uint64_t list_bytes = m.scan(&m.stream, m.d_own_size.as<uint32_t>(), m.d_own_size.as<uint32_t>(), steps + 1);
         total_bytes = list_bytes + (wrap_hi - wrap_lo);
-        d_ptext.ensure(total_bytes + 64);
-        const PathLineView pv{d_own_off.as<uint64_t>(), n_own, d_own_size.as<uint32_t>(), d_wrap_off.as<uint64_t>() + own_seq_lo, d_pre_len.as<uint32_t>() + own_seq_lo,
-                              d_suf_len.as<uint32_t>() + own_seq_lo, d_blob.as<char>(), d_blob_off.as<uint64_t>() + own_seq_lo, wrap_lo};
-        ac_launch("path_text", &stream, PathTextFullBody{(const UStrand*)tokens, nullptr, d_own_last.as<uint8_t>(), pv, d_ptext.as<char>()}, steps);
-        ac_launch("path_wrap", &stream, PathWrapBody{pv, d_ptext.as<char>()}, 2ull * n_own);
-        h_ptext.ensure(total_bytes + 64);
-        ac_d2h(h_ptext.p, d_ptext.p, total_bytes, &stream);
+        m.d_ptext.ensure(total_bytes + 64);
+        const PathLineView pv{m.d_own_off.as<uint64_t>(), n_own, m.d_own_size.as<uint32_t>(), m.d_wrap_off.as<uint64_t>() + lo, m.d_pre_len.as<uint32_t>() + lo,
+                              m.d_suf_len.as<uint32_t>() + lo, m.d_blob.as<char>(), m.d_blob_off.as<uint64_t>() + lo, wrap_lo};
+        ac_launch("path_text", &m.stream, PathTextFullBody{(const UStrand*)tokens, nullptr, m.d_own_last.as<uint8_t>(), pv, m.d_ptext.as<char>()}, steps);
+        ac_launch("path_wrap", &m.stream, PathWrapBody{pv, m.d_ptext.as<char>()}, 2ull * n_own);
+        m.h_ptext.ensure(total_bytes + 64);
+        ac_d2h(m.h_ptext.p, m.d_ptext.p, total_bytes, &m.stream);
     }
-    ac_sync(&stream);
-    path_lines_d2h = total_bytes;
-    *text = total_bytes ? h_ptext.as<char>() : nullptr; *bytes = total_bytes;
+    ac_sync(&m.stream);
+    *text = total_bytes ? m.h_ptext.as<char>() : nullptr; *bytes = total_bytes;
 }
-
-// One instantiation of every k-mer kernel per key width: W = ceil(2k / 64) words, k up to 511.
-#define AC_W_CASE(fn, n, ...) case n: fn<n>(__VA_ARGS__); break;
-#define AC_DISPATCH_W(fn, ...) switch (W) { AC_W_CASE(fn, 1, __VA_ARGS__) AC_W_CASE(fn, 2, __VA_ARGS__) AC_W_CASE(fn, 3, __VA_ARGS__) AC_W_CASE(fn, 4, __VA_ARGS__) \
-    AC_W_CASE(fn, 5, __VA_ARGS__) AC_W_CASE(fn, 6, __VA_ARGS__) AC_W_CASE(fn, 7, __VA_ARGS__) AC_W_CASE(fn, 8, __VA_ARGS__) AC_W_CASE(fn, 9, __VA_ARGS__) AC_W_CASE(fn, 10, __VA_ARGS__) \
-    AC_W_CASE(fn, 11, __VA_ARGS__) AC_W_CASE(fn, 12, __VA_ARGS__) AC_W_CASE(fn, 13, __VA_ARGS__) AC_W_CASE(fn, 14, __VA_ARGS__) AC_W_CASE(fn, 15, __VA_ARGS__) AC_W_CASE(fn, 16, __VA_ARGS__) \
-    default: throw std::runtime_error("upload() must precede build()"); }
 
 void DevicePipeline::build_local(uint32_t seq_lo, uint32_t seq_hi, bool multi) {
     Impl& m = *impl; m.make_current(); const int W = m.W;
@@ -2520,10 +2533,9 @@ void DevicePipeline::build_local(uint32_t seq_lo, uint32_t seq_hi, bool multi) {
 uint64_t DevicePipeline::count_entries() {
     Impl& m = *impl; m.make_current(); const int W = m.W;
     uint64_t count = 0;
-    AC_DISPATCH_W(count = m.do_count_entries)
+    AC_DISPATCH_W(count = m.count_entries_w)
     return count;
 }
-void DevicePipeline::export_entries(void* dst, uint64_t cap_records) { impl->make_current(); impl->do_export_entries(dst, cap_records); }
 void DevicePipeline::merge_entries(const void* dev_ptr, uint64_t n) {
     Impl& m = *impl; m.make_current(); const int W = m.W;
     AC_DISPATCH_W(m.merge_w, dev_ptr, n)
@@ -2533,28 +2545,23 @@ void DevicePipeline::runs_local() {
     AC_DISPATCH_W(m.runs_local_w)
 }
 uint64_t DevicePipeline::local_runs() const { return impl->n_runs; }
-void DevicePipeline::export_runs(void* dst, uint64_t cap_records) { impl->make_current(); impl->do_export_runs(dst, cap_records); }
-void DevicePipeline::import_runs(const void* dev_ptr, uint64_t n) { impl->make_current(); impl->do_import_runs(dev_ptr, n); }
 void DevicePipeline::import_runs_padded(const void* dev_ptr, uint64_t stride, const uint64_t* counts, uint32_t n_ranks) {
     if (n_ranks == 0 || n_ranks > AC_MAX_RANKS) throw std::runtime_error("import_runs_padded: bad rank count");
     const void* ptrs[AC_MAX_RANKS];
     for (uint32_t q = 0; q < n_ranks; ++q) { if (counts[q] > stride) throw std::runtime_error("import_runs_padded: a rank holds more records than the stride"); ptrs[q] = (const char*)dev_ptr + (size_t)q * stride * sizeof(RunRec); }
     import_runs_from(ptrs, counts, n_ranks);
 }
-void DevicePipeline::import_runs_from(const void* const* ptrs, const uint64_t* counts, uint32_t n_ranks) { impl->make_current(); impl->do_import_runs_from(ptrs, counts, n_ranks); }
 const void* DevicePipeline::export_entries_own(uint64_t* n) {
-    Impl& m = *impl; m.make_current(); const int W = m.W;
-    uint64_t count = 0;
-    AC_DISPATCH_W(count = m.do_count_entries)
-    m.own_entries.ensure((count + 1) * sizeof(SlotRec));
-    m.do_export_entries(m.own_entries.p, count);
+    const uint64_t count = count_entries();
+    impl->own_entries.ensure((count + 1) * sizeof(SlotRec));
+    export_entries(impl->own_entries.p, count);
     *n = count;
-    return m.own_entries.p;
+    return impl->own_entries.p;
 }
 const void* DevicePipeline::export_runs_own(uint64_t* n) {
     Impl& m = *impl; m.make_current();
     m.own_runs.ensure((m.n_runs + 1) * sizeof(RunRec));
-    m.do_export_runs(m.own_runs.p, m.n_runs);
+    export_runs(m.own_runs.p, m.n_runs);
     *n = m.n_runs;
     return m.own_runs.p;
 }
@@ -2575,11 +2582,6 @@ void DevicePipeline::enable_peer_access(const int* devices, int n) {
     (void)devices; (void)n;
 #endif
 }
-void DevicePipeline::finish(PipelineResult& out, bool keep_positions, bool fused, bool split_paths) {
-    Impl& m = *impl; m.make_current(); const int W = m.W;
-    if (split_paths && !fused) throw std::runtime_error("split path lines need the fused finish");
-    AC_DISPATCH_W(m.finish_w, out, keep_positions, fused, split_paths)
-}
 void* DevicePipeline::strand_block(uint32_t seq_lo, uint32_t seq_hi, uint64_t* n_bytes) {
     Impl& m = *impl;
     if (seq_lo > seq_hi || seq_hi > m.n_seqs || m.total == 0) throw std::runtime_error("strand_block: bad range, or nothing uploaded");
@@ -2588,16 +2590,12 @@ void* DevicePipeline::strand_block(uint32_t seq_lo, uint32_t seq_hi, uint64_t* n
     *n_bytes = b1 - b0;
     return m.ascii.as<uint8_t>() + b0;
 }
-void DevicePipeline::export_path_tokens(void* dst, uint64_t stride, const uint64_t* counts, uint32_t n_ranks) { impl->make_current(); impl->do_export_path_tokens(dst, stride, counts, n_ranks); }
-void DevicePipeline::render_path_lines(const void* tokens, uint64_t n_tokens, const char** text, uint64_t* bytes) { impl->make_current(); impl->do_render_path_lines(tokens, n_tokens, text, bytes); }
 void DevicePipeline::fetch_graph(PipelineResult& out, bool keep_positions) {
     Impl& m = *impl; m.make_current();
-    if (m.stage < 2 || !out.fused) throw std::runtime_error("fetch_graph follows a fused build");
+    if (m.stage < Stage::RUNS || !out.fused) throw std::runtime_error("fetch_graph follows a fused build");
     if (out.graph_fetched) return;
     m.pull_graph(out, keep_positions);
 }
-
-void DevicePipeline::complete(PipelineResult& out) { impl->make_current(); impl->do_complete(out); }
 
 void DevicePipeline::build(PipelineResult& out, bool keep_positions, bool fused) {   // single GPU: every sequence is local, nothing to exchange
     build_local(0, impl->n_seqs, false);
