@@ -97,6 +97,19 @@ class AcSubsampleInfo(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class AcGenomeSizeInfo(C.Structure):
+    _fields_ = [("estimate", C.c_uint64), ("k", C.c_uint32), ("reruns", C.c_uint32), ("reads", C.c_uint64), ("bases", C.c_uint64),
+                ("windows", C.c_uint64), ("distinct", C.c_uint64), ("valley", C.c_uint64), ("peak", C.c_uint64), ("peak_refined", C.c_double),
+                ("solid", C.c_uint64), ("partitions", C.c_uint64), ("table_bytes", C.c_uint64), ("kernel_ms", C.c_float),
+                ("scan_ms", C.c_float), ("pack_ms", C.c_float), ("count_ms", C.c_float), ("hist_ms", C.c_float), ("read_ms", C.c_double),
+                ("copy_ms", C.c_double)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+GENOME_SIZE_BINS = 16384    # AC_GENOME_SIZE_BINS
+
 EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_sequence", "ac_clear_sequences", "ac_upload",
            "ac_build", "ac_compress", "ac_simplify", "ac_merge_linear_paths", "ac_renumber_unitigs", "ac_load_gfa", "ac_bind_host_to_device", "ac_decompress_gfa", "ac_pairwise_distances", "ac_distance_matrix_text", "ac_sequence_reconstruct", "ac_counts_get", "ac_unitigs_copy", "ac_path_copy", "ac_gfa_size", "ac_gfa_copy",
            "ac_timings_get", "ac_compress_dir", "ac_compress_dir_devices", "ac_load_sequences", "ac_sequence_get",
@@ -108,7 +121,8 @@ EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_seq
            "ac_bridge_best_paths", "ac_resolve", "ac_resolve_text", "ac_resolve_stats", "ac_resolve_dir", "ac_resolve_dirs", "ac_combine_dir",
            "ac_dotplot_rgb", "ac_dotplot_dir", "ac_png_write",
            "ac_clean_gfa", "ac_clean_text", "ac_gfa_to_fasta", "ac_gfa_fasta_text", "ac_table_text",
-           "ac_subsample_dir", "ac_genome_size", "ac_subsample_words", "ac_subsample_shuffle"]
+           "ac_subsample_dir", "ac_genome_size", "ac_subsample_words", "ac_subsample_shuffle",
+           "ac_genome_size_estimate", "ac_genome_size_from_histogram"]
 
 _libs = {}
 
@@ -221,6 +235,9 @@ def load_library(path=None):
     lib.ac_genome_size.argtypes = [C.c_char_p, C.POINTER(C.c_uint64)]
     lib.ac_subsample_words.argtypes = [C.c_uint64, C.c_uint32, C.POINTER(C.c_uint32), C.c_uint64]
     lib.ac_subsample_shuffle.argtypes = [C.c_uint64, C.c_uint64, C.POINTER(C.c_uint32)]
+    lib.ac_genome_size_estimate.argtypes = [C.c_char_p, C.c_uint32, C.c_int32, C.c_char_p, C.c_int32, C.POINTER(C.c_uint64),
+                                            C.POINTER(AcGenomeSizeInfo)]
+    lib.ac_genome_size_from_histogram.argtypes = [C.POINTER(C.c_uint64), C.c_uint64, C.POINTER(AcGenomeSizeInfo)]
     lib.ac_table_text.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint64, C.c_int32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     _libs[path] = lib
     return lib
@@ -780,3 +797,27 @@ def subsample_shuffle(n, seed, lib=None):
     out = (C.c_uint32 * max(1, n))()
     _raise_unless_ok(lib, lib.ac_subsample_shuffle(n, seed, out))
     return list(out)[:n]
+
+
+def genome_size_estimate(reads, k=21, device=0, dir=None, verbose=False, lib=None):
+    """`autocycler helper genome_size`: the genome size from the reads' k-mer depth spectrum (DESIGN.md §18; not the reference's Raven
+    assembly length).  Returns the info dict, with "histogram": the AC_GENOME_SIZE_BINS bins as a list."""
+    lib = lib or load_library()
+    info = AcGenomeSizeInfo()
+    hist = (C.c_uint64 * GENOME_SIZE_BINS)()
+    _raise_unless_ok(lib, lib.ac_genome_size_estimate(os.fsencode(reads), k, device, None if dir is None else os.fsencode(dir),
+                                                      1 if verbose else 0, hist, C.byref(info)))
+    out = info.as_dict()
+    out["histogram"] = list(hist)
+    return out
+
+
+def genome_size_from_histogram(hist, windows, lib=None):
+    """The rule alone (host only) on a histogram of up to AC_GENOME_SIZE_BINS bins (zero-padded) and its window count -> the info dict."""
+    lib = lib or load_library()
+    if len(hist) > GENOME_SIZE_BINS:
+        raise ValueError(f"at most {GENOME_SIZE_BINS} bins")
+    h = (C.c_uint64 * GENOME_SIZE_BINS)(*[int(x) for x in hist])
+    info = AcGenomeSizeInfo()
+    _raise_unless_ok(lib, lib.ac_genome_size_from_histogram(h, windows, C.byref(info)))
+    return info.as_dict()

@@ -27,6 +27,7 @@
 #include "host_clean.h"
 #include "host_dotplot.h"
 #include "host_subsample.h"
+#include "host_genome_size.h"
 #include <mutex>
 #include <immintrin.h>
 #include <functional>
@@ -1631,16 +1632,17 @@ int ac_png_write(const char* path, const uint8_t* rgb, uint32_t width, uint32_t 
 // ---- `autocycler subsample` (subsample.rs) --------------------------------------------------------------------------------------
 namespace {
 // One subsample device object per device, as for dotplot: its buffers (and pinned windows) are kept for the next call on that device.
+// genome_size reads through the same object and keeps its packed stream and table beside it.
 std::mutex g_subsample_mu;
 struct SubsampleDevice {
-    DeviceContext ctx; DeviceSubsample sub;
-    explicit SubsampleDevice(int32_t device) : ctx(device, nullptr), sub(ctx) {}
+    DeviceContext ctx; DeviceSubsample sub; DeviceSpectrum spec;
+    explicit SubsampleDevice(int32_t device) : ctx(device, nullptr), sub(ctx), spec(ctx) {}
 };
-DeviceSubsample& subsample_device(int32_t device) {        // with g_subsample_mu held
+SubsampleDevice& subsample_device(int32_t device) {        // with g_subsample_mu held
     static std::vector<std::pair<int32_t, SubsampleDevice*>> devices;
-    for (auto& d : devices) if (d.first == device) return d.second->sub;
+    for (auto& d : devices) if (d.first == device) return *d.second;
     devices.emplace_back(device, new SubsampleDevice(device));
-    return devices.back().second->sub;
+    return *devices.back().second;
 }
 }  // namespace
 
@@ -1665,7 +1667,7 @@ int ac_subsample_dir(const char* reads, const char* out_dir, const char* genome_
     SubsampleRun run;
     try {
         std::lock_guard<std::mutex> lock(g_subsample_mu);
-        subsample_run(subsample_device(device), in, dir, gsize, count, min_read_depth, seed, subsample_window_size(), verbose != 0, run);
+        subsample_run(subsample_device(device).sub, in, dir, gsize, count, min_read_depth, seed, subsample_window_size(), verbose != 0, run);
     } catch (const AcIoError& e) { return set_error(nullptr, AC_EIO, e.msg); }
     catch (const std::length_error& e) { return set_error(nullptr, AC_ERANGE, e.what()); }
     if (info) {
@@ -1702,6 +1704,73 @@ int ac_genome_size(const char* text, uint64_t* size) {
     if (!text || !size) return set_error(nullptr, AC_EINVAL, "null argument");
     AC_GUARD_BEGIN
     *size = parse_genome_size(text);
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
+// ---- `autocycler helper genome_size`: a k-mer depth estimate in place of helper.rs:388-403's Raven assembly --------------------------
+static_assert(AC_GENOME_SIZE_BINS == AC_GS_BINS, "the header's bin count is the device's");
+namespace {
+void fill_gs_info(const GenomeSizeRun& r, ac_genome_size_info* info) {
+    if (!info) return;
+    *info = ac_genome_size_info{};
+    info->estimate = r.estimate; info->k = r.k; info->reruns = (uint32_t)r.spectrum.reruns;
+    info->reads = r.reads; info->bases = r.bases; info->windows = r.windows; info->distinct = r.distinct;
+    info->valley = r.valley; info->peak = r.peak; info->peak_refined = r.peak_refined; info->solid = r.solid;
+    info->partitions = r.spectrum.partitions; info->table_bytes = r.spectrum.table_bytes;
+    info->kernel_ms = r.kernel_ms; info->scan_ms = r.scan_ms; info->pack_ms = r.spectrum.pack_ms; info->count_ms = r.spectrum.count_ms;
+    info->hist_ms = r.spectrum.hist_ms; info->read_ms = r.read_ms; info->copy_ms = r.copy_ms;
+}
+}  // namespace
+
+int ac_genome_size_estimate(const char* reads, uint32_t k, int32_t device, const char* dir, int32_t verbose, uint64_t* hist,
+                            ac_genome_size_info* info) {
+    if (!reads) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    const std::string in = reads;
+    int rc;
+    if ((rc = check_file(in)) != AC_OK) return rc;
+    if (k < 11 || k > 31 || k % 2 == 0) return set_error(nullptr, AC_EINPUT, "--kmer must be odd and between 11 and 31");
+    struct stat st;
+    if (dir && stat(dir, &st) == 0 && !S_ISDIR(st.st_mode)) return set_error(nullptr, AC_EINPUT, std::string(dir) + " exists but is not a directory");
+    if (dir && !make_dirs(dir)) return set_error(nullptr, AC_EINPUT, std::string("failed to create directory ") + dir + "\n" + strerror(errno));
+    if (verbose) fprintf(stderr, "\nStarting autocycler helper genome_size\n    This build estimates the genome size from the reads' k-mer depth "
+                                 "spectrum on the GPU. The reference assembles the reads with Raven and reports the assembly's length "
+                                 "instead, so the two numbers differ.\n\nSettings:\n  --reads %s\n  --kmer %u\n\n", in.c_str(), k);
+    GenomeSizeRun run;
+    std::vector<uint64_t> h;
+    try {
+        std::lock_guard<std::mutex> lock(g_subsample_mu);
+        SubsampleDevice& d = subsample_device(device);
+        genome_size_run(d.sub, d.spec, in, k, subsample_window_size(), h, run);
+    } catch (const AcIoError& e) { return set_error(nullptr, AC_EIO, e.msg); }
+    catch (const std::length_error& e) { return set_error(nullptr, AC_ERANGE, e.what()); }
+    if (hist) memcpy(hist, h.data(), AC_GS_BINS * 8);
+    if (dir) {
+        std::string tsv;
+        for (uint64_t c = 1; c < AC_GS_BINS; ++c)
+            if (h[c]) tsv += std::to_string(c) + "\t" + std::to_string(h[c]) + "\n";
+        const std::string path = std::string(dir) + "/kmer_histogram.tsv";
+        if (!write_file(path, tsv)) return set_error(nullptr, AC_EIO, "cannot write " + path);
+    }
+    genome_size_rule(h.data(), run.windows, run);
+    fill_gs_info(run, info);
+    if (verbose) fprintf(stderr, "K-mer spectrum (k = %u):\n  reads: %llu\n  bases: %llu\n  k-mer windows: %llu\n  distinct k-mers: %llu\n"
+                                 "  valley: %llu\n  peak: %llu (refined %.3f)\n  solid k-mer occurrences: %llu\n  partitions: %llu\n\n"
+                                 "Estimated genome size: %llu bp\n\n", k, (unsigned long long)run.reads, (unsigned long long)run.bases,
+                         (unsigned long long)run.windows, (unsigned long long)run.distinct, (unsigned long long)run.valley,
+                         (unsigned long long)run.peak, run.peak_refined, (unsigned long long)run.solid,
+                         (unsigned long long)run.spectrum.partitions, (unsigned long long)run.estimate);
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
+int ac_genome_size_from_histogram(const uint64_t* hist, uint64_t windows, ac_genome_size_info* info) {
+    if (!hist) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    GenomeSizeRun run;
+    genome_size_rule(hist, windows, run);
+    fill_gs_info(run, info);
     return ok(nullptr);
     AC_GUARD_END(nullptr)
 }

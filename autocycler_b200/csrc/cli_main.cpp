@@ -1,6 +1,7 @@
 // `autocycler compress`, `autocycler decompress`, `autocycler cluster`, `autocycler trim`, `autocycler resolve`, `autocycler combine`, `autocycler dotplot`,
 // `autocycler clean`, `autocycler gfa2fasta`, `autocycler table` and `autocycler subsample` with the reference's flags (main.rs:126-162), messages and exit codes
-// (misc.rs:130-136: "Error: <text>" on stderr, exit 1), running the H100 path through the C ABI.
+// (misc.rs:130-136: "Error: <text>" on stderr, exit 1), running the H100 path through the C ABI; and `autocycler helper genome_size`,
+// which departs from the reference on purpose: a k-mer depth estimate on the GPU instead of the length of a Raven assembly.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -286,6 +287,52 @@ static int subsample_main(int argc, char** argv) {
     return finish(ac_subsample_dir(reads.c_str(), out.c_str(), gsize.c_str(), count, depth, seed, device, 1, nullptr));
 }
 
+// `autocycler helper genome_size` (main.rs:194-236, helper.rs:388-403), the one helper task this build runs, and not as the reference
+// does: the estimate comes from the reads' k-mer depth spectrum, counted on the GPU, instead of the total length of a Raven assembly.
+// The number alone goes to stdout.  -t is accepted because the pipelines pass it; the assembler tasks' flags and --args are refused.
+static const char* helper_usage =
+    "Usage: autocycler helper genome_size --reads <READS> [--threads 8] [--dir <DIR>] [--kmer 21] [--device N]\n\n"
+    "Estimates the genome size from the reads' canonical k-mer depth spectrum, counted on the GPU, and prints it (bases) on stdout.\n"
+    "This departs from the reference, which assembles the reads with Raven and prints the assembly's total length: the numbers differ.\n"
+    "A replicon present in c copies per genome counts c times, and so does each copy of a repeat.\n\n"
+    "Options:\n"
+    "  -r, --reads <READS>      Input long reads in FASTQ format, gzipped or not (required)\n"
+    "  -t, --threads <THREADS>  Accepted for the pipelines' command lines; the counting runs on the GPU [default: 8]\n"
+    "  -d, --dir <DIR>          Directory to create and write kmer_histogram.tsv into (count<TAB>k-mers)\n"
+    "      --kmer <KMER>        K-mer size, odd, 11 to 31 [default: 21]\n"
+    "      --device <ORDINAL>   CUDA device [default: 0]\n"
+    "The other helper tasks (canu, flye, metamdbg, miniasm, myloasm, necat, nextdenovo, plassembler, raven, redbean) run external\n"
+    "assemblers, which this build does not include.\n";
+static int helper_main(int argc, char** argv) {
+    Args a{argc, argv, helper_usage};
+    if (argc < 3 || argv[2][0] == '-') {
+        if (argc >= 3 && (strcmp(argv[2], "-h") == 0 || strcmp(argv[2], "--help") == 0)) return a.help();
+        return a.missing();
+    }
+    const std::string task = argv[2];
+    if (task != "genome_size") {
+        fprintf(stderr, "\nError: helper task '%s' runs an external assembler, which this build does not include; only genome_size runs here\n",
+                task.c_str());
+        return 1;
+    }
+    a.i = 2;
+    std::string reads, dir; bool has_dir = false; unsigned long k = 21; int device = 0;
+    while (a.next()) {
+        if (a.is("-r", "--reads")) reads = a.value();
+        else if (a.is("-t", "--threads")) a.number(true);
+        else if (a.is("-d", "--dir")) { dir = a.value(); has_dir = true; }
+        else if (a.is("--kmer")) k = (unsigned long)a.number(true);
+        else if (a.is("--device")) device = atoi(a.value());
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
+    }
+    if (reads.empty()) return a.missing();
+    ac_genome_size_info info;
+    const int rc = ac_genome_size_estimate(reads.c_str(), k > 0xFFFFFFFFul ? 0 : (uint32_t)k, device, has_dir ? dir.c_str() : nullptr, 1, nullptr, &info);
+    if (rc == AC_OK) printf("%llu\n", (unsigned long long)info.estimate);
+    return finish(rc);
+}
+
 int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "dotplot") == 0) return dotplot_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "resolve") == 0) return resolve_main(argc, argv);
@@ -298,6 +345,7 @@ int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "gfa2fasta") == 0) return gfa2fasta_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "table") == 0) return table_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "subsample") == 0) return subsample_main(argc, argv);
+    if (argc >= 2 && strcmp(argv[1], "helper") == 0) return helper_main(argc, argv);
     fprintf(stderr, "%s", compress_usage);
     return 2;
 }

@@ -1,4 +1,4 @@
-// The device parts of `autocycler trim`, `resolve`, `cluster`, `dotplot` and `subsample`.  Each object owns its device buffers (allocated on first
+// The device parts of `autocycler trim`, `resolve`, `cluster`, `dotplot`, `subsample` and `helper genome_size`.  Each object owns its device buffers (allocated on first
 // use, kept for the next call) and runs on the device and stream of the DeviceContext it is given, which must outlive it.
 #pragma once
 #include <cstdint>
@@ -147,6 +147,9 @@ public:
     PinBuf h_win, h_out;
     float kernel_ms = 0.f;           // the kernels of every call so far (CUDA events; 0 under emulation)
     double copy_ms = 0.0;            // host wall time of the window uploads and the gathered output's copies back
+    // The window last scanned, on the device: its bytes and its records' spans (valid until the next scan_window).
+    const uint8_t* window_bytes() { return d_bytes.as<uint8_t>(); }
+    const SubRecord* window_records() { return d_rec.as<SubRecord>(); }
 private:
     void rows(uint64_t n, const uint64_t* starts, uint32_t count, uint64_t rps, SubStats* out);
     DeviceContext& ctx;
@@ -155,3 +158,38 @@ private:
     uint64_t win_records = 0, win_bytes = 0;
     DevBuf d_bytes, d_mask, d_cnt, d_line, d_rec, d_bad, d_len, d_len_tmp, d_rank, d_starts, d_h1, d_s1, d_h2, d_s2, d_row, d_size, d_out;
 };
+
+// `autocycler helper genome_size`: the canonical k-mer depth spectrum of a FASTQ file (DESIGN.md §18).  Each window that
+// DeviceSubsample scanned is packed into a device-resident stream (2 bits and a validity bit per base, every record from a fresh
+// 32-base word); the k-mers are then counted in P partitions of an open-addressing table of 16-byte slots, and each partition's counts
+// are added to a histogram of AC_GS_BINS bins (the last one holds every count >= AC_GS_BINS - 1).
+#define AC_GS_BINS 16384u
+struct GsSlot { uint64_t key; uint32_t count, pad; };   // key: canonical k-mer + 1 (0: empty)
+// What the count ran: partitions, the largest table's bytes, partitions rerun with twice the slots, and the kernels' time by stage.
+struct SpectrumRun { uint64_t partitions = 0, table_bytes = 0, reruns = 0; float pack_ms = 0.f, count_ms = 0.f, hist_ms = 0.f; };
+
+class DeviceSpectrum {
+public:
+    explicit DeviceSpectrum(DeviceContext& ctx) : ctx(ctx) {}
+    ~DeviceSpectrum() { ctx.make_current(); }
+    // An empty packed stream for k-mers of length k (odd, 11..31).
+    void begin(uint32_t k);
+    // Appends the `records` records of the window `sub` scanned last to the packed stream, and adds their windows and bases.
+    void pack_window(DeviceSubsample& sub, uint64_t records);
+    // W: windows of k valid bases inside one read, and the bases of the records packed so far (one host round trip).
+    void totals(uint64_t* windows, uint64_t* bases);
+    // The histogram of the packed stream's canonical k-mer counts into hist[AC_GS_BINS].  budget_slots: the most slots a table may
+    // take; parts: the partitions to use (0: the smallest power of two whose 2 W / P slots fit the budget).  A partition whose probe
+    // limit is hit is counted again with twice the slots.
+    void count(uint64_t windows, uint64_t budget_slots, uint64_t parts, uint64_t* hist, SpectrumRun* run);
+    float kernel_ms = 0.f;           // the kernels of every call since begin() (CUDA events; 0 under emulation)
+private:
+    DeviceContext& ctx;
+    SerialScan<uint64_t, AC_SUB_SCAN_TILE, 8> scan_u64;          // of the records' word counts
+    uint32_t k = 21;
+    uint64_t words = 0;              // packed words so far
+    float pack_ms = 0.f;
+    DevBuf d_code, d_valid, d_woff, d_tot, d_table, d_flag, d_hist;
+};
+// Slots of device memory a k-mer table may take by default: half of the device's free memory (2^25 slots under emulation).
+uint64_t ac_gs_budget_slots();

@@ -10,6 +10,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <stdexcept>
 
 #include "host_cluster.h"
@@ -96,33 +97,6 @@ uint32_t below(ChaChaWords& rng, uint32_t bound) {
     return hi;
 }
 
-// The window reader: the file as it is, or gunzipped (every member) when it starts with the gzip magic (misc.rs:197-208, 233-245).
-struct FastqStream {
-    FILE* f = nullptr; gzFile g = nullptr; std::string path;
-    explicit FastqStream(const std::string& p) : path(p) {
-        f = fopen(p.c_str(), "rb");
-        if (!f) throw AcIoError{"cannot read " + p};
-        unsigned char magic[2] = {0, 0};
-        const size_t got = fread(magic, 1, 2, f);
-        if (got == 2 && magic[0] == 0x1f && magic[1] == 0x8b) {
-            fclose(f); f = nullptr;
-            g = gzopen(p.c_str(), "rb");
-            if (!g) throw AcIoError{"cannot read " + p};
-            gzbuffer(g, 1 << 20);
-        } else rewind(f);
-    }
-    ~FastqStream() { if (f) fclose(f); if (g) gzclose(g); }
-    size_t read(uint8_t* dst, size_t n) {
-        if (f) {
-            const size_t got = fread(dst, 1, n, f);
-            if (got < n && ferror(f)) throw AcIoError{"cannot read " + path};
-            return got;
-        }
-        const int got = gzread(g, dst, (unsigned)std::min<size_t>(n, 1u << 30));
-        if (got < 0) throw InputError{"Error reading FASTQ file: " + path + " is not a valid gzip file"};
-        return (size_t)got;
-    }
-};
 void grow_keep(PinBuf& b, size_t want, size_t keep) {    // pinned memory that keeps its first `keep` bytes
     if (want <= b.cap) return;
     PinBuf nb;
@@ -140,8 +114,34 @@ const char* reason_text(uint64_t why) {
     }
 }
 
-// One pass over the file in windows of at least `window` bytes: each_window(first record, records) runs after each window's scan.
-template <class F> void windows(DeviceSubsample& dev, const std::string& path, uint64_t& window, bool keep_lengths, SubsampleRun& run, F each_window) {
+}  // namespace
+
+FastqStream::FastqStream(const std::string& p) : path(p) {
+    f = fopen(p.c_str(), "rb");
+    if (!f) throw AcIoError{"cannot read " + p};
+    unsigned char magic[2] = {0, 0};
+    const size_t got = fread(magic, 1, 2, f);
+    if (got == 2 && magic[0] == 0x1f && magic[1] == 0x8b) {
+        fclose(f); f = nullptr;
+        g = gzopen(p.c_str(), "rb");
+        if (!g) throw AcIoError{"cannot read " + p};
+        gzbuffer(g, 1 << 20);
+    } else rewind(f);
+}
+FastqStream::~FastqStream() { if (f) fclose(f); if (g) gzclose(g); }
+size_t FastqStream::read(uint8_t* dst, size_t n) {
+    if (f) {
+        const size_t got = fread(dst, 1, n, f);
+        if (got < n && ferror(f)) throw AcIoError{"cannot read " + path};
+        return got;
+    }
+    const int got = gzread(g, dst, (unsigned)std::min<size_t>(n, 1u << 30));
+    if (got < 0) throw InputError{"Error reading FASTQ file: " + path + " is not a valid gzip file"};
+    return (size_t)got;
+}
+
+void fastq_windows(DeviceSubsample& dev, const std::string& path, uint64_t& window, bool keep_lengths, SubsampleRun& run,
+                   const std::function<void(uint64_t, uint64_t)>& each_window) {
     FastqStream in(path);
     struct stat st;
     const uint64_t file_size = in.f && stat(path.c_str(), &st) == 0 ? (uint64_t)st.st_size : 0;
@@ -177,7 +177,6 @@ template <class F> void windows(DeviceSubsample& dev, const std::string& path, u
         if (eof) break;
     }
 }
-}  // namespace
 
 uint64_t parse_genome_size(const std::string& text) {
     size_t a = 0, b = text.size();
@@ -238,7 +237,7 @@ void subsample_run(DeviceSubsample& dev, const std::string& reads, const std::st
     dev.kernel_ms = 0.f; dev.copy_ms = 0.0;
     // pass 1 (input_fastq_stats, :103-118): every record checked and its length kept on the device
     uint64_t n = 0;
-    windows(dev, reads, window, true, run, [&](uint64_t, uint64_t r) { n += r; });
+    fastq_windows(dev, reads, window, true, run, [&](uint64_t, uint64_t r) { n += r; });
     const bool one_window = run.windows == 1;
     run.input = dev.input_stats(n);
     if (verbose) fprintf(stderr, "Input FASTQ:\n  Read count: %llu\n  Read bases: %llu\n  Read N50 length: %llu bp\n\n", (unsigned long long)n,
@@ -296,7 +295,7 @@ void subsample_run(DeviceSubsample& dev, const std::string& reads, const std::st
         }
     };
     if (n && one_window) write_window(0, n);
-    else if (n) windows(dev, reads, window, false, run, write_window);
+    else if (n) fastq_windows(dev, reads, window, false, run, write_window);
     t0 = std::chrono::steady_clock::now();
     for (uint64_t i = 0; i < count; ++i) {
         const bool good = fclose(files[i]) == 0;

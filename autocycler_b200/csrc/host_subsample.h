@@ -2,7 +2,11 @@
 // shuffle, the sample files and subsample.yaml.  The record scan, the statistics and the split into subsets run on the device
 // (DeviceSubsample, subsample.cu).
 #pragma once
+#include <zlib.h>
+
 #include <cstdint>
+#include <cstdio>
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -29,3 +33,19 @@ struct AcIoError { std::string msg; };
 void subsample_run(DeviceSubsample& dev, const std::string& reads, const std::string& out_dir, uint64_t genome_size, uint64_t count,
                    double min_depth, uint64_t seed, uint64_t window, bool verbose, SubsampleRun& run);
 uint64_t subsample_window_size();   // AC_SUBSAMPLE_WINDOW (bytes) or 1 GiB
+
+// The FASTQ reader of subsample and genome_size: the file as it is, or gunzipped (every member) when it starts with the gzip magic
+// (misc.rs:197-208, 233-245).  AcIoError when it cannot be read, InputError for a broken gzip stream.
+struct FastqStream {
+    FILE* f = nullptr; gzFile g = nullptr; std::string path;
+    explicit FastqStream(const std::string& p);
+    FastqStream(const FastqStream&) = delete; FastqStream& operator=(const FastqStream&) = delete;
+    ~FastqStream();
+    size_t read(uint8_t* dst, size_t n);
+};
+// One pass over a FASTQ file in windows of at least `window` bytes (it doubles while a window holds no complete record): each window is
+// scanned by dev.scan_window (every record checked; the lengths kept when keep_lengths) and each_window(first record, records) runs
+// after each scan.  A malformed record is InputError "Error reading FASTQ file: record N: <reason>" (std::length_error for a read of
+// 2^32 bases or more).  run.read_ms gets the reading time; with keep_lengths, run.windows and run.bytes_scanned the windows and bytes.
+void fastq_windows(DeviceSubsample& dev, const std::string& path, uint64_t& window, bool keep_lengths, SubsampleRun& run,
+                   const std::function<void(uint64_t, uint64_t)>& each_window);

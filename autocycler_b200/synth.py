@@ -183,6 +183,17 @@ def make_reads(genome, depth=None, n_reads=None, n50=15_000, sigma=0.5, seed=1, 
         yield (f"read_{made} length={L}", seq.tobytes(), qual.tobytes())
 
 
+def make_noisy_reads(genome, depth=None, n_reads=None, n50=15_000, sigma=0.5, seed=1, sub=0.0, ins=0.0, dele=0.0, min_length=0):
+    """make_reads' reads (the same seed gives the same positions, strands and lengths before the errors), each then given per-base
+    substitutions, insertions and deletions at the given rates from a second seeded stream, with fresh qualities of its new length.
+    Stops on make_reads' own rule (depth counts the error-free lengths).  Yields (name, sequence bytes, quality bytes)."""
+    rng = SplitMix64(seed ^ 0x6E6F697379)
+    for name, seq, _ in make_reads(genome, depth=depth, n_reads=n_reads, n50=n50, sigma=sigma, seed=seed, min_length=min_length):
+        out = mutate(rng, np.frombuffer(seq, dtype=np.uint8), sub, ins, dele) if seq else np.zeros(0, dtype=np.uint8)
+        qual = (rng.u64((len(out) + 7) // 8).view(np.uint8)[:len(out)] % np.uint8(42)) + np.uint8(33)
+        yield (name, out.tobytes(), qual.tobytes())
+
+
 def write_reads(reads, path, gz=False, crlf=False, plus_header=False, final_newline=True):
     """reads as FASTQ at path (gzipped when gz): CRLF line ends, '+' lines that repeat the header and a last record without its
     newline on request."""

@@ -28,6 +28,8 @@
  *   subsample (the whole subcommand)        subsample.rs:29-43       -> ac_subsample_dir
  *   parse_genome_size                       subsample.rs:83-101      -> ac_genome_size
  *   StdRng::seed_from_u64 + shuffle         subsample.rs:151-153     -> ac_subsample_words, ac_subsample_shuffle
+ *   helper genome_size                      helper.rs:388-403        -> ac_genome_size_estimate, ac_genome_size_from_histogram
+ *       (a deliberate departure: a k-mer depth estimate from the reads on the GPU, not the length of a Raven assembly)
  *
  * Conventions: every function returns 0 on success and a negative AC_E* code on failure; the message
  * is available from ac_last_error(handle) (or ac_last_error(NULL) when no handle exists).  No C++
@@ -426,6 +428,42 @@ int ac_genome_size(const char* text, uint64_t* size);
 int ac_subsample_words(uint64_t seed, uint32_t rounds, uint32_t* out, uint64_t n);
 /* (0..n).shuffle(&mut StdRng::seed_from_u64(seed)) (subsample.rs:151-153): order[p] = the read at shuffled position p.  Host only. */
 int ac_subsample_shuffle(uint64_t n, uint64_t seed, uint32_t* order);
+
+/* `autocycler helper genome_size -r reads [--kmer 21] [-d dir]`: the genome size from the reads' canonical k-mer depth spectrum.  This
+ * departs from the reference on purpose: helper.rs:388-403 assembles the reads with Raven and reports the assembly's total length, which
+ * this build cannot do, so the number differs from the reference's.  A replicon present in c copies per genome counts c times, and so
+ * does each copy of a repeat (Raven's assembly holds one copy of each).  The FASTQ file streams through subsample's windows and record
+ * scan (the same messages for a malformed record); every window is packed on the GPU at 2 bits and a validity bit per base; the canonical
+ * k-mers are counted in partitions of an open-addressing table on the GPU and their counts binned into AC_GENOME_SIZE_BINS bins
+ * (hist[c] = k-mers seen c times, the last bin every count at or above it).  The rule (DESIGN.md section 18): the valley v, the peak p,
+ * the parabola vertex p*, and G = round((windows - sum_{c<v} c hist[c]) / p*).  k: odd, 11..31, else AC_EINPUT.  No k-mer windows:
+ * AC_EINPUT; no depth peak: AC_EINPUT "no k-mer depth peak: ..."; a peak at the cap: AC_ERANGE.  dir (may be NULL): created if needed,
+ * gets kmer_histogram.tsv (`count<TAB>k-mers` per non-zero bin).  hist (may be NULL): AC_GENOME_SIZE_BINS values.  The histogram file
+ * and hist are written even when the rule then fails.  AC_GS_TABLE_SLOTS and AC_GS_PARTITIONS (DESIGN.md section 8) force a table
+ * budget and a partition count.  Calls on one device run one at a time, with subsample's.  info may be NULL. */
+#define AC_GENOME_SIZE_BINS 16384
+typedef struct {
+    uint64_t estimate;                 /* G, the genome size in bases */
+    uint32_t k;
+    uint32_t reruns;                   /* partitions counted again with twice the slots after their probe limit was hit */
+    uint64_t reads, bases;             /* FASTQ records and their bases */
+    uint64_t windows;                  /* W: windows of k A/C/G/T bases (any case) inside one read */
+    uint64_t distinct;                 /* distinct canonical k-mers */
+    uint64_t valley, peak;             /* v and p */
+    double peak_refined;               /* p* */
+    uint64_t solid;                    /* W - sum_{c<v} c hist[c], the numerator of G */
+    uint64_t partitions;               /* P: passes over the packed stream, each with the table cleared */
+    uint64_t table_bytes;              /* the largest table's bytes */
+    float kernel_ms;                   /* CUDA events around every kernel, summed (0 under emulation) */
+    float scan_ms, pack_ms, count_ms, hist_ms;   /* the same by stage: record scan, packing, counting, histogram */
+    double read_ms;                    /* host: reading and gunzipping the file */
+    double copy_ms;                    /* host wall time of the window uploads */
+} ac_genome_size_info;
+int ac_genome_size_estimate(const char* reads, uint32_t k, int32_t device, const char* dir, int32_t verbose, uint64_t* hist,
+                            ac_genome_size_info* info);
+/* The rule alone on a histogram of AC_GENOME_SIZE_BINS bins and its window count: info's estimate, windows, distinct, valley, peak,
+ * peak_refined and solid (the rest 0).  AC_EINPUT for no depth peak or more occurrences below the valley than windows.  Host only. */
+int ac_genome_size_from_histogram(const uint64_t* hist, uint64_t windows, ac_genome_size_info* info);
 
 #ifdef __cplusplus
 }
