@@ -110,6 +110,16 @@ class AcGenomeSizeInfo(C.Structure):
 
 GENOME_SIZE_BINS = 16384    # AC_GENOME_SIZE_BINS
 
+
+class AcDepthInfo(C.Structure):
+    _fields_ = [("contigs", C.c_uint64), ("unique_kmers", C.c_uint64), ("assembly_windows", C.c_uint64), ("reads", C.c_uint64),
+                ("read_windows", C.c_uint64), ("read_bases", C.c_uint64), ("table_bytes", C.c_uint64), ("kept", C.c_uint64),
+                ("k", C.c_uint32), ("filtered", C.c_int32), ("kernel_ms", C.c_float), ("scan_ms", C.c_float), ("pack_ms", C.c_float),
+                ("insert_ms", C.c_float), ("probe_ms", C.c_float), ("median_ms", C.c_float), ("read_ms", C.c_double), ("copy_ms", C.c_double)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
 EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_sequence", "ac_clear_sequences", "ac_upload",
            "ac_build", "ac_compress", "ac_simplify", "ac_merge_linear_paths", "ac_renumber_unitigs", "ac_load_gfa", "ac_bind_host_to_device", "ac_decompress_gfa", "ac_pairwise_distances", "ac_distance_matrix_text", "ac_sequence_reconstruct", "ac_counts_get", "ac_unitigs_copy", "ac_path_copy", "ac_gfa_size", "ac_gfa_copy",
            "ac_timings_get", "ac_compress_dir", "ac_compress_dir_devices", "ac_load_sequences", "ac_sequence_get",
@@ -122,7 +132,8 @@ EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_seq
            "ac_dotplot_rgb", "ac_dotplot_dir", "ac_png_write",
            "ac_clean_gfa", "ac_clean_text", "ac_gfa_to_fasta", "ac_gfa_fasta_text", "ac_table_text",
            "ac_subsample_dir", "ac_genome_size", "ac_subsample_words", "ac_subsample_shuffle",
-           "ac_genome_size_estimate", "ac_genome_size_from_histogram"]
+           "ac_genome_size_estimate", "ac_genome_size_from_histogram",
+           "ac_depth_fasta", "ac_depth_filter_text", "ac_depth_from_header"]
 
 _libs = {}
 
@@ -238,6 +249,12 @@ def load_library(path=None):
     lib.ac_genome_size_estimate.argtypes = [C.c_char_p, C.c_uint32, C.c_int32, C.c_char_p, C.c_int32, C.POINTER(C.c_uint64),
                                             C.POINTER(AcGenomeSizeInfo)]
     lib.ac_genome_size_from_histogram.argtypes = [C.POINTER(C.c_uint64), C.c_uint64, C.POINTER(AcGenomeSizeInfo)]
+    lib.ac_depth_fasta.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_int32, C.c_uint32, C.POINTER(C.c_double),
+                                   C.POINTER(C.c_double), C.c_int32, C.c_int32, C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_uint64,
+                                   C.POINTER(AcDepthInfo)]
+    lib.ac_depth_filter_text.argtypes = [C.c_char_p, C.c_uint64, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_void_p, C.c_uint64,
+                                         C.POINTER(C.c_uint64)]
+    lib.ac_depth_from_header.argtypes = [C.c_char_p, C.POINTER(C.c_double)]
     lib.ac_table_text.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint64, C.c_int32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     _libs[path] = lib
     return lib
@@ -821,3 +838,54 @@ def genome_size_from_histogram(hist, windows, lib=None):
     info = AcGenomeSizeInfo()
     _raise_unless_ok(lib, lib.ac_genome_size_from_histogram(h, windows, C.byref(info)))
     return info.as_dict()
+
+
+def _fasta_records(path):
+    """The number of records of a FASTA file (gzipped or not): its lines that start with '>'."""
+    import gzip
+    with open(path, "rb") as f:
+        data = f.read()
+    if data[:2] == b"\x1f\x8b":
+        data = gzip.decompress(data)
+    return sum(1 for line in data.split(b"\n") if line.startswith(b">"))
+
+
+def depth(assembly, out_fasta, reads=None, source="reads", k=21, min_depth_abs=None, min_depth_rel=None, tsv=None, device=0, verbose=False,
+          lib=None):
+    """`autocycler depth` (DESIGN.md §19): each contig's read depth from the reads' k-mers, counted on the GPU (not in the reference), then
+    the reference's helper depth filter; source="header" is that filter alone on the headers' depths.  Returns the info dict, with
+    "depths" (per contig, None without a depth) and "unique" (per contig, its unique k-mers)."""
+    lib = lib or load_library()
+    if source not in ("reads", "header"):
+        raise ValueError("source must be 'reads' or 'header'")
+    cap = _fasta_records(assembly) if os.path.isfile(assembly) else 0
+    depths = (C.c_double * max(1, cap))()
+    unique = (C.c_uint64 * max(1, cap))()
+    info = AcDepthInfo()
+    _raise_unless_ok(lib, lib.ac_depth_fasta(os.fsencode(assembly), None if reads is None else os.fsencode(reads), os.fsencode(out_fasta),
+                                             None if tsv is None else os.fsencode(tsv), 1 if source == "header" else 0, k,
+                                             _depth_arg(min_depth_abs), _depth_arg(min_depth_rel), device, 1 if verbose else 0, depths,
+                                             unique, cap, C.byref(info)))
+    out = info.as_dict()
+    n = min(cap, out["contigs"])
+    out["depths"] = [None if d != d else d for d in list(depths)[:n]]
+    out["unique"] = list(unique)[:n]
+    return out
+
+
+def depth_filter_text(fasta_text, min_depth_abs=None, min_depth_rel=None, lib=None):
+    """helper.rs:889-921 on a FASTA text -> what the file holds afterwards ("" when nothing is kept).  Host only."""
+    lib = lib or load_library()
+    data = fasta_text.encode() if isinstance(fasta_text, str) else fasta_text
+    return _host_text(lib, lib.ac_depth_filter_text, data, len(data), _depth_arg(min_depth_abs), _depth_arg(min_depth_rel))
+
+
+def depth_from_header(header, lib=None):
+    """helper.rs:923-931: the depth a FASTA header carries, or None.  Host only."""
+    lib = lib or load_library()
+    d = C.c_double()
+    rc = lib.ac_depth_from_header(header.encode(), C.byref(d))
+    if rc == -6:
+        return None
+    _raise_unless_ok(lib, rc)
+    return d.value

@@ -5,6 +5,7 @@
 #include <dirent.h>
 #include <sys/stat.h>
 #include <unistd.h>
+#include <cmath>
 #include <zlib.h>
 
 #include <algorithm>
@@ -28,6 +29,7 @@
 #include "host_dotplot.h"
 #include "host_subsample.h"
 #include "host_genome_size.h"
+#include "host_depth.h"
 #include <mutex>
 #include <immintrin.h>
 #include <functional>
@@ -1632,11 +1634,11 @@ int ac_png_write(const char* path, const uint8_t* rgb, uint32_t width, uint32_t 
 // ---- `autocycler subsample` (subsample.rs) --------------------------------------------------------------------------------------
 namespace {
 // One subsample device object per device, as for dotplot: its buffers (and pinned windows) are kept for the next call on that device.
-// genome_size reads through the same object and keeps its packed stream and table beside it.
+// genome_size and depth read through the same object and keep their packed streams and tables beside it.
 std::mutex g_subsample_mu;
 struct SubsampleDevice {
-    DeviceContext ctx; DeviceSubsample sub; DeviceSpectrum spec;
-    explicit SubsampleDevice(int32_t device) : ctx(device, nullptr), sub(ctx), spec(ctx) {}
+    DeviceContext ctx; DeviceSubsample sub; DeviceSpectrum spec; DeviceDepth depth;
+    explicit SubsampleDevice(int32_t device) : ctx(device, nullptr), sub(ctx), spec(ctx), depth(ctx) {}
 };
 SubsampleDevice& subsample_device(int32_t device) {        // with g_subsample_mu held
     static std::vector<std::pair<int32_t, SubsampleDevice*>> devices;
@@ -1775,4 +1777,122 @@ int ac_genome_size_from_histogram(const uint64_t* hist, uint64_t windows, ac_gen
     AC_GUARD_END(nullptr)
 }
 
+// ---- `autocycler depth`: read-measured contig depth (not in the reference) and helper.rs:889-931's depth filter ----------------------
+int ac_depth_fasta(const char* assembly, const char* reads, const char* out_fasta, const char* tsv, int32_t source_header, uint32_t k,
+                   const double* min_abs, const double* min_rel, int32_t device, int32_t verbose, double* depths, uint64_t* unique,
+                   uint64_t cap, ac_depth_info* info) {
+    if (!assembly || !out_fasta) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    const std::string in = assembly, out = out_fasta;
+    int rc;
+    if ((rc = check_file(in)) != AC_OK) return rc;
+    if (!source_header) {
+        if (!reads) return set_error(nullptr, AC_EINPUT, "--reads is required with --source reads (or use --source header)");
+        if ((rc = check_file(reads)) != AC_OK) return rc;
+        if (k < 11 || k > 31 || k % 2 == 0) return set_error(nullptr, AC_EINPUT, "--kmer must be odd and between 11 and 31");
+    }
+    if (verbose) {
+        fprintf(stderr, "\nStarting autocycler depth\n    %s\n\nSettings:\n  --assembly %s\n  --out_fasta %s\n  --source %s\n",
+                source_header ? "This command applies the reference's helper depth filter to the depths the contig headers carry."
+                              : "This command measures each contig's read depth from the reads' k-mers on the GPU (an addition that is "
+                                "not in the reference), then applies the reference's helper depth filter.",
+                in.c_str(), out.c_str(), source_header ? "header" : "reads");
+        if (!source_header) fprintf(stderr, "  --reads %s\n  --kmer %u\n", reads, k);
+        if (min_abs) fprintf(stderr, "  --min_depth_abs %s\n", rust_fixed(*min_abs, 3).c_str());
+        if (min_rel) fprintf(stderr, "  --min_depth_rel %s\n", rust_fixed(*min_rel, 3).c_str());
+        fprintf(stderr, "\n");
+    }
+    ac_depth_info di{};
+    di.k = source_header ? 0 : k;
+    std::vector<FastaRecord> recs;
+    std::vector<double> depth;
+    std::vector<char> has;
+    std::vector<uint64_t> uniq;
+    if (source_header) {                                   // copy_fasta (helper.rs:577-585), then depth_filter on the copy
+        std::vector<FastaRecord> loaded = parse_fasta(read_fasta_bytes(in), in);
+        size_t bases = 0;
+        for (const FastaRecord& r : loaded) bases += r.seq.size();
+        if (bases == 0) {
+            unlink(out.c_str());
+            if (info) *info = di;
+            return ok(nullptr);
+        }
+        recs = load_fasta(in);
+        depth.assign(recs.size(), NAN); has.assign(recs.size(), 0); uniq.assign(recs.size(), 0);
+        for (size_t i = 0; i < recs.size(); ++i) has[i] = depth_from_header(recs[i].header, depth[i]);
+    } else {
+        DepthResult r;
+        {
+            std::lock_guard<std::mutex> lock(g_subsample_mu);
+            SubsampleDevice& d = subsample_device(device);
+            try {
+                depth_run(d.sub, d.spec, d.depth, in, reads, k, subsample_window_size(), r);
+            } catch (const AcIoError& e) { return set_error(nullptr, AC_EIO, e.msg); }
+            catch (const std::length_error& e) { return set_error(nullptr, AC_ERANGE, e.what()); }
+        }
+        recs = std::move(r.recs); depth = r.depth; uniq = r.unique;
+        has.assign(recs.size(), 0);
+        for (size_t i = 0; i < recs.size(); ++i) {
+            has[i] = uniq[i] != 0;
+            if (has[i]) recs[i].header += " depth=" + rust_fixed(depth[i], 2);
+        }
+        di.unique_kmers = r.unique_total; di.assembly_windows = r.device.assembly_windows; di.reads = r.reads;
+        di.read_windows = r.read_windows; di.read_bases = r.read_bases; di.table_bytes = r.device.table_bytes;
+        di.kernel_ms = r.kernel_ms; di.scan_ms = r.scan_ms; di.pack_ms = r.pack_reads_ms; di.insert_ms = r.device.pack_ms + r.device.insert_ms;
+        di.probe_ms = r.device.probe_ms; di.median_ms = r.device.median_ms; di.read_ms = r.read_ms; di.copy_ms = r.copy_ms;
+        if (verbose) {
+            fprintf(stderr, "Read depth (k = %u):\n  reads: %llu\n  read k-mer windows: %llu\n  assembly k-mer windows: %llu\n  unique k-mers: %llu\n",
+                    k, (unsigned long long)r.reads, (unsigned long long)r.read_windows, (unsigned long long)r.device.assembly_windows,
+                    (unsigned long long)r.unique_total);
+            for (size_t i = 0; i < recs.size(); ++i)
+                fprintf(stderr, "  %s: %s (%llu unique k-mers)\n", recs[i].name.c_str(), has[i] ? ("depth=" + rust_fixed(depth[i], 2)).c_str() : "no depth",
+                        (unsigned long long)uniq[i]);
+        }
+    }
+    di.contigs = recs.size();
+    std::vector<char> keep;
+    std::string report;
+    di.filtered = depth_filter(recs, depth, has, min_abs, min_rel, keep, report) ? 1 : 0;
+    if ((min_abs || min_rel) && !di.filtered && verbose)
+        fprintf(stderr, "\nNote: not every contig has a depth, so the depth filter keeps every contig, as the reference does\n");
+    if (verbose) fputs(report.c_str(), stderr);
+    std::string text;
+    for (size_t i = 0; i < recs.size(); ++i)
+        if (keep[i]) { text += ">" + recs[i].header + "\n" + recs[i].seq + "\n"; ++di.kept; }
+    if (di.kept == 0) unlink(out.c_str());
+    else if (!write_file(out, text)) return set_error(nullptr, AC_EIO, "cannot write " + out);
+    if (tsv) {
+        std::string t;
+        for (size_t i = 0; i < recs.size(); ++i)
+            t += recs[i].name + "\t" + std::to_string(recs[i].seq.size()) + "\t" + std::to_string(uniq[i]) + "\t" + (has[i] ? rust_fixed(depth[i], 2) : std::string()) + "\n";
+        if (!write_file(tsv, t)) return set_error(nullptr, AC_EIO, std::string("cannot write ") + tsv);
+    }
+    for (uint64_t i = 0; i < std::min<uint64_t>(cap, recs.size()); ++i) {
+        if (depths) depths[i] = has[i] ? depth[i] : NAN;
+        if (unique) unique[i] = uniq[i];
+    }
+    if (info) *info = di;
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
+int ac_depth_filter_text(const char* fasta_text, uint64_t length, const double* min_abs, const double* min_rel, char* out, uint64_t cap,
+                         uint64_t* out_length) {
+    if ((!fasta_text && length) || !out_length) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    std::string report;
+    const std::string kept = depth_filter_text(std::string(fasta_text ? fasta_text : "", length), "the FASTA text", min_abs, min_rel, report);
+    return copy_text(nullptr, kept, out, cap, out_length);
+    AC_GUARD_END(nullptr)
+}
+
+int ac_depth_from_header(const char* header, double* depth) {
+    if (!header || !depth) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    if (!depth_from_header(header, *depth)) return set_error(nullptr, AC_EINPUT, "the header carries no depth");
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
 }  // extern "C"
+

@@ -1,7 +1,8 @@
 // `autocycler compress`, `autocycler decompress`, `autocycler cluster`, `autocycler trim`, `autocycler resolve`, `autocycler combine`, `autocycler dotplot`,
 // `autocycler clean`, `autocycler gfa2fasta`, `autocycler table` and `autocycler subsample` with the reference's flags (main.rs:126-162), messages and exit codes
-// (misc.rs:130-136: "Error: <text>" on stderr, exit 1), running the H100 path through the C ABI; and `autocycler helper genome_size`,
-// which departs from the reference on purpose: a k-mer depth estimate on the GPU instead of the length of a Raven assembly.
+// (misc.rs:130-136: "Error: <text>" on stderr, exit 1), running the H100 path through the C ABI; `autocycler helper genome_size`,
+// which departs from the reference on purpose: a k-mer depth estimate on the GPU instead of the length of a Raven assembly; and
+// `autocycler depth`, read-measured contig depth (not in the reference) with the reference's helper depth filter.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -333,6 +334,50 @@ static int helper_main(int argc, char** argv) {
     return finish(rc);
 }
 
+// `autocycler depth`: each contig's read depth from the reads' k-mers, counted on the GPU (an addition that is not in the reference), and
+// helper.rs:889-931's depth filter; with --source header, the reference's filter alone on the depths the headers carry.  Nothing goes
+// to stdout.
+static const char* depth_usage =
+    "Usage: autocycler depth --assembly <ASSEMBLY> --out_fasta <OUT_FASTA> [--reads <READS>] [--source reads|header] [--kmer 21]\n"
+    "                        [--min_depth_abs X] [--min_depth_rel Y] [--tsv <FILE>] [--device N]\n\n"
+    "Measures each contig's read depth from the reads' k-mers on the GPU and appends depth=<median> to its header, then applies the\n"
+    "reference's helper depth filter. Read-measured depth is not in the reference; --source header is the reference's filter alone.\n\n"
+    "Options:\n"
+    "  -i, --assembly <ASSEMBLY>   Input assembly in FASTA format, gzipped or not (required)\n"
+    "  -o, --out_fasta <FASTA>     Output FASTA, one line per sequence (required)\n"
+    "  -r, --reads <READS>         Long reads in FASTQ format, gzipped or not (required with --source reads)\n"
+    "      --source <SOURCE>       reads: measure the depth from the reads; header: the depth in each header [default: reads]\n"
+    "      --kmer <KMER>           K-mer size, odd, 11 to 31 [default: 21]\n"
+    "      --min_depth_abs <X>     Exclude contigs with a depth less than this absolute value\n"
+    "      --min_depth_rel <Y>     Exclude contigs with a depth less than this fraction of the longest contig's depth\n"
+    "      --tsv <FILE>            Write name, length, unique k-mers and depth per contig\n"
+    "      --device <ORDINAL>      CUDA device [default: 0]\n";
+static int depth_main(int argc, char** argv) {
+    Args a{argc, argv, depth_usage};
+    std::string in, out, reads, tsv, source = "reads"; bool has_tsv = false, has_abs = false, has_rel = false;
+    double min_abs = 0, min_rel = 0; unsigned long k = 21; int device = 0;
+    while (a.next()) {
+        if (a.is("-i", "--assembly")) in = a.value();
+        else if (a.is("-o", "--out_fasta")) out = a.value();
+        else if (a.is("-r", "--reads")) reads = a.value();
+        else if (a.is("--source")) {
+            source = a.value();
+            if (source != "reads" && source != "header") { fprintf(stderr, "error: invalid value '%s' for '--source'\n%s", source.c_str(), depth_usage); return 2; }
+        }
+        else if (a.is("--kmer")) k = (unsigned long)a.number(true);
+        else if (a.is("--min_depth_abs")) { min_abs = a.number(false); has_abs = true; }
+        else if (a.is("--min_depth_rel")) { min_rel = a.number(false); has_rel = true; }
+        else if (a.is("--tsv")) { tsv = a.value(); has_tsv = true; }
+        else if (a.is("--device")) device = atoi(a.value());
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
+    }
+    if (in.empty() || out.empty() || (source == "reads" && reads.empty())) return a.missing();
+    return finish(ac_depth_fasta(in.c_str(), reads.empty() ? nullptr : reads.c_str(), out.c_str(), has_tsv ? tsv.c_str() : nullptr, source == "header",
+                                 k > 0xFFFFFFFFul ? 0 : (uint32_t)k, has_abs ? &min_abs : nullptr, has_rel ? &min_rel : nullptr, device, 1,
+                                 nullptr, nullptr, 0, nullptr));
+}
+
 int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "dotplot") == 0) return dotplot_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "resolve") == 0) return resolve_main(argc, argv);
@@ -346,6 +391,7 @@ int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "table") == 0) return table_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "subsample") == 0) return subsample_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "helper") == 0) return helper_main(argc, argv);
+    if (argc >= 2 && strcmp(argv[1], "depth") == 0) return depth_main(argc, argv);
     fprintf(stderr, "%s", compress_usage);
     return 2;
 }

@@ -1,4 +1,4 @@
-// The device parts of `autocycler trim`, `resolve`, `cluster`, `dotplot`, `subsample` and `helper genome_size`.  Each object owns its device buffers (allocated on first
+// The device parts of `autocycler trim`, `resolve`, `cluster`, `dotplot`, `subsample`, `helper genome_size` and `depth`.  Each object owns its device buffers (allocated on first
 // use, kept for the next call) and runs on the device and stream of the DeviceContext it is given, which must outlive it.
 #pragma once
 #include <cstdint>
@@ -183,6 +183,11 @@ public:
     // limit is hit is counted again with twice the slots.
     void count(uint64_t windows, uint64_t budget_slots, uint64_t parts, uint64_t* hist, SpectrumRun* run);
     float kernel_ms = 0.f;           // the kernels of every call since begin() (CUDA events; 0 under emulation)
+    // The packed stream so far, on the device: `packed_words()` words of codes and validity masks (DeviceDepth::probe reads it).
+    const uint64_t* packed_codes() { return d_code.as<uint64_t>(); }
+    const uint32_t* packed_valid() { return d_valid.as<uint32_t>(); }
+    uint64_t packed_words() const { return words; }
+    float packed_ms() const { return pack_ms; }      // the packing's kernels since begin()
 private:
     DeviceContext& ctx;
     SerialScan<uint64_t, AC_SUB_SCAN_TILE, 8> scan_u64;          // of the records' word counts
@@ -193,3 +198,31 @@ private:
 };
 // Slots of device memory a k-mer table may take by default: half of the device's free memory (2^25 slots under emulation).
 uint64_t ac_gs_budget_slots();
+
+// `autocycler depth`: each contig's read depth from the reads' canonical k-mers (DESIGN.md §19).  The contigs are packed like the reads
+// (DeviceSpectrum's layout, each contig from a fresh word) and every window's canonical key goes into one open-addressing table; a key
+// seen twice is marked non-unique.  The reads' packed stream then probes the table, each hit on a unique key adding 1 to its count, and
+// each contig's depth is the exact median of its unique keys' counts, selected on the device.
+struct DepthSlot { uint64_t key; uint32_t count, flags; };   // key: canonical k-mer + 1 (0: empty); flags: contig id, AC_DEPTH_DUP
+#define AC_DEPTH_DUP 0x80000000u                             // the key occurs more than once over the assembly's windows
+// What the device ran: the assembly's windows, the table's bytes and the kernels' time by stage (CUDA events; 0 under emulation).
+struct DepthRun { uint64_t assembly_windows = 0, table_bytes = 0; float pack_ms = 0.f, insert_ms = 0.f, probe_ms = 0.f, median_ms = 0.f; };
+
+class DeviceDepth {
+public:
+    explicit DeviceDepth(DeviceContext& ctx) : ctx(ctx) {}
+    ~DeviceDepth() { ctx.make_current(); }
+    // The assembly table.  bytes: every contig's bytes back to back (a circular contig followed by its first k-1 bases), contig c
+    // taking len[c] of them; windows: the windows of k A/C/G/T bases in them.  The table takes max(2 windows, 64) slots;
+    // std::length_error when that exceeds budget_slots or there are 2^31 contigs or more.
+    void build(const uint8_t* bytes, const uint64_t* len, uint32_t n_contigs, uint64_t windows, uint32_t k, uint64_t budget_slots, DepthRun* run);
+    // Counts every window of the reads `spec` packed (after build, with the same k) into the unique keys it hits.
+    void probe(DeviceSpectrum& spec, DepthRun* run);
+    // unique[c]: contig c's unique keys; median[c]: the median of their counts (NaN when unique[c] is 0).  Host arrays of n_contigs.
+    void medians(uint64_t* unique, double* median, DepthRun* run);
+private:
+    DeviceContext& ctx;
+    uint32_t k = 21, n_contigs = 0;
+    uint64_t slots = 0;
+    DevBuf d_bytes, d_contig, d_woff, d_code, d_valid, d_wcid, d_table, d_unique, d_rank, d_prefix, d_hist, d_median;
+};

@@ -75,10 +75,9 @@ static std::string slurp(const std::string& path) {
 
 static bool is_ws(char c) { return c == ' ' || c == '\t' || c == '\n' || c == '\r' || c == '\v' || c == '\f'; }
 
-std::vector<FastaRecord> load_fasta(const std::string& path) {   // misc.rs:144-159, 174-194, 248-321
-    struct stat st;
-    if (stat(path.c_str(), &st) == 0 && st.st_size == 0) fail(path + " is an empty file");
-    const std::string data = slurp(path);
+std::string read_fasta_bytes(const std::string& path) { return slurp(path); }
+
+std::vector<FastaRecord> parse_fasta(const std::string& data, const std::string& path) {   // misc.rs:248-321
     std::vector<FastaRecord> recs;
     FastaRecord cur; bool open = false;
     auto close_record = [&]() {
@@ -108,6 +107,10 @@ std::vector<FastaRecord> load_fasta(const std::string& path) {   // misc.rs:144-
         pos = eol + 1;
     }
     if (open) close_record();
+    return recs;
+}
+
+void check_fasta(const std::vector<FastaRecord>& recs, const std::string& path) {   // misc.rs:174-194
     if (recs.empty()) fail(path + " contains no sequences");
     std::unordered_set<std::string> seen;
     for (auto& r : recs) {
@@ -115,6 +118,13 @@ std::vector<FastaRecord> load_fasta(const std::string& path) {   // misc.rs:144-
         if (r.seq.empty()) fail(path + " has an empty sequence");
     }
     for (auto& r : recs) if (!seen.insert(r.name).second) fail(path + " has a duplicate name: " + r.name);
+}
+
+std::vector<FastaRecord> load_fasta(const std::string& path) {   // misc.rs:144-159
+    struct stat st;
+    if (stat(path.c_str(), &st) == 0 && st.st_size == 0) fail(path + " is an empty file");
+    std::vector<FastaRecord> recs = parse_fasta(slurp(path), path);
+    check_fasta(recs, path);
     return recs;
 }
 

@@ -23,6 +23,9 @@ struct LoadedInput {
 std::vector<std::string> find_all_assemblies(const std::string& dir);                 // misc.rs:64-95
 struct FastaRecord { std::string name, header, seq; };
 std::vector<FastaRecord> load_fasta(const std::string& path);                         // misc.rs:144-321
+std::string read_fasta_bytes(const std::string& path);                                // the file, gunzipped when it starts with the gzip magic
+std::vector<FastaRecord> parse_fasta(const std::string& data, const std::string& path);   // misc.rs:248-321 (load_fasta_allow_empty's parse)
+void check_fasta(const std::vector<FastaRecord>& recs, const std::string& path);      // misc.rs:174-194
 LoadedInput load_sequences(const std::string& dir, uint32_t k, uint32_t max_contigs, uint32_t threads, bool verbose, DevicePipeline* device);
 void sequence_end_repair_device(DevicePipeline& pipe, std::vector<std::string>& padded, uint32_t k);   // compress.rs:202-270, matches found on the GPU
 void sequence_end_repair(std::vector<std::string>& padded, uint32_t k, uint32_t threads);   // compress.rs:202-270

@@ -21,31 +21,6 @@ double ms_since(std::chrono::steady_clock::time_point t0) {
     return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
 }
 
-// str::parse::<f64> (already lowercased): [+-]? then inf, infinity, nan, or digits with an optional '.' and exponent; nothing else, so
-// no hex floats and no partial parses.  The value is strtod's, correctly rounded as Rust's is.
-bool rust_f64(const std::string& s, double& v) {
-    size_t i = 0;
-    if (i < s.size() && (s[i] == '+' || s[i] == '-')) ++i;
-    const std::string rest = s.substr(i);
-    if (rest == "inf" || rest == "infinity" || rest == "nan") {
-        v = rest == "nan" ? NAN : (s[0] == '-' ? -INFINITY : INFINITY);
-        return true;
-    }
-    size_t digits = 0;
-    while (i < s.size() && isdigit((unsigned char)s[i])) { ++i; ++digits; }
-    if (i < s.size() && s[i] == '.') { ++i; while (i < s.size() && isdigit((unsigned char)s[i])) { ++i; ++digits; } }
-    if (digits == 0) return false;
-    if (i < s.size() && s[i] == 'e') {
-        ++i;
-        if (i < s.size() && (s[i] == '+' || s[i] == '-')) ++i;
-        size_t e = 0;
-        while (i < s.size() && isdigit((unsigned char)s[i])) { ++i; ++e; }
-        if (e == 0) return false;
-    }
-    if (i != s.size()) return false;
-    v = strtod(s.c_str(), nullptr);
-    return true;
-}
 uint64_t as_u64(double x) {            // Rust's saturating `f64 as u64` of round() (half away from zero)
     x = std::round(x);
     if (!(x > 0)) return 0;
@@ -116,6 +91,31 @@ const char* reason_text(uint64_t why) {
 
 }  // namespace
 
+// str::parse::<f64> (already lowercased): [+-]? then inf, infinity, nan, or digits with an optional '.' and exponent; nothing else, so
+// no hex floats and no partial parses.  The value is strtod's, correctly rounded as Rust's is.
+bool rust_f64(const std::string& s, double& v) {
+    size_t i = 0;
+    if (i < s.size() && (s[i] == '+' || s[i] == '-')) ++i;
+    const std::string rest = s.substr(i);
+    if (rest == "inf" || rest == "infinity" || rest == "nan") {
+        v = rest == "nan" ? NAN : (s[0] == '-' ? -INFINITY : INFINITY);
+        return true;
+    }
+    size_t digits = 0;
+    while (i < s.size() && isdigit((unsigned char)s[i])) { ++i; ++digits; }
+    if (i < s.size() && s[i] == '.') { ++i; while (i < s.size() && isdigit((unsigned char)s[i])) { ++i; ++digits; } }
+    if (digits == 0) return false;
+    if (i < s.size() && s[i] == 'e') {
+        ++i;
+        if (i < s.size() && (s[i] == '+' || s[i] == '-')) ++i;
+        size_t e = 0;
+        while (i < s.size() && isdigit((unsigned char)s[i])) { ++i; ++e; }
+        if (e == 0) return false;
+    }
+    if (i != s.size()) return false;
+    v = strtod(s.c_str(), nullptr);
+    return true;
+}
 FastqStream::FastqStream(const std::string& p) : path(p) {
     f = fopen(p.c_str(), "rb");
     if (!f) throw AcIoError{"cannot read " + p};

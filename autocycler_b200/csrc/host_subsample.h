@@ -15,6 +15,8 @@
 // parse_genome_size (subsample.rs:83-101): trim, lowercase, Rust's f64 grammar, round half away from zero, a saturating `as u64`, then
 // the k/m/g suffixes.  InputError "cannot interpret genome size".
 uint64_t parse_genome_size(const std::string& text);
+// str::parse::<f64> on an already lowercased text: Rust's f64 grammar, nothing else (no hex floats, no partial parses).
+bool rust_f64(const std::string& s, double& v);
 // (0..n).shuffle(&mut StdRng::seed_from_u64(seed)) of rand 0.9 (ChaCha12, IncreasingUniform): order[p] = the read at shuffled position p.
 std::vector<uint32_t> subsample_shuffle(uint64_t n, uint64_t seed);
 // The first n u32 words of StdRng::seed_from_u64(seed), or of the same generator at another round count (20: ChaCha20).

@@ -30,6 +30,8 @@
  *   StdRng::seed_from_u64 + shuffle         subsample.rs:151-153     -> ac_subsample_words, ac_subsample_shuffle
  *   helper genome_size                      helper.rs:388-403        -> ac_genome_size_estimate, ac_genome_size_from_histogram
  *       (a deliberate departure: a k-mer depth estimate from the reads on the GPU, not the length of a Raven assembly)
+ *   depth_filter, depth_from_header         helper.rs:889-931        -> ac_depth_filter_text, ac_depth_from_header
+ *   depth (read-measured contig depth)      not in the reference     -> ac_depth_fasta
  *
  * Conventions: every function returns 0 on success and a negative AC_E* code on failure; the message
  * is available from ac_last_error(handle) (or ac_last_error(NULL) when no handle exists).  No C++
@@ -464,6 +466,47 @@ int ac_genome_size_estimate(const char* reads, uint32_t k, int32_t device, const
 /* The rule alone on a histogram of AC_GENOME_SIZE_BINS bins and its window count: info's estimate, windows, distinct, valley, peak,
  * peak_refined and solid (the rest 0).  AC_EINPUT for no depth peak or more occurrences below the valley than windows.  Host only. */
 int ac_genome_size_from_histogram(const uint64_t* hist, uint64_t windows, ac_genome_size_info* info);
+
+/* `autocycler depth -i assembly -o out.fasta [-r reads] [--source reads|header]`: each contig's read depth, and the reference's depth
+ * filter (helper.rs:889-921).  Read-measured depth is an addition that is not in the reference (DESIGN.md section 19).
+ * source_header = 0 (reads): reads is required (AC_EINPUT otherwise); the assembly is loaded as load_fasta does and a header that already
+ * carries a depth (ac_depth_from_header) is AC_EINPUT.  Every contig window of k A/C/G/T bases (a contig whose header holds
+ * "circular=true", any case, and whose length is at least k also gets the k-1 windows across its end) gives a canonical key; a key that
+ * occurs once over all contigs is unique.  Each read window (the genome_size rule) whose key is a unique key adds 1 to it, on the GPU.
+ * A contig's depth is the median of its unique keys' counts (the mean of the two middle ones for an even number); none without unique
+ * keys.  out_fasta gets `>header[ depth={:.2}]\nseq\n` per contig; tsv (may be NULL) `name\tlength\tunique_kmers\tdepth` (empty without a
+ * depth).  k: odd, 11..31, else AC_EINPUT.  A table beyond half the free device memory: AC_ERANGE.
+ * source_header = 1: no reads are read and no device work runs: the assembly copied one line per sequence into out_fasta, as copy_fasta
+ * does (nothing written, out_fasta removed, for a file without bases), then the filter.
+ * The filter runs when min_abs or min_rel is given (may be NULL): nothing is filtered when a contig has no depth; otherwise the threshold
+ * is max(min_abs or 0, min_rel x the depth of the first longest contig) and a contig is kept when its depth reaches it.  None kept: no
+ * output file, and an existing one is removed.  verbose prints the settings, the depths and the filter's report to stderr.  depths and
+ * unique (may be NULL) get the first `cap` contigs' depth (NaN: none) and unique keys (0 in header mode).  Calls on one device run one at
+ * a time, with subsample's.  info may be NULL. */
+typedef struct {
+    uint64_t contigs;                  /* assembly records */
+    uint64_t unique_kmers;             /* unique keys over all contigs */
+    uint64_t assembly_windows;         /* the contigs' windows, junction windows included */
+    uint64_t reads, read_windows, read_bases;
+    uint64_t table_bytes;              /* the assembly table */
+    uint64_t kept;                     /* records written to out_fasta */
+    uint32_t k;
+    int32_t filtered;                  /* 1 when the filter ran */
+    float kernel_ms;                   /* CUDA events around every kernel, summed (0 under emulation) */
+    float scan_ms, pack_ms, insert_ms, probe_ms, median_ms;   /* the same by stage: record scan, read packing, assembly table, probes, medians */
+    double read_ms;                    /* host: reading and gunzipping the reads */
+    double copy_ms;                    /* host wall time of the window uploads */
+} ac_depth_info;
+int ac_depth_fasta(const char* assembly, const char* reads, const char* out_fasta, const char* tsv, int32_t source_header, uint32_t k,
+                   const double* min_abs, const double* min_rel, int32_t device, int32_t verbose, double* depths, uint64_t* unique,
+                   uint64_t cap, ac_depth_info* info);
+/* helper.rs:889-921 on a FASTA text: out gets what the file would hold afterwards: the text itself when the filter does not run (no bound
+ * given, no bases, or a record without a depth), the kept records one line per sequence, or nothing when none is kept.  out NULL asks
+ * for the length only.  Host only. */
+int ac_depth_filter_text(const char* fasta_text, uint64_t length, const double* min_abs, const double* min_rel, char* out, uint64_t cap,
+                         uint64_t* out_length);
+/* helper.rs:923-931: the depth a header carries (depth=, then depth-, then coverage=).  AC_EINPUT when it carries none.  Host only. */
+int ac_depth_from_header(const char* header, double* depth);
 
 #ifdef __cplusplus
 }
