@@ -120,6 +120,18 @@ class AcDepthInfo(C.Structure):
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
+class AcQvInfo(C.Structure):
+    _fields_ = [("assemblies", C.c_uint64), ("contigs", C.c_uint64), ("k", C.c_uint32), ("min_count", C.c_uint32), ("valley", C.c_uint64),
+                ("reads", C.c_uint64), ("read_windows", C.c_uint64), ("read_bases", C.c_uint64), ("distinct", C.c_uint64),
+                ("solid_kmers", C.c_uint64), ("assembly_windows", C.c_uint64), ("table_bytes", C.c_uint64), ("spectrum_table_bytes", C.c_uint64),
+                ("partitions", C.c_uint64), ("reruns", C.c_uint64), ("kernel_ms", C.c_float), ("scan_ms", C.c_float), ("pack_ms", C.c_float),
+                ("insert_ms", C.c_float), ("probe_ms", C.c_float), ("count_ms", C.c_float), ("assembly_ms", C.c_float), ("read_ms", C.c_double),
+                ("copy_ms", C.c_double)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_sequence", "ac_clear_sequences", "ac_upload",
            "ac_build", "ac_compress", "ac_simplify", "ac_merge_linear_paths", "ac_renumber_unitigs", "ac_load_gfa", "ac_bind_host_to_device", "ac_decompress_gfa", "ac_pairwise_distances", "ac_distance_matrix_text", "ac_sequence_reconstruct", "ac_counts_get", "ac_unitigs_copy", "ac_path_copy", "ac_gfa_size", "ac_gfa_copy",
            "ac_timings_get", "ac_compress_dir", "ac_compress_dir_devices", "ac_load_sequences", "ac_sequence_get",
@@ -133,7 +145,7 @@ EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_seq
            "ac_clean_gfa", "ac_clean_text", "ac_gfa_to_fasta", "ac_gfa_fasta_text", "ac_table_text",
            "ac_subsample_dir", "ac_genome_size", "ac_subsample_words", "ac_subsample_shuffle",
            "ac_genome_size_estimate", "ac_genome_size_from_histogram",
-           "ac_depth_fasta", "ac_depth_filter_text", "ac_depth_from_header"]
+           "ac_depth_fasta", "ac_depth_filter_text", "ac_depth_from_header", "ac_qv_dir"]
 
 _libs = {}
 
@@ -255,6 +267,8 @@ def load_library(path=None):
     lib.ac_depth_filter_text.argtypes = [C.c_char_p, C.c_uint64, C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_void_p, C.c_uint64,
                                          C.POINTER(C.c_uint64)]
     lib.ac_depth_from_header.argtypes = [C.c_char_p, C.POINTER(C.c_double)]
+    lib.ac_qv_dir.argtypes = [C.c_char_p, C.POINTER(C.c_char_p), C.c_uint32, C.c_char_p, C.c_uint32, C.POINTER(C.c_uint32), C.c_int32, C.c_int32,
+                              C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.c_uint64, C.POINTER(AcQvInfo)]
     lib.ac_table_text.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint64, C.c_int32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     _libs[path] = lib
     return lib
@@ -889,3 +903,37 @@ def depth_from_header(header, lib=None):
         return None
     _raise_unless_ok(lib, rc)
     return d.value
+
+
+def qv(reads, assemblies, out_dir, k=21, min_count=None, device=0, verbose=False, lib=None):
+    """`autocycler qv` (DESIGN.md §20): each assembly's k-mer QV and completeness against the reads, counted on the GPU (not in the
+    reference).  assemblies: FASTA files or directories (expanded as find_all_assemblies does).  Returns the info dict (t is "min_count", S
+    "solid_kmers", the stage timings in ms) with "assemblies": per assembly a dict of path, kmers, unsupported, solid_found and qv (None for
+    an empty field, float("inf") for inf), and "contigs": per contig a dict of assembly, contig, length, kmers, unsupported and qv, both
+    read back from the qv.tsv and contig_qv.tsv the call wrote."""
+    lib = lib or load_library()
+    paths = [assemblies] if isinstance(assemblies, (str, bytes, os.PathLike)) else list(assemblies)
+    cap = sum(len(os.listdir(p)) if os.path.isdir(p) else 1 for p in paths)
+    arr = (C.c_char_p * max(1, len(paths)))(*[os.fsencode(p) for p in paths])
+    kmers, unsupported, found = ((C.c_uint64 * max(1, cap))() for _ in range(3))
+    info = AcQvInfo()
+    t = None if min_count is None else C.byref(C.c_uint32(min_count))
+    _raise_unless_ok(lib, lib.ac_qv_dir(os.fsencode(reads), arr, len(paths), os.fsencode(out_dir), k, t, device, 1 if verbose else 0, kmers,
+                                        unsupported, found, cap, C.byref(info)))
+    out = info.as_dict()
+
+    def rows(name):
+        with open(os.path.join(out_dir, name)) as f:
+            lines = f.read().splitlines()
+        head = lines[0].split("\t")
+        return [dict(zip(head, line.split("\t"))) for line in lines[1:]]
+
+    def qv_value(text):
+        return None if text == "" else float(text)
+
+    n = min(cap, out["assemblies"])
+    out["assemblies"] = [{"path": r["assembly"], "kmers": kmers[i], "unsupported": unsupported[i], "solid_found": found[i],
+                          "qv": qv_value(r["qv"]), "completeness": qv_value(r["completeness"])} for i, r in enumerate(rows("qv.tsv")[:n])]
+    out["contigs"] = [{"assembly": r["assembly"], "contig": r["contig"], "length": int(r["length"]), "kmers": int(r["kmers"]),
+                       "unsupported": int(r["unsupported"]), "qv": qv_value(r["qv"])} for r in rows("contig_qv.tsv")]
+    return out

@@ -30,6 +30,7 @@
 #include "host_subsample.h"
 #include "host_genome_size.h"
 #include "host_depth.h"
+#include "host_qv.h"
 #include <mutex>
 #include <immintrin.h>
 #include <functional>
@@ -1634,11 +1635,11 @@ int ac_png_write(const char* path, const uint8_t* rgb, uint32_t width, uint32_t 
 // ---- `autocycler subsample` (subsample.rs) --------------------------------------------------------------------------------------
 namespace {
 // One subsample device object per device, as for dotplot: its buffers (and pinned windows) are kept for the next call on that device.
-// genome_size and depth read through the same object and keep their packed streams and tables beside it.
+// genome_size, depth and qv read through the same object and keep their packed streams and tables beside it.
 std::mutex g_subsample_mu;
 struct SubsampleDevice {
-    DeviceContext ctx; DeviceSubsample sub; DeviceSpectrum spec; DeviceDepth depth;
-    explicit SubsampleDevice(int32_t device) : ctx(device, nullptr), sub(ctx), spec(ctx), depth(ctx) {}
+    DeviceContext ctx; DeviceSubsample sub; DeviceSpectrum spec; DeviceDepth depth; DeviceQv qv;
+    explicit SubsampleDevice(int32_t device) : ctx(device, nullptr), sub(ctx), spec(ctx), depth(ctx), qv(ctx) {}
 };
 SubsampleDevice& subsample_device(int32_t device) {        // with g_subsample_mu held
     static std::vector<std::pair<int32_t, SubsampleDevice*>> devices;
@@ -1890,6 +1891,90 @@ int ac_depth_from_header(const char* header, double* depth) {
     if (!header || !depth) return set_error(nullptr, AC_EINVAL, "null argument");
     AC_GUARD_BEGIN
     if (!depth_from_header(header, *depth)) return set_error(nullptr, AC_EINPUT, "the header carries no depth");
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
+// ---- `autocycler qv`: each assembly's k-mer QV and completeness against the reads (not in the reference) -----------------------------
+int ac_qv_dir(const char* reads, const char* const* inputs, uint32_t n_inputs, const char* out_dir, uint32_t k, const uint32_t* min_count,
+              int32_t device, int32_t verbose, uint64_t* kmers, uint64_t* unsupported, uint64_t* solid_found, uint64_t cap, ac_qv_info* info) {
+    if (!reads || !out_dir || (!inputs && n_inputs)) return set_error(nullptr, AC_EINVAL, "null argument");
+    for (uint32_t i = 0; i < n_inputs; ++i) if (!inputs[i]) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    const std::string in = reads, dir = out_dir;
+    if (!n_inputs) return set_error(nullptr, AC_EINPUT, "no assemblies given");
+    if (k < 11 || k > 31 || k % 2 == 0) return set_error(nullptr, AC_EINPUT, "--kmer must be odd and between 11 and 31");
+    if (min_count && (*min_count < 1 || *min_count > AC_GS_BINS - 1))
+        return set_error(nullptr, AC_EINPUT, "--min_count must be between 1 and " + std::to_string(AC_GS_BINS - 1));
+    int rc;
+    if ((rc = check_file(in)) != AC_OK) return rc;
+    const std::vector<std::string> paths = qv_inputs(std::vector<std::string>(inputs, inputs + n_inputs));
+    struct stat st;
+    if (stat(dir.c_str(), &st) == 0 && !S_ISDIR(st.st_mode)) return set_error(nullptr, AC_EINPUT, dir + " exists but is not a directory");
+    if (!make_dirs(dir)) return set_error(nullptr, AC_EINPUT, "failed to create directory " + dir + "\n" + strerror(errno));
+    if (verbose) {
+        fprintf(stderr, "\nStarting autocycler qv\n    This command measures each assembly's k-mer accuracy (QV) and completeness against the reads, "
+                        "counted on the GPU. It is not in the reference.\n\nSettings:\n  --reads %s\n  --assemblies", in.c_str());
+        for (const std::string& p : paths) fprintf(stderr, " %s", p.c_str());
+        fprintf(stderr, "\n  --out_dir %s\n  --kmer %u\n", dir.c_str(), k);
+        if (min_count) fprintf(stderr, "  --min_count %u\n", *min_count);
+        fprintf(stderr, "\n");
+    }
+    QvResult r;
+    {
+        std::lock_guard<std::mutex> lock(g_subsample_mu);
+        SubsampleDevice& d = subsample_device(device);
+        try {
+            qv_run(d.sub, d.spec, d.qv, paths, in, k, min_count, subsample_window_size(), r);
+        } catch (const AcIoError& e) { return set_error(nullptr, AC_EIO, e.msg); }
+        catch (const std::length_error& e) { return set_error(nullptr, AC_ERANGE, e.what()); }
+    }
+    for (const char* sub : {"/unsupported", "/spectra_cn"})
+        if (!make_dirs(dir + sub)) return set_error(nullptr, AC_EIO, "failed to create directory " + dir + sub + "\n" + strerror(errno));
+    std::vector<std::pair<std::string, std::string>> files{{"qv.tsv", qv_table(r, k)}, {"contig_qv.tsv", qv_contig_table(r, k)},
+                                                           {"kmer_histogram.tsv", qv_histogram(r)}};
+    for (size_t a = 0; a < r.assemblies.size(); ++a) {
+        files.emplace_back("unsupported/" + std::to_string(a + 1) + ".bed", r.assemblies[a].bed);
+        files.emplace_back("spectra_cn/" + std::to_string(a + 1) + ".tsv", r.assemblies[a].spectrum);
+    }
+    for (const auto& f : files)
+        if (!write_file(dir + "/" + f.first, f.second)) return set_error(nullptr, AC_EIO, "cannot write " + dir + "/" + f.first);
+    uint64_t contigs = 0;
+    for (size_t a = 0; a < r.assemblies.size(); ++a) {
+        const QvAssembly& as = r.assemblies[a];
+        contigs += as.contigs.size();
+        if (a < cap) {
+            if (kmers) kmers[a] = as.kmers;
+            if (unsupported) unsupported[a] = as.unsupported;
+            if (solid_found) solid_found[a] = as.solid_found;
+        }
+    }
+    if (verbose) {
+        fprintf(stderr, "K-mer QV (k = %u):\n  reads: %llu\n  read k-mer windows: %llu\n  distinct read k-mers: %llu\n  valley: %s\n"
+                        "  min_count: %llu%s\n  solid read k-mers: %llu\n  assembly k-mer windows: %llu\n\n", k, (unsigned long long)r.reads,
+                (unsigned long long)r.read_windows, (unsigned long long)r.distinct, r.valley ? std::to_string(r.valley).c_str() : "none",
+                (unsigned long long)r.min_count, min_count ? " (given)" : " (the valley)", (unsigned long long)r.solid,
+                (unsigned long long)r.device.assembly_windows);
+        for (const QvAssembly& as : r.assemblies) {
+            fprintf(stderr, "  %s: QV %s, %llu of %llu k-mers unsupported", as.path.c_str(), qv_text(as.unsupported, as.kmers, k).c_str(),
+                    (unsigned long long)as.unsupported, (unsigned long long)as.kmers);
+            if (r.solid) fprintf(stderr, ", completeness %.2f%%", 100.0 * (double)as.solid_found / (double)r.solid);
+            fprintf(stderr, "\n");
+        }
+        fprintf(stderr, "\nFinished!\nQV table: %s/qv.tsv\n\n", dir.c_str());
+    }
+    if (info) {
+        *info = ac_qv_info{};
+        info->assemblies = r.assemblies.size(); info->contigs = contigs; info->k = k; info->min_count = (uint32_t)r.min_count;
+        info->valley = r.valley; info->reads = r.reads; info->read_windows = r.read_windows; info->read_bases = r.read_bases;
+        info->distinct = r.distinct; info->solid_kmers = r.solid; info->assembly_windows = r.device.assembly_windows;
+        info->table_bytes = r.device.table_bytes; info->spectrum_table_bytes = r.spectrum.table_bytes; info->partitions = r.spectrum.partitions;
+        info->reruns = r.spectrum.reruns;
+        info->kernel_ms = r.kernel_ms; info->scan_ms = r.scan_ms; info->pack_ms = r.pack_reads_ms;
+        info->insert_ms = r.device.pack_ms + r.device.insert_ms; info->probe_ms = r.device.probe_ms;
+        info->count_ms = r.spectrum.count_ms + r.spectrum.hist_ms; info->assembly_ms = r.device.assembly_ms;
+        info->read_ms = r.read_ms; info->copy_ms = r.copy_ms;
+    }
     return ok(nullptr);
     AC_GUARD_END(nullptr)
 }

@@ -2,7 +2,8 @@
 // `autocycler clean`, `autocycler gfa2fasta`, `autocycler table` and `autocycler subsample` with the reference's flags (main.rs:126-162), messages and exit codes
 // (misc.rs:130-136: "Error: <text>" on stderr, exit 1), running the H100 path through the C ABI; `autocycler helper genome_size`,
 // which departs from the reference on purpose: a k-mer depth estimate on the GPU instead of the length of a Raven assembly; and
-// `autocycler depth`, read-measured contig depth (not in the reference) with the reference's helper depth filter.
+// `autocycler depth`, read-measured contig depth (not in the reference) with the reference's helper depth filter; and `autocycler qv`,
+// each assembly's k-mer QV and completeness against the reads (not in the reference).
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -378,6 +379,50 @@ static int depth_main(int argc, char** argv) {
                                  nullptr, nullptr, 0, nullptr));
 }
 
+// `autocycler qv`: each assembly's k-mer QV and completeness against the reads, counted on the GPU (not in the reference).  qv.tsv also
+// goes to stdout, byte for byte.
+static const char* qv_usage =
+    "Usage: autocycler qv --reads <READS> --assemblies <FASTA|DIR>... --out_dir <DIR> [--kmer 21] [--min_count N] [--device N]\n\n"
+    "Measures each assembly's k-mer accuracy (QV) and completeness against the reads, counted on the GPU, as Merqury defines them: QV\n"
+    "from the assembly k-mers the reads do not support, completeness from the reads' solid k-mers the assembly holds. This command is\n"
+    "not in the reference. Writes qv.tsv (also to stdout), contig_qv.tsv, kmer_histogram.tsv, unsupported/<n>.bed and spectra_cn/<n>.tsv.\n\n"
+    "Options:\n"
+    "  -r, --reads <READS>            Long reads in FASTQ format, gzipped or not (required)\n"
+    "  -i, --assemblies <FASTA|DIR>...  Assemblies in FASTA format, gzipped or not, or directories of them (required)\n"
+    "  -o, --out_dir <DIR>            Directory to create and write the tables into (required)\n"
+    "      --kmer <KMER>              K-mer size, odd, 11 to 31 [default: 21]\n"
+    "      --min_count <N>            Read count from which a k-mer supports the assembly, 1 to 16383 (1: Merqury's QV)\n"
+    "                                 [default: the valley of the reads' k-mer spectrum]\n"
+    "      --device <ORDINAL>         CUDA device [default: 0]\n";
+static int qv_main(int argc, char** argv) {
+    Args a{argc, argv, qv_usage};
+    std::string reads, out; std::vector<std::string> inputs; bool has_min = false; unsigned long k = 21, min_count = 0; int device = 0;
+    while (a.next()) {
+        if (a.is("-r", "--reads")) reads = a.value();
+        else if (a.is("-i", "--assemblies")) { const std::vector<std::string> v = a.values(); inputs.insert(inputs.end(), v.begin(), v.end()); }
+        else if (a.is("-o", "--out_dir")) out = a.value();
+        else if (a.is("--kmer")) k = (unsigned long)a.number(true);
+        else if (a.is("--min_count")) { min_count = (unsigned long)a.number(true); has_min = true; }
+        else if (a.is("--device")) device = atoi(a.value());
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
+    }
+    if (reads.empty() || out.empty() || inputs.empty()) return a.missing();
+    const std::vector<const char*> ptrs = c_strings(inputs);
+    const uint32_t t = min_count > 0xFFFFFFFFul ? 0 : (uint32_t)min_count;
+    const int rc = ac_qv_dir(reads.c_str(), ptrs.data(), (uint32_t)ptrs.size(), out.c_str(), k > 0xFFFFFFFFul ? 0 : (uint32_t)k, has_min ? &t : nullptr,
+                             device, 1, nullptr, nullptr, nullptr, 0, nullptr);
+    if (rc == AC_OK) {
+        FILE* f = fopen((out + "/qv.tsv").c_str(), "rb");
+        if (f) {
+            char buf[1 << 16]; size_t n;
+            while ((n = fread(buf, 1, sizeof buf, f)) > 0) fwrite(buf, 1, n, stdout);
+            fclose(f);
+        }
+    }
+    return finish(rc);
+}
+
 int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "dotplot") == 0) return dotplot_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "resolve") == 0) return resolve_main(argc, argv);
@@ -392,6 +437,7 @@ int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "subsample") == 0) return subsample_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "helper") == 0) return helper_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "depth") == 0) return depth_main(argc, argv);
+    if (argc >= 2 && strcmp(argv[1], "qv") == 0) return qv_main(argc, argv);
     fprintf(stderr, "%s", compress_usage);
     return 2;
 }

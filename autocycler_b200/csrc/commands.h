@@ -1,4 +1,4 @@
-// The device parts of `autocycler trim`, `resolve`, `cluster`, `dotplot`, `subsample`, `helper genome_size` and `depth`.  Each object owns its device buffers (allocated on first
+// The device parts of `autocycler trim`, `resolve`, `cluster`, `dotplot`, `subsample`, `helper genome_size`, `depth` and `qv`.  Each object owns its device buffers (allocated on first
 // use, kept for the next call) and runs on the device and stream of the DeviceContext it is given, which must outlive it.
 #pragma once
 #include <cstdint>
@@ -225,4 +225,40 @@ private:
     uint32_t k = 21, n_contigs = 0;
     uint64_t slots = 0;
     DevBuf d_bytes, d_contig, d_woff, d_code, d_valid, d_wcid, d_table, d_unique, d_rank, d_prefix, d_hist, d_median;
+};
+
+// `autocycler qv`: each assembly's k-mer accuracy and completeness against the reads (DESIGN.md §20).  Every assembly's contigs are packed
+// into one stream (depth's layout) and their canonical keys claimed in one combined DepthSlot table with the flags left 0, so the reads'
+// packed stream, probed once with DpProbeBody, counts every hit.  Then, per assembly, a multiplicity table of its own keys (each with the
+// reads' count copied from the combined table), a mask of its unsupported windows, and its copy-number spectrum.
+struct QvSlot { uint64_t key; uint32_t m, r; };              // key: canonical k-mer + 1 (0: empty); m: the assembly's windows; r: the reads'
+#define AC_QV_CN 5                                           // copy-number columns of the spectrum: m = 0 (unused on the device), 1, 2, 3, 4+
+// What the device ran: every assembly's windows, the two tables' bytes and the kernels' time by stage (CUDA events; 0 under emulation).
+struct QvRun { uint64_t assembly_windows = 0, table_bytes = 0; float pack_ms = 0.f, insert_ms = 0.f, probe_ms = 0.f, assembly_ms = 0.f; };
+
+class DeviceQv {
+public:
+    explicit DeviceQv(DeviceContext& ctx) : ctx(ctx) {}
+    ~DeviceQv() { ctx.make_current(); }
+    // The combined table and the per-assembly buffers.  bytes: every contig's bytes back to back (a circular contig followed by its first
+    // k-1 bases), contig c taking len[c] of them; assembly a holds contigs first[a] .. first[a+1]-1 and windows[a] windows of k A/C/G/T
+    // bases.  The combined table takes max(2 sum windows, 64) slots, the multiplicity table max(2 max windows, 64); std::length_error when
+    // the two exceed budget_slots.
+    void build(const uint8_t* bytes, const uint64_t* len, uint32_t n_contigs, const uint32_t* first, uint32_t n_assemblies,
+               const uint64_t* windows, uint32_t k, uint64_t budget_slots, QvRun* run);
+    // Counts every window of the reads `spec` packed (after build, with the same k) into the assembly key it hits.
+    void probe(DeviceSpectrum& spec, QvRun* run);
+    // Assembly a against the threshold t: mask[i] (one u32 per packed word of its contigs, from contig first[a]'s first word) has bit j
+    // set when the window that ends at base j of that word has a read count below t; spectrum[c * AC_QV_CN + m] (AC_GS_BINS rows) counts
+    // its distinct keys with read count bin c (min(r, AC_GS_BINS - 1)) that occur m times (4: 4 or more) over its windows.
+    void assembly(uint32_t a, uint32_t t, uint32_t* mask, uint32_t* spectrum, QvRun* run);
+    // The first packed word of every contig, and one past the last (n_contigs + 1 values), as build laid them out.
+    const std::vector<uint64_t>& word_offsets() const { return woff; }
+private:
+    DeviceContext& ctx;
+    uint32_t k = 21;
+    uint64_t slots = 0, mult_slots = 0;
+    std::vector<uint64_t> woff, win;
+    std::vector<uint32_t> first_contig;
+    DevBuf d_bytes, d_contig, d_code, d_valid, d_wcid, d_table, d_mult, d_mask, d_spec;
 };

@@ -3,7 +3,7 @@
 // filter on the depths (host_depth.cpp) is.  This file compiles with nvcc for sm_90a (product) and with g++ -DAC_EMULATE (tests/emu,
 // serial execution of the same bodies).
 #include "commands.h"
-#include "gs_kmers.h"
+#include "dp_kmers.h"
 
 #include <algorithm>
 #include <cmath>
@@ -14,51 +14,6 @@
 // depth: pack, insert, probe and median, see DESIGN.md §19
 // ------------------------------------------------------------------------------------------------
 namespace {
-struct DpContig { uint64_t off, len, woff; };      // bytes at off, len of them (junction bases included), first packed word
-
-// Adds 1 to *p.  On the device the lanes of a warp that add to the same address are grouped first, one atomic per group: in the
-// median's passes every unique key of a long contig adds to the same few bins.
-#ifdef AC_EMULATE
-inline void dp_add_one(uint32_t* p) { ++*p; }
-#else
-__device__ __forceinline__ void dp_add_one(uint32_t* p) {
-    const unsigned same = __match_any_sync(__activemask(), (unsigned long long)p);
-    if ((int)(threadIdx.x & 31) == __ffs((int)same) - 1) atomicAdd(p, (unsigned)__popc(same));
-}
-#endif
-
-// Calls f(canonical key) for each window that ends in word w: the forward and reverse keys roll over word w-1's last k-1 bases and then
-// w's 32, as GsCountBody's do.
-template <class F> AC_D void dp_each_key(const uint64_t* code, const uint32_t* valid, uint64_t w, uint32_t k, F&& f) {
-    const uint32_t ends = gs_window_ends(valid[w], w ? valid[w - 1] : 0, k);
-    if (!ends) return;
-    const uint64_t c = code[w], pc = w ? code[w - 1] : 0, mask = (1ull << (2 * k)) - 1;
-    const uint32_t top = 2 * (k - 1);
-    uint64_t fw = 0, rc = 0;
-    for (uint32_t i = 32 - (k - 1); i < 32; ++i) {
-        const uint64_t b = (pc >> (2 * i)) & 3;
-        fw = ((fw << 2) | b) & mask; rc = (rc >> 2) | ((3 - b) << top);
-    }
-    for (uint32_t i = 0; i < 32; ++i) {
-        const uint64_t b = (c >> (2 * i)) & 3;
-        fw = ((fw << 2) | b) & mask; rc = (rc >> 2) | ((3 - b) << top);
-        if ((ends >> i) & 1) f(fw < rc ? fw : rc);
-    }
-}
-
-// One thread per packed word of the assembly: its contig (a binary search over the word offsets), codes, validity mask and contig id.
-struct DpPackBody {
-    const uint8_t* bytes; const DpContig* contig; uint32_t n; uint64_t* code; uint32_t* valid; uint32_t* wcid;
-    AC_D void operator()(uint64_t w) const {
-        uint32_t lo = 0, hi = n;                             // the last contig whose first word is <= w
-        while (hi - lo > 1) { const uint32_t mid = (lo + hi) / 2; if (contig[mid].woff <= w) lo = mid; else hi = mid; }
-        const DpContig o = contig[lo];
-        uint64_t c;
-        valid[w] = gs_pack_word(bytes + o.off, o.len, w - o.woff, &c);
-        code[w] = c;
-        wcid[w] = lo;
-    }
-};
 // One thread per packed word of the assembly: each window's key is inserted by linear probing from its home slot, claimed with a CAS
 // on the empty key.  The claimer ORs its contig id into the flags; every later occurrence ORs AC_DEPTH_DUP.  The table holds at least
 // twice the windows, so a probe always finds its key or an empty slot.
@@ -74,27 +29,6 @@ struct DpInsertBody {
                 if (cur == 0) cur = ac_atomic_cas(&q->key, (uint64_t)0, tag);
                 if (cur == 0) { ac_atomic_or(&q->flags, wcid[w]); return; }
                 if (cur == tag) { ac_atomic_or(&q->flags, AC_DEPTH_DUP); return; }
-                if (++s == slots) s = 0;
-            }
-        });
-    }
-};
-// One thread per packed word of the reads: each window is a lookup that stops at its key or the first empty slot.  A hit on a unique
-// key adds 1 while a plain read shows the count below 2^31 (GsCountBody's guard).
-struct DpProbeBody {
-    const uint64_t* code; const uint32_t* valid; uint32_t k; DepthSlot* table; uint64_t slots;
-    AC_D void operator()(uint64_t w) const {
-        dp_each_key(code, valid, w, k, [&](uint64_t key) {
-            uint64_t s = ac_umul64hi(gs_mix(key), slots);
-            const uint64_t tag = key + 1;
-            for (;;) {
-                DepthSlot* q = table + s;
-                const uint64_t cur = q->key;
-                if (cur == 0) return;
-                if (cur == tag) {
-                    if (!(q->flags & AC_DEPTH_DUP) && ac_ld_volatile(&q->count) < 0x80000000u) ac_atomic_add(&q->count, 1u);
-                    return;
-                }
                 if (++s == slots) s = 0;
             }
         });

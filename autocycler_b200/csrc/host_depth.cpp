@@ -65,6 +65,22 @@ std::string depth_filter_text(const std::string& text, const std::string& name, 
     return out;
 }
 
+uint64_t pack_contig(const FastaRecord& r, uint32_t k, std::string& bytes) {
+    std::string lower = r.header;
+    for (char& ch : lower) if (ch >= 'A' && ch <= 'Z') ch = (char)(ch + 32);
+    const bool circular = lower.find("circular=true") != std::string::npos && r.seq.size() >= k;    // rotate_plassembler_contigs' test, helper.rs:866
+    const size_t start = bytes.size();
+    bytes += r.seq;
+    if (circular) bytes.append(r.seq, 0, k - 1);
+    uint64_t run = 0, windows = 0;
+    for (size_t i = start; i < bytes.size(); ++i) {
+        const char b = bytes[i];
+        run = (b == 'A' || b == 'C' || b == 'G' || b == 'T') ? run + 1 : 0;
+        windows += run >= k;
+    }
+    return windows;
+}
+
 void depth_run(DeviceSubsample& sub, DeviceSpectrum& spec, DeviceDepth& dev, const std::string& assembly, const std::string& reads, uint32_t k,
                uint64_t window, DepthResult& out) {
     out = DepthResult();
@@ -75,38 +91,19 @@ void depth_run(DeviceSubsample& sub, DeviceSpectrum& spec, DeviceDepth& dev, con
         if (depth_from_header(r.header, d))
             throw InputError{assembly + ": the header of " + r.name + " already carries a depth; use --source header to filter by it"};
     }
-    // the contigs back to back, a circular one (rotate_plassembler_contigs' test, helper.rs:866) followed by its first k-1 bases
     std::string bytes;
     std::vector<uint64_t> len(recs.size());
     uint64_t windows = 0;
     for (size_t c = 0; c < recs.size(); ++c) {
-        const std::string& seq = recs[c].seq;
-        std::string lower = recs[c].header;
-        for (char& ch : lower) if (ch >= 'A' && ch <= 'Z') ch = (char)(ch + 32);
-        const bool circular = lower.find("circular=true") != std::string::npos && seq.size() >= k;
         const size_t start = bytes.size();
-        bytes += seq;
-        if (circular) bytes.append(seq, 0, k - 1);
+        windows += pack_contig(recs[c], k, bytes);
         len[c] = bytes.size() - start;
-        uint64_t run = 0;
-        for (size_t i = start; i < bytes.size(); ++i) {
-            const char b = bytes[i];
-            run = (b == 'A' || b == 'C' || b == 'G' || b == 'T') ? run + 1 : 0;
-            windows += run >= k;
-        }
     }
     const uint64_t budget_env = genome_size_env("AC_DEPTH_TABLE_SLOTS");
     const uint64_t budget = budget_env ? budget_env : ac_gs_budget_slots();
     dev.build((const uint8_t*)bytes.data(), len.data(), (uint32_t)std::min<size_t>(recs.size(), 0xFFFFFFFFu), windows, k, budget, &out.device);
-    sub.kernel_ms = 0.f; sub.copy_ms = 0.0;
-    spec.begin(k);
-    SubsampleRun pass;
-    fastq_windows(sub, reads, window, false, pass, [&](uint64_t, uint64_t records) {
-        spec.pack_window(sub, records);
-        out.reads += records;
-    });
-    out.read_ms = pass.read_ms;
-    out.copy_ms = sub.copy_ms;
+    const ReadPass pass = pack_reads(sub, spec, reads, k, window);
+    out.reads = pass.reads; out.read_ms = pass.read_ms; out.copy_ms = pass.copy_ms;
     spec.totals(&out.read_windows, &out.read_bases);
     dev.probe(spec, &out.device);
     out.unique.assign(recs.size(), 0);

@@ -28,6 +28,10 @@ std::string depth_filter_text(const std::string& text, const std::string& name, 
 // Rust's `{:.N}` of an f64 (NaN, inf and -inf spelled as Rust does).
 std::string rust_fixed(double x, int digits);
 
+// Appends contig r to bytes as the device packs it: its sequence, followed by its first k-1 bases when its header holds
+// "circular=true" (any case) and it is at least k long.  Returns its windows of k A/C/G/T bases (shared with qv).
+uint64_t pack_contig(const FastaRecord& r, uint32_t k, std::string& bytes);
+
 struct DepthResult {
     std::vector<FastaRecord> recs;
     std::vector<uint64_t> unique;            // per contig: its unique keys

@@ -7,18 +7,25 @@
 #include "host_io.h"
 #include "host_subsample.h"
 
+const char* const genome_size_no_peak = "no k-mer depth peak: the reads are too shallow or too noisy for a k-mer estimate";
+
+uint64_t genome_size_valley(const uint64_t* h) {
+    const uint64_t H = AC_GS_BINS;
+    // s[c] = h[c-1] + h[c] + h[c+1], with h[0] taken as h[1] (the edge bin repeated: with 0 there, s[1] would sum two bins against
+    // s[2]'s three, and any k-mer seen three times would put the valley at 1); the valley is the smallest c >= 1 with s[c] < s[c+1]
+    auto s = [&](uint64_t c) { return (c > 1 ? h[c - 1] : h[1]) + h[c] + h[c + 1]; };
+    for (uint64_t c = 1; c + 2 < H; ++c)
+        if (s(c) < s(c + 1)) return c;
+    return 0;
+}
+
 void genome_size_rule(const uint64_t* h, uint64_t W, GenomeSizeRun& run) {
     const uint64_t H = AC_GS_BINS;
     run.windows = W;
     run.distinct = 0;
     for (uint64_t c = 1; c < H; ++c) run.distinct += h[c];
-    // s[c] = h[c-1] + h[c] + h[c+1], with h[0] taken as h[1] (the edge bin repeated: with 0 there, s[1] would sum two bins against
-    // s[2]'s three, and any k-mer seen three times would put the valley at 1); the valley is the smallest c >= 1 with s[c] < s[c+1]
-    auto s = [&](uint64_t c) { return (c > 1 ? h[c - 1] : h[1]) + h[c] + h[c + 1]; };
-    uint64_t v = 0;
-    for (uint64_t c = 1; c + 2 < H; ++c)
-        if (s(c) < s(c + 1)) { v = c; break; }
-    if (!v) throw InputError{"no k-mer depth peak: the reads are too shallow or too noisy for a k-mer estimate"};
+    const uint64_t v = genome_size_valley(h);
+    if (!v) throw InputError{genome_size_no_peak};
     uint64_t p = v + 1;
     for (uint64_t c = v + 1; c < H - 1; ++c)
         if (h[c] > h[p]) p = c;
@@ -42,19 +49,26 @@ uint64_t genome_size_env(const char* name) {
     return e && *e ? strtoull(e, nullptr, 10) : 0;
 }
 
-void genome_size_run(DeviceSubsample& sub, DeviceSpectrum& spec, const std::string& reads, uint32_t k, uint64_t window,
-                     std::vector<uint64_t>& hist, GenomeSizeRun& run) {
-    run = GenomeSizeRun();
-    run.k = k;
+ReadPass pack_reads(DeviceSubsample& sub, DeviceSpectrum& spec, const std::string& reads, uint32_t k, uint64_t window) {
+    ReadPass out;
     sub.kernel_ms = 0.f; sub.copy_ms = 0.0;
     spec.begin(k);
     SubsampleRun pass;
     fastq_windows(sub, reads, window, false, pass, [&](uint64_t, uint64_t records) {
         spec.pack_window(sub, records);
-        run.reads += records;
+        out.reads += records;
     });
-    run.read_ms = pass.read_ms;
-    run.copy_ms = sub.copy_ms;
+    out.read_ms = pass.read_ms;
+    out.copy_ms = sub.copy_ms;
+    return out;
+}
+
+void genome_size_run(DeviceSubsample& sub, DeviceSpectrum& spec, const std::string& reads, uint32_t k, uint64_t window,
+                     std::vector<uint64_t>& hist, GenomeSizeRun& run) {
+    run = GenomeSizeRun();
+    run.k = k;
+    const ReadPass pass = pack_reads(sub, spec, reads, k, window);
+    run.reads = pass.reads; run.read_ms = pass.read_ms; run.copy_ms = pass.copy_ms;
     spec.totals(&run.windows, &run.bases);
     if (!run.windows) throw InputError{"no k-mer windows: no read holds " + std::to_string(k) + " consecutive A, C, G or T bases"};
     hist.assign(AC_GS_BINS, 0);

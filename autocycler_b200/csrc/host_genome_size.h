@@ -22,6 +22,16 @@ struct GenomeSizeRun {
 // k-mers' occurrences exceed W, RangeError when the peak is at the cap or p* is not positive.
 void genome_size_rule(const uint64_t* hist, uint64_t windows, GenomeSizeRun& run);
 
+// The valley of hist[AC_GS_BINS]: the smallest c >= 1 whose smoothed sum h[c-1] + h[c] + h[c+1] (h[0] taken as h[1]) is below the next
+// one; 0 when there is none.  genome_size_no_peak is the message for that case.
+uint64_t genome_size_valley(const uint64_t* hist);
+extern const char* const genome_size_no_peak;
+
+// One pass of subsample's windows over a FASTQ file (gzipped or not), each window packed into spec's stream (begun here with k): the
+// records, the time reading and gunzipping the file, and the window uploads' time.  sub.kernel_ms holds the record scan's kernels after.
+struct ReadPass { uint64_t reads = 0; double read_ms = 0, copy_ms = 0; };
+ReadPass pack_reads(DeviceSubsample& sub, DeviceSpectrum& spec, const std::string& reads, uint32_t k, uint64_t window);
+
 // The spectrum of one FASTQ file (gzipped or not): one pass of windows (subsample's scan and messages), each window packed on the
 // device, then the partitions counted.  hist gets the AC_GS_BINS bins; genome_size_rule makes the estimate from them.  InputError for a
 // malformed file or no k-mer windows, AcIoError when the file cannot be read.

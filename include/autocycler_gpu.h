@@ -32,6 +32,7 @@
  *       (a deliberate departure: a k-mer depth estimate from the reads on the GPU, not the length of a Raven assembly)
  *   depth_filter, depth_from_header         helper.rs:889-931        -> ac_depth_filter_text, ac_depth_from_header
  *   depth (read-measured contig depth)      not in the reference     -> ac_depth_fasta
+ *   qv (k-mer QV and completeness)          not in the reference     -> ac_qv_dir
  *
  * Conventions: every function returns 0 on success and a negative AC_E* code on failure; the message
  * is available from ac_last_error(handle) (or ac_last_error(NULL) when no handle exists).  No C++
@@ -507,6 +508,41 @@ int ac_depth_filter_text(const char* fasta_text, uint64_t length, const double* 
                          uint64_t* out_length);
 /* helper.rs:923-931: the depth a header carries (depth=, then depth-, then coverage=).  AC_EINPUT when it carries none.  Host only. */
 int ac_depth_from_header(const char* header, double* depth);
+
+/* `autocycler qv -r reads -i assemblies... -o out_dir [--kmer 21] [--min_count N]`: each assembly's k-mer accuracy and completeness
+ * against the reads (Merqury's QV and completeness), counted on the GPU.  Not in the reference (DESIGN.md section 20).  inputs: n_inputs
+ * paths, each a FASTA file (gzipped or not, loaded as load_fasta does) or a directory, expanded as find_all_assemblies does.  Contig
+ * windows are depth's (k A/C/G/T bases; a contig whose header holds "circular=true", any case, and whose length is at least k also gets the
+ * k-1 windows across its end); read windows and the histogram are genome_size's.  r(key): the read windows with that canonical key.  The
+ * solid threshold t is *min_count (1 .. AC_GENOME_SIZE_BINS - 1, else AC_EINPUT), or the histogram's valley when min_count is NULL (no
+ * valley: AC_EINPUT "no k-mer depth peak: ...").  Per assembly: K windows, E of them with r < t, QV = -10 log10(-expm1(log1p(-E/K) / k))
+ * (`%.2f`, "inf" for E = 0); S = the distinct read keys with count >= t; completeness = 100 x (its distinct keys with r >= t) / S.
+ * out_dir (created if needed) gets qv.tsv, contig_qv.tsv, kmer_histogram.tsv (as helper genome_size -d writes it), unsupported/<n>.bed
+ * (the merged stretches of bases covered by unsupported windows) and spectra_cn/<n>.tsv (Merqury's copy-number spectrum), n the
+ * assembly's 1-based row.  k: odd, 11..31, else AC_EINPUT.  An assembly without windows, reads without windows: AC_EINPUT.  The tables
+ * beyond half the free device memory: AC_ERANGE.  kmers, unsupported and solid_found (may be NULL) get the first `cap` assemblies' K, E
+ * and found keys.  verbose prints the settings, the histogram's numbers and one line per assembly to stderr.  Calls on one device run one
+ * at a time, with subsample's.  info may be NULL. */
+typedef struct {
+    uint64_t assemblies, contigs;
+    uint32_t k;
+    uint32_t min_count;                /* t, given or the valley */
+    uint64_t valley;                   /* v of the reads' histogram (0: none) */
+    uint64_t reads, read_windows, read_bases;
+    uint64_t distinct;                 /* distinct canonical read k-mers */
+    uint64_t solid_kmers;              /* S: distinct read k-mers seen t times or more */
+    uint64_t assembly_windows;         /* every assembly's windows, junction windows included */
+    uint64_t table_bytes;              /* the combined key table and the multiplicity table */
+    uint64_t spectrum_table_bytes;     /* the read spectrum's largest table */
+    uint64_t partitions, reruns;       /* of the read spectrum */
+    float kernel_ms;                   /* CUDA events around every kernel, summed (0 under emulation) */
+    float scan_ms, pack_ms, insert_ms, probe_ms, count_ms, assembly_ms;   /* record scan, read packing, assembly pack and claim, probes,
+                                                                             spectrum count and histogram, every assembly's passes */
+    double read_ms;                    /* host: reading and gunzipping the reads */
+    double copy_ms;                    /* host wall time of the window uploads */
+} ac_qv_info;
+int ac_qv_dir(const char* reads, const char* const* inputs, uint32_t n_inputs, const char* out_dir, uint32_t k, const uint32_t* min_count,
+              int32_t device, int32_t verbose, uint64_t* kmers, uint64_t* unsupported, uint64_t* solid_found, uint64_t cap, ac_qv_info* info);
 
 #ifdef __cplusplus
 }
