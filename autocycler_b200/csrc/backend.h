@@ -65,6 +65,10 @@ template <class Body> inline void ac_launch(const char*, AcStream*, const Body& 
 // whole grid — between phases.  Emulated by one thread.
 struct AcGridSync { void operator()() const {} };
 template <class Body> inline void ac_launch_coop(const char*, AcStream*, const Body& body, uint64_t, uint64_t = 256) { AcGridSync sync; body(0, 1, sync); }
+// Events that order one stream after another (no timing): no-ops under emulation, where every copy is done when it is issued
+struct AcEvent {};
+inline void ac_record(AcEvent*, AcStream*) {}
+inline void ac_wait(AcStream*, AcEvent*) {}
 
 #else
 // ------------------------------------------------------------------------------------------------
@@ -140,6 +144,15 @@ inline int ac_smem_optin() {
     if (optin < 0) { int dev = 0; AC_CUDA_CHECK(cudaGetDevice(&dev)); AC_CUDA_CHECK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev)); }
     return optin;
 }
+// An event that orders one stream after another (no timing)
+struct AcEvent {
+    cudaEvent_t e = nullptr;
+    AcEvent() { AC_CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming)); }
+    AcEvent(const AcEvent&) = delete; AcEvent& operator=(const AcEvent&) = delete;
+    ~AcEvent() { cudaEventDestroy(e); }
+};
+inline void ac_record(AcEvent* ev, AcStream* st) { AC_CUDA_CHECK(cudaEventRecord(ev->e, st->s)); }
+inline void ac_wait(AcStream* st, AcEvent* ev) { AC_CUDA_CHECK(cudaStreamWaitEvent(st->s, ev->e, 0)); }
 // Device time of what a stream runs between the constructor and stop() (two CUDA events); ms() once the stream has synced
 class AcTimer {
     cudaEvent_t e0 = nullptr, e1 = nullptr; AcStream* st;

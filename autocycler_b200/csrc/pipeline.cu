@@ -1531,16 +1531,27 @@ struct GfaChunkCountBody {    // 64-base pieces of every unitig's sequence, so t
     GfaView v; uint32_t n_unitigs; uint32_t* pieces;
     AC_D void operator()(uint64_t n) const { pieces[n] = n == n_unitigs ? 0u : (v.rec[v.order[n]].len + 63) / 64; }
 };
-struct GfaSequenceBody {
+struct GfaSequenceBody {    // 32 threads per piece, one warp on the device: lane b copies bytes b and b + 32, so a store covers one or two sectors
     GfaView v; uint32_t n_unitigs; const uint32_t* piece_off; const uint32_t* s_off; char* text;
-    AC_D void operator()(uint64_t c) const {
+    AC_D void operator()(uint64_t t) const {
+        const uint64_t c = t >> 5; const uint32_t lane = (uint32_t)t & 31u;
         uint32_t lo = 0, hi = n_unitigs;                      // the unitig this piece belongs to: last n with piece_off[n] <= c
+#ifdef __CUDA_ARCH__
+        // the warp's 32 lanes share c and search together, 32 probes a round: 4 dependent loads for 10^5 unitigs instead of 17
+        while (hi - lo > 1) {
+            const uint32_t step = (hi - lo + 31) / 32, probe = lo + lane * step;      // lane 0 probes lo, where piece_off[lo] <= c holds
+            const unsigned le = __ballot_sync(0xFFFFFFFFu, probe < hi && piece_off[probe] <= c);
+            lo += (uint32_t)(31 - __clz((int)le)) * step;
+            hi = lo + step < hi ? lo + step : hi;
+        }
+#else
         while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (piece_off[mid] <= c) lo = mid; else hi = mid; }
+#endif
         const uint32_t idx = v.order[lo], first = ((uint32_t)c - piece_off[lo]) * 64, len = v.rec[idx].len;
         const uint32_t m = len - first < 64 ? len - first : 64;
         const char* src = v.arena + v.rec[idx].seq_off + first;
         char* dst = text + s_off[lo] + 2 + ac_dec_len(lo + 1) + 1 + first;
-        for (uint32_t i = 0; i < m; ++i) dst[i] = src[i];
+        for (uint32_t i = lane; i < m; i += 32) dst[i] = src[i];
     }
 };
 struct GfaLinkBody {          // get_links_for_gfa (:333-350): forward_next then reverse_next of every unitig, in numbering order
@@ -1595,14 +1606,15 @@ struct PathTextFullBody {
         if (!last[x]) *p++ = ',';
     }
 };
-struct PathWrapBody {       // one thread per (sequence, prefix or suffix)
+struct PathWrapBody {       // 32 threads (a warp on the device) per (sequence, prefix or suffix): consecutive lanes store consecutive bytes
     PathLineView v; char* text;
-    AC_D void operator()(uint64_t t) const {
+    AC_D void operator()(uint64_t x) const {
+        const uint64_t t = x >> 5; const uint32_t lane = (uint32_t)x & 31u;
         const uint32_t i = (uint32_t)(t >> 1); const bool suffix = t & 1;
         const char* src = v.blob + v.blob_off[i] + (suffix ? v.pre_len[i] : 0u);
         char* dst = text + (v.wrap_off[i] - v.wrap_base) + (suffix ? v.pre_len[i] + v.p_off[v.path_off[i + 1]] : v.p_off[v.path_off[i]]);
         const uint32_t n = suffix ? v.suf_len[i] : v.pre_len[i];
-        for (uint32_t b = 0; b < n; ++b) dst[b] = src[b];
+        for (uint32_t b = lane; b < n; b += 32) dst[b] = src[b];
     }
 };
 
@@ -1795,17 +1807,29 @@ struct DevicePipeline::Impl : DeviceContext {
     PinBuf h_cands, h_deps, h_spec, h_fixed, h_text, h_ptext;
 #ifndef AC_EMULATE
     cudaEvent_t ev[N_MARKS];
-    Impl(int device, void* stream) : DeviceContext(device, stream) { for (auto& e : ev) AC_CUDA_CHECK(cudaEventCreate(&e)); }
-    ~Impl() { cudaSetDevice(device); for (auto& e : ev) cudaEventDestroy(e); }      // the buffers go first (on this device), the stream last (DeviceContext)
+    AcStream copy_stream;      // the GFA text goes to the host on it section by section, each while the next one renders
+    Impl(int device, void* stream) : DeviceContext(device, stream) {
+        for (auto& e : ev) AC_CUDA_CHECK(cudaEventCreate(&e));
+        AC_CUDA_CHECK(cudaStreamCreateWithFlags(&copy_stream.s, cudaStreamNonBlocking));
+    }
+    ~Impl() { cudaSetDevice(device); for (auto& e : ev) cudaEventDestroy(e); cudaStreamDestroy(copy_stream.s); }      // the buffers go first (on this device), the stream last (DeviceContext)
     void mark(Mark m) { AC_CUDA_CHECK(cudaEventRecord(ev[m], stream.s)); }
     void wait_mark(Mark m) { AC_CUDA_CHECK(cudaEventSynchronize(ev[m])); }
     float between(Mark a, Mark b) { float ms = 0; AC_CUDA_CHECK(cudaEventElapsedTime(&ms, ev[a], ev[b])); return ms; }
 #else
+    AcStream copy_stream{};
     Impl(int device, void* stream) : DeviceContext(device, stream) {}
     void mark(Mark) {}
     void wait_mark(Mark) {}
     float between(Mark, Mark) { return 0.f; }
 #endif
+    AcEvent text_rendered, text_copied;      // a section of the GFA text rendered (on stream); all of it copied to the host (on copy_stream)
+    // The GFA text's bytes [R.gfa_copied, to) go to the host on copy_stream once what stream has queued so far is done
+    void copy_text_after_rendering(uint64_t to) {
+        ac_record(&text_rendered, &stream); ac_wait(&copy_stream, &text_rendered);
+        if (to > R.gfa_copied) ac_d2h(h_text.as<char>() + R.gfa_copied, d_text.as<char>() + R.gfa_copied, to - R.gfa_copied, &copy_stream);
+        R.gfa_copied = to;
+    }
     bool arena_pending = false;
     const std::function<void()>* before_results = nullptr;   // -> DevicePipeline::before_results
 
@@ -1834,7 +1858,7 @@ struct DevicePipeline::Impl : DeviceContext {
         uint32_t* order_built = nullptr; uint32_t* final_order = nullptr; uint8_t* fix_start = nullptr;
         DevBuf* arena_src = nullptr; uint64_t arena_final = 0;
         bool any_moved = false, gfa_on_device = false, paths_split = false;
-        uint64_t bases_removed = 0, gfa_bytes = 0;
+        uint64_t bases_removed = 0, gfa_bytes = 0, gfa_copied = 0;      // gfa_copied: the GFA text's bytes whose copy to the host is queued
     } R;
     void pull_graph(PipelineResult& out, bool keep_positions);
     std::vector<char> path_blob; std::vector<uint32_t> path_pre, path_suf; uint64_t path_wrap_total = 0;
@@ -2302,7 +2326,9 @@ void DevicePipeline::Impl::simplify() {
     unsigned long long* res = c64 + AC_PASS_WORDS;
     ac_launch("level_pred", &stream, LevelPredBody{d_cands.as<ExpandCandidate>(), d_deps.as<ExpandDeps>(), d_pred.as<int32_t>()}, n_cands);
     ac_memset(d_level.p, 0, n_cands * 4, &stream); ac_memset(d_flagmax.p, 0, 32, &stream);
-    ac_launch_coop("levels", &stream, LevelsCoopBody{d_pred.as<int32_t>(), d_level.as<uint32_t>(), d_flagmax.as<uint32_t>(), n_cands}, n_cands, 4096);
+    // 1024 candidates per CTA: each of the ~15 rounds is a sweep of dependent loads, so splitting it over more SMs beats the dearer
+    // barrier (cfg2: 69 CTAs relax 35-45 us faster than 17, DESIGN.md §5)
+    ac_launch_coop("levels", &stream, LevelsCoopBody{d_pred.as<int32_t>(), d_level.as<uint32_t>(), d_flagmax.as<uint32_t>(), n_cands}, n_cands, 1024);
     ac_memset(d_counters64.p, 0, (AC_PASS_WORDS + 8) * 8, &stream);
     const RelocBoundBody bound_body{d_cands.as<ExpandCandidate>(), d_rec.as<UnitigRec>(), d_cand_at.as<int32_t>(), c64 + AC_PASS_SET(1) + 1};     // the first pass's bound: into the set it does not use
     ac_launch("reloc_bound", &stream, bound_body, n_cands);
@@ -2389,14 +2415,19 @@ void DevicePipeline::Impl::gfa(bool split_paths) {
     char* text = d_text.as<char>();
     ac_h2d(text, head, head_bytes, &stream);       // `head` is on the stack: synchronised below before it goes out of scope (h2d from pageable memory is staged by the driver at call time)
     ac_launch("gfa_segment", &stream, GfaSegmentBody{gv, gfa_s_size.as<uint32_t>(), text + head_bytes}, U);
-    ac_launch("gfa_sequence", &stream, GfaSequenceBody{gv, U, gfa_pieces.as<uint32_t>(), gfa_s_size.as<uint32_t>(), text + head_bytes}, n_pieces);
+    ac_launch("gfa_sequence", &stream, GfaSequenceBody{gv, U, gfa_pieces.as<uint32_t>(), gfa_s_size.as<uint32_t>(), text + head_bytes}, 32 * n_pieces);
+    // H and S (most of the bytes) are final: their copy to the host runs while the L lines render, the L lines' while the P lines
+    // render (the PCIe copy is the longest step of the text; results() queues the P section's and joins the two streams)
+    h_text.ensure(R.gfa_bytes + 64);
+    copy_text_after_rendering(head_bytes + s_bytes);
     ac_launch("gfa_link", &stream, GfaLinkBody{gv, gfa_l_size.as<uint32_t>(), text + head_bytes + s_bytes}, U);
+    copy_text_after_rendering(head_bytes + s_bytes + l_bytes);
     const PathLineView pv{d_path_off.as<uint64_t>(), n_seqs, gfa_p_size.as<uint32_t>(), d_wrap_off.as<uint64_t>(), d_pre_len.as<uint32_t>(), d_suf_len.as<uint32_t>(),
                           d_blob.as<char>(), d_blob_off.as<uint64_t>(), 0};
     char* p_text = text + head_bytes + s_bytes + l_bytes;
     if (!split_paths) {
         ac_launch("path_text", &stream, PathTextFullBody{d_path.as<UStrand>(), d_pos2.as<uint32_t>(), d_last.as<uint8_t>(), pv, p_text}, steps);
-        ac_launch("path_wrap", &stream, PathWrapBody{pv, p_text}, 2ull * n_seqs);
+        ac_launch("path_wrap", &stream, PathWrapBody{pv, p_text}, 64ull * n_seqs);
     }
     R.paths_split = split_paths;
     R.gfa_on_device = true;
@@ -2409,8 +2440,9 @@ void DevicePipeline::Impl::results(PipelineResult& out, bool keep_positions, boo
     if (fused && !R.gfa_on_device) throw std::runtime_error("fused build: the device GFA writer did not run");
     uint64_t d2h = 0;
     if (R.gfa_on_device) {
-        h_text.ensure(R.gfa_bytes + 64);
-        ac_d2h(h_text.p, d_text.p, R.gfa_bytes, &stream); d2h += R.gfa_bytes;
+        copy_text_after_rendering(R.gfa_bytes);
+        ac_record(&text_copied, &copy_stream); ac_wait(&stream, &text_copied);
+        d2h += R.gfa_bytes;
     }
     uint32_t small[16];
     ac_d2h(small, d_small.p, 64, &stream); ac_sync(&stream); d2h += 64;
@@ -2518,7 +2550,7 @@ void DevicePipeline::render_path_lines(const void* tokens, uint64_t n_tokens, co
         const PathLineView pv{m.d_own_off.as<uint64_t>(), n_own, m.d_own_size.as<uint32_t>(), m.d_wrap_off.as<uint64_t>() + lo, m.d_pre_len.as<uint32_t>() + lo,
                               m.d_suf_len.as<uint32_t>() + lo, m.d_blob.as<char>(), m.d_blob_off.as<uint64_t>() + lo, wrap_lo};
         ac_launch("path_text", &m.stream, PathTextFullBody{(const UStrand*)tokens, nullptr, m.d_own_last.as<uint8_t>(), pv, m.d_ptext.as<char>()}, steps);
-        ac_launch("path_wrap", &m.stream, PathWrapBody{pv, m.d_ptext.as<char>()}, 2ull * n_own);
+        ac_launch("path_wrap", &m.stream, PathWrapBody{pv, m.d_ptext.as<char>()}, 64ull * n_own);
         m.h_ptext.ensure(total_bytes + 64);
         ac_d2h(m.h_ptext.p, m.d_ptext.p, total_bytes, &m.stream);
     }
