@@ -132,6 +132,20 @@ class AcQvInfo(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class AcUnassembledInfo(C.Structure):
+    _fields_ = [("assemblies", C.c_uint64), ("contigs", C.c_uint64), ("k", C.c_uint32), ("min_count", C.c_uint32), ("valley", C.c_uint64),
+                ("reads", C.c_uint64), ("read_windows", C.c_uint64), ("read_bases", C.c_uint64), ("distinct", C.c_uint64),
+                ("scored_reads", C.c_uint64), ("selected_reads", C.c_uint64), ("selected_bases", C.c_uint64), ("absent_kmers", C.c_uint64),
+                ("absent_median", C.c_double), ("peak", C.c_double), ("absent_copy_ratio", C.c_double), ("assembly_windows", C.c_uint64),
+                ("table_bytes", C.c_uint64), ("read_bytes", C.c_uint64), ("spectrum_table_bytes", C.c_uint64), ("partitions", C.c_uint64),
+                ("reruns", C.c_uint64), ("read_passes", C.c_uint64), ("kernel_ms", C.c_float), ("scan_ms", C.c_float), ("pack_ms", C.c_float),
+                ("claim_ms", C.c_float), ("count_ms", C.c_float), ("sweep_ms", C.c_float), ("gather_ms", C.c_float), ("read_ms", C.c_double),
+                ("copy_ms", C.c_double), ("write_ms", C.c_double)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_sequence", "ac_clear_sequences", "ac_upload",
            "ac_build", "ac_compress", "ac_simplify", "ac_merge_linear_paths", "ac_renumber_unitigs", "ac_load_gfa", "ac_bind_host_to_device", "ac_decompress_gfa", "ac_pairwise_distances", "ac_distance_matrix_text", "ac_sequence_reconstruct", "ac_counts_get", "ac_unitigs_copy", "ac_path_copy", "ac_gfa_size", "ac_gfa_copy",
            "ac_timings_get", "ac_compress_dir", "ac_compress_dir_devices", "ac_load_sequences", "ac_sequence_get",
@@ -145,7 +159,7 @@ EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_seq
            "ac_clean_gfa", "ac_clean_text", "ac_gfa_to_fasta", "ac_gfa_fasta_text", "ac_table_text",
            "ac_subsample_dir", "ac_genome_size", "ac_subsample_words", "ac_subsample_shuffle",
            "ac_genome_size_estimate", "ac_genome_size_from_histogram",
-           "ac_depth_fasta", "ac_depth_filter_text", "ac_depth_from_header", "ac_qv_dir"]
+           "ac_depth_fasta", "ac_depth_filter_text", "ac_depth_from_header", "ac_qv_dir", "ac_unassembled_dir"]
 
 _libs = {}
 
@@ -269,6 +283,8 @@ def load_library(path=None):
     lib.ac_depth_from_header.argtypes = [C.c_char_p, C.POINTER(C.c_double)]
     lib.ac_qv_dir.argtypes = [C.c_char_p, C.POINTER(C.c_char_p), C.c_uint32, C.c_char_p, C.c_uint32, C.POINTER(C.c_uint32), C.c_int32, C.c_int32,
                               C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.c_uint64, C.POINTER(AcQvInfo)]
+    lib.ac_unassembled_dir.argtypes = [C.c_char_p, C.POINTER(C.c_char_p), C.c_uint32, C.c_char_p, C.c_uint32, C.POINTER(C.c_uint32), C.c_uint64,
+                                       C.c_double, C.c_int32, C.c_int32, C.POINTER(AcUnassembledInfo)]
     lib.ac_table_text.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint64, C.c_int32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     _libs[path] = lib
     return lib
@@ -936,4 +952,28 @@ def qv(reads, assemblies, out_dir, k=21, min_count=None, device=0, verbose=False
                           "qv": qv_value(r["qv"]), "completeness": qv_value(r["completeness"])} for i, r in enumerate(rows("qv.tsv")[:n])]
     out["contigs"] = [{"assembly": r["assembly"], "contig": r["contig"], "length": int(r["length"]), "kmers": int(r["kmers"]),
                        "unsupported": int(r["unsupported"]), "qv": qv_value(r["qv"])} for r in rows("contig_qv.tsv")]
+    return out
+
+
+def unassembled(reads, assemblies, out_dir, k=21, min_count=None, min_solid=100, min_fraction=0.5, device=0, verbose=False, lib=None):
+    """`autocycler unassembled` (DESIGN.md §21): the reads the assembly does not explain, and the depth of the sequence it misses,
+    counted on the GPU (not in the reference).  assemblies: FASTA files or directories (expanded as find_all_assemblies does); together
+    they are the assembly.  Returns the info dict (t is "min_count"; absent_median, peak and absent_copy_ratio are None where summary.tsv
+    leaves them empty; the stage timings in ms) with "selected": per selected read a dict of read, length, solid_kmers and absent_kmers,
+    read back from the unassembled.tsv the call wrote."""
+    lib = lib or load_library()
+    paths = [assemblies] if isinstance(assemblies, (str, bytes, os.PathLike)) else list(assemblies)
+    arr = (C.c_char_p * max(1, len(paths)))(*[os.fsencode(p) for p in paths])
+    info = AcUnassembledInfo()
+    t = None if min_count is None else C.byref(C.c_uint32(min_count))
+    _raise_unless_ok(lib, lib.ac_unassembled_dir(os.fsencode(reads), arr, len(paths), os.fsencode(out_dir), k, t, min_solid, min_fraction, device,
+                                                 1 if verbose else 0, C.byref(info)))
+    out = info.as_dict()
+    for name in ("absent_median", "peak", "absent_copy_ratio"):
+        if out[name] != out[name]:
+            out[name] = None
+    with open(os.path.join(out_dir, "unassembled.tsv")) as f:
+        lines = f.read().splitlines()
+    out["selected"] = [{"read": r[0], "length": int(r[1]), "solid_kmers": int(r[2]), "absent_kmers": int(r[3])}
+                       for r in (line.split("\t") for line in lines[1:])]
     return out

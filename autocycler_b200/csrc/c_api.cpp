@@ -31,6 +31,7 @@
 #include "host_genome_size.h"
 #include "host_depth.h"
 #include "host_qv.h"
+#include "host_unassembled.h"
 #include <mutex>
 #include <immintrin.h>
 #include <functional>
@@ -1635,11 +1636,11 @@ int ac_png_write(const char* path, const uint8_t* rgb, uint32_t width, uint32_t 
 // ---- `autocycler subsample` (subsample.rs) --------------------------------------------------------------------------------------
 namespace {
 // One subsample device object per device, as for dotplot: its buffers (and pinned windows) are kept for the next call on that device.
-// genome_size, depth and qv read through the same object and keep their packed streams and tables beside it.
+// genome_size, depth, qv and unassembled read through the same object and keep their packed streams and tables beside it.
 std::mutex g_subsample_mu;
 struct SubsampleDevice {
-    DeviceContext ctx; DeviceSubsample sub; DeviceSpectrum spec; DeviceDepth depth; DeviceQv qv;
-    explicit SubsampleDevice(int32_t device) : ctx(device, nullptr), sub(ctx), spec(ctx), depth(ctx), qv(ctx) {}
+    DeviceContext ctx; DeviceSubsample sub; DeviceSpectrum spec; DeviceDepth depth; DeviceQv qv; DeviceUnassembled unassembled;
+    explicit SubsampleDevice(int32_t device) : ctx(device, nullptr), sub(ctx), spec(ctx), depth(ctx), qv(ctx), unassembled(ctx) {}
 };
 SubsampleDevice& subsample_device(int32_t device) {        // with g_subsample_mu held
     static std::vector<std::pair<int32_t, SubsampleDevice*>> devices;
@@ -1974,6 +1975,79 @@ int ac_qv_dir(const char* reads, const char* const* inputs, uint32_t n_inputs, c
         info->insert_ms = r.device.pack_ms + r.device.insert_ms; info->probe_ms = r.device.probe_ms;
         info->count_ms = r.spectrum.count_ms + r.spectrum.hist_ms; info->assembly_ms = r.device.assembly_ms;
         info->read_ms = r.read_ms; info->copy_ms = r.copy_ms;
+    }
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
+// ---- `autocycler unassembled`: the reads an assembly does not explain (not in the reference) --------------------------------------
+int ac_unassembled_dir(const char* reads, const char* const* inputs, uint32_t n_inputs, const char* out_dir, uint32_t k, const uint32_t* min_count,
+                       uint64_t min_solid, double min_fraction, int32_t device, int32_t verbose, ac_unassembled_info* info) {
+    if (!reads || !out_dir || (!inputs && n_inputs)) return set_error(nullptr, AC_EINVAL, "null argument");
+    for (uint32_t i = 0; i < n_inputs; ++i) if (!inputs[i]) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    const std::string in = reads, dir = out_dir;
+    if (!n_inputs) return set_error(nullptr, AC_EINPUT, "no assemblies given");
+    if (k < 11 || k > 31 || k % 2 == 0) return set_error(nullptr, AC_EINPUT, "--kmer must be odd and between 11 and 31");
+    if (min_count && (*min_count < 1 || *min_count > AC_GS_BINS - 1))
+        return set_error(nullptr, AC_EINPUT, "--min_count must be between 1 and " + std::to_string(AC_GS_BINS - 1));
+    if (min_solid < 1) return set_error(nullptr, AC_EINPUT, "--min_solid must be at least 1");
+    if (!(min_fraction > 0.0 && min_fraction <= 1.0)) return set_error(nullptr, AC_EINPUT, "--min_fraction must be above 0 and at most 1");
+    int rc;
+    if ((rc = check_file(in)) != AC_OK) return rc;
+    const std::vector<std::string> paths = qv_inputs(std::vector<std::string>(inputs, inputs + n_inputs));
+    struct stat st;
+    if (stat(dir.c_str(), &st) == 0 && !S_ISDIR(st.st_mode)) return set_error(nullptr, AC_EINPUT, dir + " exists but is not a directory");
+    if (!make_dirs(dir)) return set_error(nullptr, AC_EINPUT, "failed to create directory " + dir + "\n" + strerror(errno));
+    if (verbose) {
+        fprintf(stderr, "\nStarting autocycler unassembled\n    This command finds the reads the assembly does not explain and the depth of the sequence it "
+                        "misses, counted on the GPU. It is not in the reference.\n\nSettings:\n  --reads %s\n  --assemblies", in.c_str());
+        for (const std::string& p : paths) fprintf(stderr, " %s", p.c_str());
+        fprintf(stderr, "\n  --out_dir %s\n  --kmer %u\n", dir.c_str(), k);
+        if (min_count) fprintf(stderr, "  --min_count %u\n", *min_count);
+        fprintf(stderr, "  --min_solid %llu\n  --min_fraction %s\n\n", (unsigned long long)min_solid, format_float(min_fraction).c_str());
+    }
+    UnassembledResult r;
+    {
+        std::lock_guard<std::mutex> lock(g_subsample_mu);
+        SubsampleDevice& d = subsample_device(device);
+        try {
+            unassembled_run(d.sub, d.spec, d.unassembled, paths, in, k, min_count, min_solid, min_fraction, subsample_window_size(), dir, r);
+        } catch (const AcIoError& e) { return set_error(nullptr, AC_EIO, e.msg); }
+        catch (const std::length_error& e) { return set_error(nullptr, AC_ERANGE, e.what()); }
+    }
+    const auto t0 = std::chrono::steady_clock::now();
+    const std::pair<std::string, std::string> files[] = {{"unassembled.tsv", r.table}, {"fraction_histogram.tsv", unassembled_fractions(r)},
+                                                         {"absent_histogram.tsv", unassembled_absent(r)},
+                                                         {"kmer_histogram.tsv", unassembled_kmer_histogram(r)}, {"summary.tsv", unassembled_summary(r)}};
+    for (const auto& f : files)
+        if (!write_file(dir + "/" + f.first, f.second)) return set_error(nullptr, AC_EIO, "cannot write " + dir + "/" + f.first);
+    r.write_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    if (verbose) {
+        fprintf(stderr, "Unassembled reads (k = %u):\n  reads: %llu\n  read k-mer windows: %llu\n  valley: %s\n  min_count: %llu%s\n"
+                        "  k-mer depth peak: %s\n  assembly k-mer windows: %llu\n  scored reads: %llu\n  selected reads: %llu (%llu bases)\n"
+                        "  absent k-mers: %llu\n  absent k-mer median count: %s\n  absent copy ratio: %s\n\n", k, (unsigned long long)r.reads,
+                (unsigned long long)r.read_windows, r.valley ? std::to_string(r.valley).c_str() : "none", (unsigned long long)r.min_count,
+                min_count ? " (given)" : " (the valley)", r.has_peak ? unassembled_peak_text(r).c_str() : "none",
+                (unsigned long long)r.device.assembly_windows, (unsigned long long)r.scored, (unsigned long long)r.selected,
+                (unsigned long long)r.selected_bases, (unsigned long long)r.absent_kmers, r.has_median ? unassembled_median_text(r).c_str() : "none",
+                r.has_median && r.has_peak ? unassembled_ratio_text(r).c_str() : "none");
+        fprintf(stderr, "Finished!\nUnassembled reads: %s/unassembled.fastq\n\n", dir.c_str());
+    }
+    if (info) {
+        *info = ac_unassembled_info{};
+        info->assemblies = r.paths.size(); info->contigs = r.contigs; info->k = k; info->min_count = (uint32_t)r.min_count;
+        info->valley = r.valley; info->reads = r.reads; info->read_windows = r.read_windows; info->read_bases = r.read_bases;
+        info->distinct = r.distinct; info->scored_reads = r.scored; info->selected_reads = r.selected; info->selected_bases = r.selected_bases;
+        info->absent_kmers = r.absent_kmers; info->absent_median = r.has_median ? r.absent_median : NAN; info->peak = r.has_peak ? r.peak : NAN;
+        info->absent_copy_ratio = r.has_median && r.has_peak ? r.absent_median / r.peak : NAN;
+        info->assembly_windows = r.device.assembly_windows; info->table_bytes = r.device.table_bytes; info->read_bytes = r.device.read_bytes;
+        info->spectrum_table_bytes = r.spectrum.table_bytes; info->partitions = r.spectrum.partitions;
+        info->reruns = r.spectrum.reruns + r.device.sweep.reruns; info->read_passes = r.selected && r.windows > 1 ? 2 : 1;
+        info->kernel_ms = r.kernel_ms; info->scan_ms = r.scan_ms; info->pack_ms = r.pack_reads_ms + r.device.index_ms;
+        info->claim_ms = r.device.pack_ms + r.device.claim_ms; info->count_ms = r.spectrum.count_ms + r.spectrum.hist_ms;
+        info->sweep_ms = r.device.sweep.count_ms + r.device.attribute_ms; info->gather_ms = r.gather_ms;
+        info->read_ms = r.read_ms; info->copy_ms = r.copy_ms; info->write_ms = r.write_ms;
     }
     return ok(nullptr);
     AC_GUARD_END(nullptr)

@@ -2,8 +2,9 @@
 // `autocycler clean`, `autocycler gfa2fasta`, `autocycler table` and `autocycler subsample` with the reference's flags (main.rs:126-162), messages and exit codes
 // (misc.rs:130-136: "Error: <text>" on stderr, exit 1), running the H100 path through the C ABI; `autocycler helper genome_size`,
 // which departs from the reference on purpose: a k-mer depth estimate on the GPU instead of the length of a Raven assembly; and
-// `autocycler depth`, read-measured contig depth (not in the reference) with the reference's helper depth filter; and `autocycler qv`,
-// each assembly's k-mer QV and completeness against the reads (not in the reference).
+// `autocycler depth`, read-measured contig depth (not in the reference) with the reference's helper depth filter; `autocycler qv`,
+// each assembly's k-mer QV and completeness against the reads (not in the reference); and `autocycler unassembled`, the reads the
+// assembly does not explain (not in the reference).
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -423,6 +424,60 @@ static int qv_main(int argc, char** argv) {
     return finish(rc);
 }
 
+// `autocycler unassembled`: the reads the assembly does not explain, and the depth of the sequence it misses, counted on the GPU (not in
+// the reference).  summary.tsv also goes to stdout, byte for byte.
+static const char* unassembled_usage =
+    "Usage: autocycler unassembled --reads <READS> --assemblies <FASTA|DIR>... --out_dir <DIR> [--kmer 21] [--min_count N] [--min_solid 100]\n"
+    "                              [--min_fraction 0.5] [--device N]\n\n"
+    "Finds the reads the assembly does not explain, counted on the GPU: the reads where a large share of the solid k-mers is absent from\n"
+    "every input assembly, and the read depth of those absent k-mers against the genome's k-mer peak (a missing plasmid shows up as its\n"
+    "copy number). This command is not in the reference. Writes unassembled.fastq, unassembled.tsv, fraction_histogram.tsv,\n"
+    "absent_histogram.tsv, kmer_histogram.tsv and summary.tsv (also to stdout).\n\n"
+    "Options:\n"
+    "  -r, --reads <READS>            Long reads in FASTQ format, gzipped or not (required)\n"
+    "  -i, --assemblies <FASTA|DIR>...  Assemblies in FASTA format, gzipped or not, or directories of them; together they are the\n"
+    "                                 assembly (required)\n"
+    "  -o, --out_dir <DIR>            Directory to create and write the reads and tables into (required)\n"
+    "      --kmer <KMER>              K-mer size, odd, 11 to 31 [default: 21]\n"
+    "      --min_count <N>            Read count from which a k-mer is solid, 1 to 16383 [default: the valley of the reads' k-mer spectrum]\n"
+    "      --min_solid <N>            Solid k-mers a read needs to be scored, at least 1 [default: 100]\n"
+    "      --min_fraction <F>         Share of a scored read's solid k-mers that must be absent from the assembly to select it,\n"
+    "                                 above 0 and at most 1 [default: 0.5]\n"
+    "      --device <ORDINAL>         CUDA device [default: 0]\n";
+static int unassembled_main(int argc, char** argv) {
+    Args a{argc, argv, unassembled_usage};
+    std::string reads, out; std::vector<std::string> inputs; bool has_min = false;
+    unsigned long k = 21, min_count = 0; double min_solid = 100, min_fraction = 0.5; int device = 0;
+    auto refuse = [&]() { fprintf(stderr, "error: invalid value '%s' for '%s'\n%s", argv[a.i], a.flag.c_str(), unassembled_usage); return 2; };
+    while (a.next()) {
+        if (a.is("-r", "--reads")) reads = a.value();
+        else if (a.is("-i", "--assemblies")) { const std::vector<std::string> v = a.values(); inputs.insert(inputs.end(), v.begin(), v.end()); }
+        else if (a.is("-o", "--out_dir")) out = a.value();
+        else if (a.is("--kmer")) { k = (unsigned long)a.number(true); if (k < 11 || k > 31 || k % 2 == 0) return refuse(); }
+        else if (a.is("--min_count")) { min_count = (unsigned long)a.number(true); has_min = true; }
+        else if (a.is("--min_solid")) { min_solid = a.number(true); if (min_solid < 1) return refuse(); }
+        else if (a.is("--min_fraction")) { min_fraction = a.number(false); if (!(min_fraction > 0.0 && min_fraction <= 1.0)) return refuse(); }
+        else if (a.is("--device")) device = atoi(a.value());
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
+    }
+    if (reads.empty() || out.empty() || inputs.empty()) return a.missing();
+    const std::vector<const char*> ptrs = c_strings(inputs);
+    const uint32_t t = min_count > 0xFFFFFFFFul ? 0 : (uint32_t)min_count;
+    const uint64_t solid = min_solid >= 18446744073709551615.0 ? UINT64_MAX : (uint64_t)min_solid;
+    const int rc = ac_unassembled_dir(reads.c_str(), ptrs.data(), (uint32_t)ptrs.size(), out.c_str(), (uint32_t)k, has_min ? &t : nullptr, solid,
+                                      min_fraction, device, 1, nullptr);
+    if (rc == AC_OK) {
+        FILE* f = fopen((out + "/summary.tsv").c_str(), "rb");
+        if (f) {
+            char buf[1 << 16]; size_t n;
+            while ((n = fread(buf, 1, sizeof buf, f)) > 0) fwrite(buf, 1, n, stdout);
+            fclose(f);
+        }
+    }
+    return finish(rc);
+}
+
 int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "dotplot") == 0) return dotplot_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "resolve") == 0) return resolve_main(argc, argv);
@@ -438,6 +493,7 @@ int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "helper") == 0) return helper_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "depth") == 0) return depth_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "qv") == 0) return qv_main(argc, argv);
+    if (argc >= 2 && strcmp(argv[1], "unassembled") == 0) return unassembled_main(argc, argv);
     fprintf(stderr, "%s", compress_usage);
     return 2;
 }

@@ -1,7 +1,8 @@
-// The device parts of `autocycler trim`, `resolve`, `cluster`, `dotplot`, `subsample`, `helper genome_size`, `depth` and `qv`.  Each object owns its device buffers (allocated on first
+// The device parts of `autocycler trim`, `resolve`, `cluster`, `dotplot`, `subsample`, `helper genome_size`, `depth`, `qv` and `unassembled`.  Each object owns its device buffers (allocated on first
 // use, kept for the next call) and runs on the device and stream of the DeviceContext it is given, which must outlive it.
 #pragma once
 #include <cstdint>
+#include <functional>
 #include <vector>
 
 #include "backend.h"
@@ -182,18 +183,26 @@ public:
     // take; parts: the partitions to use (0: the smallest power of two whose 2 W / P slots fit the budget).  A partition whose probe
     // limit is hit is counted again with twice the slots.
     void count(uint64_t windows, uint64_t budget_slots, uint64_t parts, uint64_t* hist, SpectrumRun* run);
+    // A second sweep over the partitions count() made, for a rule that needs the whole histogram first: each(table, slots, P, part) runs
+    // once per partition with that partition's table on the device.  The last partition's table is the one count() left behind; every
+    // other partition is counted again at the slots count() settled on (run gets those counts' time, and any rerun).
+    void sweep(const std::function<void(const GsSlot*, uint64_t, uint64_t, uint64_t)>& each, SpectrumRun* run);
     float kernel_ms = 0.f;           // the kernels of every call since begin() (CUDA events; 0 under emulation)
     // The packed stream so far, on the device: `packed_words()` words of codes and validity masks (DeviceDepth::probe reads it).
     const uint64_t* packed_codes() { return d_code.as<uint64_t>(); }
     const uint32_t* packed_valid() { return d_valid.as<uint32_t>(); }
     uint64_t packed_words() const { return words; }
     float packed_ms() const { return pack_ms; }      // the packing's kernels since begin()
+    // The last pack_window's records' first words, relative to the words packed before it, and their total (records + 1 values).
+    const uint64_t* window_word_offsets() { return d_woff.as<uint64_t>(); }
 private:
+    uint64_t count_partition(uint64_t parts, uint64_t part, uint64_t slots, SpectrumRun* run);
     DeviceContext& ctx;
     SerialScan<uint64_t, AC_SUB_SCAN_TILE, 8> scan_u64;          // of the records' word counts
     uint32_t k = 21;
     uint64_t words = 0;              // packed words so far
     float pack_ms = 0.f;
+    std::vector<uint64_t> part_slots;                            // each partition's slots in the last count()
     DevBuf d_code, d_valid, d_woff, d_tot, d_table, d_flag, d_hist;
 };
 // Slots of device memory a k-mer table may take by default: half of the device's free memory (2^25 slots under emulation).
@@ -261,4 +270,41 @@ private:
     std::vector<uint64_t> woff, win;
     std::vector<uint32_t> first_contig;
     DevBuf d_bytes, d_contig, d_code, d_valid, d_wcid, d_table, d_mult, d_mask, d_spec;
+};
+
+// `autocycler unassembled`: the reads an assembly does not explain (DESIGN.md §21).  The contigs of every input are packed (depth's
+// layout) and their canonical keys claimed in one DepthSlot table, the assembly set A.  While the reads are packed, each packed word gets
+// its read's index and each read its length.  After DeviceSpectrum::count has given the histogram and so the solid threshold t, a second
+// sweep over its partitions counts, per read, the windows whose key the reads hold t times or more (s) and those of them A does not hold
+// (a), and bins the distinct such keys that A does not hold by their read count.
+// What the device ran: the assembly's windows, the bytes of the assembly set, the per-read counters and the word indices, and the
+// kernels' time by stage (CUDA events; 0 under emulation).  sweep: the second sweep's recounts of partitions.
+struct UaRun {
+    uint64_t assembly_windows = 0, table_bytes = 0, read_bytes = 0;
+    float pack_ms = 0.f, claim_ms = 0.f, index_ms = 0.f, attribute_ms = 0.f;
+    SpectrumRun sweep;
+};
+
+class DeviceUnassembled {
+public:
+    explicit DeviceUnassembled(DeviceContext& ctx) : ctx(ctx) {}
+    ~DeviceUnassembled() { ctx.make_current(); }
+    // The assembly set.  bytes: every contig's bytes back to back (a circular contig followed by its first k-1 bases), contig c taking
+    // len[c] of them, `windows` windows of k A/C/G/T bases in all.  The table takes max(2 windows, 64) slots; std::length_error when that
+    // exceeds budget_slots.
+    void build(const uint8_t* bytes, const uint64_t* len, uint32_t n_contigs, uint64_t windows, uint32_t k, uint64_t budget_slots, UaRun* run);
+    // After spec.pack_window of the window whose first record is `first` and which has `records` records, starting at packed word `word0`:
+    // each of its packed words gets its read's index, and each read its sequence length.
+    void index_window(DeviceSpectrum& spec, DeviceSubsample& sub, uint64_t first, uint64_t records, uint64_t word0, UaRun* run);
+    // The counters of `reads` reads and the word indices, with the assembly set, against budget_slots (16-byte slots); std::length_error
+    // when they exceed it.
+    void check_budget(uint64_t reads, uint64_t words, uint64_t budget_slots, UaRun* run);
+    // After spec.count: the second sweep at threshold t.  counts[2 i] = s_i and counts[2 i + 1] = a_i for each of the `reads` reads,
+    // lengths[i] its sequence length, absent[c] the distinct keys with bin(r) = c (r >= t) that A does not hold (host arrays).
+    void attribute(DeviceSpectrum& spec, uint64_t reads, uint32_t t, uint32_t* counts, uint32_t* lengths, uint64_t* absent, UaRun* run);
+private:
+    DeviceContext& ctx;
+    uint32_t k = 21;
+    uint64_t slots = 0;
+    DevBuf d_bytes, d_contig, d_code, d_valid, d_wcid, d_table, d_read, d_len, d_counts, d_absent;
 };

@@ -6,6 +6,7 @@
 #include "gs_kmers.h"
 
 #include <algorithm>
+#include <stdexcept>
 #include <utility>
 
 // ------------------------------------------------------------------------------------------------
@@ -130,6 +131,7 @@ uint64_t ac_gs_budget_slots() {
 void DeviceSpectrum::begin(uint32_t kk) {
     ctx.make_current();
     k = kk; words = 0; kernel_ms = 0.f; pack_ms = 0.f;
+    part_slots.clear();
     d_tot.ensure(16);
     ac_memset(d_tot.p, 0, 16, &ctx.stream);
 }
@@ -166,6 +168,31 @@ void DeviceSpectrum::totals(uint64_t* windows, uint64_t* bases) {
     *windows = t[0]; *bases = t[1];
 }
 
+// One partition's table in d_table: counted at `slots` slots, and again at twice the slots while the probe limit is hit.  Returns the
+// slot count that held it.
+uint64_t DeviceSpectrum::count_partition(uint64_t parts, uint64_t part, uint64_t slots, SpectrumRun* run) {
+    AcStream* st = &ctx.stream;
+    for (;; slots *= 2) {
+        if (slots > (1ull << 40)) throw std::runtime_error("genome_size: the k-mer table cannot hold one partition");
+        d_table.ensure(slots * sizeof(GsSlot));
+        run->table_bytes = std::max<uint64_t>(run->table_bytes, slots * sizeof(GsSlot));
+        GsSlot* table = d_table.as<GsSlot>();
+        ac_memset(table, 0, slots * sizeof(GsSlot), st);
+        ac_memset(d_flag.p, 0, 4, st);
+        const uint64_t limit = std::min<uint64_t>(slots, 4096);
+        AcTimer tc(st);
+        ac_launch("gs_count", st, GsCountBody{d_code.as<uint64_t>(), d_valid.as<uint32_t>(), k, parts, part, table, slots, limit,
+                                              d_flag.as<uint32_t>()}, words);
+        tc.stop();
+        uint32_t overflow = 0;
+        ac_d2h(&overflow, d_flag.p, 4, st);
+        ac_sync(st);
+        run->count_ms += tc.ms();
+        if (overflow) { ++run->reruns; continue; }
+        return slots;
+    }
+}
+
 void DeviceSpectrum::count(uint64_t W, uint64_t budget, uint64_t parts, uint64_t* hist, SpectrumRun* run) {
     ctx.make_current();
     AcStream* st = &ctx.stream;
@@ -177,40 +204,39 @@ void DeviceSpectrum::count(uint64_t W, uint64_t budget, uint64_t parts, uint64_t
     const uint64_t base_slots = std::max<uint64_t>(1, std::min((want + parts - 1) / parts, budget));
     d_hist.ensure(AC_GS_BINS * 8); d_flag.ensure(4);
     ac_memset(d_hist.p, 0, AC_GS_BINS * 8, st);
+    part_slots.clear();
     for (uint64_t part = 0; part < parts; ++part) {
-        for (uint64_t slots = base_slots;; slots *= 2) {
-            if (slots > (1ull << 40)) throw std::runtime_error("genome_size: the k-mer table cannot hold one partition");
-            d_table.ensure(slots * sizeof(GsSlot));
-            run->table_bytes = std::max<uint64_t>(run->table_bytes, slots * sizeof(GsSlot));
-            GsSlot* table = d_table.as<GsSlot>();
-            ac_memset(table, 0, slots * sizeof(GsSlot), st);
-            ac_memset(d_flag.p, 0, 4, st);
-            const uint64_t limit = std::min<uint64_t>(slots, 4096);
-            AcTimer tc(st);
-            ac_launch("gs_count", st, GsCountBody{d_code.as<uint64_t>(), d_valid.as<uint32_t>(), k, parts, part, table, slots, limit,
-                                                  d_flag.as<uint32_t>()}, words);
-            tc.stop();
-            uint32_t overflow = 0;
-            ac_d2h(&overflow, d_flag.p, 4, st);
-            ac_sync(st);
-            run->count_ms += tc.ms();
-            if (overflow) { ++run->reruns; continue; }
-            AcTimer th(st);
+        const uint64_t slots = count_partition(parts, part, base_slots, run);
+        part_slots.push_back(slots);
+        const GsSlot* table = d_table.as<GsSlot>();
+        AcTimer th(st);
 #ifndef AC_EMULATE
-            const uint64_t blocks = std::min<uint64_t>((slots + 1023) / 1024, 2 * ac_sm_count());
-            ac_launch_kernel("gs_hist", st, ac_gs_hist_kernel, (unsigned)blocks, 1024, AC_GS_BINS * 4, (const GsSlot*)table, slots,
-                             d_hist.as<unsigned long long>());
+        const uint64_t blocks = std::min<uint64_t>((slots + 1023) / 1024, 2 * ac_sm_count());
+        ac_launch_kernel("gs_hist", st, ac_gs_hist_kernel, (unsigned)blocks, 1024, AC_GS_BINS * 4, table, slots,
+                         d_hist.as<unsigned long long>());
 #else
-            ac_launch("gs_hist", st, GsHistBody{table, d_hist.as<uint64_t>()}, slots);
+        ac_launch("gs_hist", st, GsHistBody{table, d_hist.as<uint64_t>()}, slots);
 #endif
-            th.stop();
-            ac_sync(st);
-            run->hist_ms += th.ms();
-            break;
-        }
+        th.stop();
+        ac_sync(st);
+        run->hist_ms += th.ms();
     }
     ac_d2h(hist, d_hist.p, AC_GS_BINS * 8, st);
     ac_sync(st);
     run->partitions = parts;
     kernel_ms = run->pack_ms + run->count_ms + run->hist_ms;
+}
+
+void DeviceSpectrum::sweep(const std::function<void(const GsSlot*, uint64_t, uint64_t, uint64_t)>& each, SpectrumRun* run) {
+    ctx.make_current();
+    const uint64_t parts = part_slots.size();
+    if (!parts) throw std::logic_error("genome_size: a second sweep before the count");
+    // the last partition's table is still in d_table, so it goes first; every other one is counted again at its settled slots
+    for (uint64_t i = 0; i < parts; ++i) {
+        const uint64_t part = (parts - 1 + i) % parts;
+        uint64_t slots = part_slots[part];
+        if (i) slots = count_partition(parts, part, slots, run);
+        each(d_table.as<GsSlot>(), slots, parts, part);
+    }
+    run->partitions = parts;
 }

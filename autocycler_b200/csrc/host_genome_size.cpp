@@ -49,14 +49,18 @@ uint64_t genome_size_env(const char* name) {
     return e && *e ? strtoull(e, nullptr, 10) : 0;
 }
 
-ReadPass pack_reads(DeviceSubsample& sub, DeviceSpectrum& spec, const std::string& reads, uint32_t k, uint64_t window) {
+ReadPass pack_reads(DeviceSubsample& sub, DeviceSpectrum& spec, const std::string& reads, uint32_t k, uint64_t window,
+                    const std::function<void(uint64_t, uint64_t, uint64_t)>& each) {
     ReadPass out;
     sub.kernel_ms = 0.f; sub.copy_ms = 0.0;
     spec.begin(k);
     SubsampleRun pass;
-    fastq_windows(sub, reads, window, false, pass, [&](uint64_t, uint64_t records) {
+    fastq_windows(sub, reads, window, false, pass, [&](uint64_t first, uint64_t records) {
+        const uint64_t word0 = spec.packed_words();
         spec.pack_window(sub, records);
+        if (each) each(first, records, word0);
         out.reads += records;
+        ++out.windows;
     });
     out.read_ms = pass.read_ms;
     out.copy_ms = sub.copy_ms;

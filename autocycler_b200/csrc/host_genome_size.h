@@ -3,6 +3,7 @@
 // length, which this build cannot do.  The number here is a k-mer estimate and will not equal Raven's (DESIGN.md §18).
 #pragma once
 #include <cstdint>
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -28,9 +29,11 @@ uint64_t genome_size_valley(const uint64_t* hist);
 extern const char* const genome_size_no_peak;
 
 // One pass of subsample's windows over a FASTQ file (gzipped or not), each window packed into spec's stream (begun here with k): the
-// records, the time reading and gunzipping the file, and the window uploads' time.  sub.kernel_ms holds the record scan's kernels after.
-struct ReadPass { uint64_t reads = 0; double read_ms = 0, copy_ms = 0; };
-ReadPass pack_reads(DeviceSubsample& sub, DeviceSpectrum& spec, const std::string& reads, uint32_t k, uint64_t window);
+// records, the windows, the time reading and gunzipping the file, and the window uploads' time.  sub.kernel_ms holds the record scan's
+// kernels after.  each (when given) runs after each window is packed, with its first record, its records and its first packed word.
+struct ReadPass { uint64_t reads = 0, windows = 0; double read_ms = 0, copy_ms = 0; };
+ReadPass pack_reads(DeviceSubsample& sub, DeviceSpectrum& spec, const std::string& reads, uint32_t k, uint64_t window,
+                    const std::function<void(uint64_t, uint64_t, uint64_t)>& each = nullptr);
 
 // The spectrum of one FASTQ file (gzipped or not): one pass of windows (subsample's scan and messages), each window packed on the
 // device, then the partitions counted.  hist gets the AC_GS_BINS bins; genome_size_rule makes the estimate from them.  InputError for a

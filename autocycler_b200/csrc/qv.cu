@@ -14,34 +14,6 @@
 // qv: pack, claim, probe, then multiplicity, support and spectrum per assembly, see DESIGN.md §20
 // ------------------------------------------------------------------------------------------------
 namespace {
-// One thread per packed word of every assembly: each window's key is claimed by linear probing from its home slot with a CAS on the
-// empty key; the flags stay 0, so DpProbeBody counts every read window that hits the key.
-struct QvClaimBody {
-    const uint64_t* code; const uint32_t* valid; uint32_t k; DepthSlot* table; uint64_t slots;
-    AC_D void operator()(uint64_t w) const {
-        dp_each_key(code, valid, w, k, [&](uint64_t key) {
-            uint64_t s = ac_umul64hi(gs_mix(key), slots);
-            const uint64_t tag = key + 1;
-            for (;;) {
-                DepthSlot* q = table + s;
-                uint64_t cur = ac_ld_volatile(&q->key);
-                if (cur == 0) cur = ac_atomic_cas(&q->key, (uint64_t)0, tag);
-                if (cur == 0 || cur == tag) return;
-                if (++s == slots) s = 0;
-            }
-        });
-    }
-};
-// The reads' count of a key the combined table holds.
-AC_D uint32_t qv_read_count(const DepthSlot* table, uint64_t slots, uint64_t key) {
-    uint64_t s = ac_umul64hi(gs_mix(key), slots);
-    for (;;) {
-        const DepthSlot* q = table + s;
-        if (q->key == key + 1) return q->count;
-        if (q->key == 0) return 0;
-        if (++s == slots) s = 0;
-    }
-}
 // One thread per packed word of one assembly (from word w0): each window adds 1 to its key's m in the multiplicity table; the thread
 // that claims the slot copies the key's read count from the combined table.
 struct QvMultBody {

@@ -33,6 +33,7 @@
  *   depth_filter, depth_from_header         helper.rs:889-931        -> ac_depth_filter_text, ac_depth_from_header
  *   depth (read-measured contig depth)      not in the reference     -> ac_depth_fasta
  *   qv (k-mer QV and completeness)          not in the reference     -> ac_qv_dir
+ *   unassembled (reads the assembly lacks)  not in the reference     -> ac_unassembled_dir
  *
  * Conventions: every function returns 0 on success and a negative AC_E* code on failure; the message
  * is available from ac_last_error(handle) (or ac_last_error(NULL) when no handle exists).  No C++
@@ -543,6 +544,49 @@ typedef struct {
 } ac_qv_info;
 int ac_qv_dir(const char* reads, const char* const* inputs, uint32_t n_inputs, const char* out_dir, uint32_t k, const uint32_t* min_count,
               int32_t device, int32_t verbose, uint64_t* kmers, uint64_t* unsupported, uint64_t* solid_found, uint64_t cap, ac_qv_info* info);
+
+/* `autocycler unassembled -r reads -i assemblies... -o out_dir [--kmer 21] [--min_count N] [--min_solid 100] [--min_fraction 0.5]`: the
+ * reads the assembly does not explain, and the depth of the sequence it misses, counted on the GPU.  Not in the reference (DESIGN.md
+ * section 21).  inputs: n_inputs paths, each a FASTA file or a directory, expanded as in ac_qv_dir; the contigs of all of them together are
+ * the assembly, and A is the set of their canonical keys (qv's contig windows, junction windows included).  Read windows, r(key) and the
+ * histogram are genome_size's; the solid threshold t is *min_count (1 .. AC_GENOME_SIZE_BINS - 1, else AC_EINPUT) or the valley when
+ * min_count is NULL (no valley: AC_EINPUT "no k-mer depth peak: ...").  Per read i: s_i = its windows whose key has r >= t, a_i = those
+ * of them whose key is not in A; the read is scored when s_i >= min_solid (>= 1, else AC_EINPUT) and selected when it is scored and
+ * (double)a_i >= min_fraction * (double)s_i (0 < min_fraction <= 1, else AC_EINPUT).  The absent keys are the distinct keys with r >= t
+ * not in A.  out_dir (created if needed) gets unassembled.fastq (the selected records in input order), unassembled.tsv,
+ * fraction_histogram.tsv, absent_histogram.tsv, kmer_histogram.tsv (as helper genome_size -d writes it) and summary.tsv.  k: odd, 11..31,
+ * else AC_EINPUT.  An assembly without windows (naming the inputs), reads without windows: AC_EINPUT.  The assembly set, the per-read
+ * counters and the word indices beyond half the free device memory: AC_ERANGE.  verbose prints the settings and the counts to stderr.
+ * Calls on one device run one at a time, with subsample's.  info may be NULL. */
+typedef struct {
+    uint64_t assemblies, contigs;
+    uint32_t k;
+    uint32_t min_count;                /* t, given or the valley */
+    uint64_t valley;                   /* v of the reads' histogram (0: none) */
+    uint64_t reads, read_windows, read_bases;
+    uint64_t distinct;                 /* distinct canonical read k-mers */
+    uint64_t scored_reads, selected_reads, selected_bases;
+    uint64_t absent_kmers;             /* distinct keys with r >= t that the assembly lacks */
+    double absent_median;              /* the median of their bins (NaN: no absent key) */
+    double peak;                       /* genome_size's refined peak p* (NaN: the rule refuses the histogram) */
+    double absent_copy_ratio;          /* absent_median / peak (NaN when either is) */
+    uint64_t assembly_windows;         /* the assembly's windows, junction windows included */
+    uint64_t table_bytes;              /* the assembly set */
+    uint64_t read_bytes;               /* the per-read counters and lengths, and the word indices */
+    uint64_t spectrum_table_bytes;     /* the read spectrum's largest table */
+    uint64_t partitions, reruns;       /* of the read spectrum, over both sweeps */
+    uint64_t read_passes;              /* 1, or 2 when the selected reads were gathered from a second read of the file */
+    float kernel_ms;                   /* CUDA events around every kernel, summed (0 under emulation) */
+    float scan_ms, pack_ms, claim_ms, count_ms, sweep_ms, gather_ms;   /* record scans, read packing and word indices, assembly pack and
+                                                                          claim, spectrum count and histogram, attribution sweep (its
+                                                                          recounts included), the FASTQ gather (with
+                                                                          the second read's record scans) */
+    double read_ms;                    /* host: reading and gunzipping the reads, both passes */
+    double copy_ms;                    /* host wall time of the window uploads */
+    double write_ms;                   /* host: writing the output files */
+} ac_unassembled_info;
+int ac_unassembled_dir(const char* reads, const char* const* inputs, uint32_t n_inputs, const char* out_dir, uint32_t k, const uint32_t* min_count,
+                       uint64_t min_solid, double min_fraction, int32_t device, int32_t verbose, ac_unassembled_info* info);
 
 #ifdef __cplusplus
 }
