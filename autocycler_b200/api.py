@@ -146,6 +146,20 @@ class AcUnassembledInfo(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class AcPolishInfo(C.Structure):
+    _fields_ = [("contigs", C.c_uint64), ("k", C.c_uint32), ("min_count", C.c_uint32), ("valley", C.c_uint64), ("reads", C.c_uint64),
+                ("read_windows", C.c_uint64), ("read_bases", C.c_uint64), ("distinct", C.c_uint64), ("kmers_before", C.c_uint64),
+                ("unsupported_before", C.c_uint64), ("kmers_after", C.c_uint64), ("unsupported_after", C.c_uint64), ("edits", C.c_uint64),
+                ("rounds", C.c_uint64), ("loci", C.c_uint64), ("table_bytes", C.c_uint64), ("candidate_table_bytes", C.c_uint64),
+                ("batches", C.c_uint64), ("spectrum_table_bytes", C.c_uint64), ("partitions", C.c_uint64), ("reruns", C.c_uint64),
+                ("kernel_ms", C.c_float), ("scan_ms", C.c_float), ("pack_ms", C.c_float), ("count_ms", C.c_float), ("contig_ms", C.c_float),
+                ("fill_ms", C.c_float), ("recount_ms", C.c_float), ("candidate_ms", C.c_float), ("choose_ms", C.c_float),
+                ("read_ms", C.c_double), ("copy_ms", C.c_double), ("host_ms", C.c_double), ("write_ms", C.c_double)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_sequence", "ac_clear_sequences", "ac_upload",
            "ac_build", "ac_compress", "ac_simplify", "ac_merge_linear_paths", "ac_renumber_unitigs", "ac_load_gfa", "ac_bind_host_to_device", "ac_decompress_gfa", "ac_pairwise_distances", "ac_distance_matrix_text", "ac_sequence_reconstruct", "ac_counts_get", "ac_unitigs_copy", "ac_path_copy", "ac_gfa_size", "ac_gfa_copy",
            "ac_timings_get", "ac_compress_dir", "ac_compress_dir_devices", "ac_load_sequences", "ac_sequence_get",
@@ -159,7 +173,8 @@ EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_seq
            "ac_clean_gfa", "ac_clean_text", "ac_gfa_to_fasta", "ac_gfa_fasta_text", "ac_table_text",
            "ac_subsample_dir", "ac_genome_size", "ac_subsample_words", "ac_subsample_shuffle",
            "ac_genome_size_estimate", "ac_genome_size_from_histogram",
-           "ac_depth_fasta", "ac_depth_filter_text", "ac_depth_from_header", "ac_qv_dir", "ac_unassembled_dir"]
+           "ac_depth_fasta", "ac_depth_filter_text", "ac_depth_from_header", "ac_qv_dir", "ac_unassembled_dir",
+           "ac_polish_fasta"]
 
 _libs = {}
 
@@ -285,6 +300,8 @@ def load_library(path=None):
                               C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.c_uint64, C.POINTER(AcQvInfo)]
     lib.ac_unassembled_dir.argtypes = [C.c_char_p, C.POINTER(C.c_char_p), C.c_uint32, C.c_char_p, C.c_uint32, C.POINTER(C.c_uint32), C.c_uint64,
                                        C.c_double, C.c_int32, C.c_int32, C.POINTER(AcUnassembledInfo)]
+    lib.ac_polish_fasta.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint32, C.POINTER(C.c_uint32), C.c_uint32, C.c_uint32, C.c_int32,
+                                    C.c_int32, C.POINTER(AcPolishInfo)]
     lib.ac_table_text.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint64, C.c_int32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     _libs[path] = lib
     return lib
@@ -976,4 +993,27 @@ def unassembled(reads, assemblies, out_dir, k=21, min_count=None, min_solid=100,
         lines = f.read().splitlines()
     out["selected"] = [{"read": r[0], "length": int(r[1]), "solid_kmers": int(r[2]), "absent_kmers": int(r[3])}
                        for r in (line.split("\t") for line in lines[1:])]
+    return out
+
+
+def polish(reads, assembly, out_dir, k=21, min_count=None, max_indel=3, rounds=3, device=0, verbose=False, lib=None):
+    """`autocycler polish` (DESIGN.md §22): the consensus corrected where the reads' k-mers do not support it, with candidate edits
+    scored on the GPU (not in the reference).  Returns the info dict (t is "min_count", the stage timings in ms) with "qv_before" and
+    "qv_after" (None for an empty field, float("inf") for inf) and "applied": per applied edit a dict of round, contig, position, ref, alt
+    and score, both read back from the summary.tsv and edits.tsv the call wrote."""
+    lib = lib or load_library()
+    info = AcPolishInfo()
+    t = None if min_count is None else C.byref(C.c_uint32(min_count))
+    _raise_unless_ok(lib, lib.ac_polish_fasta(os.fsencode(reads), os.fsencode(assembly), os.fsencode(out_dir), k, t, max_indel, rounds, device,
+                                              1 if verbose else 0, C.byref(info)))
+    out = info.as_dict()
+    with open(os.path.join(out_dir, "summary.tsv")) as f:
+        head, row = (line.split("\t") for line in f.read().splitlines())
+    summary = dict(zip(head, row))
+    for name in ("qv_before", "qv_after"):
+        out[name] = None if summary[name] == "" else float(summary[name])
+    with open(os.path.join(out_dir, "edits.tsv")) as f:
+        lines = f.read().splitlines()
+    out["applied"] = [{"round": int(r[0]), "contig": r[1], "position": int(r[2]), "ref": r[3], "alt": r[4], "score": int(r[5])}
+                    for r in (line.split("\t") for line in lines[1:])]
     return out

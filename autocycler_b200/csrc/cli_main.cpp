@@ -3,8 +3,9 @@
 // (misc.rs:130-136: "Error: <text>" on stderr, exit 1), running the H100 path through the C ABI; `autocycler helper genome_size`,
 // which departs from the reference on purpose: a k-mer depth estimate on the GPU instead of the length of a Raven assembly; and
 // `autocycler depth`, read-measured contig depth (not in the reference) with the reference's helper depth filter; `autocycler qv`,
-// each assembly's k-mer QV and completeness against the reads (not in the reference); and `autocycler unassembled`, the reads the
-// assembly does not explain (not in the reference).
+// each assembly's k-mer QV and completeness against the reads (not in the reference); `autocycler unassembled`, the reads the
+// assembly does not explain (not in the reference); and `autocycler polish`, the consensus corrected from the reads' k-mers (not in the
+// reference).
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -478,6 +479,56 @@ static int unassembled_main(int argc, char** argv) {
     return finish(rc);
 }
 
+// `autocycler polish`: the consensus corrected where the reads' k-mers do not support it, with candidate edits scored on the GPU (not in
+// the reference).  summary.tsv also goes to stdout, byte for byte.
+static const char* polish_usage =
+    "Usage: autocycler polish --reads <READS> --input <FASTA> --out_dir <DIR> [--kmer 21] [--min_count N] [--max_indel 3] [--rounds 3]\n"
+    "                         [--device N]\n\n"
+    "Corrects the consensus where the reads' k-mers do not support it, with candidate edits scored on the GPU: at each run of\n"
+    "unsupported k-mers it tries every substitution and every insertion or deletion of up to --max_indel bases, and keeps the one that\n"
+    "makes every k-mer it touches solid. This command is not in the reference. Writes polished.fasta, edits.tsv, rounds.tsv,\n"
+    "remaining.bed and summary.tsv (also to stdout). Paired short reads go in as one file: cat R1.fq.gz R2.fq.gz > reads.fq.gz.\n\n"
+    "Options:\n"
+    "  -r, --reads <READS>            Reads in FASTQ format, gzipped or not (required)\n"
+    "  -i, --input <FASTA>            Assembly in FASTA format, gzipped or not (required)\n"
+    "  -o, --out_dir <DIR>            Directory to create and write the polished assembly and tables into (required)\n"
+    "      --kmer <KMER>              K-mer size, odd, 11 to 31 [default: 21]\n"
+    "      --min_count <N>            Read count from which a k-mer is solid, 1 to 16383 [default: the valley of the reads' k-mer spectrum]\n"
+    "      --max_indel <L>            Longest insertion or deletion tried, 1 to 4 [default: 3]\n"
+    "      --rounds <N>               Most rounds of edits, 1 to 10 [default: 3]\n"
+    "      --device <ORDINAL>         CUDA device [default: 0]\n";
+static int polish_main(int argc, char** argv) {
+    Args a{argc, argv, polish_usage};
+    std::string reads, in, out; bool has_min = false;
+    unsigned long k = 21, min_count = 0, max_indel = 3, rounds = 3; int device = 0;
+    auto refuse = [&]() { fprintf(stderr, "error: invalid value '%s' for '%s'\n%s", argv[a.i], a.flag.c_str(), polish_usage); return 2; };
+    while (a.next()) {
+        if (a.is("-r", "--reads")) reads = a.value();
+        else if (a.is("-i", "--input")) in = a.value();
+        else if (a.is("-o", "--out_dir")) out = a.value();
+        else if (a.is("--kmer")) { k = (unsigned long)a.number(true); if (k < 11 || k > 31 || k % 2 == 0) return refuse(); }
+        else if (a.is("--min_count")) { min_count = (unsigned long)a.number(true); if (min_count < 1 || min_count > 16383) return refuse(); has_min = true; }
+        else if (a.is("--max_indel")) { max_indel = (unsigned long)a.number(true); if (max_indel < 1 || max_indel > 4) return refuse(); }
+        else if (a.is("--rounds")) { rounds = (unsigned long)a.number(true); if (rounds < 1 || rounds > 10) return refuse(); }
+        else if (a.is("--device")) device = atoi(a.value());
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
+    }
+    if (reads.empty() || in.empty() || out.empty()) return a.missing();
+    const uint32_t t = (uint32_t)min_count;
+    const int rc = ac_polish_fasta(reads.c_str(), in.c_str(), out.c_str(), (uint32_t)k, has_min ? &t : nullptr, (uint32_t)max_indel,
+                                   (uint32_t)rounds, device, 1, nullptr);
+    if (rc == AC_OK) {
+        FILE* f = fopen((out + "/summary.tsv").c_str(), "rb");
+        if (f) {
+            char buf[1 << 16]; size_t n;
+            while ((n = fread(buf, 1, sizeof buf, f)) > 0) fwrite(buf, 1, n, stdout);
+            fclose(f);
+        }
+    }
+    return finish(rc);
+}
+
 int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "dotplot") == 0) return dotplot_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "resolve") == 0) return resolve_main(argc, argv);
@@ -494,6 +545,7 @@ int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "depth") == 0) return depth_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "qv") == 0) return qv_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "unassembled") == 0) return unassembled_main(argc, argv);
+    if (argc >= 2 && strcmp(argv[1], "polish") == 0) return polish_main(argc, argv);
     fprintf(stderr, "%s", compress_usage);
     return 2;
 }

@@ -1,5 +1,6 @@
-// The device parts of `autocycler trim`, `resolve`, `cluster`, `dotplot`, `subsample`, `helper genome_size`, `depth`, `qv` and `unassembled`.  Each object owns its device buffers (allocated on first
-// use, kept for the next call) and runs on the device and stream of the DeviceContext it is given, which must outlive it.
+// The device parts of `autocycler trim`, `resolve`, `cluster`, `dotplot`, `subsample`, `helper genome_size`, `depth`, `qv`, `unassembled`
+// and `polish`.  Each object owns its device buffers (allocated on first use, kept for the next call) and runs on the device and stream
+// of the DeviceContext it is given, which must outlive it.
 #pragma once
 #include <cstdint>
 #include <functional>
@@ -183,9 +184,10 @@ public:
     // take; parts: the partitions to use (0: the smallest power of two whose 2 W / P slots fit the budget).  A partition whose probe
     // limit is hit is counted again with twice the slots.
     void count(uint64_t windows, uint64_t budget_slots, uint64_t parts, uint64_t* hist, SpectrumRun* run);
-    // A second sweep over the partitions count() made, for a rule that needs the whole histogram first: each(table, slots, P, part) runs
-    // once per partition with that partition's table on the device.  The last partition's table is the one count() left behind; every
-    // other partition is counted again at the slots count() settled on (run gets those counts' time, and any rerun).
+    // A further sweep over the partitions count() made, for a rule that needs the whole histogram first: each(table, slots, P, part) runs
+    // once per partition with that partition's table on the device.  The table the last count or sweep left behind goes first (after
+    // count(), the last partition's); every other partition is counted again at the slots count() settled on (run gets those counts'
+    // time, and any rerun).  With one partition a sweep counts nothing.
     void sweep(const std::function<void(const GsSlot*, uint64_t, uint64_t, uint64_t)>& each, SpectrumRun* run);
     float kernel_ms = 0.f;           // the kernels of every call since begin() (CUDA events; 0 under emulation)
     // The packed stream so far, on the device: `packed_words()` words of codes and validity masks (DeviceDepth::probe reads it).
@@ -201,6 +203,7 @@ private:
     SerialScan<uint64_t, AC_SUB_SCAN_TILE, 8> scan_u64;          // of the records' word counts
     uint32_t k = 21;
     uint64_t words = 0;              // packed words so far
+    uint64_t resident = 0;           // the partition whose table d_table holds
     float pack_ms = 0.f;
     std::vector<uint64_t> part_slots;                            // each partition's slots in the last count()
     DevBuf d_code, d_valid, d_woff, d_tot, d_table, d_flag, d_hist;
@@ -307,4 +310,61 @@ private:
     uint32_t k = 21;
     uint64_t slots = 0;
     DevBuf d_bytes, d_contig, d_code, d_valid, d_wcid, d_table, d_read, d_len, d_counts, d_absent;
+};
+
+// `autocycler polish`: the consensus corrected where the reads' k-mers do not support it (DESIGN.md §22).  Each round packs the contigs
+// (depth's layout) and claims their canonical keys in a DepthSlot query table; a sweep over the read spectrum's partitions copies each
+// key's read count r into the table, and a mask of the windows with r < t goes back to the host, which builds the loci.  For every
+// attempted locus and each of its candidate edits, the k + s windows of the edited sequence that cover the edit are claimed in a candidate
+// table, filled by a second sweep, and scored by their minimum r; one warp per locus then picks the best score and counts the candidates
+// that hold it.
+struct PlLocus { uint64_t word0, len, a; uint32_t circular, pad; };   // its contig's first packed word and length; the first unsupported window
+// Candidate c of a locus at a largest indel of L (cur: the round's base at p0, 0..3 for A, C, G, T): the bases it puts at p0 (base i in
+// bits 2i..2i+1, mlen of them) and the round's bases from p0 on that they replace (skip).  0..2: the other three bases in A, C, G, T
+// order; 3..L+2: deletion of c-2 bases; then the insertions of 1, 2, ... L bases, each length's strings in lexicographic order.
+struct PlEdit { uint32_t mid, mlen, skip; };
+AC_HD PlEdit pl_edit(uint32_t c, uint32_t L, uint32_t cur) {
+    if (c < 3) return PlEdit{c < cur ? c : c + 1, 1, 1};
+    if (c < 3 + L) return PlEdit{0, 0, c - 2};
+    uint32_t i = c - 3 - L, s = 1, n = 4;
+    while (i >= n) { i -= n; ++s; n *= 4; }
+    uint32_t mid = 0;
+    for (uint32_t j = 0; j < s; ++j) mid |= ((i >> (2 * (s - 1 - j))) & 3u) << (2 * j);
+    return PlEdit{mid, s, 0};
+}
+// What the device ran: the window table's bytes, the largest candidate table's, the candidate batches, and the kernels' time by stage
+// (CUDA events; 0 under emulation).  sweep: the sweeps' recounts of partitions (none with one partition).
+struct PlRun {
+    uint64_t table_bytes = 0, candidate_bytes = 0, batches = 0;
+    float pack_ms = 0.f, fill_ms = 0.f, candidate_ms = 0.f, choose_ms = 0.f;
+    SpectrumRun sweep;
+};
+
+class DevicePolish {
+public:
+    explicit DevicePolish(DeviceContext& ctx) : ctx(ctx) {}
+    ~DevicePolish() { ctx.make_current(); }
+    // The candidates per locus at a largest indel of L (3 + L + sum_{s=1..L} 4^s) and their checked windows (sum of k + s).
+    static uint64_t candidates(uint32_t max_indel);
+    static uint64_t candidate_windows(uint32_t k, uint32_t max_indel);
+    // The buffers for every round, before the read spectrum takes its share of the device: contigs of up to `bytes` bytes (junction bases
+    // included) in `words` packed words with `windows` windows.  The window table takes max(2 windows, 64) slots; std::length_error when
+    // that exceeds budget_slots.
+    void reserve(uint64_t bytes, uint64_t words, uint64_t windows, uint32_t k, uint64_t budget_slots, PlRun* run);
+    // One round's contigs (after reserve, within its sizes; after spec.count with the same k): bytes back to back, contig c taking len[c]
+    // of them (a circular contig followed by its first k-1 bases).  mask[i] (one u32 per packed word, each contig from a fresh word) has
+    // bit j set when the window that ends at base j of that word has a read count below t.
+    void windows(DeviceSpectrum& spec, const uint8_t* bytes, const uint64_t* len, uint32_t n_contigs, uint64_t windows, uint32_t t, uint32_t* mask,
+                 PlRun* run);
+    // The candidates of n loci of the round windows() packed last, in batches whose candidate tables fit budget_slots (std::length_error
+    // when one locus's does not).  out[3 i .. 3 i + 2] = locus i's best score (0: no candidate passes), the candidates that hold it and
+    // the first of them.
+    void choose(DeviceSpectrum& spec, const PlLocus* loci, uint64_t n, uint32_t max_indel, uint32_t t, uint64_t budget_slots, uint32_t* out,
+                PlRun* run);
+private:
+    void fill(DeviceSpectrum& spec, DepthSlot* table, uint64_t slots, PlRun* run);
+    DeviceContext& ctx;
+    uint32_t k = 21;
+    uint64_t slots = 0, words = 0;
+    DevBuf d_bytes, d_contig, d_code, d_valid, d_wcid, d_table, d_mask, d_loci, d_cand, d_score, d_out;
 };

@@ -1,6 +1,7 @@
-// The assembly side of the packed k-mer stream, shared by `depth` (depth.cu), `qv` (qv.cu) and `unassembled` (unassembled.cu): contigs
-// packed like the reads, each from a fresh word that keeps its contig id, the canonical keys of the windows that end in a word, the
-// claim of an assembly's keys and the read probe into a DepthSlot table, its lookups, and the warp-grouped add (DESIGN.md §19-§21).
+// The assembly side of the packed k-mer stream, shared by `depth` (depth.cu), `qv` (qv.cu), `unassembled` (unassembled.cu) and `polish`
+// (polish.cu): contigs packed like the reads, each from a fresh word that keeps its contig id, the canonical keys of the windows that end
+// in a word, the claim of an assembly's keys and the read probe into a DepthSlot table, its lookups, a key's count in a spectrum
+// partition's table, and the warp-grouped add (DESIGN.md §19-§22).
 // Device code only.  The bodies sit in an anonymous namespace on purpose: each
 // file that includes this header launches its own kernels of them, as depth.cu did when they were its own.
 #pragma once
@@ -74,22 +75,24 @@ struct DpProbeBody {
         });
     }
 };
-// One thread per packed word of every assembly: each window's key is claimed by linear probing from its home slot with a CAS on the
-// empty key; the flags stay 0, so DpProbeBody counts every read window that hits the key.
+// Claims a key in a DepthSlot table by linear probing from its home slot with a CAS on the empty key.
+AC_D void dp_claim(DepthSlot* table, uint64_t slots, uint64_t key) {
+    uint64_t s = ac_umul64hi(gs_mix(key), slots);
+    const uint64_t tag = key + 1;
+    for (;;) {
+        DepthSlot* q = table + s;
+        uint64_t cur = ac_ld_volatile(&q->key);
+        if (cur == 0) cur = ac_atomic_cas(&q->key, (uint64_t)0, tag);
+        if (cur == 0 || cur == tag) return;
+        if (++s == slots) s = 0;
+    }
+}
+// One thread per packed word of every assembly: each window's key is claimed (dp_claim); the flags stay 0, so DpProbeBody counts every
+// read window that hits the key.
 struct QvClaimBody {
     const uint64_t* code; const uint32_t* valid; uint32_t k; DepthSlot* table; uint64_t slots;
     AC_D void operator()(uint64_t w) const {
-        dp_each_key(code, valid, w, k, [&](uint64_t key) {
-            uint64_t s = ac_umul64hi(gs_mix(key), slots);
-            const uint64_t tag = key + 1;
-            for (;;) {
-                DepthSlot* q = table + s;
-                uint64_t cur = ac_ld_volatile(&q->key);
-                if (cur == 0) cur = ac_atomic_cas(&q->key, (uint64_t)0, tag);
-                if (cur == 0 || cur == tag) return;
-                if (++s == slots) s = 0;
-            }
-        });
+        dp_each_key(code, valid, w, k, [&](uint64_t key) { dp_claim(table, slots, key); });
     }
 };
 // The reads' count of a key the combined table holds.
@@ -99,6 +102,16 @@ AC_D uint32_t qv_read_count(const DepthSlot* table, uint64_t slots, uint64_t key
         const DepthSlot* q = table + s;
         if (q->key == key + 1) return q->count;
         if (q->key == 0) return 0;
+        if (++s == slots) s = 0;
+    }
+}
+// The read count of a key of partition `part` of the read spectrum (h: its mix) in that partition's table, which holds every such key.
+AC_D uint32_t ua_read_count(const GsSlot* table, uint64_t slots, uint64_t parts, uint64_t h, uint64_t key) {
+    uint64_t s = ac_umul64hi(h * parts, slots);
+    for (;;) {
+        const GsSlot q = table[s];
+        if (q.key == key + 1) return q.count;
+        if (q.key == 0) return 0;
         if (++s == slots) s = 0;
     }
 }

@@ -189,6 +189,7 @@ uint64_t DeviceSpectrum::count_partition(uint64_t parts, uint64_t part, uint64_t
         ac_sync(st);
         run->count_ms += tc.ms();
         if (overflow) { ++run->reruns; continue; }
+        resident = part;
         return slots;
     }
 }
@@ -231,9 +232,10 @@ void DeviceSpectrum::sweep(const std::function<void(const GsSlot*, uint64_t, uin
     ctx.make_current();
     const uint64_t parts = part_slots.size();
     if (!parts) throw std::logic_error("genome_size: a second sweep before the count");
-    // the last partition's table is still in d_table, so it goes first; every other one is counted again at its settled slots
+    // the partition whose table is still in d_table goes first; every other one is counted again at its settled slots
+    const uint64_t first = resident;
     for (uint64_t i = 0; i < parts; ++i) {
-        const uint64_t part = (parts - 1 + i) % parts;
+        const uint64_t part = (first + i) % parts;
         uint64_t slots = part_slots[part];
         if (i) slots = count_partition(parts, part, slots, run);
         each(d_table.as<GsSlot>(), slots, parts, part);

@@ -43,8 +43,8 @@ std::string percent(uint64_t num, uint64_t den) {
     return buf;
 }
 
-// One contig's BED lines from its masks (one u32 per packed word): each unsupported window ending at e covers [e-k+1, e], split at the
-// end of a circular contig's sequence; touching and overlapping intervals merged.
+}  // namespace
+
 void contig_bed(const std::string& name, uint64_t L, const uint32_t* mask, uint64_t words, uint32_t k, std::string& bed) {
     std::vector<std::pair<uint64_t, uint64_t>> iv;
     for (uint64_t j = 0; j < words; ++j)
@@ -61,7 +61,6 @@ void contig_bed(const std::string& name, uint64_t L, const uint32_t* mask, uint6
         bed += name + "\t" + std::to_string(s) + "\t" + std::to_string(e) + "\n";
     }
 }
-}  // namespace
 
 void qv_run(DeviceSubsample& sub, DeviceSpectrum& spec, DeviceQv& dev, const std::vector<std::string>& paths, const std::string& reads,
             uint32_t k, const uint32_t* min_count, uint64_t window, QvResult& out) {

@@ -37,6 +37,9 @@ std::vector<std::string> qv_inputs(const std::vector<std::string>& args);
 void qv_run(DeviceSubsample& sub, DeviceSpectrum& spec, DeviceQv& dev, const std::vector<std::string>& assemblies, const std::string& reads,
             uint32_t k, const uint32_t* min_count, uint64_t window, QvResult& out);
 
+// One contig's BED lines (appended to bed) from its masks, one u32 per packed word of its L bases and junction bases: each unsupported
+// window ending at e covers [e-k+1, e], split at the end of a circular contig's sequence; touching and overlapping intervals merged.
+void contig_bed(const std::string& name, uint64_t L, const uint32_t* mask, uint64_t words, uint32_t k, std::string& bed);
 // -10 log10(p), p = -expm1(log1p(-E / K) / k), as `%.2f`; "inf" for E = 0 and "" for K = 0.
 std::string qv_text(uint64_t unsupported, uint64_t kmers, uint32_t k);
 // The files under out_dir: qv.tsv, contig_qv.tsv and kmer_histogram.tsv (the BED and spectrum texts are in each QvAssembly).

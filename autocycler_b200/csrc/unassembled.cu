@@ -25,16 +25,6 @@ struct UaIndexBody {
         if (lane == 0) len[first + r] = rec[r].seq_len;
     }
 };
-// The read count of a key of this partition (h: its mix) in the partition's table, which holds every such key.
-AC_D uint32_t ua_read_count(const GsSlot* table, uint64_t slots, uint64_t parts, uint64_t h, uint64_t key) {
-    uint64_t s = ac_umul64hi(h * parts, slots);
-    for (;;) {
-        const GsSlot q = table[s];
-        if (q.key == key + 1) return q.count;
-        if (q.key == 0) return 0;
-        if (++s == slots) s = 0;
-    }
-}
 // *p += s | a << 32 (the read's two u32 counters; s < 2^32 for any read).  On the device the lanes of a warp that add to the same read
 // are grouped first, one atomic per group: consecutive words almost always belong to one read.
 #ifdef AC_EMULATE

@@ -34,6 +34,7 @@
  *   depth (read-measured contig depth)      not in the reference     -> ac_depth_fasta
  *   qv (k-mer QV and completeness)          not in the reference     -> ac_qv_dir
  *   unassembled (reads the assembly lacks)  not in the reference     -> ac_unassembled_dir
+ *   polish (k-mer consensus correction)     not in the reference     -> ac_polish_fasta
  *
  * Conventions: every function returns 0 on success and a negative AC_E* code on failure; the message
  * is available from ac_last_error(handle) (or ac_last_error(NULL) when no handle exists).  No C++
@@ -587,6 +588,48 @@ typedef struct {
 } ac_unassembled_info;
 int ac_unassembled_dir(const char* reads, const char* const* inputs, uint32_t n_inputs, const char* out_dir, uint32_t k, const uint32_t* min_count,
                        uint64_t min_solid, double min_fraction, int32_t device, int32_t verbose, ac_unassembled_info* info);
+
+/* `autocycler polish -r reads -i assembly -o out_dir [--kmer 21] [--min_count N] [--max_indel 3] [--rounds 3]`: the consensus corrected
+ * where the reads' k-mers do not support it, with candidate edits scored on the GPU.  Not in the reference (DESIGN.md section 22).
+ * assembly: one FASTA file (gzipped or not, loaded as load_fasta does).  Contig windows, r(key), the histogram and the solid threshold t
+ * (*min_count, 1 .. AC_GENOME_SIZE_BINS - 1, else AC_EINPUT; the valley when min_count is NULL) are ac_qv_dir's, on each round's sequence.
+ * Each round: a locus is a maximal run [a, b] of window starts with r < t (cyclic on a circular contig), tried when window a-1 exists and
+ * has r >= t (and a circular contig is at least 2k + 2 max_indel long); at p0 = a + k - 1 its 3 substitutions, deletions of 1 .. max_indel
+ * bases and insertions of every string of 1 .. max_indel bases before p0 are scored by the minimum r over the k + s windows of the edited
+ * sequence that cover the edit; a candidate passes when all of them are windows (inside a linear contig) with r >= t.  A unique best is
+ * accepted; accepted edits whose spans [a, p0 + d + k) overlap a kept one's (ascending a) wait for the next round.  The rounds stop after
+ * `rounds` (1..10, else AC_EINPUT) or at the first that applies no edit.  max_indel: 1..4, else AC_EINPUT.  out_dir (created if needed)
+ * gets polished.fasta, edits.tsv, rounds.tsv, remaining.bed (qv's unsupported/1.bed of polished.fasta) and summary.tsv.  k: odd, 11..31,
+ * else AC_EINPUT.  An assembly or reads without windows: AC_EINPUT.  The window table beyond half the free device memory, or one locus's
+ * candidate table beyond half of what the read spectrum leaves: AC_ERANGE.  verbose prints the settings, the counts and one line per round
+ * to stderr.  Calls on one device run one at a time, with subsample's.  info may be NULL. */
+typedef struct {
+    uint64_t contigs;
+    uint32_t k;
+    uint32_t min_count;                /* t, given or the valley */
+    uint64_t valley;                   /* v of the reads' histogram (0: none) */
+    uint64_t reads, read_windows, read_bases;
+    uint64_t distinct;                 /* distinct canonical read k-mers */
+    uint64_t kmers_before, unsupported_before, kmers_after, unsupported_after;   /* the input's and polished.fasta's K and E */
+    uint64_t edits, rounds, loci;      /* applied edits, rounds run, loci over every round */
+    uint64_t table_bytes;              /* the contigs' window table */
+    uint64_t candidate_table_bytes;    /* the largest candidate table */
+    uint64_t batches;                  /* candidate batches over every round */
+    uint64_t spectrum_table_bytes;     /* the read spectrum's largest table */
+    uint64_t partitions, reruns;       /* of the read spectrum, over the count and every sweep */
+    float kernel_ms;                   /* CUDA events around every kernel, summed (0 under emulation) */
+    float scan_ms, pack_ms, count_ms, contig_ms, fill_ms, recount_ms, candidate_ms, choose_ms;   /* record scan, read packing, spectrum count
+                                                                                                    and histogram, contig pack and claim, read
+                                                                                                    count fills and unsupported masks, the
+                                                                                                    sweeps' recounts of partitions, candidate
+                                                                                                    claims and scores, choices */
+    double read_ms;                    /* host: reading and gunzipping the reads */
+    double copy_ms;                    /* host wall time of the window uploads */
+    double host_ms;                    /* host: loci, overlaps, edits and the contigs' packing */
+    double write_ms;                   /* host: writing the output files */
+} ac_polish_info;
+int ac_polish_fasta(const char* reads, const char* assembly, const char* out_dir, uint32_t k, const uint32_t* min_count, uint32_t max_indel,
+                    uint32_t rounds, int32_t device, int32_t verbose, ac_polish_info* info);
 
 #ifdef __cplusplus
 }
