@@ -107,7 +107,9 @@ struct PlChooseBody {
         for (uint32_t c = 0; c < C; ++c) pl_take(s[c], c, best, count, first);
 #else
         for (uint32_t c = lane; c < C; c += 32) pl_take(s[c], c, best, count, first);
-        const unsigned all = __activemask();
+        // Every lane of the warp gets here (the launch is 32 threads per locus), but after the loop above, whose trip count differs
+        // between lanes when C is not a multiple of 32, __activemask() need not name them all: the reductions take the whole warp.
+        const unsigned all = 0xFFFFFFFFu;
         const uint32_t top = __reduce_max_sync(all, best);
         count = __reduce_add_sync(all, best == top ? count : 0u);
         first = __reduce_min_sync(all, best == top ? first : 0xFFFFFFFFu);

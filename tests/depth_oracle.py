@@ -78,7 +78,8 @@ def depths(assembly, reads, k):
             counts += np.bincount(idx[hit], minlength=len(uniq))
     unique, dep = [], []
     for p in per:
-        mine = p[np.isin(p, uniq)]
+        at = np.minimum(np.searchsorted(uniq, p), max(len(uniq) - 1, 0))
+        mine = p[uniq[at] == p] if len(uniq) else p[:0]           # np.isin(p, uniq), without a sort of uniq per contig
         unique.append(len(mine))
         if not len(mine):
             dep.append(None)
