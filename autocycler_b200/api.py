@@ -160,6 +160,21 @@ class AcPolishInfo(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class AcVariantsInfo(C.Structure):
+    _fields_ = [("contigs", C.c_uint64), ("k", C.c_uint32), ("min_count", C.c_uint32), ("valley", C.c_uint64), ("reads", C.c_uint64),
+                ("read_windows", C.c_uint64), ("read_bases", C.c_uint64), ("distinct", C.c_uint64), ("kmers", C.c_uint64),
+                ("positions", C.c_uint64), ("screened", C.c_uint64), ("candidates", C.c_uint64), ("loci", C.c_uint64), ("passing", C.c_uint64),
+                ("variants", C.c_uint64), ("substitutions", C.c_uint64), ("insertions", C.c_uint64), ("deletions", C.c_uint64),
+                ("paralog", C.c_uint64), ("alt_major", C.c_uint64), ("table_bytes", C.c_uint64), ("candidate_table_bytes", C.c_uint64),
+                ("batches", C.c_uint64), ("spectrum_table_bytes", C.c_uint64), ("partitions", C.c_uint64), ("reruns", C.c_uint64),
+                ("kernel_ms", C.c_float), ("scan_ms", C.c_float), ("pack_ms", C.c_float), ("count_ms", C.c_float), ("contig_ms", C.c_float),
+                ("fill_ms", C.c_float), ("screen_ms", C.c_float), ("recount_ms", C.c_float), ("candidate_ms", C.c_float), ("ref_ms", C.c_float),
+                ("read_ms", C.c_double), ("copy_ms", C.c_double), ("host_ms", C.c_double), ("write_ms", C.c_double)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
 EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_sequence", "ac_clear_sequences", "ac_upload",
            "ac_build", "ac_compress", "ac_simplify", "ac_merge_linear_paths", "ac_renumber_unitigs", "ac_load_gfa", "ac_bind_host_to_device", "ac_decompress_gfa", "ac_pairwise_distances", "ac_distance_matrix_text", "ac_sequence_reconstruct", "ac_counts_get", "ac_unitigs_copy", "ac_path_copy", "ac_gfa_size", "ac_gfa_copy",
            "ac_timings_get", "ac_compress_dir", "ac_compress_dir_devices", "ac_load_sequences", "ac_sequence_get",
@@ -174,7 +189,7 @@ EXPORTS = ["ac_last_error", "ac_version", "ac_create", "ac_destroy", "ac_add_seq
            "ac_subsample_dir", "ac_genome_size", "ac_subsample_words", "ac_subsample_shuffle",
            "ac_genome_size_estimate", "ac_genome_size_from_histogram",
            "ac_depth_fasta", "ac_depth_filter_text", "ac_depth_from_header", "ac_qv_dir", "ac_unassembled_dir",
-           "ac_polish_fasta"]
+           "ac_polish_fasta", "ac_variants_fasta"]
 
 _libs = {}
 
@@ -302,6 +317,8 @@ def load_library(path=None):
                                        C.c_double, C.c_int32, C.c_int32, C.POINTER(AcUnassembledInfo)]
     lib.ac_polish_fasta.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint32, C.POINTER(C.c_uint32), C.c_uint32, C.c_uint32, C.c_int32,
                                     C.c_int32, C.POINTER(AcPolishInfo)]
+    lib.ac_variants_fasta.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint32, C.POINTER(C.c_uint32), C.c_uint32, C.c_double,
+                                      C.c_int32, C.c_int32, C.POINTER(AcVariantsInfo)]
     lib.ac_table_text.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint64, C.c_int32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     _libs[path] = lib
     return lib
@@ -1016,4 +1033,27 @@ def polish(reads, assembly, out_dir, k=21, min_count=None, max_indel=3, rounds=3
         lines = f.read().splitlines()
     out["applied"] = [{"round": int(r[0]), "contig": r[1], "position": int(r[2]), "ref": r[3], "alt": r[4], "score": int(r[5])}
                     for r in (line.split("\t") for line in lines[1:])]
+    return out
+
+
+def variants(reads, assembly, out_dir, k=21, min_count=None, max_indel=1, min_fraction=0.1, device=0, verbose=False, lib=None):
+    """`autocycler variants` (DESIGN.md §23): the alleles the reads carry beside the consensus, with every position's alternatives
+    screened on the GPU (not in the reference).  Returns the info dict (t is "min_count", the stage timings in ms) with "rows": per row of
+    the variants.vcf the call wrote a dict of contig, pos, ref, alt, af, ak, rk and pk."""
+    lib = lib or load_library()
+    info = AcVariantsInfo()
+    t = None if min_count is None else C.byref(C.c_uint32(min_count))
+    _raise_unless_ok(lib, lib.ac_variants_fasta(os.fsencode(reads), os.fsencode(assembly), os.fsencode(out_dir), k, t, max_indel, min_fraction,
+                                                device, 1 if verbose else 0, C.byref(info)))
+    out = info.as_dict()
+    rows = []
+    with open(os.path.join(out_dir, "variants.vcf")) as f:
+        for line in f:
+            if line.startswith("#"):
+                continue
+            c = line.rstrip("\n").split("\t")
+            tags = dict(x.split("=") for x in c[7].split(";"))
+            rows.append({"contig": c[0], "pos": int(c[1]), "ref": c[3], "alt": c[4], "af": float(tags["AF"]), "ak": int(tags["AK"]),
+                         "rk": int(tags["RK"]), "pk": int(tags["PK"])})
+    out["rows"] = rows
     return out

@@ -33,6 +33,7 @@
 #include "host_qv.h"
 #include "host_unassembled.h"
 #include "host_polish.h"
+#include "host_variants.h"
 #include <mutex>
 #include <immintrin.h>
 #include <functional>
@@ -1637,11 +1638,13 @@ int ac_png_write(const char* path, const uint8_t* rgb, uint32_t width, uint32_t 
 // ---- `autocycler subsample` (subsample.rs) --------------------------------------------------------------------------------------
 namespace {
 // One subsample device object per device, as for dotplot: its buffers (and pinned windows) are kept for the next call on that device.
-// genome_size, depth, qv, unassembled and polish read through the same object and keep their packed streams and tables beside it.
+// genome_size, depth, qv, unassembled, polish and variants read through the same object and keep their packed streams and tables beside it.
 std::mutex g_subsample_mu;
 struct SubsampleDevice {
     DeviceContext ctx; DeviceSubsample sub; DeviceSpectrum spec; DeviceDepth depth; DeviceQv qv; DeviceUnassembled unassembled; DevicePolish polish;
-    explicit SubsampleDevice(int32_t device) : ctx(device, nullptr), sub(ctx), spec(ctx), depth(ctx), qv(ctx), unassembled(ctx), polish(ctx) {}
+    DeviceVariants variants;
+    explicit SubsampleDevice(int32_t device)
+        : ctx(device, nullptr), sub(ctx), spec(ctx), depth(ctx), qv(ctx), unassembled(ctx), polish(ctx), variants(ctx) {}
 };
 SubsampleDevice& subsample_device(int32_t device) {        // with g_subsample_mu held
     static std::vector<std::pair<int32_t, SubsampleDevice*>> devices;
@@ -2121,6 +2124,73 @@ int ac_polish_fasta(const char* reads, const char* assembly, const char* out_dir
         info->kernel_ms = r.kernel_ms; info->scan_ms = r.scan_ms; info->pack_ms = r.pack_reads_ms; info->count_ms = r.spectrum.count_ms + r.spectrum.hist_ms;
         info->contig_ms = r.device.pack_ms; info->fill_ms = r.device.fill_ms; info->recount_ms = r.device.sweep.count_ms;
         info->candidate_ms = r.device.candidate_ms; info->choose_ms = r.device.choose_ms;
+        info->read_ms = r.read_ms; info->copy_ms = r.copy_ms; info->host_ms = r.host_ms; info->write_ms = write_ms;
+    }
+    return ok(nullptr);
+    AC_GUARD_END(nullptr)
+}
+
+// ---- `autocycler variants`: the alleles the reads carry beside the consensus (not in the reference) -------------------------------------
+int ac_variants_fasta(const char* reads, const char* assembly, const char* out_dir, uint32_t k, const uint32_t* min_count, uint32_t max_indel,
+                      double min_fraction, int32_t device, int32_t verbose, ac_variants_info* info) {
+    if (!reads || !assembly || !out_dir) return set_error(nullptr, AC_EINVAL, "null argument");
+    AC_GUARD_BEGIN
+    const std::string in = reads, fasta = assembly, dir = out_dir;
+    if (k < 11 || k > 31 || k % 2 == 0) return set_error(nullptr, AC_EINPUT, "--kmer must be odd and between 11 and 31");
+    if (min_count && (*min_count < 1 || *min_count > AC_GS_BINS - 1))
+        return set_error(nullptr, AC_EINPUT, "--min_count must be between 1 and " + std::to_string(AC_GS_BINS - 1));
+    if (max_indel > 3) return set_error(nullptr, AC_EINPUT, "--max_indel must be between 0 and 3");
+    if (!(min_fraction > 0.0 && min_fraction <= 1.0)) return set_error(nullptr, AC_EINPUT, "--min_fraction must be above 0 and at most 1");
+    int rc;
+    if ((rc = check_file(in)) != AC_OK) return rc;
+    if ((rc = check_file(fasta)) != AC_OK) return rc;
+    struct stat st;
+    if (stat(dir.c_str(), &st) == 0 && !S_ISDIR(st.st_mode)) return set_error(nullptr, AC_EINPUT, dir + " exists but is not a directory");
+    if (!make_dirs(dir)) return set_error(nullptr, AC_EINPUT, "failed to create directory " + dir + "\n" + strerror(errno));
+    if (verbose) {
+        fprintf(stderr, "\nStarting autocycler variants\n    This command finds the alleles the reads carry beside the consensus, with every "
+                        "position's alternatives screened on the GPU. It is not in the reference.\n\nSettings:\n  --reads %s\n  --input %s\n"
+                        "  --out_dir %s\n  --kmer %u\n", in.c_str(), fasta.c_str(), dir.c_str(), k);
+        if (min_count) fprintf(stderr, "  --min_count %u\n", *min_count);
+        fprintf(stderr, "  --max_indel %u\n  --min_fraction %s\n\n", max_indel, format_float(min_fraction).c_str());
+    }
+    VariantsResult r;
+    {
+        std::lock_guard<std::mutex> lock(g_subsample_mu);
+        SubsampleDevice& d = subsample_device(device);
+        try {
+            variants_run(d.sub, d.spec, d.polish, d.variants, fasta, in, k, min_count, max_indel, min_fraction, subsample_window_size(), r);
+        } catch (const AcIoError& e) { return set_error(nullptr, AC_EIO, e.msg); }
+        catch (const std::length_error& e) { return set_error(nullptr, AC_ERANGE, e.what()); }
+    }
+    const auto t0 = std::chrono::steady_clock::now();
+    const std::pair<std::string, std::string> files[] = {{"variants.vcf", variants_vcf(r)}, {"summary.tsv", variants_summary(r)}};
+    for (const auto& f : files)
+        if (!write_file(dir + "/" + f.first, f.second)) return set_error(nullptr, AC_EIO, "cannot write " + dir + "/" + f.first);
+    const double write_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    if (verbose) {
+        fprintf(stderr, "K-mer variants (k = %u):\n  reads: %llu\n  read k-mer windows: %llu\n  valley: %s\n  min_count: %llu%s\n"
+                        "  positions: %llu\n  screened: %llu\n  candidates: %llu (%llu passing)\n  variants: %llu (%llu substitutions, %llu insertions, "
+                        "%llu deletions)\n  paralog: %llu\n  alt_major: %llu\n\nFinished!\nVariants: %s/variants.vcf\n\n", k,
+                (unsigned long long)r.reads, (unsigned long long)r.read_windows, r.valley ? std::to_string(r.valley).c_str() : "none",
+                (unsigned long long)r.min_count, min_count ? " (given)" : " (the valley)", (unsigned long long)r.positions,
+                (unsigned long long)r.screened, (unsigned long long)r.candidates, (unsigned long long)r.passing, (unsigned long long)r.rows.size(),
+                (unsigned long long)r.substitutions, (unsigned long long)r.insertions, (unsigned long long)r.deletions,
+                (unsigned long long)r.paralog, (unsigned long long)r.alt_major, dir.c_str());
+    }
+    if (info) {
+        *info = ac_variants_info{};
+        info->contigs = r.recs.size(); info->k = k; info->min_count = (uint32_t)r.min_count; info->valley = r.valley;
+        info->reads = r.reads; info->read_windows = r.read_windows; info->read_bases = r.read_bases; info->distinct = r.distinct;
+        info->kmers = r.kmers; info->positions = r.positions; info->screened = r.screened; info->candidates = r.candidates;
+        info->loci = r.loci; info->passing = r.passing; info->variants = r.rows.size(); info->substitutions = r.substitutions;
+        info->insertions = r.insertions; info->deletions = r.deletions; info->paralog = r.paralog; info->alt_major = r.alt_major;
+        info->table_bytes = r.device.table_bytes; info->candidate_table_bytes = r.device.candidate_bytes; info->batches = r.device.batches;
+        info->spectrum_table_bytes = r.spectrum.table_bytes; info->partitions = r.spectrum.partitions;
+        info->reruns = r.spectrum.reruns + r.device.sweep.reruns;
+        info->kernel_ms = r.kernel_ms; info->scan_ms = r.scan_ms; info->pack_ms = r.pack_reads_ms; info->count_ms = r.spectrum.count_ms + r.spectrum.hist_ms;
+        info->contig_ms = r.device.pack_ms; info->fill_ms = r.device.fill_ms; info->screen_ms = r.va.screen_ms; info->recount_ms = r.device.sweep.count_ms;
+        info->candidate_ms = r.device.candidate_ms; info->ref_ms = r.va.ref_ms;
         info->read_ms = r.read_ms; info->copy_ms = r.copy_ms; info->host_ms = r.host_ms; info->write_ms = write_ms;
     }
     return ok(nullptr);

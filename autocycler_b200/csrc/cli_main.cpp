@@ -4,8 +4,8 @@
 // which departs from the reference on purpose: a k-mer depth estimate on the GPU instead of the length of a Raven assembly; and
 // `autocycler depth`, read-measured contig depth (not in the reference) with the reference's helper depth filter; `autocycler qv`,
 // each assembly's k-mer QV and completeness against the reads (not in the reference); `autocycler unassembled`, the reads the
-// assembly does not explain (not in the reference); and `autocycler polish`, the consensus corrected from the reads' k-mers (not in the
-// reference).
+// assembly does not explain (not in the reference); `autocycler polish`, the consensus corrected from the reads' k-mers (not in the
+// reference); and `autocycler variants`, the alleles the reads carry beside the consensus (not in the reference).
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -529,6 +529,57 @@ static int polish_main(int argc, char** argv) {
     return finish(rc);
 }
 
+// `autocycler variants`: the alleles the reads carry beside the consensus, with every position's alternatives screened on the GPU (not in
+// the reference).  summary.tsv also goes to stdout, byte for byte.
+static const char* variants_usage =
+    "Usage: autocycler variants --reads <READS> --input <FASTA> --out_dir <DIR> [--kmer 21] [--min_count N] [--max_indel 1]\n"
+    "                           [--min_fraction 0.1] [--device N]\n\n"
+    "Finds the alleles the reads carry beside the consensus, with every position's alternatives screened on the GPU: a substitution,\n"
+    "or an insertion or deletion of up to --max_indel bases, whose k-mers the reads hold at least --min_count times, at a fraction of at\n"
+    "least --min_fraction beside the consensus's own k-mers. This command is not in the reference. Writes variants.vcf (indels\n"
+    "left-aligned) and summary.tsv (also to stdout).\n\n"
+    "Options:\n"
+    "  -r, --reads <READS>            Reads in FASTQ format, gzipped or not (required)\n"
+    "  -i, --input <FASTA>            Assembly in FASTA format, gzipped or not (required)\n"
+    "  -o, --out_dir <DIR>            Directory to create and write the VCF and summary into (required)\n"
+    "      --kmer <KMER>              K-mer size, odd, 11 to 31 [default: 21]\n"
+    "      --min_count <N>            Read count an alternative allele's k-mers need, 1 to 16383 [default: the valley of the reads'\n"
+    "                                 k-mer spectrum]\n"
+    "      --max_indel <L>            Longest insertion or deletion tried, 0 to 3 [default: 1]\n"
+    "      --min_fraction <F>         Least alternative allele fraction, above 0 and at most 1 [default: 0.1]\n"
+    "      --device <ORDINAL>         CUDA device [default: 0]\n";
+static int variants_main(int argc, char** argv) {
+    Args a{argc, argv, variants_usage};
+    std::string reads, in, out; bool has_min = false;
+    unsigned long k = 21, min_count = 0, max_indel = 1; double min_fraction = 0.1; int device = 0;
+    auto refuse = [&]() { fprintf(stderr, "error: invalid value '%s' for '%s'\n%s", argv[a.i], a.flag.c_str(), variants_usage); return 2; };
+    while (a.next()) {
+        if (a.is("-r", "--reads")) reads = a.value();
+        else if (a.is("-i", "--input")) in = a.value();
+        else if (a.is("-o", "--out_dir")) out = a.value();
+        else if (a.is("--kmer")) { k = (unsigned long)a.number(true); if (k < 11 || k > 31 || k % 2 == 0) return refuse(); }
+        else if (a.is("--min_count")) { min_count = (unsigned long)a.number(true); if (min_count < 1 || min_count > 16383) return refuse(); has_min = true; }
+        else if (a.is("--max_indel")) { max_indel = (unsigned long)a.number(true); if (max_indel > 3) return refuse(); }
+        else if (a.is("--min_fraction")) { min_fraction = a.number(false); if (!(min_fraction > 0.0 && min_fraction <= 1.0)) return refuse(); }
+        else if (a.is("--device")) device = atoi(a.value());
+        else if (a.is("-h", "--help")) return a.help();
+        else return a.unexpected();
+    }
+    if (reads.empty() || in.empty() || out.empty()) return a.missing();
+    const uint32_t t = (uint32_t)min_count;
+    const int rc = ac_variants_fasta(reads.c_str(), in.c_str(), out.c_str(), (uint32_t)k, has_min ? &t : nullptr, (uint32_t)max_indel,
+                                     min_fraction, device, 1, nullptr);
+    if (rc == AC_OK) {
+        FILE* f = fopen((out + "/summary.tsv").c_str(), "rb");
+        if (f) {
+            char buf[1 << 16]; size_t n;
+            while ((n = fread(buf, 1, sizeof buf, f)) > 0) fwrite(buf, 1, n, stdout);
+            fclose(f);
+        }
+    }
+    return finish(rc);
+}
+
 int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "dotplot") == 0) return dotplot_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "resolve") == 0) return resolve_main(argc, argv);
@@ -546,6 +597,7 @@ int main(int argc, char** argv) {
     if (argc >= 2 && strcmp(argv[1], "qv") == 0) return qv_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "unassembled") == 0) return unassembled_main(argc, argv);
     if (argc >= 2 && strcmp(argv[1], "polish") == 0) return polish_main(argc, argv);
+    if (argc >= 2 && strcmp(argv[1], "variants") == 0) return variants_main(argc, argv);
     fprintf(stderr, "%s", compress_usage);
     return 2;
 }

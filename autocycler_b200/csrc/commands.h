@@ -1,5 +1,5 @@
-// The device parts of `autocycler trim`, `resolve`, `cluster`, `dotplot`, `subsample`, `helper genome_size`, `depth`, `qv`, `unassembled`
-// and `polish`.  Each object owns its device buffers (allocated on first use, kept for the next call) and runs on the device and stream
+// The device parts of `autocycler trim`, `resolve`, `cluster`, `dotplot`, `subsample`, `helper genome_size`, `depth`, `qv`, `unassembled`,
+// `polish` and `variants`.  Each object owns its device buffers (allocated on first use, kept for the next call) and runs on the device and stream
 // of the DeviceContext it is given, which must outlive it.
 #pragma once
 #include <cstdint>
@@ -361,10 +361,51 @@ public:
     // the first of them.
     void choose(DeviceSpectrum& spec, const PlLocus* loci, uint64_t n, uint32_t max_indel, uint32_t t, uint64_t budget_slots, uint32_t* out,
                 PlRun* run);
+    // windows()'s first steps: the contigs packed and their keys claimed in the query table, with every count 0 (fill it in a sweep).
+    void pack(const uint8_t* bytes, const uint64_t* len, uint32_t n_contigs, uint64_t windows, PlRun* run);
+    // choose()'s claim, fill and score of the candidates of n loci, batch by batch: each(first locus, loci, device scores) runs after a
+    // batch's scores (score[i * C + c], as PlScoreBody writes them) are on the device's stream.
+    void score(DeviceSpectrum& spec, const PlLocus* loci, uint64_t n, uint32_t max_indel, uint32_t t, uint64_t budget_slots,
+               const std::function<void(uint64_t, uint64_t, const uint32_t*)>& each, PlRun* run);
+    // The round packed last, on the device: its codes, validity masks and packed words, and the query table of its keys.
+    const uint64_t* packed_codes() { return d_code.as<uint64_t>(); }
+    const uint32_t* packed_valid() { return d_valid.as<uint32_t>(); }
+    uint64_t packed_words() const { return words; }
+    DepthSlot* query_table() { return d_table.as<DepthSlot>(); }
+    uint64_t query_slots() const { return slots; }
+    uint32_t kmer() const { return k; }
 private:
     void fill(DeviceSpectrum& spec, DepthSlot* table, uint64_t slots, PlRun* run);
     DeviceContext& ctx;
     uint32_t k = 21;
     uint64_t slots = 0, words = 0;
     DevBuf d_bytes, d_contig, d_code, d_valid, d_wcid, d_table, d_mask, d_loci, d_cand, d_score, d_out;
+};
+
+// `autocycler variants`: the alleles the reads carry beside the consensus (DESIGN.md §23).  The input is packed and its keys claimed and
+// filled as polish's first round (DevicePolish::pack and a sweep of PlFillBody); in the same sweep VaScreenBody looks up, for the window
+// that ends at each base p, the three windows S(p, b) with the last base swapped, and sets a bit where r >= t.  The host turns the masks
+// into candidates, DevicePolish::score scores them, and VaRefBody gives each passing candidate the input's ref count and PK.
+// One candidate to measure: its position as a polish locus (a = p - k + 1) and its index in pl_edit's order.
+struct VaCandidate { PlLocus lo; uint32_t c, pad; };
+// What the device ran beyond the polish object's steps: the screen's and the ref pass's time (CUDA events; 0 under emulation).
+struct VaRun { float screen_ms = 0.f, ref_ms = 0.f; };
+
+class DeviceVariants {
+public:
+    explicit DeviceVariants(DeviceContext& ctx) : ctx(ctx) {}
+    ~DeviceVariants() { ctx.make_current(); }
+    // After pl.pack: one sweep over the spectrum's partitions fills pl's query table and screens every window.  mask[3 w + j] (host, three
+    // u32 per packed word) has bit i set when the window ending at base i of word w, its last base replaced by the j-th of the other three
+    // bases in A, C, G, T order, has r >= t.
+    void screen(DeviceSpectrum& spec, DevicePolish& pl, uint32_t t, uint32_t* mask, PlRun* prun, VaRun* run);
+    // pl.score for n loci of the input: score[i * C + c] (host) as PlScoreBody writes it, C = DevicePolish::candidates(max_indel).
+    void scores(DeviceSpectrum& spec, DevicePolish& pl, const PlLocus* loci, uint64_t n, uint32_t max_indel, uint32_t t, uint64_t budget_slots,
+                uint32_t* score, PlRun* prun);
+    // out[2 i] = candidate i's ref (the least r over the input's windows that start at a .. p + d, 0 for a missing one) and out[2 i + 1] its
+    // PK (checked windows whose key pl's query table holds, the last one left out for an indel).  Host arrays.
+    void ref(DevicePolish& pl, const VaCandidate* cand, uint64_t n, uint32_t max_indel, uint32_t* out, VaRun* run);
+private:
+    DeviceContext& ctx;
+    DevBuf d_mask, d_cand, d_out;
 };

@@ -1,9 +1,11 @@
 // Device part of `autocycler polish`: each round's contigs packed and their canonical keys claimed in a query table whose read counts a
 // sweep over the read spectrum's partitions fills, the mask of the windows the reads do not support, and for each attempted locus its
-// candidate edits' checked windows claimed, filled, scored and reduced to a choice.  Not in the reference (DESIGN.md §22).  This file
-// compiles with nvcc for sm_90a (product) and with g++ -DAC_EMULATE (tests/emu, serial execution of the same bodies).
+// candidate edits' checked windows claimed, filled, scored and reduced to a choice.  Not in the reference (DESIGN.md §22).  The fill, the
+// candidates' windows, their claim and their score are in pl_kmers.h, which `variants` shares.  This file compiles with nvcc for sm_90a
+// (product) and with g++ -DAC_EMULATE (tests/emu, serial execution of the same bodies).
 #include "commands.h"
 #include "dp_kmers.h"
+#include "pl_kmers.h"
 
 #include <algorithm>
 #include <stdexcept>
@@ -14,16 +16,6 @@
 // polish: pack, claim, fill and mask per round, then candidates, fill, score and choice per batch of loci, see DESIGN.md §22
 // ------------------------------------------------------------------------------------------------
 namespace {
-// One thread per slot of a query table, for the keys of spectrum partition `part`: the key's read count r.
-struct PlFillBody {
-    DepthSlot* table; const GsSlot* spec; uint64_t spec_slots, parts, part;
-    AC_D void operator()(uint64_t s) const {
-        const uint64_t tag = table[s].key;
-        if (!tag) return;
-        const uint64_t h = gs_mix(tag - 1);
-        if (ac_umul64hi(h, parts) == part) table[s].count = ua_read_count(spec, spec_slots, parts, h, tag - 1);
-    }
-};
 // One thread per packed word of the round's contigs: bit j of mask[w] is set when the window that ends at base j has r < t.
 struct PlSupportBody {
     const uint64_t* code; const uint32_t* valid; uint32_t k; const DepthSlot* table; uint64_t slots; uint32_t t; uint32_t* mask;
@@ -38,59 +30,6 @@ struct PlSupportBody {
     }
 };
 
-// Calls f(canonical key) for each checked window of candidate c at locus lo, in order: the windows of the edited sequence that start
-// at a, k + s of them, rolled over the round's bases [a, p0), the edit's bases and the round's bases from p0 + skip to the span's end
-// p0 + d + k.  False (possibly after some calls) when the candidate is not allowed, a deletion past the contig's last base or, on a linear
-// contig, a window past its end, or when a checked base is not A/C/G/T.
-template <class F> AC_D bool pl_each_key(const uint64_t* code, const uint32_t* valid, const PlLocus& lo, uint32_t c, uint32_t k, uint32_t L,
-                                         F&& f) {
-    const uint64_t n = lo.len, p0 = lo.a + k - 1 < n ? lo.a + k - 1 : lo.a + k - 1 - n;
-    uint32_t b = 0;
-    auto base = [&](uint64_t i) {                            // the round's base at i (cyclic on a circular contig); false: not A/C/G/T
-        if (i >= n) i -= n;
-        const uint64_t w = lo.word0 + i / 32;
-        const uint32_t o = (uint32_t)(i % 32);
-        b = (uint32_t)(code[w] >> (2 * o)) & 3u;
-        return ((valid[w] >> o) & 1u) != 0;
-    };
-    base(p0);
-    const PlEdit e = pl_edit(c, L, b);
-    const uint64_t d = e.mlen ? 0 : e.skip;
-    if (p0 + d > n || (!lo.circular && p0 + d + k > n)) return false;
-    const uint32_t len = 2 * k - 1 + e.mlen + (uint32_t)d - e.skip, top = 2 * (k - 1);
-    const uint64_t mask = (1ull << (2 * k)) - 1;
-    uint64_t fw = 0, rc = 0;
-    for (uint32_t x = 0; x < len; ++x) {
-        if (x < k - 1) { if (!base(lo.a + x)) return false; }
-        else if (x < k - 1 + e.mlen) b = (e.mid >> (2 * (x - (k - 1)))) & 3u;
-        else if (!base(p0 + e.skip + (x - (k - 1) - e.mlen))) return false;
-        fw = ((fw << 2) | b) & mask; rc = (rc >> 2) | ((uint64_t)(3 - b) << top);
-        if (x >= k - 1) f(fw < rc ? fw : rc);
-    }
-    return true;
-}
-
-// One thread per (locus, candidate): the candidate's checked windows claimed in the candidate table.
-struct PlCandidateBody {
-    const uint64_t* code; const uint32_t* valid; const PlLocus* loci; uint32_t k, L, C; DepthSlot* table; uint64_t slots;
-    AC_D void operator()(uint64_t i) const {
-        pl_each_key(code, valid, loci[i / C], (uint32_t)(i % C), k, L, [&](uint64_t key) { dp_claim(table, slots, key); });
-    }
-};
-// One thread per (locus, candidate), after the fill: score[i] = the minimum r over its checked windows when it passes (every window
-// allowed, of A/C/G/T bases and with r >= t), else 0.
-struct PlScoreBody {
-    const uint64_t* code; const uint32_t* valid; const PlLocus* loci; uint32_t k, L, C; const DepthSlot* table; uint64_t slots; uint32_t t;
-    uint32_t* score;
-    AC_D void operator()(uint64_t i) const {
-        uint32_t m = 0xFFFFFFFFu;
-        const bool ok = pl_each_key(code, valid, loci[i / C], (uint32_t)(i % C), k, L, [&](uint64_t key) {
-            const uint32_t r = qv_read_count(table, slots, key);
-            m = r < m ? r : m;
-        });
-        score[i] = ok && m >= t ? m : 0;
-    }
-};
 AC_D void pl_take(uint32_t v, uint32_t c, uint32_t& best, uint32_t& count, uint32_t& first) {
     if (v > best) { best = v; count = 1; first = c; }
     else if (v && v == best) ++count;
@@ -155,8 +94,7 @@ void DevicePolish::fill(DeviceSpectrum& spec, DepthSlot* table, uint64_t n_slots
     }, &run->sweep);
 }
 
-void DevicePolish::windows(DeviceSpectrum& spec, const uint8_t* bytes, const uint64_t* len, uint32_t n, uint64_t windows, uint32_t t,
-                           uint32_t* mask, PlRun* run) {
+void DevicePolish::pack(const uint8_t* bytes, const uint64_t* len, uint32_t n, uint64_t windows, PlRun* run) {
     ctx.make_current();
     AcStream* st = &ctx.stream;
     std::vector<DpContig> contig(n + 1);
@@ -181,6 +119,12 @@ void DevicePolish::windows(DeviceSpectrum& spec, const uint8_t* bytes, const uin
     tp.stop();
     ac_sync(st);
     run->pack_ms += tp.ms();
+}
+
+void DevicePolish::windows(DeviceSpectrum& spec, const uint8_t* bytes, const uint64_t* len, uint32_t n, uint64_t windows, uint32_t t,
+                           uint32_t* mask, PlRun* run) {
+    pack(bytes, len, n, windows, run);
+    AcStream* st = &ctx.stream;
     fill(spec, d_table.as<DepthSlot>(), slots, run);
     AcTimer ts(st);
     ac_launch("pl_support", st, PlSupportBody{d_code.as<uint64_t>(), d_valid.as<uint32_t>(), k, d_table.as<DepthSlot>(), slots, t,
@@ -191,8 +135,8 @@ void DevicePolish::windows(DeviceSpectrum& spec, const uint8_t* bytes, const uin
     run->fill_ms += ts.ms();
 }
 
-void DevicePolish::choose(DeviceSpectrum& spec, const PlLocus* loci, uint64_t n, uint32_t L, uint32_t t, uint64_t budget, uint32_t* out,
-                          PlRun* run) {
+void DevicePolish::score(DeviceSpectrum& spec, const PlLocus* loci, uint64_t n, uint32_t L, uint32_t t, uint64_t budget,
+                         const std::function<void(uint64_t, uint64_t, const uint32_t*)>& each, PlRun* run) {
     if (!n) return;
     ctx.make_current();
     AcStream* st = &ctx.stream;
@@ -221,11 +165,21 @@ void DevicePolish::choose(DeviceSpectrum& spec, const PlLocus* loci, uint64_t n,
         ac_launch("pl_score", st, PlScoreBody{d_code.as<uint64_t>(), d_valid.as<uint32_t>(), d_loci.as<PlLocus>(), k, L, (uint32_t)C, cand,
                                               cslots, t, d_score.as<uint32_t>()}, nb * C);
         ts.stop();
+        each(b0, nb, d_score.as<uint32_t>());                // synchronizes the stream
+        run->candidate_ms += ts.ms();
+    }
+}
+
+void DevicePolish::choose(DeviceSpectrum& spec, const PlLocus* loci, uint64_t n, uint32_t L, uint32_t t, uint64_t budget, uint32_t* out,
+                          PlRun* run) {
+    AcStream* st = &ctx.stream;
+    const uint32_t C = (uint32_t)candidates(L);
+    score(spec, loci, n, L, t, budget, [&](uint64_t b0, uint64_t nb, const uint32_t* score) {
         AcTimer tx(st);
-        ac_launch("pl_choose", st, PlChooseBody{d_score.as<uint32_t>(), (uint32_t)C, d_out.as<uint32_t>()}, nb * 32);
+        ac_launch("pl_choose", st, PlChooseBody{score, C, d_out.as<uint32_t>()}, nb * 32);
         tx.stop();
         ac_d2h(out + 3 * b0, d_out.p, nb * 12, st);
         ac_sync(st);
-        run->candidate_ms += ts.ms(); run->choose_ms += tx.ms();
-    }
+        run->choose_ms += tx.ms();
+    }, run);
 }

@@ -35,6 +35,7 @@
  *   qv (k-mer QV and completeness)          not in the reference     -> ac_qv_dir
  *   unassembled (reads the assembly lacks)  not in the reference     -> ac_unassembled_dir
  *   polish (k-mer consensus correction)     not in the reference     -> ac_polish_fasta
+ *   variants (alleles beside the consensus) not in the reference     -> ac_variants_fasta
  *
  * Conventions: every function returns 0 on success and a negative AC_E* code on failure; the message
  * is available from ac_last_error(handle) (or ac_last_error(NULL) when no handle exists).  No C++
@@ -630,6 +631,55 @@ typedef struct {
 } ac_polish_info;
 int ac_polish_fasta(const char* reads, const char* assembly, const char* out_dir, uint32_t k, const uint32_t* min_count, uint32_t max_indel,
                     uint32_t rounds, int32_t device, int32_t verbose, ac_polish_info* info);
+
+/* `autocycler variants -r reads -i assembly -o out_dir [--kmer 21] [--min_count N] [--max_indel 1] [--min_fraction 0.1]`: the alleles the
+ * reads carry beside the consensus, with every position's alternatives screened on the GPU.  Not in the reference (DESIGN.md section 23).
+ * Inputs, windows, r(key) and t (*min_count, 1 .. AC_GENOME_SIZE_BINS - 1, else AC_EINPUT; the valley when min_count is NULL) are
+ * ac_polish_fasta's, on the input sequence only; t is the least count an alternative allele needs.  A position p is tried when it can be
+ * polish's p0 with a = p - k + 1 (a linear contig: p >= k - 1; a circular one: every p when it is at least 2k + 2 max_indel long) and the
+ * window that ends at p has k A/C/G/T bases.  S(p, b): the input's bases [p - k + 1, p) followed by b; p is screened when r(S(p, e)) >= t
+ * for some e other than its base.  Its candidates are polish's (3 substitutions, deletions of 1 .. max_indel bases, insertions of every
+ * string of 1 .. max_indel bases before p), each taken only in its rightmost form, where its first base e in the edited sequence at p
+ * differs from the input's (a deletion of d: base p + d, cyclic, A/C/G/T; an insertion: its first base), and only when S(p, e) passes the
+ * screen.  Such a candidate passes as in polish (every checked window a window inside a linear contig, with r >= t); alt = the least r over
+ * its checked windows, ref = the least r over the input's windows that start at a .. p + d (0 for a missing one; d = 0 but for a deletion),
+ * PK = its checked windows whose key the input holds (an indel's last one left out).  A variant: alt >= min_fraction * (alt + ref) in f64,
+ * 0 < min_fraction <= 1 (else AC_EINPUT).  max_indel: 0..3, else AC_EINPUT.  out_dir (created if needed) gets variants.vcf (VCF 4.2, indels
+ * left-aligned, AF = alt / (alt + ref), AK, RK, PK) and summary.tsv.  k: odd, 11..31, else AC_EINPUT.  An assembly or reads without
+ * windows: AC_EINPUT.  The window table beyond half the free device memory, or one position's candidate table beyond half of what the read
+ * spectrum leaves: AC_ERANGE.  verbose prints the settings and the counts to stderr.  Calls on one device run one at a time, with
+ * subsample's.  info may be NULL. */
+typedef struct {
+    uint64_t contigs;
+    uint32_t k;
+    uint32_t min_count;                /* t, given or the valley */
+    uint64_t valley;                   /* v of the reads' histogram (0: none) */
+    uint64_t reads, read_windows, read_bases;
+    uint64_t distinct;                 /* distinct canonical read k-mers */
+    uint64_t kmers;                    /* the input's windows */
+    uint64_t positions, screened, candidates;   /* tried positions, those with an alternative window at or above t, rightmost candidates
+                                                   whose first window passes */
+    uint64_t loci;                     /* positions whose candidates were scored */
+    uint64_t passing, variants;        /* candidates that pass, and of them the rows of variants.vcf */
+    uint64_t substitutions, insertions, deletions, paralog, alt_major;
+    uint64_t table_bytes;              /* the input's window table */
+    uint64_t candidate_table_bytes;    /* the largest candidate table */
+    uint64_t batches;                  /* candidate batches */
+    uint64_t spectrum_table_bytes;     /* the read spectrum's largest table */
+    uint64_t partitions, reruns;       /* of the read spectrum, over the count and every sweep */
+    float kernel_ms;                   /* CUDA events around every kernel, summed (0 under emulation) */
+    float scan_ms, pack_ms, count_ms, contig_ms, fill_ms, screen_ms, recount_ms, candidate_ms, ref_ms;   /* record scan, read packing,
+                                                                                                    spectrum count and histogram, contig pack
+                                                                                                    and claim, read count fills, the screen,
+                                                                                                    the sweeps' recounts of partitions,
+                                                                                                    candidate claims and scores, ref and PK */
+    double read_ms;                    /* host: reading and gunzipping the reads */
+    double copy_ms;                    /* host wall time of the window uploads */
+    double host_ms;                    /* host: the contigs' packing, the candidates from the masks, the fraction test and left-alignment */
+    double write_ms;                   /* host: writing the output files */
+} ac_variants_info;
+int ac_variants_fasta(const char* reads, const char* assembly, const char* out_dir, uint32_t k, const uint32_t* min_count, uint32_t max_indel,
+                      double min_fraction, int32_t device, int32_t verbose, ac_variants_info* info);
 
 #ifdef __cplusplus
 }
