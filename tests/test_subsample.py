@@ -173,7 +173,7 @@ def test_inputs(lib, name, tmp_path):
 
 
 @pytest.mark.parametrize("lib", builds(), indirect=True)
-@pytest.mark.parametrize("count", [2, 3, 4, 7, 100])
+@pytest.mark.parametrize("count", [2, 3, 4, 7, 64, 65, 100, 128, 129])
 def test_counts(lib, count, tmp_path):
     path = str(tmp_path / "r.fq")
     synth.write_reads(synth.make_reads(GENOME, depth=60, n50=2500, seed=count), path)
@@ -205,11 +205,11 @@ def test_subset_sizes(lib, setting, tmp_path):
 
 
 @pytest.mark.parametrize("lib", builds(), indirect=True)
-@pytest.mark.parametrize("crlf", [False, True])
-def test_window_at_every_byte(lib, crlf, tmp_path, monkeypatch):
-    path = str(tmp_path / "r.fq")
-    synth.write_reads(reads_of([7, 0, 12, 3]), path, crlf=crlf, plus_header=True)
-    size = os.path.getsize(path)
+@pytest.mark.parametrize("crlf,gz", [(False, False), (True, False), (False, True), (True, True)], ids=["False", "True", "False-gz", "True-gz"])
+def test_window_at_every_byte(lib, crlf, gz, tmp_path, monkeypatch):
+    path = str(tmp_path / ("r.fq.gz" if gz else "r.fq"))
+    synth.write_reads(reads_of([7, 0, 12, 3]), path, gz=gz, crlf=crlf, plus_header=True)
+    size = len(O.read_bytes(path))
     want = O.subsample(path, "10", count=3, min_read_depth=1.0, seed=9)
     for w in range(1, size + 2):
         monkeypatch.setenv("AC_SUBSAMPLE_WINDOW", str(w))
